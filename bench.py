@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the torchcde_b200 hot path against BASELINE.json's metric.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one fused fixed-step solve ``cdeint(CubicSpline(hermite coeffs), linear func, z0,
 t=[0, L-1], method='rk4', options={'step_size': 1})`` over one synthetic batch at BASELINE
@@ -9,10 +9,15 @@ config 3: batch 65536 per GPU, length 256, 8 input channels, 32 hidden channels,
 Prints ONE JSON line (rank 0).  See DESIGN.md "Measurement" for what every key means.
 
 Timing rules: inputs resident in HBM for ``value`` (CUDA events, max over ranks, barrier +
-synchronize both sides); the coefficient tensor is 2.1 GB per GPU, far larger than the 126 MB
-L2, so no flush is needed between iterations.  ``e2e`` runs the user pipeline from pinned HOST
+synchronize both sides); the coefficient tensor is 2.1 GB per GPU, far larger than the 50 MB
+L2 of an H100, so no flush is needed between iterations.  ``e2e`` runs the user pipeline from pinned HOST
 series through ``torchcde_b200.hostio.cdeint_from_host_series`` (H2D of x and z0, fused gap fill +
 Hermite coefficients on the device, fused solve, D2H) with the copies inside the timed region.
+
+``--dump-outputs DIR`` writes, after the timed steps, what the last timed solve returned:
+``DIR/solution.npy``, float32 [65536, 2, 32] (16.8 MB) on one GPU; a fixed sample per rank on several
+(``dump_solution``); with ``--impl reference`` the CPU arm's [8192, 2, 32] solution.  The inputs are seeded,
+so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -42,7 +47,7 @@ WORKLOAD = ("cdeint rk4 step_size=1 (255 steps, 1020 stage evals), CubicSpline(h
 
 def config_for(world):
     return {"workload": WORKLOAD, "parallelism": "batch-sharded x{}".format(world), "global_batch": world * BATCH,
-            "l2": "inputs (2.1 GB coeffs per GPU) exceed the 126 MB L2; no flush"}
+            "l2": "inputs (2.1 GB coeffs per GPU) exceed the 50 MB L2; no flush"}
 
 
 _T0 = time.perf_counter()
@@ -59,10 +64,31 @@ def measured_peaks():
     if os.path.isfile(path):
         with open(path) as f:
             p = json.load(f)
-        return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p["bf16_tflops"], "sm_max_mhz": p.get("sm_max_mhz", 1965.0),
+        return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p["bf16_tflops"], "sm_max_mhz": p.get("sm_max_mhz", 1980.0),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "sm_max_mhz": 1965.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "sm_max_mhz": 1980.0,
+            "source": "fallback (H100 SXM datasheet: 3.35 TB/s HBM3, 989 dense bf16 TFLOP/s, 1980 MHz)"}
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_solution(directory, out, rank, world):
+    """What the last timed solve returned.  One GPU: the whole [BATCH, n_out, HIDDEN] result as DIR/solution.npy.  N GPUs:
+    every rank writes DIR/solution_rank<r>.npy, the same fixed, sorted sample of its shard's paths (seeded, identical
+    on every rank) such that all ranks together stay within 64 MB, and rank 0 writes the sampled path indices as
+    DIR/solution_paths.npy (float64)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    if world == 1:
+        np.save(os.path.join(directory, "solution.npy"), out.float().cpu().numpy())
+        return
+    per_path = out[0].numel() * 4
+    n = min(out.shape[0], DUMP_BYTES // (world * per_path))
+    paths = torch.randperm(out.shape[0], generator=torch.Generator().manual_seed(0))[:n].sort().values
+    np.save(os.path.join(directory, "solution_rank{}.npy".format(rank)), out[paths.to(out.device)].float().cpu().numpy())
+    if rank == 0:
+        np.save(os.path.join(directory, "solution_paths.npy"), paths.double().numpy())
 
 
 # ------------------------------------------------------------------------------- synthetic data
@@ -202,7 +228,7 @@ def host_threads():
 
 
 def cpu_reference_solver(sample_paths):
-    """The reference's OWN ``cdeint`` (unmodified torchcde from /root/reference or oracle/_ref: its
+    """The reference's OWN ``cdeint`` (unmodified torchcde from its checkout or oracle/_ref: its
     ``_check_compatability``, ``_VectorField.forward`` with 63 aten calls and 4 ``item()`` per evaluation,
     ``CubicSpline.derivative``, output permute) on host cores.  torchdiffeq, which it dispatches to at
     solver.py:226-227, is not installable offline: ``oracle/odeint_port.py`` stands in for it (kind "_ref+port").
@@ -278,8 +304,10 @@ def run_reference_arm(args):
         run()
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        run()
+        result = run()
     total = time.perf_counter() - t0
+    if args.dump_outputs:                 # the sampled CPU workload's solution, [CPU_SAMPLE_PATHS, 2, HIDDEN]
+        dump_solution(args.dump_outputs, result, 0, 1)
     value = CPU_SAMPLE_PATHS * args.steps / total
     base = {"value": value, "unit": "sequences/s", "cores": torch.get_num_threads(), "kind": kind,
             "host_cpus": os.cpu_count(),
@@ -359,6 +387,8 @@ def run_gpu_arm(args):
         if rank != 0:
             clocks = None
         assert bool(torch.isfinite(holder["out"]).all())
+        if args.dump_outputs:
+            dump_solution(args.dump_outputs, holder["out"], rank, world)
 
         note("device-resident: {:.3f} ms per solve".format(ms / args.steps))
         # ---- end to end from pinned host buffers (copies inside the timed region) ------------
@@ -462,7 +492,7 @@ def run_gpu_arm(args):
                 t_ms = min(time_loop(train_step, 1, 0, device) for _ in range(3))
                 extra["cdeint_rk4_forward_plus_adjoint_backward"] = {
                     "ms": t_ms, "sequences_per_s": BATCH / (t_ms * 1e-3), "bound": "tensor (bf16 / f16 MMAs)", "runs": "best of 3",
-                    "note": "backward = two tensor-core solves that keep their stage inputs + one tcgen05 GEMM for dL/dW, dL/db "
+                    "note": "backward = two tensor-core solves that keep their stage inputs + one tensor-core product for dL/dW, dL/db "
                             "(tcde_cdeint_fixed_linear_stages x2, tcde_linear_field_param_grads); not the headline"}
             except Exception as exc:      # never lose the headline line over the extra
                 extra["cdeint_rk4_forward_plus_adjoint_backward"] = {"error": repr(exc)}
@@ -531,7 +561,7 @@ def run_gpu_arm(args):
                     "adjoint_stats": getattr(cde.cdeint, "last_adjoint_stats", None),
                     "note": "backward = dopri5 on (z, adjoint state) as one virtual batch with the controller on the device "
                             "(tcde_dopri5_linear_paired_attempts), dL/dW, dL/db by quadrature over the accepted steps' stage "
-                            "inputs (one tcgen05 GEMM per 256 accepted steps); round 1 / host-driven: ~1.4 s"}
+                            "inputs (one parameter-gradient launch per 256 accepted steps)"}
             except Exception as exc:
                 config4["error"] = repr(exc)
             extra["config4_dopri5_adjoint"] = config4
@@ -547,17 +577,18 @@ def run_gpu_arm(args):
     kernel_s = ms_step * 1e-3                       # one launch per step: the step IS the kernel
     achieved_gbs = BATCH * BYTES_PER_SEQ / kernel_s / 1e9
     achieved_tf = BATCH * FLOPS_PER_SEQ / kernel_s / 1e12
-    fp32_peak_tf = 148 * 128 * 2 * peaks["sm_max_mhz"] * 1e6 / 1e12
+    n_sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    fp32_peak_tf = n_sms * 128 * 2 * peaks["sm_max_mhz"] * 1e6 / 1e12
     e2e_value = world * BATCH * e2e_steps / (e2e_ms * 1e-3)
     variant = (args.variant if args.variant is not None else 0) & 15
     tensor_kernel = variant != 1
     fp16_split = variant in (0, 4, 5)
-    mmas_per_stage = 7 if fp16_split else 13        # 128 x 256 x (16 halves | 8 tf32) each: the same 2 * 128 * 256 * 16 / 2 ... flops per cycle-slot
-    mma_flops = BATCH / 128 * 255 * 4 * mmas_per_stage * 2 * 128 * 256 * (16 if fp16_split else 8)
+    # executed tensor-core work: three split products (lo.hi + hi.lo + hi.hi) of [path x 32] . [32 x 256] per stage
+    mma_flops = BATCH * 255 * 4 * 3 * 2 * HIDDEN * HIDDEN * CHANNELS
     mma_peak = peaks["bf16_tflops"] if fp16_split else peaks["bf16_tflops"] / 2
-    kernel_name = {0: "cdeint_tc_kernel<1> (tcgen05.mma kind::f16, 2xFP16 split, TMA rows, persistent)", 2: "cdeint_umma_kernel<8> (round 1, 3xTF32)",
-                   3: "cdeint_tc_kernel<0> (3xTF32)", 4: "cdeint_tc_kernel<1> (2xFP16)", 5: "cdeint_tc_kernel<1> (2xFP16)",
-                   6: "cdeint_tc_kernel<0> (3xTF32)"}.get(variant, "?")
+    kernel_name = {0: "cdeint_tc_kernel<1> (mma.sync m16n8k16 f16, 2xFP16 split)", 2: "cdeint_tc_kernel<0> (mma.sync m16n8k8 tf32, 3xTF32)",
+                   3: "cdeint_tc_kernel<0> (mma.sync m16n8k8 tf32, 3xTF32)", 4: "cdeint_tc_kernel<1> (mma.sync m16n8k16 f16, 2xFP16)",
+                   5: "cdeint_tc_kernel<1> (2xFP16)", 6: "cdeint_tc_kernel<0> (3xTF32)"}.get(variant, "?")
     secondary = dict(extra)
     config4 = secondary.get("config4_dopri5_adjoint")
     line = {
@@ -582,29 +613,26 @@ def run_gpu_arm(args):
         "gpu_launches": args.steps,
         "roofline": ({
             "bound": "tensor", "achieved": achieved_tf, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s",
-            "frac": achieved_tf / peaks["bf16_tflops"], "traffic": 2225915168, "peak_source": peaks["source"],
+            "frac": achieved_tf / peaks["bf16_tflops"], "peak_source": peaks["source"],
             "kernel": kernel_name,
             "algorithmic_flops_per_launch": BATCH * FLOPS_PER_SEQ,
-            "note": "achieved = ALGORITHMIC flops (17.6 MFLOP/seq) / time against the measured dense bf16 peak, as the "
-                    "contract asks. fp32 accuracy on the tensor pipe costs a 2-way operand split: 3 partial products + 1 bias "
-                    "block = 7 FP16 MMAs (13 TF32 MMAs in round 1) per 128 x 256 x 32 product, so the kernel's own ceiling is "
-                    "peak * 2 / 7; see mma below (executed MMA flops against the same peak). The pace is set by the serial "
-                    "chain MMA -> TMEM read -> Runge-Kutta -> operand split of the two tiles TMEM can hold, not by the pipe "
-                    "(profiles/README.md). traffic = dram bytes of one launch from the ncu capture in profiles/ "
-                    "(algorithmic bytes: 1.63e9; whole 128-byte coefficient rows are fetched).",
+            "note": "achieved = ALGORITHMIC flops (17.6 MFLOP/seq) / time against the dense bf16 peak. fp32 accuracy on "
+                    "the tensor pipe costs a 2-way operand split: 3 partial products per [32 x 32] . [32 x 256] field "
+                    "evaluation (the bias is the accumulator's initial value), so the kernel's own ceiling is peak / 3; "
+                    "see mma below (executed MMA flops against the same peak).",
             "mma": {"executed_mma_tflops": mma_flops / kernel_s / 1e12, "peak_tflops": mma_peak,
-                    "frac": mma_flops / kernel_s / 1e12 / mma_peak, "mmas_per_tile_stage": mmas_per_stage,
-                    "peak_source": "measured dense bf16 (kind::f16 rate)" if fp16_split else "measured dense bf16 / 2 (tf32 rate)"},
+                    "frac": mma_flops / kernel_s / 1e12 / mma_peak, "split_products_per_stage": 3,
+                    "peak_source": "dense bf16 (f16 rate)" if fp16_split else "dense bf16 / 2 (tf32 rate)"},
             "hbm": {"achieved_gbs": achieved_gbs, "peak_gbs": peaks["hbm_gbs"], "frac": achieved_gbs / peaks["hbm_gbs"],
                     "note": "the north_star's HBM framing: this solve is ~700 flop/B, compute bound by ~60x"},
             "secondary": secondary,
         } if tensor_kernel else {
             "bound": "hbm", "achieved": achieved_gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-            "frac": achieved_gbs / peaks["hbm_gbs"], "traffic": 2176804000, "peak_source": peaks["source"],
+            "frac": achieved_gbs / peaks["hbm_gbs"], "peak_source": peaks["source"],
             "kernel": "cdeint_simt_kernel<float,8,8>", "algorithmic_bytes_per_launch": BATCH * BYTES_PER_SEQ,
             "note": "this kernel is FP32-FMA bound (708 flop/B), not HBM bound; see fp32 below and DESIGN.md",
             "fp32": {"achieved_tflops": achieved_tf, "peak_tflops": fp32_peak_tf, "frac": achieved_tf / fp32_peak_tf,
-                     "peak_source": "148 SMs x 128 FMA lanes x 2 x clocks.max.sm"},
+                     "peak_source": "{} SMs x 128 FMA lanes x 2 x clocks.max.sm".format(n_sms)},
             "secondary": secondary}),
         "config4": config4,
     }
@@ -622,7 +650,10 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--variant", type=int, default=None, help="solve kernel: 1 = CUDA-core, 2 = tcgen05 (default: the library's choice)")
+    ap.add_argument("--variant", type=int, default=None,
+                    help="solve kernel: 1 = CUDA-core, 3 = tensor cores 3xTF32, 4 = tensor cores 2xFP16 (default: the library's choice)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed solve returned to DIR (float32 .npy; see dump_solution)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * torchcde_b200 -- C ABI of the B200-native Neural-CDE hot path.
+ * torchcde_b200 -- C ABI of the H100-native Neural-CDE hot path.
  *
  * The reference (patrick-kidger/torchcde) is pure Python and has no FFI of its own; the
  * drop-in boundary is its Python API (SURVEY.md 8b).  This header is the boundary one level
@@ -275,20 +275,16 @@ TCDE_API int tcde_logsignature_windows(const void* x, int64_t n_paths, int64_t l
                               const int32_t* window_index, int64_t n_windows, int depth, const int32_t* words, int64_t n_words,
                               void* out, int dtype, void* stream);
 
-/* Profiling aid: a device buffer of 64 x 8 int64 that the tensor-core solve kernel (variant 2)
- * fills with clock64 stamps of CTA 0 / tile 0 for its first 64 stages; NULL (default) disables. */
-TCDE_API int tcde_set_trace_buffer(void* device_buffer);
-
 /* Natural-cubic / gap-fill kernel choice: 0 = the parallel kernels (windowed sweeps, warp per path)
  * when the path fits shared memory (default), 1 = one thread per series, 2 = parallel kernels
  * but the CTA-per-path natural-cubic kernel instead of the warp-per-path one.  For tests / benchmarks. */
 TCDE_API int tcde_set_natural_variant(int variant);
 
-/* Which kernel tcde_cdeint_fixed_linear launches for float32: 0 = automatic (the tcgen05 kernel
+/* Which kernel tcde_cdeint_fixed_linear launches for float32: 0 = automatic (the tensor-core kernel
  * where it is built for the shape: hidden = 32, channels = 8; the CUDA-core kernel otherwise),
- * 1 = CUDA-core kernel, 2 = round-1 tcgen05 kernel (3xTF32, Runge-Kutta slopes parked in shared memory), 3 / 4 = round-2
- * tcgen05 kernel (solve_tc.cu: slopes in registers) with the 3xTF32 / the 2xFP16 operand split (TCDE_ERR_UNSUPPORTED
- * for other shapes).  Process-wide; meant for tests and benchmarks. */
+ * 1 = CUDA-core kernel, 3 / 4 = tensor-core kernel (solve_tc.cu) with the 3xTF32 / the 2xFP16 operand split
+ * (TCDE_ERR_UNSUPPORTED for other shapes); 2 and 6 are aliases of 3, 5 of 4; bits above 15 are ignored.
+ * Process-wide; meant for tests and benchmarks. */
 TCDE_API int tcde_set_solve_variant(int variant);
 
 #ifdef __cplusplus

@@ -8,7 +8,7 @@ missing; it never routes here).
 
 Pinning status (see DESIGN.md "Oracle"):
   * path (i)  coefficient construction + spline evaluation: PINNED.  Every function is
-    checked bit-for-bit against the live reference (imported from /root/reference with
+    checked bit-for-bit against the live reference (imported from its checkout with
     the two absent solver packages stubbed, ``oracle/reference_loader.py``) and against
     the reference tests' own known-answer vectors; the generated vectors are committed
     under ``tests/golden/`` by ``oracle/make_golden.py``.

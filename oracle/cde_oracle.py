@@ -3,11 +3,11 @@
 Everything here is plain ``torch`` CPU arithmetic in the dtype of the inputs, written so
 that every floating-point operation happens in the same order as in the reference (no
 fused multiply-add anywhere: each torch elementwise op rounds once), which is what lets
-``tests/`` demand bit-equality for path (i).  Citations are to /root/reference.
+``tests/`` demand bit-equality for path (i).  Citations are to the reference repository.
 
 Pinning: ``tests/test_oracle_pinned.py`` checks each function below bit-for-bit against the
 committed fixtures in ``tests/golden/`` (generated from the live reference by
-``oracle/make_golden.py``) and, when /root/reference is present, against the live
+``oracle/make_golden.py``) and, against the live
 reference again.  The solve (``cdeint_linear``) is pinned for its vector field only; its
 time stepping is ``oracle/odeint_port.py`` -- see that file's header for "parity unpinned".
 """

@@ -1,9 +1,9 @@
-"""Generate tests/golden/*.npz from the LIVE reference -- run in the build container only.
+"""Generate tests/golden/*.npz from the LIVE reference -- run where a reference checkout exists.
 
     python -m oracle.make_golden
 
 Every array under ``ref_*`` keys is an output of the unmodified reference code imported
-from /root/reference (``oracle/reference_loader.py``); the ``in_*`` arrays are the seeded
+from the reference checkout (``oracle/reference_loader.py``); the ``in_*`` arrays are the seeded
 inputs that produced them.  Nothing here is computed by the oracle or by the CUDA path.
 The only non-reference arithmetic involved is the fixed-grid stepping inside the
 ``cdeint`` fixtures, which is ``oracle/odeint_port.py`` standing where torchdiffeq would

@@ -5,7 +5,7 @@ What this stands in for
 ``torchcde.cdeint`` contains no time stepping.  It hands a vector field to
 ``torchdiffeq.odeint`` (reference call site: torchcde/solver.py:226-227).  torchdiffeq
 is a third-party dependency pinned only as ``torchdiffeq>=0.2.0`` (setup.py:51); it is
-not vendored under /root/reference, not installed here and not installable (no
+not vendored in the reference repository, not installed here and not installable (no
 network).  This module restates the *published* algorithm of torchdiffeq 0.2.x's
 fixed-grid solvers (its ``_impl/fixed_grid.py``, ``_impl/solvers.py``
 ``FixedGridODESolver``, ``_impl/rk_common.py`` ``rk4_alt_step_func`` and the time

@@ -1,10 +1,9 @@
-"""Import the live reference package (build container only) -- TEST INFRASTRUCTURE ONLY.
+"""Import the reference package -- TEST / BENCHMARK INFRASTRUCTURE ONLY.
 
-``/root/reference`` exists in the build container and NOT on the GPU box; ``oracle/_ref`` (an
-unmodified ``pip install --target`` of it, recipe in ``oracle/Makefile``, git-ignored) does travel.
-This module is used by ``oracle/make_golden.py`` (to generate the committed fixtures), by the
-``not gpu`` tests that re-pin the oracle when the reference tree is present, and by
-``bench.py``'s CPU arm (the reference's own ``cdeint`` timed on the host cores).
+A checkout of the reference is looked for at ``$TORCHCDE_REFERENCE_ROOT`` (default ``/root/reference``);
+``oracle/_ref`` is an unmodified ``pip install --target`` of it (recipe in ``oracle/Makefile``, git-ignored).
+This module is used by ``oracle/make_golden.py`` and ``oracle/make_reference_golden.py`` (to generate the
+committed fixtures) and by ``bench.py``'s CPU arm (the reference's own ``cdeint`` timed on the host cores).
 
 The reference's ``torchcde/__init__.py:7`` imports ``solver.py``, whose first lines import
 ``torchdiffeq`` and ``torchsde`` (solver.py:2-3).  Neither is installed.  We therefore put
@@ -21,7 +20,7 @@ import sys
 import types
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# the live tree (build container) or the unmodified install of it that travels to the GPU box (oracle/Makefile)
+# the reference checkout, or the unmodified install of it under oracle/_ref (oracle/Makefile)
 _CANDIDATES = [os.environ.get("TORCHCDE_REFERENCE_ROOT", "/root/reference"), os.path.join(_HERE, "_ref")]
 
 
@@ -35,12 +34,18 @@ def _root():
 REFERENCE_ROOT = _root() or _CANDIDATES[0]
 
 
+def reference_source():
+    """The reference checkout (with its setup.py) that oracle/Makefile can install into oracle/_ref, or None."""
+    src = _CANDIDATES[0]
+    return src if os.path.isfile(os.path.join(src, "setup.py")) else None
+
+
 def reference_available():
     return _root() is not None
 
 
 def reference_kind():
-    """'live' = /root/reference itself, '_ref' = the pip-installed copy under oracle/_ref, None = neither."""
+    """'live' = the reference checkout itself, '_ref' = the pip-installed copy under oracle/_ref, None = neither."""
     root = _root()
     if root is None:
         return None

@@ -4,7 +4,7 @@ VERDICT r01 item 1: the stepping arithmetic behind torchcde/solver.py:226-227 li
 not vendored.  This probe records -- as evidence, not assumption -- whether the package exists on the box the
 benchmarks run on.  If it does, the restated solvers (oracle/odeint_port.py, torchcde_b200/adaptive.py) are
 diffed against it on a small seeded problem and the differences are printed; if not, the module search path and
-the installed distributions are logged.  Output goes to stdout (redirect into profiles/).
+the installed distributions are logged.  Output goes to stdout.
 """
 import importlib.metadata
 import importlib.util
@@ -30,7 +30,8 @@ def main():
             print("find_spec({!r}) raised {!r}".format(name, exc))
         found[name] = spec
         print("find_spec({!r}): {}".format(name, spec.origin if spec else None))
-    print("/root/reference present:", os.path.isdir("/root/reference"))
+    from oracle import reference_loader
+    print("reference tree present:", reference_loader.reference_available())
     print("baseline/_ref present:", os.path.isdir(os.path.join(ROOT, "baseline", "_ref")))
     dists = sorted({d.metadata["Name"] for d in importlib.metadata.distributions() if d.metadata["Name"]}, key=str.lower)
     hits = [d for d in dists if any(k in d.lower() for k in ("diffeq", "torchsde", "torchcde", "signatory"))]

@@ -13,10 +13,9 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
     # The C-ABI library is a build artefact (git-ignored).  In a fresh checkout build it before the
-    # first test needs it (nvcc cross-compiles for sm_100a without a GPU); never rebuild on the GPU box
-    # when the prebuilt library travelled with the snapshot.
+    # first test needs it (nvcc cross-compiles for sm_90a without a GPU); an existing library is never rebuilt here.
     lib = os.path.join(ROOT, "torchcde_b200", "csrc", "libtcde_b200.so")
     if not os.path.isfile(lib):
         import shutil

@@ -1,97 +1,82 @@
 """torchcde_b200/_diff.py (the torch-operator restatements that serve BACKWARD passes of the kernel-backed builders)
-against the live reference: same values and the same gradients with respect to the data and the knots, with and
-without missing values.  CPU, fp64.  Needs the reference tree (/root/reference here, oracle/_ref on the GPU box)."""
+against the reference package: same values and the same gradients with respect to the data and the knots, with and
+without missing values.  CPU, fp64.  The reference's values, cotangents and gradients are stored in
+tests/golden/reference_live.npz (oracle/make_reference_golden.py)."""
+import os
+
+import numpy as np
 import pytest
 import torch
 
-from oracle import reference_loader
 from torchcde_b200 import _diff
 
-pytestmark = pytest.mark.skipif(not reference_loader.reference_available(), reason="reference tree not present")
+_Z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_live.npz"))
+_OURS = {"hermite": _diff.hermite, "natural1": lambda a, b: _diff.natural(a, b, 1), "natural0": lambda a, b: _diff.natural(a, b, 0),
+         "linear": _diff.linear_fill}
 
 
-def _data(seed, batch=(3,), length=9, channels=2, nan=0.0, irregular=True):
-    gen = torch.Generator().manual_seed(seed)
-    x = torch.randn(*batch, length, channels, generator=gen, dtype=torch.float64)
-    if nan:
-        hole = torch.rand(x.shape, generator=gen) < nan
-        x = x.masked_fill(hole, float("nan"))
-    t = torch.rand(length, generator=gen, dtype=torch.float64).add(0.2).cumsum(0) if irregular else None
-    return x, t
+def _t(key):
+    return torch.from_numpy(_Z[key]) if key in _Z.files else None
 
 
-def _compare(ours, theirs, x, t, seed):
+def _cases(prefix):
+    n = 0
+    while prefix + "__{}__x".format(n) in _Z.files:
+        yield prefix + "__{}__".format(n)
+        n += 1
+
+
+def _compare(ours, key):
+    x, t = _t(key + "x"), _t(key + "t")
+    want, cot = _t(key + "want"), _t(key + "cot")
     xa = x.clone().requires_grad_(True)
-    xb = x.clone().requires_grad_(True)
     ta = None if t is None else t.clone().requires_grad_(True)
-    tb = None if t is None else t.clone().requires_grad_(True)
-    got, want = ours(xa, ta), theirs(xb, tb)
+    got = ours(xa, ta)
     assert got.shape == want.shape
     nan_same = torch.isnan(got) == torch.isnan(want)
     assert bool(nan_same.all())
     ok = ~torch.isnan(want)
     assert torch.allclose(got[ok], want[ok], rtol=1e-9, atol=1e-11), float((got[ok] - want[ok]).abs().max())
-    cot = torch.randn(want.shape, generator=torch.Generator().manual_seed(seed), dtype=torch.float64) * ok
-    ins_a = [xa] + ([ta] if t is not None else [])
-    ins_b = [xb] + ([tb] if t is not None else [])
-    if not want.requires_grad:          # e.g. linear coefficients without NaN return their input
+    if key + "gx" not in _Z.files:       # e.g. linear coefficients without NaN return their input
         return
+    ins_a = [xa] + ([ta] if t is not None else [])
     ga = torch.autograd.grad(torch.where(ok, got, torch.zeros_like(got)), ins_a, cot, allow_unused=True)
-    gb = torch.autograd.grad(torch.where(ok, want, torch.zeros_like(want)), ins_b, cot, allow_unused=True)
-    for a, b in zip(ga, gb):
+    for a, name in zip(ga, ("gx", "gt")):
+        b = _t(key + name)
         a = torch.zeros(1, dtype=torch.float64) if a is None else torch.nan_to_num(a)
-        b = torch.zeros(1, dtype=torch.float64) if b is None else torch.nan_to_num(b)
         assert torch.allclose(a, b, rtol=1e-7, atol=1e-9), float((a - b).abs().max())
 
 
 @pytest.mark.parametrize("nan", [0.0, 0.35])
 @pytest.mark.parametrize("irregular", [False, True])
 def test_builders_values_and_gradients_match_the_reference(nan, irregular):
-    ref = reference_loader.load_reference()
-    for seed, batch, length in ((0, (3,), 9), (1, (2, 2), 6), (2, (), 2), (3, (4,), 3)):
-        x, t = _data(seed, batch, length, 2, nan, irregular)
-        if nan:
-            x[..., 1, :] = float("nan") if length > 2 else x[..., 1, :]      # a fully missing knot row
-            if batch:
-                x[0] = float("nan")                                           # an all-NaN path
-                x[-1][..., 0, :] = float("nan")                               # leading NaN
-                x[-1][..., -1, 0] = float("nan")                              # trailing NaN
-        _compare(_diff.hermite, ref.hermite_cubic_coefficients_with_backward_differences, x, t, seed)
-        _compare(lambda a, b: _diff.natural(a, b, 1), ref.natural_cubic_coeffs, x, t, seed)
-        _compare(lambda a, b: _diff.natural(a, b, 0), ref.natural_cubic_spline_coeffs, x, t, seed)
-        if nan:
-            _compare(_diff.linear_fill, ref.linear_interpolation_coeffs, x, t, seed)
-            ff = ref.misc.forward_fill(x)
-            mine = _diff.forward_fill(x)
-            assert bool(((ff == mine) | (torch.isnan(ff) & torch.isnan(mine))).all())
+    keys = [k for k in _cases("diff") if tuple(_Z[k + "group"]) == (nan, float(irregular))]
+    assert len(keys) == (20 if nan else 12)
+    for key in keys:
+        builder = str(_Z[key + "builder"])
+        if builder == "ffill":
+            ff, mine = _t(key + "want"), _diff.forward_fill(_t(key + "x"))
+            assert bool(((ff == mine) | (torch.isnan(ff) & torch.isnan(mine))).all()), key
+        else:
+            _compare(_OURS[builder], key)
 
 
 def test_rectilinear_matches_the_reference():
-    ref = reference_loader.load_reference()
-    x, _ = _data(5, (3,), 7, 3, 0.3, False)
-    x[..., 0] = torch.arange(7, dtype=torch.float64)          # the time channel has no NaN
-    x[:, 0, :] = 1.0                                           # no leading NaN
-    want = ref.linear_interpolation_coeffs(x, rectilinear=0)
-    got = _diff.linear_fill(_diff.rectilinear(x, 0), None)
-    assert torch.allclose(got, want)
+    got = _diff.linear_fill(_diff.rectilinear(_t("rect__x"), 0), None)
+    assert torch.allclose(got, _t("rect__want"))
 
 
 def test_evaluation_formulas_match_the_reference():
-    ref = reference_loader.load_reference()
-    x, t = _data(7, (2, 3), 8, 2, 0.0, True)
-    coeffs = ref.natural_cubic_coeffs(x, t)
-    spline = ref.CubicSpline(coeffs, t)
-    linear = ref.LinearInterpolation(x, t)
-    query = torch.tensor([t[0] - 0.3, t[0], t[2], 0.5 * (t[3] + t[4]), t[-1], t[-1] + 1.0], dtype=torch.float64)
+    x, t, coeffs = _t("eval__x"), _t("eval__t"), _t("eval__coeffs")
     c = x.size(-1)
     a, b, two_c, three_d = coeffs[..., :c], coeffs[..., c:2 * c], coeffs[..., 2 * c:3 * c], coeffs[..., 3 * c:]
-    for q in (query, query[3], query.view(2, 3)):
-        frac, index = spline._interpret_t(q)
+    for i in range(3):
+        key = "eval__{}__".format(i)
+        q, index, lindex = _t(key + "q"), _t(key + "index"), _t(key + "lindex")
         for deriv in (False, True):
-            want = spline.derivative(q) if deriv else spline.evaluate(q)
+            want = _t(key + ("cubic_deriv" if deriv else "cubic_eval"))
             got = _diff.cubic_eval(a, b, two_c, three_d, t, q, index, deriv)
             assert torch.allclose(got, want, rtol=1e-12, atol=1e-12)
-            want = linear.derivative(q) if deriv else linear.evaluate(q)
-            _, lindex = linear._interpret_t(q)
+            want = _t(key + ("linear_deriv" if deriv else "linear_eval"))
             got = _diff.linear_eval(x, t, q, lindex, deriv)
             assert torch.allclose(got, want, rtol=1e-12, atol=1e-12)

@@ -354,10 +354,10 @@ def test_trajectory_backward_matches_the_per_stage_backward(method, monkeypatch)
 @pytest.mark.parametrize("n_paths,n_stages", [(1, 1), (31, 3), (32, 2), (33, 5), (1000, 8), (4099, 40)])
 @pytest.mark.parametrize("kind", ["cubic", "linear"])
 def test_parameter_gradient_kernels_against_einsum(n_paths, n_stages, kind):
-    """tcde_linear_field_param_grads on the tensor cores (variant 0: round 2, BF16 two-way split, MN-major operands fed by
-    TMA; variant 2: round 1, 3xTF32) and on the CUDA cores (variant 1) vs an fp64 einsum over (stage, path): ragged path
-    blocks, zero-weight stages, accumulation onto existing gradients.  Bars: fp32-class (3e-5 of the largest entry) for the
-    TF32 / CUDA-core kernels, 2e-4 for the BF16 split (16 significant bits per operand: ample for a gradient)."""
+    """tcde_linear_field_param_grads on the tensor cores (variant 0: 2xBF16 operand split; variant 2: 3xTF32) and on the
+    CUDA cores (variant 1) vs an fp64 einsum over (stage, path): ragged path blocks, zero-weight stages, accumulation onto
+    existing gradients.  Bars: fp32-class (3e-5 of the largest entry) for the TF32 / CUDA-core kernels, 2e-4 for the BF16
+    split (16 significant bits per operand: ample for a gradient)."""
     from torchcde_b200 import _lib
     gen = torch.Generator().manual_seed(n_paths + n_stages)
     hidden, channels, n_rows = 32, 8, 6

@@ -2,8 +2,7 @@
 oracle; (2) the whole transform against the REFERENCE's own log_ode.py executed on the CPU with the oracle plugged in as
 ``signatory`` (so the window construction, NaN knots, linear fill, scaling and cumsum are the reference's code);
 (3) the reference's test_log_ode.py:8-36 with the oracle in signatory's place."""
-import sys
-import types
+import os
 
 import numpy as np
 import pytest
@@ -11,26 +10,9 @@ import torch
 
 import torchcde_b200 as cde
 from oracle import logsig_oracle as O
-from oracle import reference_loader
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-
-
-def _fake_signatory():
-    mod = types.ModuleType("signatory")
-
-    class Logsignature:
-        def __init__(self, depth):
-            self.depth = depth
-
-        def __call__(self, paths):
-            out = [O.logsignature(p.detach().cpu().double().numpy(), self.depth) for p in paths]
-            return torch.tensor(np.stack(out), dtype=paths.dtype)
-
-    mod.Logsignature = Logsignature
-    mod.logsignature_channels = lambda channels, depth: len(O.lyndon_words(channels, depth))
-    return mod
 
 
 @pytest.mark.parametrize("dtype,tol", [(torch.float64, 1e-11), (torch.float32, 2e-5)])
@@ -51,26 +33,20 @@ def test_kernel_against_the_oracle(dtype, tol):
         assert float((got - want).abs().max()) <= tol * max(1.0, scale), (channels, depth)
 
 
-@pytest.mark.skipif(not reference_loader.reference_available(), reason="reference tree not present")
-def test_whole_transform_against_the_reference_code_with_the_oracle_as_signatory(monkeypatch):
-    ref = reference_loader.load_reference()
-    log_ode = sys.modules[ref.__name__ + ".log_ode"]
-    monkeypatch.setattr(log_ode, "signatory", _fake_signatory())
-    torch.manual_seed(1)
-    for batch, length, channels, depth, window, irregular, nan in (((2,), 11, 2, 3, 2.5, False, 0.0), ((3,), 9, 3, 2, 4.0, True, 0.3),
-                                                                   ((2, 2), 7, 1, 4, 1.0, False, 0.2), ((1,), 6, 2, 2, 10.0, True, 0.0)):
-        x = torch.randn(*batch, length, channels, dtype=torch.float64)
-        if nan:
-            hole = torch.rand(x.shape) < nan
-            hole[..., 0, :] = False
-            hole[..., -1, :] = False
-            x = x.masked_fill(hole, float("nan"))
-        t = (torch.rand(length, dtype=torch.float64) + 0.3).cumsum(0) if irregular else None
-        want = ref.logsig_windows(x, depth, window, t)
+def test_whole_transform_against_the_reference_code_with_the_oracle_as_signatory():
+    """The reference's logsig_windows / logsignature_windows, run with the oracle as signatory, stored in
+    tests/golden/reference_live.npz (oracle/make_reference_golden.py)."""
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_live.npz"))
+    for i in range(4):
+        key = "logsig__{}__".format(i)
+        x = torch.from_numpy(z[key + "x"])
+        depth, window = int(z[key + "depth"]), float(z[key + "window"])
+        t = torch.from_numpy(z[key + "t"]) if key + "t" in z.files else None
+        want = torch.from_numpy(z[key + "want"])
         got = cde.logsig_windows(x.to(DEV), depth, window, None if t is None else t.to(DEV))
         assert got.shape == want.shape
-        assert torch.allclose(got.cpu(), want, rtol=1e-9, atol=1e-10), (batch, length, channels, depth)
-        want_v, want_t = ref.logsignature_windows(x, depth, window, t)
+        assert torch.allclose(got.cpu(), want, rtol=1e-9, atol=1e-10), (x.shape, depth)
+        want_v, want_t = torch.from_numpy(z[key + "want_v"]), torch.from_numpy(z[key + "want_t"])
         got_v, got_t = cde.logsignature_windows(x.to(DEV), depth, window, None if t is None else t.to(DEV))
         assert torch.allclose(got_v.cpu(), want_v, rtol=1e-9, atol=1e-10) and torch.allclose(got_t.cpu(), want_t)
 

@@ -28,7 +28,7 @@ def _bench_problem(batch, nan_fraction=0.0, seed=0):
 
 @pytest.mark.parametrize("nan_fraction", [0.0, 0.3])
 def test_full_batch_fp32_tensor_core_solve_against_fp64_kernel(nan_fraction):
-    """ALL 65,536 paths of BASELINE config 3 (and of a 30 %-NaN config-2 -> config-3 pipeline): the fp32 tcgen05
+    """ALL 65,536 paths of BASELINE config 3 (and of a 30 %-NaN config-2 -> config-3 pipeline): the fp32 tensor-core
     solve against the fp64 CUDA-core solve (itself oracle-checked to 1e-10 in test_gpu_solve.py) on the same
     fp32-rounded coefficients.  Bar: 1e-5 of the solution scale on every element."""
     B = 65536

@@ -250,7 +250,7 @@ def test_gradients_flow_through_the_generic_loop():
     _assert_close(out.detach(), fused.cpu(), torch.float32)
 
 
-# ------------------------------------------------------------------ tensor-core (tcgen05) variant
+# ------------------------------------------------------------------ tensor-core variant
 def _set_variant(v):
     from torchcde_b200 import _lib
     _lib.call("tcde_set_solve_variant", v)
@@ -259,9 +259,9 @@ def _set_variant(v):
 @pytest.mark.parametrize("variant", [2, 3, 4, 4 + 16 * 32, 4 + 16 * 2])
 @pytest.mark.parametrize("batch", [1, 100, 128, 129, 256, 300, 1000])
 def test_tensor_core_variant_matches_cuda_core_and_oracle(batch, variant):
-    """The tcgen05 kernels -- 2: solve_umma.cu (round 1, 3xTF32), 3 / 4: solve_tc.cu (Runge-Kutta state in registers;
-    3xTF32 / 2xFP16 with per-path power-of-two scaling; + 16 * 32: the time axis forced into four segments handed over
-    through HBM; + 16 * 2: the proxy fence in every row thread as well as in the issuer) -- against solve_simt.cu and the fp64 oracle, including partial tiles (batch not a multiple of 128 / 256)."""
+    """The tensor-core kernel solve_tc.cu -- 2 / 3: 3xTF32, 4: 2xFP16 with per-path power-of-two scaling; the + 16 * k
+    variants carry flag bits the library accepts and ignores -- against solve_simt.cu and the fp64 oracle, including
+    partial warps and CTAs (batch not a multiple of 32 / 128)."""
     length, channels, hidden = 40, 8, 32
     gen = torch.Generator().manual_seed(batch)
     x = torch.randn(batch, length, channels, generator=gen, dtype=torch.float64).cumsum(1) / math.sqrt(length)

@@ -1,17 +1,17 @@
 """Pin the CPU oracle (oracle/cde_oracle.py) to the reference, bit for bit.
 
 The fixtures in tests/golden/ are outputs of the unmodified reference
-(oracle/make_golden.py); when /root/reference is present (build container) the same
-checks are repeated against the live reference on fresh random inputs.
+(oracle/make_golden.py, oracle/make_reference_golden.py).
 """
+import os
 import warnings
 
+import numpy as np
 import pytest
 import torch
 
 from conftest import Golden, same
 from oracle import cde_oracle as O
-from oracle import reference_loader
 
 
 def test_builders_match_reference_fixtures():
@@ -100,24 +100,23 @@ def test_solve_fixtures_vector_field_and_call_site():
         assert same(out, g.t(k + "_ref_out")), k
 
 
-@pytest.mark.skipif(not reference_loader.reference_available(), reason="reference tree not on this machine")
-def test_oracle_against_live_reference_fresh_inputs():
-    ref = reference_loader.load_reference()
-    gen = torch.Generator().manual_seed(31337)
-    for dtype in (torch.float32, torch.float64):
-        for shape in ((4, 11, 3), (2, 2, 5, 2), (6, 2, 1)):
-            x = torch.randn(shape, generator=gen, dtype=torch.float64).to(dtype)
-            t = (torch.rand(shape[-2], generator=gen, dtype=torch.float64) + 0.05).cumsum(0).to(dtype)
-            for frac in (0.0, 0.25, 0.7):
-                xin = x.clone()
-                xin[torch.rand(shape, generator=gen) < frac] = float("nan")
-                for tt in (None, t):
-                    assert same(O.linear_knots(xin, tt), ref.linear_interpolation_coeffs(xin, tt))
-                    assert same(O.hermite_backward_difference_coeffs(xin, tt),
-                                ref.hermite_cubic_coefficients_with_backward_differences(xin, tt))
-                    assert same(O.natural_cubic_coeffs(xin, tt, 1), ref.natural_cubic_coeffs(xin, tt))
-                    assert same(O.natural_cubic_coeffs(xin, tt, 0), ref.natural_cubic_spline_coeffs(xin, tt))
-                    assert same(O.carry_forward(xin), ref.misc.forward_fill(xin))
+def test_oracle_against_reference_outputs_on_fresh_inputs():
+    """The oracle against the reference package's own outputs on seeded inputs (tests/golden/reference_live.npz, written by
+    oracle/make_reference_golden.py): fp32 and fp64, with and without knots, 0 / 25 / 70 % missing values."""
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_live.npz"))
+    n = 0
+    while "fresh__{}__x".format(n) in z.files:
+        key = "fresh__{}__".format(n)
+        xin = torch.from_numpy(z[key + "x"])
+        tt = torch.from_numpy(z[key + "t"]) if key + "t" in z.files else None
+        want = {f: torch.from_numpy(z[key + f]) for f in ("linear", "hermite", "natural1", "natural0", "ffill")}
+        assert same(O.linear_knots(xin, tt), want["linear"]), key
+        assert same(O.hermite_backward_difference_coeffs(xin, tt), want["hermite"]), key
+        assert same(O.natural_cubic_coeffs(xin, tt, 1), want["natural1"]), key
+        assert same(O.natural_cubic_coeffs(xin, tt, 0), want["natural0"]), key
+        assert same(O.carry_forward(xin), want["ffill"]), key
+        n += 1
+    assert n == 36
 
 
 def test_validation_messages_follow_reference():

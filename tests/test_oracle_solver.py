@@ -88,7 +88,7 @@ def test_reversed_time():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# Independent anchors (VERDICT r01 item 1; torchdiffeq is absent here and on the B200 image, profiles/r02_torchdiffeq_probe.txt):
+# Independent anchors (torchdiffeq is not installed, scripts/probe_torchdiffeq.py):
 # a generic explicit Runge-Kutta written from the published Butcher tableaux in numpy fp64 -- no code shared with
 # oracle/odeint_port.py -- and scipy's adaptive integrators as ground truth.
 _TABLEAUX = {

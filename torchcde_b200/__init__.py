@@ -1,4 +1,4 @@
-"""torchcde_b200 -- a B200-native (sm_100a) Neural-CDE solve path with the torchcde API.
+"""torchcde_b200 -- an H100-native (sm_90a) Neural-CDE solve path with the torchcde API.
 
 Drop-in names (reference torchcde/__init__.py:1-9): ``cdeint``, ``CubicSpline``,
 ``LinearInterpolation``, ``natural_cubic_coeffs``, ``natural_cubic_spline_coeffs``,

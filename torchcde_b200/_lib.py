@@ -59,7 +59,6 @@ SIGNATURES = {
     "tcde_logsignature_windows": ([_p, _i64, _i64, _i64, _p, _i64, _int, _p, _i64, _p, _int, _p], _int),
     "tcde_set_solve_variant": ([_int], _int),
     "tcde_set_natural_variant": ([_int], _int),
-    "tcde_set_trace_buffer": ([_p], _int),
 }
 
 _lib = None
@@ -102,7 +101,7 @@ def require_cuda(*tensors):
     for x in tensors:
         if x is not None and not x.is_cuda:
             raise RuntimeError(
-                "torchcde_b200 runs on CUDA (B200, sm_100a) only and has no CPU path; got a tensor on '{}'. "
+                "torchcde_b200 runs on CUDA (H100, sm_90a) only and has no CPU path; got a tensor on '{}'. "
                 "Move the inputs to the GPU first.".format(x.device))
 
 

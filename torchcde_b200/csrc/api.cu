@@ -19,14 +19,16 @@ int cuda_failed(cudaError_t e, const char* what) {
     return TCDE_ERR_CUDA;
 }
 
+// SMs of the current device; 132 (an H100 SXM) only if the runtime cannot say, which the launches that follow report
 int sm_count() {
+    constexpr int kFallback = 132;
     static thread_local int cached_dev = -1;
     static thread_local int cached = 0;
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return kFallback;
     if (dev != cached_dev) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) n = kFallback;
         cached = n;
         cached_dev = dev;
     }

@@ -7,13 +7,13 @@ namespace tcde {
 
 static constexpr int kThreads = 256;
 
-// packed fp32x2 arithmetic (sm_100 FADD2 / FMUL2): two IEEE-rounded operations per instruction
-typedef uint64_t f2;
-__device__ __forceinline__ f2 pk2(float a, float b) { f2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk2(f2 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) { f2 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f2 sub2(f2 a, f2 b) { f2 d; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) { f2 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
+// two-float arithmetic: one IEEE rounding per lane and operation, never contracted into an FMA
+typedef float2 f2;
+__device__ __forceinline__ f2 pk2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void upk2(f2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 sub2(f2 a, f2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 // kernel selectors for tests / benchmarks (tcde_set_natural_variant, defined in fill.cu)
 extern int g_fill_variant;            // 0 = scan / ballot warp-per-path gap fill when they fit, 1 = one thread per

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the torchcde_b200 kernels (sm_100a only).
+// Shared device/host helpers for the torchcde_b200 kernels (sm_90a).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -90,7 +90,7 @@ template <int N> __device__ __forceinline__ void cp_async_wait() {
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-// ---- arguments of the tensor-core solve (solve_umma.cu), filled in by the C entry points of solve_simt.cu ----
+// ---- arguments of the tensor-core solve (solve_tc.cu), filled in by the C entry points of solve_simt.cu ----
 struct UmmaArgs {
     const float* control;
     const float* weight;
@@ -107,30 +107,18 @@ struct UmmaArgs {
     int64_t n_rows;
     int control_kind, method, n_stages, n_steps, n_out;
     float sign;
-    long long* trace;     // optional [64][8] clock64 stamps of CTA 0 / tile 0 (profiling aid), else nullptr
     float* stage_dump;    // optional [n_steps * n_stages][n_paths][32]: the input of every stage (for the adjoint)
-    int debug;            // solve_tc.cu: profiling experiments with WRONG results (1 no row fetch, 4 no TMEM reads,
-                          // 8 no split) and switches with right results (2 proxy fence in every row thread too, 16 one segment, 32 force four segments, 64 no stagger)
 };
-bool solve_umma_supported(int H, int C);
-int solve_umma_f32(const UmmaArgs& a, int H, int C, cudaStream_t stream);
-// round-2 kernel (solve_tc.cu): Runge-Kutta state in registers; mode 0 = 3xTF32 (13 MMAs per stage), mode 1 = 2xFP16 with
-// per-path power-of-two scaling (7 MMAs per stage)
+bool solve_tc_supported(int H, int C);
+// tensor-core kernel (solve_tc.cu): Runge-Kutta state in registers; mode 0 = 3xTF32 operand split, mode 1 = 2xFP16 with
+// per-path power-of-two scaling
 int solve_tc_f32(const UmmaArgs& a, int H, int C, int mode, cudaStream_t stream);
-int current_solve_variant();          // tcde_set_solve_variant: 0 auto, 1 CUDA-core, 2 tcgen05 round 1, 3 tcgen05 TF32 r2, 4 tcgen05 FP16 r2
+int current_solve_variant();          // tcde_set_solve_variant: 0 auto, 1 CUDA-core, 2 / 3 tensor cores 3xTF32, 4 tensor cores 2xFP16
 
-// parameter gradients of a whole backward solve on the tensor cores (param_grad_umma.cu)
-int param_grad_umma_grid(int64_t n_paths, int64_t n_stage_total);
-int param_grad_umma_f32(const float* control, int control_kind, int64_t n_rows, const float* z_stages,
-                        const float* a_stages, const int32_t* stage_index, const float* stage_frac,
-                        const float* stage_weight, int n_stage_total, float* scratch, int64_t n_paths, int grid,
-                        cudaStream_t stream);
-
-// round 2: the same product with U on the N side (6 MMAs of N = 256 per 32 pairs instead of 24 of N = 48), BF16 two-way split,
-// MN-major operands, TMA-fed (param_grad_bf16.cu)
-int param_grad_bf16_grid(int64_t n_paths, int64_t n_stage_total);
-int param_grad_bf16_f32(const float* control, int control_kind, int64_t n_rows, const float* z_stages, const float* a_stages,
-                        const int32_t* stage_index, const float* stage_frac, const float* stage_weight, int n_stage_total,
-                        float* scratch, int64_t n_paths, int grid, cudaStream_t stream);
+// parameter gradients of a whole backward solve on the tensor cores (param_grad_mma.cu): mode 0 = 3xTF32, 1 = 2xBF16 split
+int param_grad_mma_grid(int64_t n_paths, int64_t n_stage_total);
+int param_grad_mma_f32(const float* control, int control_kind, int64_t n_rows, const float* z_stages, const float* a_stages,
+                       const int32_t* stage_index, const float* stage_frac, const float* stage_weight, int n_stage_total,
+                       float* scratch, int64_t n_paths, int mode, int grid, cudaStream_t stream);
 
 }  // namespace tcde

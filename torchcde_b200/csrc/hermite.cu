@@ -1,4 +1,4 @@
-// Hot path (i): batched spline-coefficient construction (sm_100a) -- Hermite cubic with backward differences.
+// Hot path (i): batched spline-coefficient construction (sm_90a) -- Hermite cubic with backward differences.
 //
 // The builders are HBM-bound streaming kernels (SURVEY.md 8d: ~1 flop per byte).  The design rules
 // that matter are the memory ones: coalesced 128-bit loads, results staged in shared memory and

@@ -1,4 +1,4 @@
-// Hot path (i): batched spline-coefficient construction (sm_100a) -- natural cubic splines (NaN-free knots and the per-series version with missing values).
+// Hot path (i): batched spline-coefficient construction (sm_90a) -- natural cubic splines (NaN-free knots and the per-series version with missing values).
 //
 // The builders are HBM-bound streaming kernels (SURVEY.md 8d: ~1 flop per byte).  The design rules
 // that matter are the memory ones: coalesced 128-bit loads, results staged in shared memory and

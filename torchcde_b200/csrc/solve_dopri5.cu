@@ -14,9 +14,9 @@
 //     reads the done flag once per chunk; launches after the end are no-ops.
 //   * on acceptance each thread evaluates torchdiffeq's 4th-order dense output for its own path at every requested
 //     time inside the accepted step (y0, y1, y_mid, f0, f1 are all still in HBM / L2: the state is double buffered);
-//   * then the attempt itself: the six new slopes k2..k7 (k1 is FSAL) through the same tcgen05 pipeline as the
-//     fixed-step solve (tc_common.cuh: 2xFP16 split, 7 MMAs per tile-stage, accumulators in TMEM, two tiles of 128
-//     paths ping-pong per CTA); y, k1, k2/k6 live in registers, k3..k5 in shared memory (k2's coefficient is zero in
+//   * then the attempt itself: the six new slopes k2..k7 (k1 is FSAL) through the same warp-level tensor-core field as the
+//     fixed-step solve (tc_common.cuh: 2xFP16 split, each warp evaluates its own 32 paths); y, k1, k2/k6 live in
+//     registers, k3..k5 in shared memory (k2's coefficient is zero in
 //     the 5th-order weights, the error weights and the dense output, so k6 takes its registers); stage times ->
 //     spline interval and fraction with the reference's bucketize semantics on the device; error partial sums of
 //     (err / (atol + rtol max(|y0|, |y1|)))^2 in double; candidate (y1, k7) into the other state buffer.
@@ -30,7 +30,7 @@
 // every attempt leaves the inputs of its stages 1, 3, 4, 5, 6 (the non-zero b_i) in slot [number of accepted steps so far]
 // of two trajectories (a rejected attempt is simply overwritten by the next one), the controller writes the accepted steps'
 // quadrature nodes (spline interval, fraction, dt * b_i), and ONE launch of the parameter-gradient GEMM
-// (param_grad_bf16.cu) contracts them afterwards.  (Not part of the error norm: in the host-driven adjoint the 8,448
+// (tcde_linear_field_param_grads) contracts them afterwards.  (Not part of the error norm: in the host-driven adjoint the 8,448
 // parameter-gradient components are 0.2 % of the packed state's RMS.)
 #include "tc_common.cuh"
 
@@ -40,8 +40,9 @@ namespace dp5 {
 
 using namespace tc;
 
+constexpr int kRows = 128;                        // paths per tile
 constexpr int kTiles = 2;
-constexpr int kThreads = kRows * kTiles;          // 256: thread = path; lane 0 of a tile's first warp issues its MMAs
+constexpr int kThreads = kRows * kTiles;          // 256: thread = path
 constexpr int kCtl = 24;                          // doubles per control slot
 
 // control slot fields (doubles; the integer ones hold exact small integers)
@@ -89,15 +90,12 @@ struct Args {
 };
 
 struct Smem {
-    static constexpr int b = 0;                                   // 256 rows x 128 B  (W_hi | W_lo)
-    static constexpr int a = b + kCols * 128;                     // [kTiles][128 rows x 128 B]
-    static constexpr int raw = a + kTiles * kRows * 128;          // [kTiles][6][128] float4
+    static constexpr int b = 0;                                   // operand B (W_hi | W_lo) + bias: tc_common.cuh
+    static constexpr int a = (BSmem<1>::bytes + 127) & ~127;      // [kThreads / 32] per-warp operand scratch
+    static constexpr int raw = a + (kThreads / 32) * WarpSmem<1>::bytes;   // [kTiles][6][128] float4
     static constexpr int park = raw + kTiles * 6 * kRows * 16;    // [kTiles][3][32][128] floats: k3, k4, k5
-    static constexpr int b_aug = park + kTiles * 3 * kHid * kRows * 4;
-    static constexpr int a_aug = b_aug + kCols * 32;
-    static constexpr int misc = a_aug + kTiles * kRows * 32;      // decision + coefficient tables
-    static constexpr int bars = misc + 1024;
-    static constexpr int total = bars + 64;
+    static constexpr int misc = park + kTiles * 3 * kHid * kRows * 4;      // decision + coefficient tables
+    static constexpr int total = misc + 1024;
 };
 
 // what thread 0 decides for the whole CTA (identically in every CTA)
@@ -141,13 +139,9 @@ __device__ __forceinline__ double next_step(double dt, double ratio) {          
 
 __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args a) {
     extern __shared__ unsigned char smem_unaligned[];
-    unsigned char* smem = smem_unaligned + ((1024u - (smem_u32(smem_unaligned) & 1023u)) & 1023u);
+    unsigned char* smem = smem_unaligned + ((128u - (smem_u32(smem_unaligned) & 127u)) & 127u);
     Plan* plan = reinterpret_cast<Plan*>(smem + Smem::misc);
-    float* red = reinterpret_cast<float*>(smem + Smem::misc + 640);
     double* cta_sums = reinterpret_cast<double*>(smem + Smem::misc + 896);
-    uint64_t* a_ready = reinterpret_cast<uint64_t*>(smem + Smem::bars);
-    uint64_t* d_ready = a_ready + kTiles;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(d_ready + kTiles);
     const int tid = threadIdx.x, warp = tid >> 5;
     const int64_t n_elem = a.n_paths * kHid;
     const int64_t plane = n_elem;                     // floats per state buffer
@@ -248,7 +242,7 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
 
     const int64_t n_pairs = (a.n_paths + kRows * kTiles - 1) / (kRows * kTiles);
     const int t_ = warp >> 2;                         // tile of this thread
-    const int r = tid & (kRows - 1);
+    const int r = (warp & 3) * 32 + lane_row(tid & 31);   // its row in the tile: the row warp_field evaluates for this lane
 
     // ---- 2. dense output of the step that was just accepted, for the thread's own paths ---------------------------
     if (plan->emit_hi > plan->emit_lo) {
@@ -292,33 +286,15 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
     if (plan->done) return;
 
     // ---- 3. the attempt --------------------------------------------------------------------------------------------
-    float w_scale, inv_w_scale, beta;
-    prepare_b_fp16(smem + Smem::b, smem + Smem::b_aug, a.weight, a.bias, red, tid, kThreads, w_scale, inv_w_scale, beta);
-    for (int e = tid; e < kTiles * kRows * 2; e += kThreads)
-        *reinterpret_cast<uint4*>(smem + Smem::a_aug + (e >> 8) * (kRows * 32) + aug_off((e >> 1) & 127, e & 1)) = make_uint4(0u, 0u, 0u, 0u);
-    if (tid == 0) {
-        for (int t = 0; t < kTiles; ++t) {
-            mbar_init(&a_ready[t], kRows);
-            mbar_init(&d_ready[t], 1);
-        }
-        fence_barrier_init();
-    }
-    if (warp == 0) tmem_alloc(tmem_slot, 512);
-    fence_proxy_async_smem();
-    tc_fence_before();
+    float inv_w_scale, beta;
+    prepare_b<1>(smem + Smem::b, a.weight, a.bias, tid, kThreads, inv_w_scale, beta);
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    unsigned char* a_tile = smem + Smem::a + t_ * kRows * 128;
-    unsigned char* a_aug = smem + Smem::a_aug + t_ * kRows * 32;
+    unsigned char* ws = smem + Smem::a + warp * WarpSmem<1>::bytes;
     float4* raw = reinterpret_cast<float4*>(smem + Smem::raw) + (size_t)t_ * 6 * kRows + r;
     float* park = reinterpret_cast<float*>(smem + Smem::park) + (size_t)t_ * 3 * kHid * kRows + r;      // [slot][h][row]
-    const uint32_t taddr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(t_ * kCols);
     const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
     const int row_stride = cubic ? 4 * kCh : kCh;
-    const bool issuer_warp = (warp & 3) == 0;
-    uint32_t phase_a = 0, phase_d = 0;
     const float* Ycur = a.state + (size_t)plan->cur * plane;
     const float* Fcur = a.state + (size_t)(2 + plan->cur) * plane;
     float* Ynew = a.state + (size_t)(plan->cur ^ 1) * plane;
@@ -335,10 +311,8 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
         const bool tile_live = (pair * kTiles + t_) * kRows < a.n_paths;
         const int half = (paired && pair * kTiles * kRows >= a.n_ctrl) ? 1 : 0;
         if (half != cur_half) {                       // CTA-uniform: switch the operand B to the adjoint state's weights
-            tc_fence_before();
-            __syncthreads();                          // every MMA that read the old weights has been waited for
-            prepare_b_fp16(smem + Smem::b, smem + Smem::b_aug, a.weight2, a.bias2, red, tid, kThreads, w_scale, inv_w_scale, beta);
-            fence_proxy_async_smem();
+            __syncthreads();                          // every warp is done reading the old weights
+            prepare_b<1>(smem + Smem::b, a.weight2, a.bias2, tid, kThreads, inv_w_scale, beta);
             __syncthreads();
             cur_half = half;
         }
@@ -361,22 +335,8 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
             for (int j = 0; j < parts; ++j) cp_async16(&raw[j * kRows], src + 4 * j);
             cp_async_commit();
         };
-        float inv_scale = 1.f;
-        // one field evaluation: operand rows of `z` -> MMAs -> dX/dt of stage s -> contraction into kv
+        // one field evaluation: dX/dt of stage s, the next stage's row requested, then the tensor-core product + contraction
         auto evaluate = [&](const float* z, int s, float* kv, auto&& shadow) {
-            inv_scale = split_store_fp16(z, a_tile, a_aug, r, beta, inv_w_scale);
-            fence_proxy_async_smem();
-            tc_fence_before();
-            mbar_arrive(&a_ready[t_]);
-            if (issuer_warp) {
-                mbar_wait(&a_ready[t_], phase_a);
-                tc_fence_after();
-                if ((tid & 31) == 0)
-                    issue_fp16(tmem_base + (uint32_t)(t_ * kCols), a_tile, a_aug, smem + Smem::b, smem + Smem::b_aug, &d_ready[t_]);
-                __syncwarp();
-            }
-            phase_a ^= 1;
-            // ---- in the MMAs' shadow -----------------------------------------------------------------------------
             cp_async_wait<0>();
             f2 dx2[kCh / 2];
             {
@@ -392,17 +352,16 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
                 } else {
                     dx2[0] = pk(b0.x, b0.y); dx2[1] = pk(b0.z, b0.w); dx2[2] = pk(b1.x, b1.y); dx2[3] = pk(b1.z, b1.w);
                 }
-                const float post = sign * inv_scale;
-                const f2 p2 = pk(post, post);
+                const f2 p2 = pk(sign, sign);
 #pragma unroll
                 for (int q = 0; q < 4; ++q) dx2[q] = mul2(dx2[q], p2);
             }
+            float dx[kCh];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) upk(dx2[q], dx[2 * q], dx[2 * q + 1]);
             if (s + 1 < 6) fetch_row(plan->stage_index[s + 1]);
             shadow();
-            mbar_wait(&d_ready[t_], phase_d);
-            phase_d ^= 1;
-            tc_fence_after();
-            contract_row<32>(taddr, dx2, kv);
+            warp_field<1>(z, dx, kv, ws, smem + Smem::b, beta, inv_w_scale);
         };
         auto nothing = [] {};
 
@@ -522,14 +481,12 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) err_acc += __shfl_down_sync(0xffffffffu, err_acc, off);
     if ((tid & 31) == 0) cta_sums[warp] = err_acc;
-    tc_fence_before();
     __syncthreads();
     if (tid == 0) {
         double s = 0.0;
         for (int w = 0; w < kThreads / 32; ++w) s += cta_sums[w];
         a.partials[(size_t)(a.seq & 1) * gridDim.x + blockIdx.x] = s;
     }
-    if (warp == 0) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace dp5

@@ -1,4 +1,4 @@
-// Hot path (ii): the fused fixed-step CDE solve on the FP32/FP64 CUDA-core pipe (sm_100a).
+// Hot path (ii): the fused fixed-step CDE solve on the FP32/FP64 CUDA-core pipe (sm_90a).
 //
 // One persistent-state kernel replaces what the reference does with ~10^4 small launches and
 // ~4*10^3 host syncs per solve (SURVEY.md 3.1): for every Runge-Kutta stage it evaluates the
@@ -14,7 +14,7 @@
 // consecutive paths and accumulates an ST x CT tile of  z . W^T  per channel chunk, with the
 // stage input z^T and W^T staged in shared memory ([k][path] and [k][chunk][h][4] so that
 // every shared-memory access is a conflict-free or broadcast 128-bit load).  The tensor-core
-// (tcgen05) variant lives in solve_umma.cu; this file is also the generic-shape path.
+// variant lives in solve_tc.cu; this file is also the generic-shape path.
 #include "common.cuh"
 
 namespace tcde {
@@ -500,30 +500,22 @@ static int launch_field(const void* control, int control_kind, int64_t n_rows, c
     return TCDE_OK;
 }
 
-// ---- tensor-core variant (solve_umma.cu) -------------------------------------------------------
+// ---- tensor-core variant (solve_tc.cu) ---------------------------------------------------------
 #ifndef TCDE_DEFAULT_TC_MODE
-#define TCDE_DEFAULT_TC_MODE 1      // bit 0: 2xFP16 operand split (7 MMAs per stage) instead of 3xTF32 (13)
+#define TCDE_DEFAULT_TC_MODE 1      // bit 0: 2xFP16 operand split (6 MMAs per 16 x 8 block) instead of 3xTF32 (12)
 #endif
-static long long* g_trace = nullptr;   // profiling aid: device buffer for in-kernel clock stamps (see tcde_set_trace_buffer)
-static int g_debug_flags = 0;
-static int g_solve_variant = 0;     // 0 auto, 1 CUDA-core kernel, 2 tcgen05 kernel (round 1), 3 / 4 round-2 kernel TF32 / FP16
+static int g_solve_variant = 0;     // 0 auto, 1 CUDA-core kernel, 2 / 3 tensor cores 3xTF32, 4 tensor cores 2xFP16
 int current_solve_variant() { return g_solve_variant; }
 
 }  // namespace tcde
 
 using namespace tcde;
 
-extern "C" int tcde_set_trace_buffer(void* device_buffer) {
-    g_trace = static_cast<long long*>(device_buffer);
-    return TCDE_OK;
-}
-
 extern "C" int tcde_set_solve_variant(int variant) {
     TCDE_CHECK_ARG(variant >= 0 && (variant & 15) <= 6,
-                   "variant=%d (0 auto, 1 CUDA-core kernel, 2 tcgen05 round-1 kernel, 3 / 4 round-2 kernel with the 3xTF32 / 2xFP16 "
-                   "operand split; 6 / 5 are aliases of 3 / 4)", variant);
-    g_solve_variant = variant & 15;
-    g_debug_flags = variant >> 4;        // profiling experiments (timing only, wrong results); 0 in normal use
+                   "variant=%d (0 auto, 1 CUDA-core kernel, 3 / 4 tensor-core kernel with the 3xTF32 / 2xFP16 operand split; "
+                   "2, 6 / 5 are aliases of 3 / 4)", variant);
+    g_solve_variant = variant & 15;      // bits above 15 (profiling switches of earlier kernels) are accepted and ignored
     return TCDE_OK;
 }
 
@@ -564,21 +556,20 @@ static int solve_fixed_linear(const void* control, int control_kind, int64_t n_r
     const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (dtype == TCDE_F32) {
-        // auto: the tcgen05 kernel wherever it is built for the shape (parity-tested against the
+        // auto: the tensor-core kernel wherever it is built for the shape (parity-tested against the
         // CUDA-core kernel and the fp64 oracle), the CUDA-core kernel for every other shape
-        const bool umma_ok = solve_umma_supported((int)hidden, (int)channels) &&
-                             ((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z0) |
-                               reinterpret_cast<uintptr_t>(out)) & 15) == 0;
-        const bool want_umma = (g_solve_variant >= 2) || (g_solve_variant == 0 && umma_ok);
-        if (want_umma) {
+        const bool tc_ok = solve_tc_supported((int)hidden, (int)channels) &&
+                           ((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z0) |
+                             reinterpret_cast<uintptr_t>(out)) & 15) == 0;
+        const bool want_tc = (g_solve_variant >= 2) || (g_solve_variant == 0 && tc_ok);
+        if (want_tc) {
             UmmaArgs u{(const float*)control, (const float*)weight, (const float*)bias, (const float*)z0, (float*)out,
                        (const float*)step_dt, stage_index, (const float*)stage_frac, out_step, out_mode,
                        (const float*)out_slope, n_paths, n_rows, control_kind, method, n_stages, (int)n_steps,
-                       (int)n_out, (float)sign, g_trace, (float*)stage_dump, g_debug_flags};
-            if (g_solve_variant == 2) return solve_umma_f32(u, (int)hidden, (int)channels, s);        // the round-1 kernel, kept for comparison
-            // round-2 kernel: 3 / 6 = 3xTF32 split, 4 / 5 = 2xFP16 split (5, 6: aliases from the development history)
-            const int mode = (g_solve_variant == 3 || g_solve_variant == 6) ? 0 : (g_solve_variant == 4 || g_solve_variant == 5) ? 1
-                                                                                                                                  : TCDE_DEFAULT_TC_MODE;
+                       (int)n_out, (float)sign, (float*)stage_dump};
+            // 2 / 3 / 6 = 3xTF32 split, 4 / 5 = 2xFP16 split (2, 5, 6: aliases from the development history)
+            const int mode = (g_solve_variant == 2 || g_solve_variant == 3 || g_solve_variant == 6) ? 0
+                             : (g_solve_variant == 4 || g_solve_variant == 5) ? 1 : TCDE_DEFAULT_TC_MODE;
             return solve_tc_f32(u, (int)hidden, (int)channels, mode, s);
         }
         TCDE_CHECK_SUPPORTED(stage_dump == nullptr, "the stage dump is written by the tensor-core solve only "

@@ -1,584 +1,212 @@
-// Hot path (ii), round 2: the fused fixed-step CDE solve on tcgen05 -- persistent, balanced, warp-specialised.
+// Hot path (ii): the fused fixed-step CDE solve on the tensor cores (sm_90a, warp-level mma.sync).
 //
-// What changed against solve_umma.cu (round 1, kept as variant 2), each step measured (profiles/r02_*):
-//   * r01 trace: one tile-stage was a 4,065-cycle serial chain of which 1,664 are tensor work (13 MMAs x 128 cycles), and
-//     256 CTAs on 148 SMs ran as 1.73 waves.  The chain, not the tensor pipe, sets the pace (two tiles of 128 paths is all
-//     that TMEM's 512 columns allow in flight), so every change below shortens the chain or removes work from it:
-//   * the Runge-Kutta slopes k1, k2 (+k3) never leave registers: the row warps get 240 registers by setmaxnreg from a third
-//     warpgroup (warps 8, 9 = one MMA issuer per tile; 10, 11 only donate); the old 64 LDS + 32-64 STS per thread and
-//     stage of "parked" slopes are gone;
-//   * MODE 1 halves the tensor work: operands are split into TWO FP16 pieces instead of two TF32 pieces.  An FP16 MMA
-//     carries K = 16 per instruction at the cycle cost of a K = 8 TF32 one, so z_lo.W_hi + z_hi.W_lo + z_hi.W_hi are
-//     6 MMAs instead of 12 (+1 for the bias in both modes).  FP16 has TF32's 11-bit significand (hi + lo = 22 bits,
-//     error ~2^-22 like 3xTF32) but only 5 exponent bits, so every path's row is scaled by its own power of two (exact)
-//     so that max(|z_k|, bias floor) lands in [2^13, 2^14); the weights get one global power of two; elements more than
-//     2^-27 below the row maximum lose relative -- not absolute -- precision, which is what a dot product needs.  The
-//     scale is undone for free by folding its inverse into the path's dX/dt before the contraction.  hi | lo of a row
-//     share ONE 128-byte swizzled A row (K = 64);
-//   * the spline rows come by TMA: one cp.async.bulk.tensor per tile and stage (box = 128 paths x one interval's
-//     a|b|2c|3d, 128B swizzle, double buffered, issued by the tile's MMA issuer a stage ahead).  The per-thread cp.async
-//     of round 1 touched 32 cache lines per warp instruction: 1,536 L1 cycles per stage on the SM's one LSU pipe;
-//   * 16-column TMEM loads, the next in flight while the current is contracted (the contraction runs at 82 % of the TMEM
-//     read rate of 64 B/cycle per sub-partition: 626 cycles for a tile's 128 KB), a tree for the row maximum;
-//   * ONE proxy fence per tile and stage, executed by the issuer after it has acquired a_ready, instead of one per row
-//     thread on the critical chain (the arrivals' release + the issuer's acquire order the rows' generic-proxy stores
-//     before that fence; scripts/soak_fence.py checks bit-identity with the row-fenced variant, debug bit 1);
-//   * the two tiles run in anti-phase (a nanosleep for tile 1 once per unit): started together they stay in lockstep and
-//     queue behind each other's 7 MMAs every stage;
-//   * DUMP (the adjoint's stage trajectory): staged in a swizzled tile, one TMA tensor store per tile and stage issued
-//     after the commit -- 32 threads storing 128 B each straight to HBM cost 32 lines per instruction (5.9 vs 3.56 ms);
-//   * persistent CTAs (one per SM) over work units (pair of tiles, segment of the time axis): 256 pairs x 4 segments over
-//     148 SMs is 6.9 -> 7 rounds of a quarter solve = 1.75 solves per SM instead of 2.  A unit starts from the state its
-//     predecessor left in HBM (32 floats per path) once that unit's flag is up; units are dealt round-robin in
-//     (segment, pair) order, so a predecessor is always a full round older and nobody waits in steady state.
-//
-// CTA anatomy (384 threads): warps 0-3 / 4-7 = the 128 rows of tile 0 / 1 (thread = path); warp 8 / 9 = MMA + TMA
-// issuer of tile 0 / 1; accumulators [128 x 256] fp32 per tile in TMEM (all 512 columns).  mbarriers: a_ready[t]
-// (128 arrivals: operand rows written), d_ready[t] (tcgen05.commit), raw_full[t][2] (TMA bytes landed).
+// Thread = path, warp = 32 paths, and the warps of a CTA never wait for each other after the one-time setup of operand B.
+// Each Runge-Kutta stage of a warp is
+//   * dX/dt of the stage from the path's spline row (read straight from HBM: b | 2c | 3d of the interval, 96 bytes per path;
+//     the next stage's row is requested before the current stage's products so that its latency hides behind them);
+//   * the field W z + b of the warp's 32 paths as a [32 x 32] . [32 x 256] product on the tensor cores with a two-way
+//     operand split (tc_common.cuh: MODE 1 = 2xFP16 with per-path power-of-two scaling, 6 MMAs per 16 x 8 block; MODE 0 =
+//     3xTF32, 12 MMAs), contracted with dX/dt in registers; every lane ends with the 32 slopes of its own path;
+//   * the Runge-Kutta combination in registers, one rounding per operation in the order of oracle/odeint_port.py.
+// The Runge-Kutta state y, k1 and the running k2 + k3 stay in registers for the whole solve.  With a stage dump (the adjoint's
+// stage trajectory) every stage input is also written to HBM.
 #include "tc_common.cuh"
 
 namespace tcde {
 
 namespace tc {
 
-using namespace umma;
+constexpr int kWarps = 4;
+constexpr int kThreads = 32 * kWarps;            // 128 paths per CTA
 
-constexpr int kH = 32;
-constexpr int kC = 8;
-constexpr int kN = kH * kC;       // 256 accumulator columns per tile
-constexpr int kTile = 128;
-constexpr int kTiles = 2;
-constexpr int kRowThreads = kTile * kTiles;     // 256 row threads: thread = path
-constexpr int kThreads = kRowThreads + 128;     // + the issuer warpgroup
-#ifndef TCDE_TC_LD_WIDTH
-#define TCDE_TC_LD_WIDTH 16                     // columns per TMEM load in the contraction (32 does not fit 240 registers)
-#endif
-
-// how the time axis is cut and where the hand-over state lives (all device pointers; n_seg == 1: nothing is handed over)
-struct Units {
-    int n_seg;
-    int steps_per_seg;
-    const int32_t* seg_first_out;   // [n_seg]: first output index whose step is >= the segment's first step
-    float* ystate;                  // [n_paths][32]: state at the end of a path's last finished segment
-    int* progress;                  // [n_pairs]: segments finished, zero before the launch
-};
-
-// shared-memory map (bytes).  MODE 0: TF32 hi / lo tiles (K = 32 floats = one 128-byte row each);
-// MODE 1: one FP16 tile per operand, row = [hi(32) | lo(32)] halves = 128 bytes.
 template <int MODE> struct Smem {
-    static constexpr int b_bytes = (MODE == 0 ? 2 : 1) * kN * 128;
-    static constexpr int a_tile_bytes = (MODE == 0 ? 2 : 1) * kTile * 128;          // per tile: hi (+ lo tile in MODE 0)
     static constexpr int b = 0;
-    static constexpr int a = b + b_bytes;
-    static constexpr int raw = a + kTiles * a_tile_bytes;                            // [kTiles][2 buffers][128 rows x 128 B] (TMA, swizzled)
-    static constexpr int raw_buf = kTile * 128;
-    static constexpr int b_aug = raw + kTiles * 2 * raw_buf;                         // N rows x 32 B (no swizzle, K-major)
-    static constexpr int a_aug = b_aug + kN * 32;                                    // [kTiles][128 rows x 32 B] (MODE 0: one 8-row group)
-    static constexpr int red = a_aug + kTiles * kTile * 32;                          // 64 floats of reduction scratch
-    static constexpr int bars = red + 256;                                           // a_ready[2], d_ready[2], raw_full[2][2], tmem slot
-    static constexpr int total = bars + 128;
-    // MODE 1 with a stage dump: two [128 rows x 128 B] staging tiles per tile (TMA store source, 128-byte swizzle), used
-    // alternately: the store of stage s may still be reading its tile while the rows stage the input of stage s + 1
-    static constexpr int dump = (total + 1023) & ~1023;
-    static constexpr int dump_buf = kTile * 128;
-    static constexpr int total_dump = dump + kTiles * 2 * dump_buf;
+    static constexpr int warps = (BSmem<MODE>::bytes + 127) & ~127;
+    static constexpr int total = warps + kWarps * WarpSmem<MODE>::bytes;
 };
 
-__device__ __forceinline__ void reg_dealloc_24() { asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory"); }
-__device__ __forceinline__ void reg_alloc_240() { asm volatile("setmaxnreg.inc.sync.aligned.u32 240;\n" ::: "memory"); }
-__device__ __forceinline__ int ld_acquire(const int* p) {
-    int v;
-    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release(int* p, int v) { asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-
-// The MMAs of one tile-stage, issued by ONE thread: D[128 x 256] = split(A) . split(B)^T + bias, then commit -> d_ready
-template <int MODE>
-__device__ __forceinline__ void issue_tile(uint32_t d, unsigned char* smem, unsigned char* a_tile, unsigned char* a_aug, uint64_t* d_ready) {
+template <int MODE, bool DUMP>
+__global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a) {
     using S = Smem<MODE>;
-    // instruction descriptor: D = F32 (bit 4), A/B format (bits 7 / 10: 2 = TF32, 0 = F16), N >> 3 (bit 17), M >> 4 (bit 24)
-    constexpr uint32_t fmt = (MODE == 0) ? 2u : 0u;
-    constexpr uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(kN >> 3) << 17) | ((uint32_t)(kTile >> 4) << 24);
-    const uint64_t db = make_desc(smem + S::b);
-    // K-major no-swizzle descriptors: LBO = 128 B (next 16 bytes of K), SBO = 256 B (next 8 rows), version 1
-    const uint64_t db_aug = (uint64_t)((smem_u32(smem + S::b_aug) & 0x3FFFF) >> 4) | (8ull << 16) | (16ull << 32) | (1ull << 46);
-    if (MODE == 0) {
-        const uint64_t db_lo = make_desc(smem + S::b + kN * 128);
-        const uint64_t dah = make_desc(a_tile);
-        const uint64_t dal = make_desc(a_tile + kTile * 128);
-        const uint64_t da_aug = (uint64_t)((smem_u32(smem + S::a_aug) & 0x3FFFF) >> 4) | (8ull << 16) | (0ull << 32) | (1ull << 46);
-        // small terms first; each K block is 8 tf32 = 32 bytes = +2 in the descriptor's address field
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb) mma_tf32(d, dal + 2 * kb, db + 2 * kb, idesc, kb > 0);
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb) mma_tf32(d, dah + 2 * kb, db_lo + 2 * kb, idesc, 1);
-#pragma unroll
-        for (int kb = 0; kb < 4; ++kb) mma_tf32(d, dah + 2 * kb, db + 2 * kb, idesc, 1);
-        mma_tf32(d, da_aug, db_aug, idesc, 1);                // + bias (1 * bias_hi + 1 * bias_lo)
-    } else {
-        const uint64_t da = make_desc(a_tile);
-        const uint64_t da_aug = (uint64_t)((smem_u32(a_aug) & 0x3FFFF) >> 4) | (8ull << 16) | (16ull << 32) | (1ull << 46);
-        // K block = 16 halves = 32 bytes = +2; A row = [hi: blocks 0,1 | lo: blocks 2,3], B row likewise
-        mma_f16(d, da + 4, db + 0, idesc, 0);                 // z_lo . W_hi
-        mma_f16(d, da + 6, db + 2, idesc, 1);
-        mma_f16(d, da + 0, db + 4, idesc, 1);                 // z_hi . W_lo
-        mma_f16(d, da + 2, db + 6, idesc, 1);
-        mma_f16(d, da + 0, db + 0, idesc, 1);                 // z_hi . W_hi
-        mma_f16(d, da + 2, db + 2, idesc, 1);
-        mma_f16(d, da_aug, db_aug, idesc, 1);                 // + row_scale * bias
-    }
-    if (d_ready) mma_commit(d_ready);
-}
-
-template <int MODE, bool TRACE, bool DUMP>
-__global__ void __launch_bounds__(kThreads, 1) cdeint_tc_kernel(const UmmaArgs a, const Units un, const __grid_constant__ CUtensorMap rows_map,
-                                                                const __grid_constant__ CUtensorMap dump_map) {
-    using S = Smem<MODE>;
-    // the stage dump of the adjoint goes through a swizzled staging tile and ONE TMA tensor store per tile and stage (MODE 1;
-    // MODE 0 has no shared memory left for it): 32 row threads storing 128 B each straight to HBM touch 32 lines per
-    // instruction -- measured 5.9 ms per dumping solve against 3.0 ms without the dump
-    constexpr bool kStaged = DUMP && MODE == 1;
     using E = exact<float>;
     extern __shared__ unsigned char smem_unaligned[];
-    unsigned char* smem = smem_unaligned + ((1024u - (smem_u32(smem_unaligned) & 1023u)) & 1023u);
-    uint64_t* a_ready = reinterpret_cast<uint64_t*>(smem + S::bars);
-    uint64_t* d_ready = a_ready + kTiles;
-    uint64_t* raw_full = d_ready + kTiles;                    // [tile][buffer]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(raw_full + 2 * kTiles);
-    float* red = reinterpret_cast<float*>(smem + S::red);
-    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
-    const int row_floats = cubic ? 4 * kC : kC;
-    const uint32_t row_bytes_tile = (uint32_t)(kTile * row_floats * 4);
-
-    const int tid = threadIdx.x;
-    const int warp = tid >> 5;
-    constexpr int kAllocWarp = kRowThreads / 32;              // warp 8
-
-    // ---- one-time setup: operand B (the weights, split) and the bias K-block -------------------------------------
-    float inv_w_scale = 1.f, beta = 0.f;                      // MODE 1: global power-of-two scales
-    if (MODE == 0) {
-        float* b_hi = reinterpret_cast<float*>(smem + S::b);
-        float* b_lo = b_hi + kN * 32;
-        for (int e = tid; e < kN * kH; e += kThreads) {
-            const int n = e >> 5, k = e & 31;
-            const float w = a.weight[e];                     // weight[n][k], n = h*C + c
-            const float hi = tf32_hi(w);
-            b_hi[swz(n, k)] = hi;
-            b_lo[swz(n, k)] = w - hi;
-        }
-        float* a_aug = reinterpret_cast<float*>(smem + S::a_aug);
-        float* b_aug = reinterpret_cast<float*>(smem + S::b_aug);
-        for (int e = tid; e < 8 * 8; e += kThreads) {
-            const int row = e >> 3, k = e & 7;
-            a_aug[(k >> 2) * 32 + row * 4 + (k & 3)] = (k < 2) ? 1.f : 0.f;         // (1, 1, 0...): SBO = 0 serves all rows
-        }
-        for (int e = tid; e < kN * 8; e += kThreads) {
-            const int row = e >> 3, k = e & 7;
-            const float bv = a.bias[row];
-            const float hi = tf32_hi(bv);
-            b_aug[(row >> 3) * 64 + (k >> 2) * 32 + (row & 7) * 4 + (k & 3)] = (k == 0) ? hi : (k == 1) ? (bv - hi) : 0.f;
-        }
-    } else {
-        float w_scale;
-        prepare_b_fp16(smem + S::b, smem + S::b_aug, a.weight, a.bias, red, tid, kThreads, w_scale, inv_w_scale, beta);
-        for (int e = tid; e < kTiles * kTile * 2; e += kThreads)                     // per-row scale goes to k = 0, 1 each stage
-            *reinterpret_cast<uint4*>(smem + S::a_aug + (e >> 8) * (kTile * 32) + aug_off((e >> 1) & 127, e & 1)) = make_uint4(0u, 0u, 0u, 0u);
-    }
-    if (tid == 0) {
-        for (int t = 0; t < kTiles; ++t) {
-            mbar_init(&a_ready[t], kTile);
-            mbar_init(&d_ready[t], 1);
-            mbar_init(&raw_full[2 * t], 1);
-            mbar_init(&raw_full[2 * t + 1], 1);
-        }
-        fence_barrier_init();
-        tma_prefetch_desc(&rows_map);
-    }
-    if (warp == kAllocWarp) tmem_alloc(tmem_slot, 512);
-    fence_proxy_async_smem();
-    tc_fence_before();
+    unsigned char* smem = smem_unaligned + ((128u - (smem_u32(smem_unaligned) & 127u)) & 127u);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    float inv_w_scale, beta;
+    prepare_b<MODE>(smem + S::b, a.weight, a.bias, tid, kThreads, inv_w_scale, beta);
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    const bool is_row = warp < kRowThreads / 32;
-    const int n_pairs = (int)((a.n_paths + kRowThreads - 1) / kRowThreads);
-    const int n_units = n_pairs * un.n_seg;
-    const int t = is_row ? (warp >> 2) : (warp - kRowThreads / 32);      // tile served by this warp (issuers: 0, 1; donors: 2, 3)
-    const int r = tid & (kTile - 1);
-    uint32_t phase_a = 0, phase_d = 0;                       // issuer / row side of the two hand-shakes
-    uint32_t kcount = 0;                                     // stages this warp's tile has gone through: raw buffer kcount & 1
+    const int64_t warp_path0 = (int64_t)blockIdx.x * kThreads + warp * 32;
+    if (warp_path0 >= a.n_paths) return;                      // no CTA-wide barrier follows
+    unsigned char* ws = smem + S::warps + warp * WarpSmem<MODE>::bytes;
+    const int64_t path = warp_path0 + lane_row(lane);
+    const bool live = path < a.n_paths;
+    const int64_t lpath = live ? path : a.n_paths - 1;
+    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
+    const int row_floats = cubic ? 4 * kCh : kCh;
+    // the part of a spline row that dX/dt reads: b | 2c | 3d (cubic), the slope (linear)
+    const float4* crow = reinterpret_cast<const float4*>(a.control + lpath * a.n_rows * row_floats + (cubic ? kCh : 0));
+    const int row_f4 = row_floats / 4;
+    const float sign = (a.sign < 0.f) ? -1.f : 1.f;
 
-    // the two roles run the SAME unit loop (same CTA barriers per unit) in separate code regions: setmaxnreg gives each
-    // region its own register budget
-#define TCDE_UNIT_PROLOGUE()                                                                                          \
-        const int seg = u / n_pairs, pair = u - seg * n_pairs;                                                        \
-        const int step_lo = seg * un.steps_per_seg;                                                                   \
-        const int step_hi = min(a.n_steps, step_lo + un.steps_per_seg);                                               \
-        const int st_lo = step_lo * a.n_stages, st_hi = step_hi * a.n_stages;                                         \
-        const int64_t tile_path0 = (int64_t)pair * kRowThreads + (int64_t)t * kTile;                                  \
-        const bool tile_live = t < kTiles && tile_path0 < a.n_paths;                                                  \
-        if (seg > 0) {                      /* the unit that ends where this one starts must be done */              \
-            if (tid == 0)                                                                                             \
-                while (ld_acquire(un.progress + pair) < seg) __nanosleep(64);                                         \
-            __syncthreads();                                                                                          \
+    auto fetch = [&](int interval, float4* raw) {
+        const float4* src = crow + (int64_t)interval * row_f4;
+        raw[0] = __ldg(src); raw[1] = __ldg(src + 1);
+        if (cubic) { raw[2] = __ldg(src + 2); raw[3] = __ldg(src + 3); raw[4] = __ldg(src + 4); raw[5] = __ldg(src + 5); }
+    };
+    auto write_out = [&](int j, const float* v) {
+        if (!live) return;
+        float4* dst = reinterpret_cast<float4*>(a.out + (path * a.n_out + j) * kHid);
+#pragma unroll
+        for (int c4 = 0; c4 < 8; ++c4) dst[c4] = make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
+    };
+    auto dump = [&](int stage_no, const float* z) {
+        if (!DUMP || !live) return;
+        float4* dst = reinterpret_cast<float4*>(a.stage_dump + ((int64_t)stage_no * a.n_paths + path) * kHid);
+#pragma unroll
+        for (int c4 = 0; c4 < 8; ++c4) dst[c4] = make_float4(z[4 * c4], z[4 * c4 + 1], z[4 * c4 + 2], z[4 * c4 + 3]);
+    };
+
+    float y[kHid], k1[kHid], s23[kHid], zin[kHid];
+    {
+        const float4* zp = reinterpret_cast<const float4*>(a.z0 + lpath * kHid);
+#pragma unroll
+        for (int c4 = 0; c4 < 8; ++c4) {
+            const float4 v = zp[c4];
+            y[4 * c4] = v.x; y[4 * c4 + 1] = v.y; y[4 * c4 + 2] = v.z; y[4 * c4 + 3] = v.w;
         }
-#define TCDE_UNIT_EPILOGUE()                                                                                          \
-        if (seg + 1 < un.n_seg) {                                                                                     \
-            __syncthreads();                                                                                          \
-            if (tid == 0) st_release(un.progress + pair, seg + 1);                                                    \
-        }
+#pragma unroll
+        for (int h = 0; h < kHid; ++h) { k1[h] = 0.f; s23[h] = 0.f; zin[h] = y[h]; }
+    }
+    int jn = 0;
+    int next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
+    while (jn < a.n_out && next_out < 0) {                    // outputs at the initial time
+        write_out(jn, y);
+        ++jn;
+        next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
+    }
 
-    if (!is_row) {
-        reg_dealloc_24();
-        for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-            TCDE_UNIT_PROLOGUE()
-            // ================================ MMA + TMA issuer of tile t ==========================
-            if (tile_live && (tid & 31) == 0) {
-                auto fetch_rows = [&](uint32_t k, int interval) {     // rows of one interval -> raw[t][k & 1]
-                    if (a.debug & 1) return;
-                    uint64_t* bar = &raw_full[2 * t + (k & 1)];
-                    mbar_expect_tx(bar, row_bytes_tile);
-                    tma_load_2d(smem + S::raw + (2 * t + (k & 1)) * S::raw_buf, &rows_map, interval * row_floats, (int)tile_path0, bar);
-                };
-                int idx_next = (st_lo + 1 < st_hi) ? a.stage_index[st_lo + 1] : 0;   // schedule entries are read a stage ahead
-                fetch_rows(kcount, a.stage_index[st_lo]);
-                for (int st = st_lo; st < st_hi; ++st) {
-                    const int idx_fetch = idx_next;
-                    if (st + 2 < st_hi) idx_next = a.stage_index[st + 2];
-                    mbar_wait(&a_ready[t], phase_a);
-                    phase_a ^= 1;
-                    fence_proxy_async_smem();                 // the row threads' operand (and staging) stores -> async proxy
-                    tc_fence_after();
-                    const bool tr = TRACE && a.trace && u == 0 && t == 0 && st < 64;
-                    if (tr) a.trace[st * 8 + 0] = clock64();
-                    issue_tile<MODE>(tmem_base + (uint32_t)(t * kN), smem, smem + S::a + t * S::a_tile_bytes,
-                                     smem + S::a_aug + t * kTile * 32, kStaged ? nullptr : &d_ready[t]);
-                    if (kStaged) {
-                        // the commit releases the row threads into the next stage, where they refill the staging tile of the
-                        // PREVIOUS stage: its store (issued a full period ago) must have read it
-                        bulk_wait_read<0>();
-                        mma_commit(&d_ready[t]);
-                    }
-                    if (tr) a.trace[st * 8 + 1] = clock64();
-                    ++kcount;
-                    // the rows of the NEXT stage: their buffer was last read two stages ago, before the arrivals just waited for
-                    if (st + 1 < st_hi) fetch_rows(kcount, idx_fetch);
-                    if (kStaged) {
-                        // this stage's input rows (staged by the row threads before their arrival) -> the trajectory in HBM,
-                        // off the chain: nobody waits for this store before the next stage's commit
-                        tma_store_3d(&dump_map, smem + S::dump + (2 * t + (st & 1)) * S::dump_buf, 0, (int)tile_path0, st);
-                        bulk_commit();
-                    }
-                }
+    const int n_st = a.n_steps * a.n_stages;
+    const float third = (float)(1.0 / 3.0);
+    float4 raw[6], nxt[6];
+    fetch(a.stage_index[0], raw);
+    int step = 0, sub = 0;
+    float dt = a.step_dt[0];
+    for (int st = 0; st < n_st; ++st) {
+        dump(st, zin);
+        // dX/dt of this stage (interpolation_cubic.py:331-336) times the sign of the time direction
+        float dx[kCh];
+        {
+            const float fr = a.stage_frac[st];
+            if (cubic) {
+                const float* b = reinterpret_cast<const float*>(raw);
+#pragma unroll
+                for (int c = 0; c < kCh; ++c) dx[c] = E::mul(E::add(b[c], E::mul(E::add(b[kCh + c], E::mul(b[2 * kCh + c], fr)), fr)), sign);
+            } else {
+                const float* b = reinterpret_cast<const float*>(raw);
+#pragma unroll
+                for (int c = 0; c < kCh; ++c) dx[c] = E::mul(b[c], sign);
             }
-            if (kStaged && (tid & 31) == 0) bulk_wait_all();  // the unit's trajectory rows are in HBM before the unit is released
-            __syncwarp();                                     // lanes 1-31 wait here for lane 0: the CTA barriers below are warp-aligned
-            TCDE_UNIT_EPILOGUE()
         }
-    } else {
-        reg_alloc_240();
-        for (int u = blockIdx.x; u < n_units; u += gridDim.x) {
-            TCDE_UNIT_PROLOGUE()
-            if (tile_live) {
-            // ================================ row threads =========================================
-            const int64_t path = tile_path0 + r;
-            const bool live = path < a.n_paths;
-            const int64_t lpath = live ? path : a.n_paths - 1;
-            unsigned char* a_tile = smem + S::a + t * S::a_tile_bytes;
-            unsigned char* a_aug = smem + S::a_aug + t * kTile * 32;
-            const unsigned char* raw_tile = smem + S::raw + 2 * t * S::raw_buf;      // two buffers
-            const uint32_t taddr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(t * kN);
-            const float sign = (a.sign < 0.f) ? -1.f : 1.f;
-            float inv_scale = 1.f;                        // MODE 1: 1 / (row scale * weight scale) of the stage in flight
+        if (st + 1 < n_st) fetch(a.stage_index[st + 1], nxt);
 
-            auto write_a = [&](const float* z, int stage_no) {   // next stage input -> split operand rows
-                if (kStaged) {                            // ... and, for the adjoint, to the trajectory in HBM (via a staging tile)
-                    unsigned char* row = smem + S::dump + (2 * t + (stage_no & 1)) * S::dump_buf + r * 128;
-#pragma unroll
-                    for (int c4 = 0; c4 < 8; ++c4)
-                        *reinterpret_cast<float4*>(row + ((c4 ^ (r & 7)) << 4)) = make_float4(z[4 * c4], z[4 * c4 + 1], z[4 * c4 + 2], z[4 * c4 + 3]);
-                } else if (DUMP && live) {
-                    float4* dst = reinterpret_cast<float4*>(a.stage_dump + ((int64_t)stage_no * a.n_paths + path) * kH);
-#pragma unroll
-                    for (int c4 = 0; c4 < 8; ++c4) dst[c4] = make_float4(z[4 * c4], z[4 * c4 + 1], z[4 * c4 + 2], z[4 * c4 + 3]);
-                }
-                if (MODE == 0) {
-                    float* a_hi = reinterpret_cast<float*>(a_tile);
-                    float* a_lo = a_hi + kTile * 32;
-#pragma unroll
-                    for (int c4 = 0; c4 < 8; ++c4) {
-                        float4 hi, lo;
-                        hi.x = tf32_hi(z[4 * c4 + 0]); hi.y = tf32_hi(z[4 * c4 + 1]);
-                        hi.z = tf32_hi(z[4 * c4 + 2]); hi.w = tf32_hi(z[4 * c4 + 3]);
-                        upk(sub2(pk(z[4 * c4 + 0], z[4 * c4 + 1]), pk(hi.x, hi.y)), lo.x, lo.y);
-                        upk(sub2(pk(z[4 * c4 + 2], z[4 * c4 + 3]), pk(hi.z, hi.w)), lo.z, lo.w);
-                        const uint32_t off = (uint32_t)r * 32u + (uint32_t)((c4 ^ (r & 7)) << 2);
-                        *reinterpret_cast<float4*>(a_hi + off) = hi;
-                        *reinterpret_cast<float4*>(a_lo + off) = lo;
-                    }
-                } else if (!(a.debug & 8)) {
-                    inv_scale = split_store_fp16(z, a_tile, a_aug, r, beta, inv_w_scale);
-                }
-                // no proxy fence here: the arrival (release) publishes these generic-proxy stores to the issuer thread, which
-                // executes ONE fence.proxy.async after its acquire and before it hands the rows to the tensor core / TMA unit.
-                // A fence per row thread (MEMBAR.ALL.CTA + FENCE.VIEW.ASYNC) sat on the critical chain: ~330 cycles per stage
-                // (debug bit 1 (2): put it back, for A/B timing)
-                if (a.debug & 2) fence_proxy_async_smem();
-                tc_fence_before();
-                mbar_arrive(&a_ready[t]);
-            };
-            auto write_out = [&](int j, const float* v) {
-                if (!live) return;
-                float4* dst = reinterpret_cast<float4*>(a.out + (path * a.n_out + j) * kH);
-#pragma unroll
-                for (int c4 = 0; c4 < 8; ++c4) dst[c4] = make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
-            };
+        float kv[kHid];
+        warp_field<MODE>(zin, dx, kv, ws, smem + S::b, beta, inv_w_scale);
 
-            float y[kH], k1[kH], s23[kH];
-            {
-                // the hand-over state was written by another SM during this launch: read it through L2 (ld.global.cg), never
-                // from this SM's L1, which may still hold the line from an earlier segment of the same paths
-                const float4* zp = reinterpret_cast<const float4*>((seg == 0 ? a.z0 : un.ystate) + lpath * kH);
+        // Runge-Kutta combination; the next stage input ends up in zin
+        bool step_done = false;
+        const f2 dt2 = pk(dt, dt);
+        if (a.method == TCDE_RK4_38) {
+            const f2 th2 = pk(third, third);
+            if (sub == 0) {
 #pragma unroll
-                for (int c4 = 0; c4 < 8; ++c4) {
-                    const float4 v = (seg == 0) ? zp[c4] : __ldcg(zp + c4);
-                    y[4 * c4] = v.x; y[4 * c4 + 1] = v.y; y[4 * c4 + 2] = v.z; y[4 * c4 + 3] = v.w;
+                for (int h = 0; h < kHid; h += 2) {
+                    k1[h] = kv[h]; k1[h + 1] = kv[h + 1];
+                    upk(add2(pk(y[h], y[h + 1]), mul2(mul2(dt2, pk(kv[h], kv[h + 1])), th2)), zin[h], zin[h + 1]);
                 }
+            } else if (sub == 1) {
 #pragma unroll
-                for (int h = 0; h < kH; ++h) { k1[h] = 0.f; s23[h] = 0.f; }
+                for (int h = 0; h < kHid; h += 2) {
+                    s23[h] = kv[h]; s23[h + 1] = kv[h + 1];
+                    upk(add2(pk(y[h], y[h + 1]), mul2(dt2, sub2(pk(kv[h], kv[h + 1]), mul2(pk(k1[h], k1[h + 1]), th2)))),
+                        zin[h], zin[h + 1]);
+                }
+            } else if (sub == 2) {
+#pragma unroll
+                for (int h = 0; h < kHid; h += 2) {
+                    const f2 k2p = pk(s23[h], s23[h + 1]), k3p = pk(kv[h], kv[h + 1]);
+                    upk(add2(pk(y[h], y[h + 1]), mul2(dt2, add2(sub2(pk(k1[h], k1[h + 1]), k2p), k3p))), zin[h], zin[h + 1]);
+                    upk(add2(k2p, k3p), s23[h], s23[h + 1]);
+                }
+            } else {
+                const f2 three = pk(3.f, 3.f), eighth = pk(0.125f, 0.125f);
+#pragma unroll
+                for (int h = 0; h < kHid; h += 2) {
+                    const f2 sum = add2(add2(pk(k1[h], k1[h + 1]), mul2(three, pk(s23[h], s23[h + 1]))), pk(kv[h], kv[h + 1]));
+                    upk(add2(pk(y[h], y[h + 1]), mul2(mul2(sum, dt2), eighth)), zin[h], zin[h + 1]);
+                }
+                step_done = true;
             }
-            int jn = (seg == 0) ? 0 : un.seg_first_out[seg];
-            int next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
-            while (seg == 0 && jn < a.n_out && next_out < 0) {         // outputs at the initial time
-                write_out(jn, y);
+        } else if (a.method == TCDE_MIDPOINT) {
+            if (sub == 0) {
+                const float half = E::mul(0.5f, dt);
+#pragma unroll
+                for (int h = 0; h < kHid; ++h) zin[h] = E::add(y[h], E::mul(kv[h], half));
+            } else {
+#pragma unroll
+                for (int h = 0; h < kHid; ++h) zin[h] = E::add(y[h], E::mul(dt, kv[h]));
+                step_done = true;
+            }
+        } else {
+#pragma unroll
+            for (int h = 0; h < kHid; ++h) zin[h] = E::add(y[h], E::mul(dt, kv[h]));
+            step_done = true;
+        }
+        if (step_done) {
+            while (next_out == step) {
+                const int mode = a.out_mode[jn];
+                if (mode == 0) write_out(jn, y);
+                else if (mode == 1) write_out(jn, zin);
+                else {
+                    const float slope_w = a.out_slope[jn];
+                    float v[kHid];
+#pragma unroll
+                    for (int h = 0; h < kHid; ++h) v[h] = E::add(y[h], E::mul(slope_w, E::sub(zin[h], y[h])));
+                    write_out(jn, v);
+                }
                 ++jn;
                 next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
             }
-            // the two tiles of a CTA share one tensor pipe: started together they stay in lockstep and each waits for the
-            // other's 7 MMAs every stage (measured: 1,990 cycles from issue to d_ready instead of ~1,150); half a stage of
-            // head start for tile 0, once per unit, keeps them in anti-phase
-            if (t == 1 && !(a.debug & 64)) __nanosleep(800);
-            write_a(y, st_lo);
-
-            const float third = (float)(1.0 / 3.0);
-            int step = step_lo, sub = 0;
-            float dt = a.step_dt[step_lo];
-            float dt_next = (step_lo + 1 < a.n_steps) ? a.step_dt[step_lo + 1] : 0.f;
-            float frac0 = a.stage_frac[st_lo];                            // this stage's fraction
-            float frac1 = (st_lo + 1 < st_hi) ? a.stage_frac[st_lo + 1] : 0.f;   // next stage's, read a full stage ahead
-            for (int st = st_lo; st < st_hi; ++st) {
-                const bool more = st + 1 < st_hi;
-                // ---- in the MMA's shadow: dX/dt from the rows the TMA unit delivered (interpolation_cubic.py:331-336),
-                //      times the sign of the time direction and (MODE 1) the inverse of the operand scales
-                if (!(a.debug & 1)) mbar_wait(&raw_full[2 * t + (kcount & 1)], (kcount >> 1) & 1);
-                f2 dx2[kC / 2];
-                {
-                    const unsigned char* rows = raw_tile + (kcount & 1) * S::raw_buf;
-                    if (cubic) {
-                        // row r of the TMA box = [a | b | 2c | 3d], 16-byte chunk c at position c ^ (r & 7)
-                        const unsigned char* row = rows + r * 128;
-                        const int x = r & 7;
-                        const float4 b0 = *reinterpret_cast<const float4*>(row + ((2 ^ x) << 4)), b1 = *reinterpret_cast<const float4*>(row + ((3 ^ x) << 4));
-                        const float4 c0 = *reinterpret_cast<const float4*>(row + ((4 ^ x) << 4)), c1 = *reinterpret_cast<const float4*>(row + ((5 ^ x) << 4));
-                        const float4 d0 = *reinterpret_cast<const float4*>(row + ((6 ^ x) << 4)), d1 = *reinterpret_cast<const float4*>(row + ((7 ^ x) << 4));
-                        const f2 fr = pk(frac0, frac0);
-                        dx2[0] = add2(pk(b0.x, b0.y), mul2(add2(pk(c0.x, c0.y), mul2(pk(d0.x, d0.y), fr)), fr));
-                        dx2[1] = add2(pk(b0.z, b0.w), mul2(add2(pk(c0.z, c0.w), mul2(pk(d0.z, d0.w), fr)), fr));
-                        dx2[2] = add2(pk(b1.x, b1.y), mul2(add2(pk(c1.x, c1.y), mul2(pk(d1.x, d1.y), fr)), fr));
-                        dx2[3] = add2(pk(b1.z, b1.w), mul2(add2(pk(c1.z, c1.w), mul2(pk(d1.z, d1.w), fr)), fr));
-                    } else {
-                        const float4 b0 = *reinterpret_cast<const float4*>(rows + r * 32), b1 = *reinterpret_cast<const float4*>(rows + r * 32 + 16);
-                        dx2[0] = pk(b0.x, b0.y); dx2[1] = pk(b0.z, b0.w); dx2[2] = pk(b1.x, b1.y); dx2[3] = pk(b1.z, b1.w);
-                    }
-                    const float post = sign * inv_scale;          // +-1 in MODE 0; a power of two (exact) in MODE 1
-                    const f2 p2 = pk(post, post);
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) dx2[q] = mul2(dx2[q], p2);
-                }
-                ++kcount;
-                frac0 = frac1;
-                if (st + 2 < st_hi) frac1 = a.stage_frac[st + 2];
-
-                const bool tr = TRACE && a.trace && u == 0 && t == 0 && r == 0 && st < 64;
-                if (tr) a.trace[st * 8 + 2] = clock64();
-                mbar_wait(&d_ready[t], phase_d);
-                phase_d ^= 1;
-                tc_fence_after();
-                if (tr) a.trace[st * 8 + 3] = clock64();
-
-                // ---- kv[h] = sum_c D[h*C + c] * dX[c]  (the bias is already in D); packed FFMA2
-                float kv[kH];
-                if (a.debug & 4) {
-#pragma unroll
-                    for (int h = 0; h < kH; ++h) kv[h] = y[h] * 1e-3f;
-                } else {
-                    contract_row<TCDE_TC_LD_WIDTH>(taddr, dx2, kv);
-                }
-
-                if (tr) a.trace[st * 8 + 4] = clock64();
-                // ---- Runge-Kutta combination in registers, one rounding per operation in the order of
-                //      oracle/odeint_port.py, two hidden units per instruction; zn ends up in kv's registers
-                bool step_done = false;
-                const f2 dt2 = pk(dt, dt);
-                if (a.method == TCDE_RK4_38) {
-                    const f2 th2 = pk(third, third);
-                    if (sub == 0) {
-#pragma unroll
-                        for (int h = 0; h < kH; h += 2) {
-                            k1[h] = kv[h]; k1[h + 1] = kv[h + 1];
-                            upk(add2(pk(y[h], y[h + 1]), mul2(mul2(dt2, pk(kv[h], kv[h + 1])), th2)), kv[h], kv[h + 1]);
-                        }
-                    } else if (sub == 1) {
-#pragma unroll
-                        for (int h = 0; h < kH; h += 2) {
-                            s23[h] = kv[h]; s23[h + 1] = kv[h + 1];
-                            upk(add2(pk(y[h], y[h + 1]), mul2(dt2, sub2(pk(kv[h], kv[h + 1]), mul2(pk(k1[h], k1[h + 1]), th2)))),
-                                kv[h], kv[h + 1]);
-                        }
-                    } else if (sub == 2) {
-#pragma unroll
-                        for (int h = 0; h < kH; h += 2) {
-                            const f2 k2p = pk(s23[h], s23[h + 1]), k3p = pk(kv[h], kv[h + 1]);
-                            upk(add2(pk(y[h], y[h + 1]), mul2(dt2, add2(sub2(pk(k1[h], k1[h + 1]), k2p), k3p))), kv[h], kv[h + 1]);
-                            upk(add2(k2p, k3p), s23[h], s23[h + 1]);
-                        }
-                    } else {
-                        const f2 three = pk(3.f, 3.f), eighth = pk(0.125f, 0.125f);
-#pragma unroll
-                        for (int h = 0; h < kH; h += 2) {
-                            const f2 sum = add2(add2(pk(k1[h], k1[h + 1]), mul2(three, pk(s23[h], s23[h + 1]))), pk(kv[h], kv[h + 1]));
-                            upk(add2(pk(y[h], y[h + 1]), mul2(mul2(sum, dt2), eighth)), kv[h], kv[h + 1]);
-                        }
-                        step_done = true;
-                    }
-                } else if (a.method == TCDE_MIDPOINT) {
-                    if (sub == 0) {
-                        const float half = E::mul(0.5f, dt);
-#pragma unroll
-                        for (int h = 0; h < kH; ++h) kv[h] = E::add(y[h], E::mul(kv[h], half));
-                    } else {
-#pragma unroll
-                        for (int h = 0; h < kH; ++h) kv[h] = E::add(y[h], E::mul(dt, kv[h]));
-                        step_done = true;
-                    }
-                } else {
-#pragma unroll
-                    for (int h = 0; h < kH; ++h) kv[h] = E::add(y[h], E::mul(dt, kv[h]));
-                    step_done = true;
-                }
-                if (tr) a.trace[st * 8 + 5] = clock64();
-                if (more) write_a(kv, st + 1);            // hand the next stage to the tensor core first ...
-                if (tr) a.trace[st * 8 + 6] = clock64();
-                if (step_done) {                          // ... then the bookkeeping that nobody waits for
-                    while (next_out == step) {
-                        const int mode = a.out_mode[jn];
-                        if (mode == 0) write_out(jn, y);
-                        else if (mode == 1) write_out(jn, kv);
-                        else {
-                            const float slope_w = a.out_slope[jn];
-                            float v[kH];
-#pragma unroll
-                            for (int h = 0; h < kH; ++h) v[h] = E::add(y[h], E::mul(slope_w, E::sub(kv[h], y[h])));
-                            write_out(jn, v);
-                        }
-                        ++jn;
-                        next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
-                    }
-#pragma unroll
-                    for (int h = 0; h < kH; ++h) y[h] = kv[h];
-                    ++step;
-                    sub = 0;
-                    dt = dt_next;
-                    if (step + 1 < a.n_steps) dt_next = a.step_dt[step + 1];
-                } else {
-                    ++sub;
-                }
-            }
-            if (seg + 1 < un.n_seg && live) {             // hand the state over to whoever runs the next segment
-                float4* dst = reinterpret_cast<float4*>(un.ystate + path * kH);
-#pragma unroll
-                for (int c4 = 0; c4 < 8; ++c4) dst[c4] = make_float4(y[4 * c4], y[4 * c4 + 1], y[4 * c4 + 2], y[4 * c4 + 3]);
-                __threadfence();
-            }
-            }
-            TCDE_UNIT_EPILOGUE()
+            for (int h = 0; h < kHid; ++h) y[h] = zin[h];
+            ++step;
+            sub = 0;
+            if (step < a.n_steps) dt = a.step_dt[step];
+        } else {
+            ++sub;
         }
+#pragma unroll
+        for (int j = 0; j < 6; ++j) raw[j] = nxt[j];
     }
-#undef TCDE_UNIT_PROLOGUE
-#undef TCDE_UNIT_EPILOGUE
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kAllocWarp) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace tc
 
-// n_seg: the smallest power of two (<= 8, segments of >= 8 steps) that minimises ceil(units / SMs) / n_seg
-static int choose_segments(int64_t n_pairs, int n_steps, int sms) {
-    int best = 1;
-    double best_cost = (double)((n_pairs + sms - 1) / sms);
-    for (int s = 2; s <= 8; s *= 2) {
-        if (n_steps / s < 8) break;
-        const int64_t units = n_pairs * s;
-        const double cost = (double)((units + sms - 1) / sms) / s;
-        if (cost < best_cost * 0.97) { best_cost = cost; best = s; }
-    }
-    return best;
-}
+bool solve_tc_supported(int H, int C) { return H == tc::kHid && C == tc::kCh; }
 
 template <int MODE> static int launch_tc(const UmmaArgs& a, cudaStream_t stream) {
-    const int64_t n_pairs = (a.n_paths + tc::kRowThreads - 1) / tc::kRowThreads;
-    TCDE_CHECK_SUPPORTED(n_pairs < (1ll << 28), "too many paths");
-    const int sms = sm_count();
-    // debug bit 4 (16): never cut the time axis; bit 5 (32): always cut it in (up to) four segments -- the tests use it to
-    // exercise the hand-over on small batches
-    const int n_seg = (a.debug & 16) ? 1 : (a.debug & 32) ? (a.n_steps >= 4 ? 4 : a.n_steps) : choose_segments(n_pairs, a.n_steps, sms);
-    const int steps_per_seg = (a.n_steps + n_seg - 1) / n_seg;
-    const int64_t n_units = n_pairs * n_seg;
-    const int grid = (int)(n_units < sms ? n_units : sms);
-    auto kern = a.stage_dump ? tc::cdeint_tc_kernel<MODE, false, true>
-                             : a.trace ? tc::cdeint_tc_kernel<MODE, true, false> : tc::cdeint_tc_kernel<MODE, false, false>;
-    const bool staged = a.stage_dump != nullptr && MODE == 1;
-    const int smem = (staged ? tc::Smem<MODE>::total_dump : tc::Smem<MODE>::total) + 1024;   // slack for the 1024-byte alignment of the tiles
+    const int64_t grid = (a.n_paths + tc::kThreads - 1) / tc::kThreads;
+    TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
+    auto kern = a.stage_dump ? tc::cdeint_tc_kernel<MODE, true> : tc::cdeint_tc_kernel<MODE, false>;
+    const int smem = tc::Smem<MODE>::total + 128;             // slack for the 128-byte alignment of the tiles
     TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    alignas(64) CUtensorMap rows_map;
-    const int row_floats = (a.control_kind == TCDE_CONTROL_CUBIC) ? 4 * tc::kC : tc::kC;
-    const int rc = tc::make_rows_tensor_map(&rows_map, a.control, a.n_paths, a.n_rows, row_floats);
-    TCDE_CHECK_SUPPORTED(rc == 0, "tensor-core solve: cuTensorMapEncodeTiled failed (%d) for control [%lld][%lld x %d floats]", rc,
-                         (long long)a.n_paths, (long long)a.n_rows, row_floats);
-
-    tc::Units un{n_seg, steps_per_seg, nullptr, nullptr, nullptr};
-    void* workspace = nullptr;
-    if (n_seg > 1) {
-        // hand-over state + flags + the per-segment output cursor: stream-ordered scratch, freed right after the launch
-        // (nothing outlives the call; the caller's buffers stay the only persistent memory, as the C ABI promises)
-        const size_t y_bytes = (size_t)a.n_paths * tc::kH * sizeof(float);
-        const size_t flag_bytes = ((size_t)n_pairs * sizeof(int) + 255) & ~(size_t)255;
-        const size_t cur_bytes = ((size_t)n_seg * sizeof(int32_t) + 255) & ~(size_t)255;
-        TCDE_CHECK_CUDA(cudaMallocAsync(&workspace, y_bytes + flag_bytes + cur_bytes, stream));
-        un.ystate = static_cast<float*>(workspace);
-        un.progress = reinterpret_cast<int*>(static_cast<char*>(workspace) + y_bytes);
-        int32_t* cursor = reinterpret_cast<int32_t*>(static_cast<char*>(workspace) + y_bytes + flag_bytes);
-        un.seg_first_out = cursor;
-        TCDE_CHECK_CUDA(cudaMemsetAsync(un.progress, 0, flag_bytes, stream));
-        tc::segment_cursor_kernel<<<1, 32, 0, stream>>>(a.out_step, a.n_out, n_seg, steps_per_seg, cursor);
-    }
-    alignas(64) CUtensorMap dump_map = rows_map;            // only read by the dumping MODE 1 kernel
-    if (staged) {
-        const int rc2 = tc::make_stage_tensor_map(&dump_map, a.stage_dump, a.n_paths, (int64_t)a.n_steps * a.n_stages);
-        TCDE_CHECK_SUPPORTED(rc2 == 0, "tensor-core solve: cuTensorMapEncodeTiled failed (%d) for the stage trajectory", rc2);
-    }
-    kern<<<grid, tc::kThreads, smem, stream>>>(a, un, rows_map, dump_map);
-    const cudaError_t launch_err = cudaGetLastError();
-    if (workspace) cudaFreeAsync(workspace, stream);
-    TCDE_CHECK_CUDA(launch_err);
+    kern<<<(unsigned)grid, tc::kThreads, smem, stream>>>(a);
+    TCDE_CHECK_CUDA(cudaGetLastError());
     return TCDE_OK;
 }
 
 int solve_tc_f32(const UmmaArgs& a, int H, int C, int mode, cudaStream_t stream) {
-    TCDE_CHECK_SUPPORTED(H == tc::kH && C == tc::kC, "tensor-core solve: built for hidden=32, channels=8 (got %d, %d)", H, C);
+    TCDE_CHECK_SUPPORTED(solve_tc_supported(H, C), "tensor-core solve: built for hidden=32, channels=8 (got %d, %d)", H, C);
     TCDE_CHECK_SUPPORTED((reinterpret_cast<uintptr_t>(a.control) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.z0) & 15) == 0 &&
                              (reinterpret_cast<uintptr_t>(a.out) & 15) == 0,
                          "tensor-core solve: control, z0 and out must be 16-byte aligned");

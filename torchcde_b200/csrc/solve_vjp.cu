@@ -1,5 +1,5 @@
 // One stage of the continuous adjoint of hot path (ii): the README-form linear vector field and
-// its vector-Jacobian products in ONE launch (sm_100a, fp32, hidden = 32, channels = 8).
+// its vector-Jacobian products in ONE launch (sm_90a, fp32, hidden = 32, channels = 8).
 //
 // torchdiffeq's odeint_adjoint (the reference's default, solver.py:144 / 226-227) integrates the
 // augmented state (z, a, dL/dW, dL/db) backwards in time; every stage of that solve needs
@@ -374,10 +374,8 @@ extern "C" int tcde_vector_field_linear_vjp(const void* control, int control_kin
 extern "C" int64_t tcde_linear_field_param_grads_scratch_bytes(int64_t n_paths, int64_t n_stages_total, int64_t channels,
                                                               int64_t hidden) {
     if (n_paths < 0 || n_stages_total < 1 || channels != vjp::C || hidden != vjp::H) return -1;
-    const int64_t g1 = vjp::param_grad_grid(n_paths, n_stages_total), g2 = param_grad_umma_grid(n_paths, n_stages_total);
-    const int64_t g3 = param_grad_bf16_grid(n_paths, n_stages_total);
-    const int64_t g = g1 > g2 ? (g1 > g3 ? g1 : g3) : (g2 > g3 ? g2 : g3);
-    return g * vjp::kParams * (int64_t)sizeof(float);
+    const int64_t g1 = vjp::param_grad_grid(n_paths, n_stages_total), g2 = param_grad_mma_grid(n_paths, n_stages_total);
+    return (g1 > g2 ? g1 : g2) * vjp::kParams * (int64_t)sizeof(float);
 }
 
 extern "C" int tcde_linear_field_param_grads(const void* control, int control_kind, int64_t n_rows, const void* z_stages,
@@ -398,21 +396,15 @@ extern "C" int tcde_linear_field_param_grads(const void* control, int control_ki
     if (n_paths == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     int grid;
-    if (current_solve_variant() != 1 && current_solve_variant() != 2 && aligned16(control)) {
-        // tensor cores, round 2: U on the N side, BF16 two-way split, MN-major operands fed by TMA
-        grid = param_grad_bf16_grid(n_paths, n_stages_total);
-        const int rc = param_grad_bf16_f32((const float*)control, control_kind, n_rows, (const float*)z_stages,
-                                           (const float*)a_stages, stage_index, (const float*)stage_frac,
-                                           (const float*)stage_weight, (int)n_stages_total, (float*)scratch, n_paths,
-                                           grid, s);
-        if (rc != TCDE_OK) return rc;
-    } else if (current_solve_variant() == 2 && aligned16(control)) {
-        // tensor cores, round 1 (3xTF32, U^T on the M side): kept for comparison
-        grid = param_grad_umma_grid(n_paths, n_stages_total);
-        const int rc = param_grad_umma_f32((const float*)control, control_kind, n_rows, (const float*)z_stages,
-                                           (const float*)a_stages, stage_index, (const float*)stage_frac,
-                                           (const float*)stage_weight, (int)n_stages_total, (float*)scratch, n_paths,
-                                           grid, s);
+    const int variant = current_solve_variant();
+    if (variant != 1) {
+        // tensor cores: 2xBF16 split by default (and for 4 / 5), 3xTF32 for the variants that select it for the solve
+        const int mode = (variant == 2 || variant == 3 || variant == 6) ? 0 : 1;
+        grid = param_grad_mma_grid(n_paths, n_stages_total);
+        const int rc = param_grad_mma_f32((const float*)control, control_kind, n_rows, (const float*)z_stages,
+                                          (const float*)a_stages, stage_index, (const float*)stage_frac,
+                                          (const float*)stage_weight, (int)n_stages_total, (float*)scratch, n_paths, mode,
+                                          grid, s);
         if (rc != TCDE_OK) return rc;
     } else {
         grid = vjp::param_grad_grid(n_paths, n_stages_total);

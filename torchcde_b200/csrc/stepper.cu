@@ -1,4 +1,4 @@
-// Elementwise pieces of the adaptive (dopri5) driver as single launches (sm_100a).
+// Elementwise pieces of the adaptive (dopri5) driver as single launches (sm_90a).
 //
 // One attempted Dormand-Prince step forms six stage states  y + dt * sum_j beta_ij k_j  and one
 // error estimate  |sum_j e_j k_j| / (atol + rtol * max(|y0|, |y1|)).  Written with torch operators

@@ -1,4 +1,5 @@
-// tcgen05 / TMEM / mbarrier helpers shared by the tensor-core kernels (solve_umma.cu, param_grad_umma.cu).
+// Small device helpers shared by the tensor-core kernels (solve_tc.cu, solve_dopri5.cu, param_grad_mma.cu):
+// shared-memory addresses, the 128-byte swizzle of the operand tiles, TF32 rounding and two-float arithmetic.
 #pragma once
 #include "common.cuh"
 
@@ -7,73 +8,9 @@ namespace umma {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done)
-                     : "r"(addr), "r"(parity)
-                     : "memory");
-    } while (!done);
-}
-// the same wait for a warp that expects to wait long and shares its scheduler with warps doing real work: sleep between
-// polls instead of spending issue slots on try_wait + branch (ncu on the param-grad kernel: half of all executed
-// instructions were the polls of its fold / TMA warps)
-__device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity, unsigned ns) {
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    for (;;) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done)
-                     : "r"(addr), "r"(parity)
-                     : "memory");
-        if (done) break;
-        __nanosleep(ns);
-    }
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)), "r"(cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] . B[smem desc], kind::tf32, issued by one thread
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// K-major, 128-byte-swizzled operand tile: row r (M or N index) is the 128 bytes at r*128; its
-// 16-byte chunk c lives at chunk position c ^ (r & 7).  Descriptor fields (cute mma_sm100_desc.hpp):
-// start address >> 4, LBO = 1 (unused for swizzled K-major), SBO = 1024 B between 8-row groups,
-// version = 1 (Blackwell), layout type 2 = SWIZZLE_128B.  Tiles are 1024-byte aligned.
-__device__ __forceinline__ uint64_t make_desc(const void* tile) {
-    const uint64_t addr = (uint64_t)((smem_u32(tile) & 0x3FFFF) >> 4);
-    return addr | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
+// 128-byte-swizzled tile of 32-float rows: row r is the 128 bytes at r*128; its 16-byte chunk c lives at chunk position
+// c ^ (r & 7), so that eight consecutive rows read at the same chunk hit eight different bank groups (ldmatrix).
 __device__ __forceinline__ uint32_t swz(int row, int k) {          // element offset of (row, k) in floats
     return (uint32_t)row * 32u + (uint32_t)((((k >> 2) ^ (row & 7)) << 2) | (k & 3));
 }
@@ -83,60 +20,14 @@ __device__ __forceinline__ float tf32_hi(float x) {
     return __uint_as_float(u);
 }
 
-// ---- packed fp32x2 arithmetic (sm_100: FADD2 / FMUL2 / FFMA2, IEEE rounding per lane) ----------
-typedef uint64_t f2;
-__device__ __forceinline__ f2 pk(float a, float b) { f2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk(f2 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) { f2 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f2 sub2(f2 a, f2 b) { f2 d; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) { f2 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { f2 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-
-
-// 32 lanes x 16 columns, issue and wait separated so that the next load overlaps the arithmetic on the
-// current one.  The destination registers go through the wait statement ("+r") so that the compiler
-// cannot schedule a use above it.
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16_wait(uint32_t* r) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                   "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :
-                 : "memory");
-}
-
-// 32 lanes x 32 columns in one instruction (4 KB per warp): with one such load in flight behind the one being consumed the
-// TMEM read port, not the load latency, paces the epilogue.  tcgen05.wait::ld waits for ALL outstanding loads of the thread,
-// so deeper pipelining than "issue next, consume current" is not expressible.
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]),
-          "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]),
-          "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld32_wait(uint32_t* r) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]),
-                   "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]), "+r"(r[16]),
-                   "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]), "+r"(r[24]),
-                   "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-                 :
-                 : "memory");
-}
+// ---- two-float arithmetic, one IEEE rounding per lane and operation (never contracted into an FMA except fma2) ------
+typedef float2 f2;
+__device__ __forceinline__ f2 pk(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void upk(f2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 sub2(f2 a, f2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 
 }  // namespace umma
 }  // namespace tcde

@@ -751,7 +751,7 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     if not hasattr(X, 'derivative'):
         raise ValueError("X must have a 'derivative' method.")
     if isinstance(z0, (tuple, list)):
-        raise NotImplementedError("torchcde_b200.cdeint: tuple / list states (TupleControl) are outside the B200 hot "
+        raise NotImplementedError("torchcde_b200.cdeint: tuple / list states (TupleControl) are outside the fused hot "
                                   "path; pass a single tensor state.")
     if not isinstance(z0, torch.Tensor):
         raise ValueError("z0 must either a tensor or a tuple/list of tensors.")
