@@ -237,6 +237,21 @@ def odeint_dopri5(field, y0, times, rtol, atol, options=None, targets=None):
 # ----------------------------------------------------- dopri5 with the controller on the device (linear field)
 _DEVICE_CHUNK = 48          # launches enqueued between two reads of the done flag
 
+# One control slot of solve_dopri5.cu: CTL_SIZE doubles, fields in the order of its C_* enum.  Launch n reads slot
+# (n - 1) & 1 and writes slot n & 1; the integer fields hold exact small integers.
+CTL_SIZE = 24
+(CTL_T, CTL_DT, CTL_TEND, CTL_RTOL, CTL_ATOL, CTL_CUR, CTL_DONE, CTL_PENDING, CTL_NACC, CTL_NREJ, CTL_NEXT_OUT,
+ CTL_NPART, CTL_NEED_MID, CTL_RATIO, CTL_LAUNCHES, CTL_OVERFLOW, CTL_BASE) = range(17)
+
+
+def initial_control(t0, dt, t_end, rtol, atol):
+    """The two control slots before launch 0: slot 1 (what launch 0 reads) holds the start, no attempt pending."""
+    ctl = torch.zeros(2, CTL_SIZE, dtype=torch.float64)
+    ctl[1, CTL_T], ctl[1, CTL_DT], ctl[1, CTL_TEND] = t0, dt, t_end
+    ctl[1, CTL_RTOL], ctl[1, CTL_ATOL] = rtol, atol
+    ctl[1, CTL_NEXT_OUT] = 1
+    return ctl
+
 
 def device_dopri5_available(z0, channels):
     return (z0.is_cuda and z0.dtype == torch.float32 and z0.size(-1) == 32 and channels == 8 and z0.numel() > 0)
@@ -262,11 +277,7 @@ def odeint_dopri5_device(control, kind, n_rows, knots, weight, bias, field, y0, 
         state[2].copy_(f0)
         grid = lib.tcde_dopri5_linear_grid(n_paths)
         partials = torch.zeros(2, grid, dtype=torch.float64, device=dev)
-        ctl_host = torch.zeros(2, 24, dtype=torch.float64)
-        ctl_host[1, 0], ctl_host[1, 1], ctl_host[1, 2] = t0, dt, times[-1]
-        ctl_host[1, 3], ctl_host[1, 4] = rtol, atol
-        ctl_host[1, 10] = 1                       # next output index
-        ctl = ctl_host.to(dev)
+        ctl = initial_control(t0, dt, times[-1], rtol, atol).to(dev)
         out = torch.empty(n_paths, len(times), hidden, dtype=torch.float32, device=dev)
         out[:, 0].copy_(yf)
         out_times = torch.tensor(times, dtype=torch.float64, device=dev)
@@ -280,11 +291,12 @@ def odeint_dopri5_device(control, kind, n_rows, knots, weight, bias, field, y0, 
                           _lib.F32, stream)
                 seq += _DEVICE_CHUNK
                 last = ctl[(seq - 1) & 1].cpu()              # the one host read per chunk
-                if last[6] != 0:
+                if last[CTL_DONE] != 0:
                     break
-                if not math.isfinite(float(last[1])) or float(last[1]) == 0.0 or seq > 10_000_000:
-                    raise RuntimeError("dopri5: step size underflow / non-finite error estimate at t = {}".format(float(last[0])))
-    stats = {"n_accepted": int(last[8]), "n_rejected": int(last[9]), "launches": seq, "device_controlled": True}
+                if not math.isfinite(float(last[CTL_DT])) or float(last[CTL_DT]) == 0.0 or seq > 10_000_000:
+                    raise RuntimeError("dopri5: step size underflow / non-finite error estimate at t = {}".format(
+                        float(last[CTL_T])))
+    stats = {"n_accepted": int(last[CTL_NACC]), "n_rejected": int(last[CTL_NREJ]), "launches": seq, "device_controlled": True}
     return out.movedim(1, 0).reshape(len(times), *shape), stats
 
 

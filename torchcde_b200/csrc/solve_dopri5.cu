@@ -45,7 +45,7 @@ constexpr int kTiles = 2;
 constexpr int kThreads = kRows * kTiles;          // 256: thread = path
 constexpr int kCtl = 24;                          // doubles per control slot
 
-// control slot fields (doubles; the integer ones hold exact small integers)
+// control slot fields (doubles; the integer ones hold exact small integers); the host side names them adaptive.CTL_*
 enum { C_T = 0, C_DT, C_TEND, C_RTOL, C_ATOL, C_CUR, C_DONE, C_PENDING, C_NACC, C_NREJ, C_NEXT_OUT, C_NPART, C_NEED_MID, C_RATIO, C_LAUNCHES,
        C_OVERFLOW,     // paired mode: the trajectory slots are full -- the solve pauses (done = 1) until the caller has contracted them
        C_BASE };       // paired mode: accepted steps already contracted; slot of an attempt = accepted steps - base

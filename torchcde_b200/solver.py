@@ -616,11 +616,7 @@ def _kernel_vjp(X, weight, bias, z0, params):
             state[2].copy_(f0)
             grid = lib.tcde_dopri5_linear_grid(2 * n_paths)
             partials = torch.zeros(2, grid, dtype=torch.float64, device=dev)
-            ctl_host = torch.zeros(2, 24, dtype=torch.float64)
-            ctl_host[1, 0], ctl_host[1, 1], ctl_host[1, 2] = s0, dt, s1
-            ctl_host[1, 3], ctl_host[1, 4] = rtol, atol
-            ctl_host[1, 10] = 1
-            ctl = ctl_host.to(dev)
+            ctl = adaptive.initial_control(s0, dt, s1, rtol, atol).to(dev)
             out = torch.empty(2 * n_paths, 2, hidden, dtype=torch.float32, device=dev)
             out[:, 0].copy_(v0)
             out_times = torch.tensor([s0, s1], dtype=torch.float64, device=dev)
@@ -656,22 +652,24 @@ def _kernel_vjp(X, weight, bias, z0, params):
                           adaptive._DEVICE_CHUNK, _lib.F32, stream)
                 seq += adaptive._DEVICE_CHUNK
                 last = ctl[(seq - 1) & 1].cpu()
-                if last[6] != 0:
-                    contract(int(last[8]) - base)
-                    if last[15] == 0:
+                if last[adaptive.CTL_DONE] != 0:
+                    contract(int(last[adaptive.CTL_NACC]) - base)
+                    if last[adaptive.CTL_OVERFLOW] == 0:
                         break
                     # slots full: the filled ones are contracted; hand the slots back and resume where the device paused
-                    base = int(last[8])
+                    base = int(last[adaptive.CTL_NACC])
                     flushes += 1
                     resume = last.clone()
-                    resume[6], resume[15], resume[16] = 0.0, 0.0, float(base)
+                    resume[adaptive.CTL_DONE], resume[adaptive.CTL_OVERFLOW] = 0.0, 0.0
+                    resume[adaptive.CTL_BASE] = float(base)
                     ctl[(seq - 1) & 1].copy_(resume)
                     continue
-                if not math.isfinite(float(last[1])) or float(last[1]) == 0.0 or seq > 10_000_000:
-                    raise RuntimeError("dopri5 adjoint: step size underflow / non-finite error estimate at s = {}".format(float(last[0])))
-            n_acc = int(last[8])
-            stage.adaptive_stats = {"n_accepted": n_acc, "n_rejected": int(last[9]), "launches": seq, "slots": max_slots,
-                                    "flushes": flushes}
+                if not math.isfinite(float(last[adaptive.CTL_DT])) or float(last[adaptive.CTL_DT]) == 0.0 or seq > 10_000_000:
+                    raise RuntimeError("dopri5 adjoint: step size underflow / non-finite error estimate at s = {}".format(
+                        float(last[adaptive.CTL_T])))
+            n_acc = int(last[adaptive.CTL_NACC])
+            stage.adaptive_stats = {"n_accepted": n_acc, "n_rejected": int(last[adaptive.CTL_NREJ]), "launches": seq,
+                                    "slots": max_slots, "flushes": flushes}
             return out[n_paths:, 1].reshape(a_hi.shape).clone()
 
     fields = []
