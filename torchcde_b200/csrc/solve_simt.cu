@@ -502,7 +502,7 @@ static int launch_field(const void* control, int control_kind, int64_t n_rows, c
 
 // ---- tensor-core variant (solve_tc.cu) ---------------------------------------------------------
 #ifndef TCDE_DEFAULT_TC_MODE
-#define TCDE_DEFAULT_TC_MODE 1      // bit 0: 2xFP16 operand split (6 MMAs per 16 x 8 block) instead of 3xTF32 (12)
+#define TCDE_DEFAULT_TC_MODE 1      // bit 0: 2xFP16 operand split (warpgroup wgmma) instead of 3xTF32 (warp-level mma.sync)
 #endif
 static int g_solve_variant = 0;     // 0 auto, 1 CUDA-core kernel, 2 / 3 tensor cores 3xTF32, 4 tensor cores 2xFP16
 int current_solve_variant() { return g_solve_variant; }

@@ -1,12 +1,15 @@
-// Hot path (ii): the fused fixed-step CDE solve on the tensor cores (sm_90a, warp-level mma.sync).
+// Hot path (ii): the fused fixed-step CDE solve on the tensor cores (sm_90a).
 //
-// Thread = path, warp = 32 paths, and the warps of a CTA never wait for each other after the one-time setup of operand B.
-// Each Runge-Kutta stage of a warp is
-//   * dX/dt of the stage from the path's spline row (read straight from HBM: b | 2c | 3d of the interval, 96 bytes per path;
-//     the next stage's row is requested before the current stage's products so that its latency hides behind them);
-//   * the field W z + b of the warp's 32 paths as a [32 x 32] . [32 x 256] product on the tensor cores with a two-way
-//     operand split (tc_common.cuh: MODE 1 = 2xFP16 with per-path power-of-two scaling, 6 MMAs per 16 x 8 block; MODE 0 =
-//     3xTF32, 12 MMAs), contracted with dX/dt in registers; every lane ends with the 32 slopes of its own path;
+// Two kernels share the schedule, the controls, the Runge-Kutta combination and the outputs:
+//   * cdeint_wgmma_kernel (2xFP16 split, the default): one warpgroup per 64 paths, warpgroup-level wgmma.mma_async with the
+//     Runge-Kutta state kept in the MMA fragment layout (below);
+//   * cdeint_tc_kernel (3xTF32 split): thread = path, warp = 32 paths, warp-level mma.sync through tc_common.cuh's
+//     warp_field<0>.
+// Each Runge-Kutta stage is
+//   * dX/dt of the stage from the path's spline row (read straight from HBM: b | 2c | 3d of the interval; the next stage's
+//     row is requested before the current stage's products so that its latency hides behind them);
+//   * the field W z + b as a [paths x 32] . [32 x 256] product on the tensor cores with a two-way operand split
+//     (tc_common.cuh), contracted with dX/dt in registers;
 //   * the Runge-Kutta combination in registers, one rounding per operation in the order of oracle/odeint_port.py.
 // The Runge-Kutta state y, k1 and the running k2 + k3 stay in registers for the whole solve.  With a stage dump (the adjoint's
 // stage trajectory) every stage input is also written to HBM.
@@ -16,29 +19,109 @@ namespace tcde {
 
 namespace tc {
 
+// One Runge-Kutta combination on NV state values of the calling thread: kv = the stage's slopes, the next stage input ends
+// up in zin.  Returns true when the stage completed a step.
+template <int NV>
+__device__ __forceinline__ bool rk_combine(const UmmaArgs& a, int sub, float dt, const float* y, float* k1, float* s23,
+                                           const float* kv, float* zin) {
+    using E = exact<float>;
+    const f2 dt2 = pk(dt, dt);
+    if (a.method == TCDE_RK4_38) {
+        const float third = (float)(1.0 / 3.0);
+        const f2 th2 = pk(third, third);
+        if (sub == 0) {
+#pragma unroll
+            for (int h = 0; h < NV; h += 2) {
+                k1[h] = kv[h]; k1[h + 1] = kv[h + 1];
+                upk(add2(pk(y[h], y[h + 1]), mul2(mul2(dt2, pk(kv[h], kv[h + 1])), th2)), zin[h], zin[h + 1]);
+            }
+        } else if (sub == 1) {
+#pragma unroll
+            for (int h = 0; h < NV; h += 2) {
+                s23[h] = kv[h]; s23[h + 1] = kv[h + 1];
+                upk(add2(pk(y[h], y[h + 1]), mul2(dt2, sub2(pk(kv[h], kv[h + 1]), mul2(pk(k1[h], k1[h + 1]), th2)))),
+                    zin[h], zin[h + 1]);
+            }
+        } else if (sub == 2) {
+#pragma unroll
+            for (int h = 0; h < NV; h += 2) {
+                const f2 k2p = pk(s23[h], s23[h + 1]), k3p = pk(kv[h], kv[h + 1]);
+                upk(add2(pk(y[h], y[h + 1]), mul2(dt2, add2(sub2(pk(k1[h], k1[h + 1]), k2p), k3p))), zin[h], zin[h + 1]);
+                upk(add2(k2p, k3p), s23[h], s23[h + 1]);
+            }
+        } else {
+            const f2 three = pk(3.f, 3.f), eighth = pk(0.125f, 0.125f);
+#pragma unroll
+            for (int h = 0; h < NV; h += 2) {
+                const f2 sum = add2(add2(pk(k1[h], k1[h + 1]), mul2(three, pk(s23[h], s23[h + 1]))), pk(kv[h], kv[h + 1]));
+                upk(add2(pk(y[h], y[h + 1]), mul2(mul2(sum, dt2), eighth)), zin[h], zin[h + 1]);
+            }
+            return true;
+        }
+        return false;
+    }
+    if (a.method == TCDE_MIDPOINT) {
+        if (sub == 0) {
+            const float half = E::mul(0.5f, dt);
+#pragma unroll
+            for (int h = 0; h < NV; ++h) zin[h] = E::add(y[h], E::mul(kv[h], half));
+            return false;
+        }
+#pragma unroll
+        for (int h = 0; h < NV; ++h) zin[h] = E::add(y[h], E::mul(dt, kv[h]));
+        return true;
+    }
+#pragma unroll
+    for (int h = 0; h < NV; ++h) zin[h] = E::add(y[h], E::mul(dt, kv[h]));
+    return true;
+}
+
+// The outputs that fall on the step just completed (y = its start, zin = its end); write(j, v) stores output j.
+template <int NV, typename Write>
+__device__ __forceinline__ void step_outputs(const UmmaArgs& a, int step, int& jn, int& next_out, const float* y,
+                                             const float* zin, Write write) {
+    using E = exact<float>;
+    while (next_out == step) {
+        const int mode = a.out_mode[jn];
+        if (mode == 0) write(jn, y);
+        else if (mode == 1) write(jn, zin);
+        else {
+            const float slope_w = a.out_slope[jn];
+            float v[NV];
+#pragma unroll
+            for (int h = 0; h < NV; ++h) v[h] = E::add(y[h], E::mul(slope_w, E::sub(zin[h], y[h])));
+            write(jn, v);
+        }
+        ++jn;
+        next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
+    }
+}
+
+// ---- 3xTF32 split: thread = path, warp-level mma.sync ---------------------------------------------------------------
+
 constexpr int kWarps = 4;
 constexpr int kThreads = 32 * kWarps;            // 128 paths per CTA
 
-template <int MODE> struct Smem {
+struct Smem {
     static constexpr int b = 0;
-    static constexpr int warps = (BSmem<MODE>::bytes + 127) & ~127;
-    static constexpr int total = warps + kWarps * WarpSmem<MODE>::bytes;
+    static constexpr int warps = (BSmem<0>::bytes + 127) & ~127;
+    static constexpr int total = warps + kWarps * WarpSmem<0>::bytes;
 };
 
-template <int MODE, bool DUMP>
+template <bool DUMP>
 __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a) {
-    using S = Smem<MODE>;
+    using S = Smem;
     using E = exact<float>;
     extern __shared__ unsigned char smem_unaligned[];
     unsigned char* smem = smem_unaligned + ((128u - (smem_u32(smem_unaligned) & 127u)) & 127u);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     float inv_w_scale, beta;
-    prepare_b<MODE>(smem + S::b, a.weight, a.bias, tid, kThreads, inv_w_scale, beta);
+    prepare_b<0>(smem + S::b, a.weight, a.bias, tid, kThreads, inv_w_scale, beta);
     __syncthreads();
 
     const int64_t warp_path0 = (int64_t)blockIdx.x * kThreads + warp * 32;
     if (warp_path0 >= a.n_paths) return;                      // no CTA-wide barrier follows
-    unsigned char* ws = smem + S::warps + warp * WarpSmem<MODE>::bytes;
+    unsigned char* ws = smem + S::warps + warp * WarpSmem<0>::bytes;
     const int64_t path = warp_path0 + lane_row(lane);
     const bool live = path < a.n_paths;
     const int64_t lpath = live ? path : a.n_paths - 1;
@@ -87,7 +170,6 @@ __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a
     }
 
     const int n_st = a.n_steps * a.n_stages;
-    const float third = (float)(1.0 / 3.0);
     float4 raw[6], nxt[6];
     fetch(a.stage_index[0], raw);
     int step = 0, sub = 0;
@@ -111,72 +193,10 @@ __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a
         if (st + 1 < n_st) fetch(a.stage_index[st + 1], nxt);
 
         float kv[kHid];
-        warp_field<MODE>(zin, dx, kv, ws, smem + S::b, beta, inv_w_scale);
+        warp_field<0>(zin, dx, kv, ws, smem + S::b, beta, inv_w_scale);
 
-        // Runge-Kutta combination; the next stage input ends up in zin
-        bool step_done = false;
-        const f2 dt2 = pk(dt, dt);
-        if (a.method == TCDE_RK4_38) {
-            const f2 th2 = pk(third, third);
-            if (sub == 0) {
-#pragma unroll
-                for (int h = 0; h < kHid; h += 2) {
-                    k1[h] = kv[h]; k1[h + 1] = kv[h + 1];
-                    upk(add2(pk(y[h], y[h + 1]), mul2(mul2(dt2, pk(kv[h], kv[h + 1])), th2)), zin[h], zin[h + 1]);
-                }
-            } else if (sub == 1) {
-#pragma unroll
-                for (int h = 0; h < kHid; h += 2) {
-                    s23[h] = kv[h]; s23[h + 1] = kv[h + 1];
-                    upk(add2(pk(y[h], y[h + 1]), mul2(dt2, sub2(pk(kv[h], kv[h + 1]), mul2(pk(k1[h], k1[h + 1]), th2)))),
-                        zin[h], zin[h + 1]);
-                }
-            } else if (sub == 2) {
-#pragma unroll
-                for (int h = 0; h < kHid; h += 2) {
-                    const f2 k2p = pk(s23[h], s23[h + 1]), k3p = pk(kv[h], kv[h + 1]);
-                    upk(add2(pk(y[h], y[h + 1]), mul2(dt2, add2(sub2(pk(k1[h], k1[h + 1]), k2p), k3p))), zin[h], zin[h + 1]);
-                    upk(add2(k2p, k3p), s23[h], s23[h + 1]);
-                }
-            } else {
-                const f2 three = pk(3.f, 3.f), eighth = pk(0.125f, 0.125f);
-#pragma unroll
-                for (int h = 0; h < kHid; h += 2) {
-                    const f2 sum = add2(add2(pk(k1[h], k1[h + 1]), mul2(three, pk(s23[h], s23[h + 1]))), pk(kv[h], kv[h + 1]));
-                    upk(add2(pk(y[h], y[h + 1]), mul2(mul2(sum, dt2), eighth)), zin[h], zin[h + 1]);
-                }
-                step_done = true;
-            }
-        } else if (a.method == TCDE_MIDPOINT) {
-            if (sub == 0) {
-                const float half = E::mul(0.5f, dt);
-#pragma unroll
-                for (int h = 0; h < kHid; ++h) zin[h] = E::add(y[h], E::mul(kv[h], half));
-            } else {
-#pragma unroll
-                for (int h = 0; h < kHid; ++h) zin[h] = E::add(y[h], E::mul(dt, kv[h]));
-                step_done = true;
-            }
-        } else {
-#pragma unroll
-            for (int h = 0; h < kHid; ++h) zin[h] = E::add(y[h], E::mul(dt, kv[h]));
-            step_done = true;
-        }
-        if (step_done) {
-            while (next_out == step) {
-                const int mode = a.out_mode[jn];
-                if (mode == 0) write_out(jn, y);
-                else if (mode == 1) write_out(jn, zin);
-                else {
-                    const float slope_w = a.out_slope[jn];
-                    float v[kHid];
-#pragma unroll
-                    for (int h = 0; h < kHid; ++h) v[h] = E::add(y[h], E::mul(slope_w, E::sub(zin[h], y[h])));
-                    write_out(jn, v);
-                }
-                ++jn;
-                next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
-            }
+        if (rk_combine<kHid>(a, sub, dt, y, k1, s23, kv, zin)) {
+            step_outputs<kHid>(a, step, jn, next_out, y, zin, write_out);
 #pragma unroll
             for (int h = 0; h < kHid; ++h) y[h] = zin[h];
             ++step;
@@ -190,17 +210,276 @@ __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a
     }
 }
 
+// ---- 2xFP16 split: one warpgroup per 64 paths, wgmma.mma_async ------------------------------------------------------
+//
+// The CTA is one warpgroup and its 64 paths are the M = 64 rows of every wgmma.  Lane (g, q) = (lane >> 2, lane & 3) of
+// warp w owns rows 16 w + g and 16 w + g + 8 (the rows of its A and accumulator fragments) and, of each of these rows, the
+// hidden units 8 i + 2 q + e (i < 4, e < 2): exactly the columns of the A fragment of the next stage, so the operand is
+// built in registers from the Runge-Kutta state.  Its 16 values of a state vector sit at index 8 r + 2 i + e (r = row).
+// The product runs in chunks of kN = 32 output columns (four hidden units x eight channels): z_lo.W_hi, z_hi.W_lo and
+// z_hi.W_hi (small terms first) are six m64n32k16 wgmmas onto an accumulator that starts at the scaled bias, with A from
+// registers and B (prepare_b<1>'s [256 rows][hi 32 | lo 32] halves, 128-byte swizzled) through one shared-memory
+// descriptor per product and k step.  Two accumulators alternate: the chunk after the current one is in flight on the
+// tensor core while the current one is contracted with dX/dt.  A contraction leaves each lane with the partial sums of its
+// two channels; a reduce-scatter over the quad (xor 1 after every chunk, xor 2 after every pair of chunks) hands each lane
+// the sums of the hidden units it owns, added in the order (q, q ^ 1) + (q ^ 2, q ^ 3).
+
+namespace wg {
+
+constexpr int kThreads = 128;                    // one warpgroup
+constexpr int kPaths = 64;                       // the M of the wgmma tile
+constexpr int kNV = 16;                          // state values per lane: 2 rows x 8 hidden units
+constexpr int kN = 32;                           // output columns per chunk
+constexpr int kChunks = kCols / kN;
+constexpr int kAcc = kN / 2;                     // accumulator registers per chunk
+constexpr int kSmem = BSmem<1>::bytes + 1024;    // slack for the 1024-byte alignment of the swizzled B tile
+
+// shared-memory matrix descriptor of a K-major, 128-byte-swizzled operand whose 8-row swizzle atoms are 1024 bytes apart
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t addr) {
+    return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+}
+
+__device__ __forceinline__ void mma_m64n32k16(float* d, const uint32_t* a, uint64_t b) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+}
+__device__ __forceinline__ void mma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void mma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void mma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving reads or writes of an accumulator across the asynchronous MMAs that own it
+__device__ __forceinline__ void pin(float* d) {
+#pragma unroll
+    for (int i = 0; i < kAcc; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+}  // namespace wg
+
+template <bool DUMP>
+__global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const UmmaArgs a) {
+    using S = BSmem<1>;
+    using E = exact<float>;
+    extern __shared__ unsigned char smem_unaligned[];
+    unsigned char* smem = smem_unaligned + ((1024u - (smem_u32(smem_unaligned) & 1023u)) & 1023u);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
+    float inv_w_scale, beta;
+    prepare_b<1>(smem, a.weight, a.bias, tid, wg::kThreads, inv_w_scale, beta);
+    if (a.sign < 0.f) inv_w_scale = -inv_w_scale;       // the sign of the time direction: dX/dt is negated exactly either way
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // the tile is read by wgmma (the async proxy)
+    __syncthreads();
+
+    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
+    const int row_f2 = (cubic ? 4 * kCh : kCh) / 2;
+    int64_t path[2];
+    bool live[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        path[r] = (int64_t)blockIdx.x * wg::kPaths + 16 * warp + g + 8 * r;
+        live[r] = path[r] < a.n_paths;
+    }
+    // channels 2q, 2q + 1 of b (cubic; +4, +8: 2c, 3d) or of the slope (linear) in the spline rows of row 0; row 1's are
+    // row1 paths further (8, or fewer where the batch ends and the reads are clamped)
+    const int64_t lpath0 = live[0] ? path[0] : a.n_paths - 1;
+    const int row1 = (int)((live[1] ? path[1] : a.n_paths - 1) - lpath0);
+    const float2* crow = reinterpret_cast<const float2*>(a.control + lpath0 * a.n_rows * (2 * row_f2) + (cubic ? kCh : 0)) + q;
+
+    auto fetch = [&](int interval, float2 (*raw)[3]) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const float2* src = crow + (r * row1 * a.n_rows + interval) * row_f2;
+            raw[r][0] = __ldg(src);
+            if (cubic) { raw[r][1] = __ldg(src + 4); raw[r][2] = __ldg(src + 8); }
+        }
+    };
+    // the lane's 16 values of a [path][32] row pair: float2 at column 8 i + 2 q of row r
+    auto store_rows = [&](float* base, int64_t stride_rows, int64_t row_off, const float* v) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            if (!live[r]) continue;
+            float2* dst = reinterpret_cast<float2*>(base + (path[r] * stride_rows + row_off) * kHid) + q;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) dst[4 * i] = make_float2(v[8 * r + 2 * i], v[8 * r + 2 * i + 1]);
+        }
+    };
+    auto write_out = [&](int j, const float* v) { store_rows(a.out, a.n_out, j, v); };
+
+    float y[wg::kNV], k1[wg::kNV], s23[wg::kNV], zin[wg::kNV];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        const int64_t lpath = live[r] ? path[r] : a.n_paths - 1;
+        const float2* zp = reinterpret_cast<const float2*>(a.z0 + lpath * kHid) + q;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float2 v = zp[4 * i];
+            y[8 * r + 2 * i] = v.x; y[8 * r + 2 * i + 1] = v.y;
+        }
+    }
+#pragma unroll
+    for (int h = 0; h < wg::kNV; ++h) { k1[h] = 0.f; s23[h] = 0.f; zin[h] = y[h]; }
+    int jn = 0;
+    int next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
+    while (jn < a.n_out && next_out < 0) {                    // outputs at the initial time
+        write_out(jn, y);
+        ++jn;
+        next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
+    }
+
+    const float* b_bias = reinterpret_cast<const float*>(smem + S::bias);
+    const uint32_t b_tile = smem_u32(smem + S::tile);
+    const bool odd = q & 1, upper = q >> 1;
+    const int n_st = a.n_steps * a.n_stages;
+    // dX/dt (interpolation_cubic.py:331-336) of a stage at fraction fr of its interval, channels 2q, 2q + 1 of both rows
+    auto slope = [&](const float2 (*raw)[3], float fr, float (*dx)[2]) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            if (cubic) {
+                dx[r][0] = E::add(raw[r][0].x, E::mul(E::add(raw[r][1].x, E::mul(raw[r][2].x, fr)), fr));
+                dx[r][1] = E::add(raw[r][0].y, E::mul(E::add(raw[r][1].y, E::mul(raw[r][2].y, fr)), fr));
+            } else {
+                dx[r][0] = raw[r][0].x;
+                dx[r][1] = raw[r][0].y;
+            }
+        }
+    };
+    float* dump_at = a.stage_dump;                 // stage st's [path][32] block
+    float dx[2][2];
+    {
+        float2 raw[2][3];
+        fetch(a.stage_index[0], raw);
+        slope(raw, a.stage_frac[0], dx);
+    }
+    int step = 0, sub = 0;
+    float dt = a.step_dt[0];
+    for (int st = 0; st < n_st; ++st) {
+        if (DUMP) {
+            store_rows(dump_at, 1, 0, zin);
+            dump_at += a.n_paths * kHid;
+        }
+        // the next stage's spline rows; their latency hides behind the first half of this stage's products
+        float2 nxt[2][3];
+        float dx_next[2][2];
+        if (st + 1 < n_st) fetch(a.stage_index[st + 1], nxt);
+
+        // Each row scaled by its own power of two so that max(|z|, bias floor) lands in [2^13, 2^14), split into FP16
+        // hi + lo A fragments [k step][4]; the inverse scales are folded into dX/dt.
+        float rs[2];
+        uint32_t ahi[2][4], alo[2][4];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            float m = beta;
+#pragma unroll
+            for (int h = 0; h < 8; ++h) m = fmaxf(m, fabsf(zin[8 * r + h]));
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+            const int e = min(max(exponent_of(m), 30), 224);
+            rs[r] = pow2_biased(127 + 13 - (e - 127));
+            const float inv = pow2_biased(127 - 13 + (e - 127)) * inv_w_scale;
+            dx[r][0] = __fmul_rn(dx[r][0], inv);
+            dx[r][1] = __fmul_rn(dx[r][1], inv);
+        }
+#pragma unroll
+        for (int k = 0; k < 2; ++k)
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {                     // register t: row t & 1, columns 16 k + 8 (t >> 1) + 2q, +1
+                const int r = t & 1, v = 8 * r + 4 * k + 2 * (t >> 1);
+                const float s0 = __fmul_rn(zin[v], rs[r]), s1 = __fmul_rn(zin[v + 1], rs[r]);
+                float h0, h1;
+                ahi[k][t] = pack_h2(s0, s1);
+                unpack_h2(ahi[k][t], h0, h1);
+                alo[k][t] = pack_h2(__fsub_rn(s0, h0), __fsub_rn(s1, h1));
+            }
+
+        float acc[2][wg::kAcc];
+        auto issue = [&](int chunk, float* d) {
+#pragma unroll
+            for (int j = 0; j < wg::kN / 8; ++j) {                // bias of columns 8 (4 chunk + j) + 2q, +1 times the row scales
+                const float2 bb = *reinterpret_cast<const float2*>(b_bias + chunk * wg::kN + 8 * j + 2 * q);
+                d[4 * j + 0] = bb.x * rs[0]; d[4 * j + 1] = bb.y * rs[0];
+                d[4 * j + 2] = bb.x * rs[1]; d[4 * j + 3] = bb.y * rs[1];
+            }
+            wg::mma_fence();
+            const uint32_t rows = b_tile + chunk * wg::kN * 128;
+            wg::mma_m64n32k16(d, alo[0], wg::desc_sw128(rows + 0));    // z_lo . W_hi
+            wg::mma_m64n32k16(d, alo[1], wg::desc_sw128(rows + 32));
+            wg::mma_m64n32k16(d, ahi[0], wg::desc_sw128(rows + 64));   // z_hi . W_lo
+            wg::mma_m64n32k16(d, ahi[1], wg::desc_sw128(rows + 96));
+            wg::mma_m64n32k16(d, ahi[0], wg::desc_sw128(rows + 0));    // z_hi . W_hi
+            wg::mma_m64n32k16(d, ahi[1], wg::desc_sw128(rows + 32));
+            wg::mma_commit();
+        };
+        float kv[wg::kNV], u_even[2][2];
+        issue(0, acc[0]);
+#pragma unroll
+        for (int c = 0; c < wg::kChunks; ++c) {
+            float* d = acc[c & 1];
+            if (c + 1 < wg::kChunks) {
+                issue(c + 1, acc[(c + 1) & 1]);
+                wg::mma_wait<1>();
+            } else {
+                wg::mma_wait<0>();
+            }
+            wg::pin(d);
+            if (c == wg::kChunks / 2 && st + 1 < n_st) slope(nxt, a.stage_frac[st + 1], dx_next);
+            // partial contraction of the lane's two channels for hidden units 4c + j, rows g and g + 8
+            float p[4][2];
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) p[j][r] = fmaf(d[4 * j + 2 * r + 1], dx[r][1], __fmul_rn(d[4 * j + 2 * r], dx[r][0]));
+            // xor 1: keep the hidden units whose owner has the parity of q (4c + 2 (q & 1) + e)
+            float u[2][2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const float got = __shfl_xor_sync(0xffffffffu, odd ? p[e][r] : p[2 + e][r], 1);
+                    u[e][r] = (odd ? p[2 + e][r] : p[e][r]) + got;
+                }
+            if ((c & 1) == 0) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) u_even[e][r] = u[e][r];
+            } else {
+                // xor 2: lanes 0, 1 keep the even chunk's units, lanes 2, 3 the odd chunk's: 8 (c >> 1) + 2q + e
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {
+                        const float got = __shfl_xor_sync(0xffffffffu, upper ? u_even[e][r] : u[e][r], 2);
+                        kv[8 * r + 2 * (c >> 1) + e] = (upper ? u[e][r] : u_even[e][r]) + got;
+                    }
+            }
+        }
+
+        if (rk_combine<wg::kNV>(a, sub, dt, y, k1, s23, kv, zin)) {
+            step_outputs<wg::kNV>(a, step, jn, next_out, y, zin, write_out);
+#pragma unroll
+            for (int h = 0; h < wg::kNV; ++h) y[h] = zin[h];
+            ++step;
+            sub = 0;
+            if (step < a.n_steps) dt = a.step_dt[step];
+        } else {
+            ++sub;
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r) { dx[r][0] = dx_next[r][0]; dx[r][1] = dx_next[r][1]; }
+    }
+}
+
 }  // namespace tc
 
 bool solve_tc_supported(int H, int C) { return H == tc::kHid && C == tc::kCh; }
 
-template <int MODE> static int launch_tc(const UmmaArgs& a, cudaStream_t stream) {
-    const int64_t grid = (a.n_paths + tc::kThreads - 1) / tc::kThreads;
+template <typename Kernel>
+static int launch(Kernel kern, int64_t grid, int threads, int smem, const UmmaArgs& a, cudaStream_t stream) {
     TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
-    auto kern = a.stage_dump ? tc::cdeint_tc_kernel<MODE, true> : tc::cdeint_tc_kernel<MODE, false>;
-    const int smem = tc::Smem<MODE>::total + 128;             // slack for the 128-byte alignment of the tiles
     TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    kern<<<(unsigned)grid, tc::kThreads, smem, stream>>>(a);
+    kern<<<(unsigned)grid, threads, smem, stream>>>(a);
     TCDE_CHECK_CUDA(cudaGetLastError());
     return TCDE_OK;
 }
@@ -213,7 +492,12 @@ int solve_tc_f32(const UmmaArgs& a, int H, int C, int mode, cudaStream_t stream)
     TCDE_CHECK_SUPPORTED(a.stage_dump == nullptr || (reinterpret_cast<uintptr_t>(a.stage_dump) & 15) == 0,
                          "tensor-core solve: the stage dump must be 16-byte aligned");
     // mode: bit 0 = operand split (0 = 3xTF32, 1 = 2xFP16)
-    return (mode & 1) ? launch_tc<1>(a, stream) : launch_tc<0>(a, stream);
+    if (mode & 1)
+        return launch(a.stage_dump ? tc::cdeint_wgmma_kernel<true> : tc::cdeint_wgmma_kernel<false>,
+                      (a.n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths, tc::wg::kThreads, tc::wg::kSmem, a, stream);
+    return launch(a.stage_dump ? tc::cdeint_tc_kernel<true> : tc::cdeint_tc_kernel<false>,
+                  (a.n_paths + tc::kThreads - 1) / tc::kThreads, tc::kThreads,
+                  tc::Smem::total + 128, a, stream);               // slack for the 128-byte alignment of the tiles
 }
 
 }  // namespace tcde

@@ -1,5 +1,6 @@
-// The linear vector field of one warp's 32 paths on the tensor cores (warp-level mma.sync, sm_90a), shared by the fixed-step
-// solve (solve_tc.cu) and the device-controlled dopri5 attempts (solve_dopri5.cu).
+// The linear vector field of one warp's 32 paths on the tensor cores (warp-level mma.sync, sm_90a), used by the 3xTF32
+// fixed-step solve (solve_tc.cu) and the device-controlled dopri5 attempts (solve_dopri5.cu).  prepare_b<1>'s operand B is
+// also the B of the 2xFP16 fixed-step solve's wgmma (a K-major 128-byte-swizzled tile).
 //
 // One evaluation is the product D[32 paths x 256] = z[32 x 32] . W^T[32 x 256] + bias followed by the contraction
 // kv[h] = sum_c D[h * 8 + c] dX/dt[c].  fp32 accuracy on the tensor pipe comes from a two-way operand split:
