@@ -19,7 +19,7 @@ linear vector field it is one fused kernel launch (``tcde_vector_field_linear``)
 
 The backward pass of ``adjoint=True`` for the flagship linear field (fp32, hidden 32, channels 8) does not go
 through autograd: a fixed-step backward solve is three launches per segment (``_fused_fixed_backward`` ->
-``solver._kernel_vjp.segment``), an adaptive one gets the field and its vector-Jacobian products from one launch
+``linear_field.AdjointStage.segment``), an adaptive one gets the field and its vector-Jacobian products from one launch
 per evaluation (``tcde_vector_field_linear_vjp``); the stage combinations and the error ratio of a dopri5
 attempt are single launches too (``tcde_linear_combination`` / ``tcde_error_ratio_sumsq``).
 """
@@ -257,47 +257,41 @@ def device_dopri5_available(z0, channels):
     return (z0.is_cuda and z0.dtype == torch.float32 and z0.size(-1) == 32 and channels == 8 and z0.numel() > 0)
 
 
-def odeint_dopri5_device(control, kind, n_rows, knots, weight, bias, field, y0, times, rtol, atol, sign, first_step=None):
-    """The same algorithm as ``Dopri5.integrate`` with accept / reject, the step-size rule and the dense output on the
-    device (``tcde_dopri5_linear_attempts``: one launch per attempted step, no host read per attempt).  ``field`` is only
-    used for the slope at the start and Hairer's initial step.  ``times``: increasing floats (already negated when
-    ``sign`` < 0).  Returns ``(out (len(times), *y0.shape), stats)``."""
-    lib = _lib.load()
-    shape = y0.shape
-    hidden = shape[-1]
-    yf = y0.detach().reshape(-1, hidden).contiguous()
-    n_paths = yf.size(0)
-    dev = yf.device
-    t0 = times[0]
-    with torch.no_grad():
-        f0 = field(t0, yf)
-        dt = first_step if first_step is not None else _initial_step(field, t0, yf, f0, rtol, atol)
+def device_controller(launch, field, v0, times, rtol, atol, first_step, underflow, on_overflow=None):
+    """The host loop of the device-controlled dopri5 kernels: ``launch(state, partials, ctl, out, out_times, first_seq)``
+    enqueues ``_DEVICE_CHUNK`` attempts from ``v0``, one control slot is read per chunk; ``field`` only gives the start
+    slope and Hairer's first step.  ``on_overflow(last)`` empties full trajectory slots before the solve resumes;
+    ``underflow`` is the error message.  Returns ``(out (paths, len(times), H), the last control slot, stats)``."""
+    dev = v0.device
+    n_paths, hidden = v0.shape
+    with torch.cuda.device(dev), torch.no_grad():
+        f0 = field(times[0], v0)
+        dt = first_step if first_step is not None else _initial_step(field, times[0], v0, f0, rtol, atol)
         state = torch.empty(5, n_paths, hidden, dtype=torch.float32, device=dev)
-        state[0].copy_(yf)
+        state[0].copy_(v0)
         state[2].copy_(f0)
-        grid = lib.tcde_dopri5_linear_grid(n_paths)
-        partials = torch.zeros(2, grid, dtype=torch.float64, device=dev)
-        ctl = initial_control(t0, dt, times[-1], rtol, atol).to(dev)
+        partials = torch.zeros(2, _lib.load().tcde_dopri5_linear_grid(n_paths), dtype=torch.float64, device=dev)
+        ctl = initial_control(times[0], dt, times[-1], rtol, atol).to(dev)
         out = torch.empty(n_paths, len(times), hidden, dtype=torch.float32, device=dev)
-        out[:, 0].copy_(yf)
+        out[:, 0].copy_(v0)
         out_times = torch.tensor(times, dtype=torch.float64, device=dev)
         seq = 0
-        with torch.cuda.device(dev):
-            stream = _lib.stream_of(yf)
-            while True:
-                _lib.call("tcde_dopri5_linear_attempts", _lib.ptr(control), kind, n_rows, _lib.ptr(knots), _lib.ptr(weight),
-                          _lib.ptr(bias), _lib.ptr(state), _lib.ptr(partials), _lib.ptr(ctl), _lib.ptr(out),
-                          _lib.ptr(out_times), len(times), n_paths, 8, hidden, float(sign), seq, _DEVICE_CHUNK,
-                          _lib.F32, stream)
-                seq += _DEVICE_CHUNK
-                last = ctl[(seq - 1) & 1].cpu()              # the one host read per chunk
-                if last[CTL_DONE] != 0:
+        while True:
+            launch(state, partials, ctl, out, out_times, seq)
+            seq += _DEVICE_CHUNK
+            last = ctl[(seq - 1) & 1].cpu()              # the one host read per chunk
+            if last[CTL_DONE] != 0:
+                if last[CTL_OVERFLOW] == 0:
                     break
-                if not math.isfinite(float(last[CTL_DT])) or float(last[CTL_DT]) == 0.0 or seq > 10_000_000:
-                    raise RuntimeError("dopri5: step size underflow / non-finite error estimate at t = {}".format(
-                        float(last[CTL_T])))
-    stats = {"n_accepted": int(last[CTL_NACC]), "n_rejected": int(last[CTL_NREJ]), "launches": seq, "device_controlled": True}
-    return out.movedim(1, 0).reshape(len(times), *shape), stats
+                on_overflow(last)
+                # hand the slots back and resume where the device paused
+                resume = last.clone()
+                resume[CTL_DONE], resume[CTL_OVERFLOW], resume[CTL_BASE] = 0.0, 0.0, last[CTL_NACC]
+                ctl[(seq - 1) & 1].copy_(resume)
+                continue
+            if not math.isfinite(float(last[CTL_DT])) or float(last[CTL_DT]) == 0.0 or seq > 10_000_000:
+                raise RuntimeError(underflow.format(float(last[CTL_T])))
+    return out, last, {"n_accepted": int(last[CTL_NACC]), "n_rejected": int(last[CTL_NREJ]), "launches": seq}
 
 
 # ------------------------------------------------------------------------- fixed grids (generic)
@@ -307,7 +301,6 @@ def odeint_fixed(field, y0, times, method, step_size):
     if step_size is None:
         grid = list(times)
     else:
-        import math
         n = int(math.ceil((t_end - t0) / step_size + 1))
         grid = [t0 + i * step_size for i in range(n)]
         grid[-1] = t_end
@@ -337,6 +330,23 @@ def odeint_fixed(field, y0, times, method, step_size):
 
 
 # ------------------------------------------------------------------------------------- adjoint
+def _packing(shapes):
+    """``pack(parts)`` / ``unpack(flat)`` of the adjoint's augmented state: tensors of ``shapes`` end to end."""
+    sizes = [s.numel() for s in shapes]
+
+    def pack(parts):
+        return torch.cat([p.reshape(-1) for p in parts])
+
+    def unpack(flat):
+        outs, off = [], 0
+        for shape, n in zip(shapes, sizes):
+            outs.append(flat[off:off + n].view(shape))
+            off += n
+        return outs
+
+    return pack, unpack
+
+
 class _Adjoint(torch.autograd.Function):
     """Continuous adjoint (torchdiffeq ``odeint_adjoint``): the forward pass keeps only the outputs;
     the backward pass integrates ``(y, a_y, a_params)`` backwards between consecutive output times
@@ -364,23 +374,12 @@ class _Adjoint(torch.autograd.Function):
             return (None, None, None, None, None, None, None, None, a_y, *a_p)
         if ctx.t_needs_grad:
             return _Adjoint._backward_with_times(ctx, ys, params, grad_ys)
-        if ctx.fused_vjp is not None and getattr(ctx.fused_vjp, "adaptive_spec", None) is not None:
+        if ctx.fused_vjp is not None and ctx.fused_vjp.adaptive_spec is not None:
             with torch.no_grad():
                 done = _device_adaptive_backward(ctx.fused_vjp, times, ys, grad_ys)
             if done is not None:
                 return (None, None, None, None, None, None, None, None, done[0], *done[1])
-        shapes = [ys[0].shape, ys[0].shape] + [p.shape for p in params]
-        sizes = [s.numel() for s in shapes]
-
-        def pack(parts):
-            return torch.cat([p.reshape(-1) for p in parts])
-
-        def unpack(flat):
-            outs, off = [], 0
-            for shape, n in zip(shapes, sizes):
-                outs.append(flat[off:off + n].view(shape))
-                off += n
-            return outs
+        pack, unpack = _packing([ys[0].shape, ys[0].shape] + [p.shape for p in params])
 
         def aug_field(t, flat):
             y, a_y, *_ = unpack(flat)
@@ -415,18 +414,7 @@ class _Adjoint(torch.autograd.Function):
         the integral of -a^T df/dt, and every output time t_i gets dL/dt_i = <f(t_i, y_i), dL/dy_i> (``odeint_adjoint``
         with ``t.requires_grad``).  Autograd serves the field (its time dependence is the control's dX/dt)."""
         vf, times = ctx.vf, ctx.times
-        shapes = [torch.Size([]), ys[0].shape, ys[0].shape] + [p.shape for p in params]
-        sizes = [max(1, s.numel()) for s in shapes]
-
-        def pack(parts):
-            return torch.cat([p.reshape(-1) for p in parts])
-
-        def unpack(flat):
-            outs, off = [], 0
-            for shape, n in zip(shapes, sizes):
-                outs.append(flat[off:off + n].view(shape))
-                off += n
-            return outs
+        pack, unpack = _packing([torch.Size([]), ys[0].shape, ys[0].shape] + [p.shape for p in params])
 
         def aug_field(t, flat):
             _, y, a_y, *_ = unpack(flat)
@@ -471,12 +459,11 @@ def _device_adaptive_backward(stage, times, ys, grad_ys):
     gw = next((g for g, r in zip(grads, stage.roles) if r == "w"), None)
     gb = next((g for g, r in zip(grads, stage.roles) if r == "b"), None)
     from .solver import cdeint
-    hint = getattr(stage, "slots_hint", None) or 256
     totals = {}
     a_y = grad_ys[-1].clone()
     for i in range(len(times) - 1, 0, -1):
         try:
-            a_lo = stage.adaptive_segment(times[i], times[i - 1], ys[i], a_y, rtol, atol, gw, gb, hint)
+            a_lo = stage.adaptive_segment(times[i], times[i - 1], ys[i], a_y, rtol, atol, gw, gb, stage.slots_hint)
         except NotImplementedError:           # TCDE_ERR_UNSUPPORTED from a kernel: the host-driven backward takes any problem
             a_lo = None
         if a_lo is None:
@@ -497,7 +484,6 @@ def _fused_fixed_backward(stage, times, ys, grad_ys, method, step_size):
     state, but (z, a) stay one (2, ..., H) tensor that the kernel reads and writes directly, and the parameter
     gradients -- whose slopes do not depend on themselves -- are accumulated in place by the kernel with the
     stage's weight, instead of being carried through ``torch.cat`` as 8,448 extra state components."""
-    import math
     grads = stage.new_grads()
     gw = next((g for g, r in zip(grads, stage.roles) if r == "w"), None)
     gb = next((g for g, r in zip(grads, stage.roles) if r == "b"), None)

@@ -48,6 +48,15 @@ def _schedule_knots(X):
     return knots.detach().cpu()
 
 
+def _control_signature(X):
+    """(kind, batch shape, channels, n_intervals) of a built-in control without evaluating it."""
+    if isinstance(X, CubicSpline):
+        return _lib.CONTROL_CUBIC, tuple(X._b.shape[:-2]), X._b.size(-1), X._b.size(-2)
+    if isinstance(X, LinearInterpolation):
+        return _lib.CONTROL_LINEAR, tuple(X._coeffs.shape[:-2]), X._coeffs.size(-1), X._coeffs.size(-2) - 1
+    return None
+
+
 def _eval_kernel(control, knots, n_rows, channels, index, frac, kind, derivative):
     """control: (..., n_rows, width) -> (..., *t.shape, channels) through the C ABI."""
     _lib.require_cuda(control)

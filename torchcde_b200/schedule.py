@@ -16,8 +16,10 @@ Because it is literally ``torch.bucketize`` on the same numbers, the interval in
 bit-exact with the reference by construction (a knot t_n, n > 0, belongs to interval n-1).
 Everything here is O(number of steps) scalar work on the CPU.
 """
+import bisect
 import collections
 
+import numpy as np
 import torch
 
 _ONE_THIRD = 1 / 3
@@ -60,6 +62,29 @@ def locate(knots, times, n_intervals):
     times = torch.as_tensor(times, dtype=knots.dtype, device=knots.device)
     index = torch.bucketize(times.detach(), knots.detach()).sub(1).clamp(0, n_intervals - 1)
     return times - knots[index], index
+
+
+def host_locator(knots, n_rows, state_dtype):
+    """``(t_float, nudge) -> (interval index, fraction)``: the scalar version of ``locate`` with exactly the casts the
+    reference stack applies to a stage time (to the state dtype by the solver, to the coefficient dtype by
+    ``_interpret_t``), evaluated on the CPU so that no device sync is needed per stage.  ``knots``: CPU tensor."""
+    # numpy scalars round exactly like the tensor casts, ``bisect_left`` is ``torch.bucketize`` (right=False), and none
+    # of it goes through the torch dispatcher (this runs once per vector-field evaluation of the adaptive and adjoint
+    # drivers)
+    state_t = np.dtype(str(state_dtype).replace("torch.", "")).type
+    knot_t = np.dtype(str(knots.dtype).replace("torch.", "")).type
+    knot_list = knots.tolist()
+    knot_vals = [knot_t(v) for v in knot_list]
+
+    def where(t, nudge=0):
+        tt = state_t(t)
+        if nudge:
+            tt = np.nextafter(tt, tt + state_t(1))
+        tk = knot_t(tt)
+        index = min(max(bisect.bisect_left(knot_list, float(tk)) - 1, 0), n_rows - 1)
+        return index, float(tk - knot_vals[index])
+
+    return where
 
 
 def build_schedule(t, knots, n_intervals, method, step_size, state_dtype):

@@ -9,129 +9,14 @@ kernel (``tcde_cdeint_fixed_linear``) when the vector field is the README-form l
 any other ``func`` runs through this package's own on-GPU stage loop, which keeps the
 reference's arithmetic but issues no per-stage host syncs.
 """
-import bisect
-import math
 import warnings
-import weakref
-
-import numpy as np
 
 import torch
 
 from . import _lib, adaptive
-from .controls import CubicSpline, LinearInterpolation, _schedule_knots
-from .schedule import FIXED_METHODS, ScheduleCache, build_schedule, locate
-
-_schedules = ScheduleCache()
-
-
-# ------------------------------------------------------------------------------ vector fields
-class LinearVectorField(torch.nn.Module):
-    """The README's vector field (README.md:42-49): ``Linear(H, H*C)(z).view(..., H, C)``.
-
-    ``cdeint`` recognises this class (and structurally identical user modules) and fuses it.
-    """
-
-    def __init__(self, hidden_channels, input_channels, bias=True, device=None, dtype=None):
-        super().__init__()
-        self.hidden_channels = hidden_channels
-        self.input_channels = input_channels
-        self.linear = torch.nn.Linear(hidden_channels, hidden_channels * input_channels, bias=bias, device=device,
-                                      dtype=dtype)
-
-    def forward(self, t, z):
-        return self.linear(z).view(*z.shape[:-1], self.hidden_channels, self.input_channels)
-
-
-_recognised = weakref.WeakKeyDictionary()
-
-
-def _single_linear(func):
-    """The one ``nn.Linear`` of ``func`` if ``func`` consists of nothing else, otherwise None."""
-    if not isinstance(func, torch.nn.Module) or hasattr(func, "prod"):
-        return None
-    mods = [m for m in func.modules() if m is not func]
-    if len(mods) != 1 or not isinstance(mods[0], torch.nn.Linear):
-        return None
-    if len(list(func.parameters())) != len(list(mods[0].parameters())) or len(list(func.buffers())) != 0:
-        return None
-    return mods[0]
-
-
-def linear_field_of(func, z0, channels, times):
-    """Return ``(weight, bias)`` if ``func(t, z)`` is exactly ``Linear(H, H*C)(z).view(..., H, C)``.
-
-    ``LinearVectorField`` is trusted; any other module made of a single ``nn.Linear`` of the
-    right shape is *probed*: it must reproduce the linear map bit for bit on random states at
-    several distinct times of the integration interval (so a module that adds an activation, or
-    scales by a function of ``t``, is never mistaken for a linear field -- probing at ``(t[0], z0)``
-    alone is degenerate for ``z0 == 0`` or ``t[0] in {0, 1}``)."""
-    hidden = z0.size(-1)
-    if isinstance(func, LinearVectorField):
-        lin = func.linear
-        if lin.in_features == hidden and lin.out_features == hidden * channels:
-            return lin.weight, lin.bias
-        return None
-    lin = _single_linear(func)
-    if lin is None or lin.in_features != hidden or lin.out_features != hidden * channels:
-        return None
-    try:
-        known = _recognised.get(func)
-    except TypeError:
-        known = None
-    if known is None:
-        known = _probe(func, lin, z0, channels, times)
-        try:
-            _recognised[func] = known
-        except TypeError:
-            pass
-    return (lin.weight, lin.bias) if known else None
-
-
-def _probe(func, lin, z0, channels, times):
-    """Bit-exact comparison of ``func`` with its ``nn.Linear`` on random (non-degenerate) states of z0's own
-    shape (user modules may hard-code the batch size) at four distinct times, none of them 0 or 1."""
-    hidden = z0.size(-1)
-    if z0.numel() * channels > (1 << 27):
-        # too large to probe at full shape: only the explicit LinearVectorField gets the fused kernel
-        return False
-    lo, hi = float(times[0]), float(times[-1])
-    span = hi - lo if hi != lo else 1.0
-    probe_times = [lo + 0.6180339887 * span, lo + 0.2718281828 * span + 0.0137, hi + 0.5772156649, lo - 0.4142135624]
-    gen = torch.Generator(device=z0.device).manual_seed(0x5eed)
-    with torch.no_grad():
-        for i, tv in enumerate(probe_times):
-            zp = torch.randn(z0.shape, generator=gen, device=z0.device, dtype=z0.dtype) * (0.5 + 1.3 * i) + 0.21 * i
-            tp = torch.tensor(tv, dtype=z0.dtype, device=z0.device)
-            try:
-                got = func(tp, zp)
-            except Exception:
-                warnings.warn("torchcde_b200.cdeint: `func` looks like a single nn.Linear but could not be probed. "
-                              "Falling back to the generic stage loop; use torchcde_b200.LinearVectorField to get the "
-                              "fused kernel.")
-                return False
-            want = torch.nn.functional.linear(zp, lin.weight, lin.bias).view(*zp.shape[:-1], hidden, channels)
-            if not (isinstance(got, torch.Tensor) and got.shape == want.shape and got.dtype == want.dtype
-                    and torch.equal(got, want)):
-                return False
-    return True
-
-
-def _check_linear_problem(control, weight, bias, z0):
-    """One validator for every kernel-backed route (fused solve, kernel field, kernel vjp): the control's
-    coefficients, the weight and the bias must share z0's dtype and CUDA device -- the kernels receive raw
-    pointers, so a mismatch would be reinterpreted memory, not an exception (the reference raises a dtype /
-    device RuntimeError from its torch ops in the same situations)."""
-    _lib.require_cuda(z0, control, weight, bias)
-    for name, ten in (("the control's coefficients", control), ("func's weight", weight), ("func's bias", bias)):
-        if ten is None:
-            continue
-        if ten.dtype != z0.dtype:
-            raise RuntimeError("torchcde_b200.cdeint: z0 is {} but {} are {}; they must match."
-                               .format(z0.dtype, name, ten.dtype))
-        if ten.device != z0.device:
-            raise RuntimeError("torchcde_b200.cdeint: z0 is on {} but {} are on {}; they must be on the same device."
-                               .format(z0.device, name, ten.device))
+from .controls import CubicSpline, _control_signature, _schedule_knots
+from .linear_field import LinearFieldKernels, LinearVectorField, _reverse, linear_field_of  # noqa: F401
+from .schedule import FIXED_METHODS, build_schedule, host_locator
 
 
 # ------------------------------------------------------------------------------- validation
@@ -170,41 +55,6 @@ def _shape_error_prod(control_shape, field_shape, z0):
         raise ValueError("func.prod did not return a tensor with the same shape as z0. func.prod returned shape {} "
                          "whilst z0 has shape {}."
                          "".format(tuple(field_shape), tuple(z0.shape)))
-
-
-def _control_signature(X):
-    """(kind, batch shape, channels, n_intervals) of a built-in control without evaluating it."""
-    if isinstance(X, CubicSpline):
-        return _lib.CONTROL_CUBIC, tuple(X._b.shape[:-2]), X._b.size(-1), X._b.size(-2)
-    if isinstance(X, LinearInterpolation):
-        return _lib.CONTROL_LINEAR, tuple(X._coeffs.shape[:-2]), X._coeffs.size(-1), X._coeffs.size(-2) - 1
-    return None
-
-
-# --------------------------------------------------------------------------------- the solve
-def _fused_solve(X, weight, bias, z0, t, method, step_size):
-    kind, batch, channels, n_rows = _control_signature(X)
-    hidden = z0.size(-1)
-    dtype = z0.dtype
-    code = _lib.dtype_code(dtype)
-    control = X._rows() if kind == _lib.CONTROL_CUBIC else X._derivs
-    _check_linear_problem(control, weight, bias, z0)
-    with torch.cuda.device(z0.device):
-        control = control.detach().reshape(-1, control.size(-2), control.size(-1))
-        if not control.is_contiguous():
-            control = control.contiguous()
-        zf = z0.detach().reshape(-1, hidden).contiguous()
-        w = weight.detach().contiguous()
-        b = (bias.detach() if bias is not None else torch.zeros(hidden * channels, dtype=dtype, device=z0.device))
-        b = b.contiguous()
-        sched, (floats, ints, v) = _schedules.get(t, _schedule_knots(X), n_rows, method, step_size, dtype, z0.device)
-        out = torch.empty(zf.size(0), sched.n_out, hidden, dtype=dtype, device=z0.device)
-        _lib.call("tcde_cdeint_fixed_linear", _lib.ptr(control), kind, n_rows, _lib.ptr(w), _lib.ptr(b),
-                  _lib.ptr(zf), _lib.ptr(out), zf.size(0), channels, hidden, _lib.METHODS[method], sched.n_steps,
-                  _lib.ptr(v["step_dt"]), _lib.ptr(v["stage_index"]), _lib.ptr(v["stage_frac"]), sched.n_out,
-                  _lib.ptr(v["out_step"]), _lib.ptr(v["out_mode"]), _lib.ptr(v["out_slope"]), float(sched.sign), code,
-                  _lib.stream_of(zf))
-    return out.view(*z0.shape[:-1], sched.n_out, hidden)
 
 
 def _derivative_at(X, index, frac):
@@ -411,276 +261,18 @@ def _generic_solve_kernels(X, func, z0, t, method, step_size, is_prod, use_graph
     return static_out.clone()
 
 
-# ------------------------------------------------------- fields for the host-driven drivers
 def _host_locator(X, state_dtype):
-    """``(t_float, nudge) -> (interval index, fraction)`` with exactly the casts the reference stack
-    applies to a stage time (to the state dtype by the solver, to the coefficient dtype by
-    ``_interpret_t``), evaluated on the CPU so that no device sync is needed per stage."""
-    knots = _schedule_knots(X)
-    n_rows = _control_signature(X)[3]
-    # scalar version of ``schedule.locate``: numpy scalars round exactly like the tensor casts, ``bisect_left`` is
-    # ``torch.bucketize`` (right=False), and none of it goes through the torch dispatcher (this runs once per
-    # vector-field evaluation of the adaptive and adjoint drivers)
-    state_t = np.dtype(str(state_dtype).replace("torch.", "")).type
-    knot_t = np.dtype(str(knots.dtype).replace("torch.", "")).type
-    knot_list = knots.tolist()
-    knot_vals = [knot_t(v) for v in knot_list]
-
-    def where(t, nudge=0):
-        tt = state_t(t)
-        if nudge:
-            tt = np.nextafter(tt, tt + state_t(1))
-        tk = knot_t(tt)
-        index = min(max(bisect.bisect_left(knot_list, float(tk)) - 1, 0), n_rows - 1)
-        return index, float(tk - knot_vals[index])
-
-    return where
+    """``schedule.host_locator`` of a built-in control: ``(t_float, nudge) -> (interval index, fraction)``."""
+    return host_locator(_schedule_knots(X), _control_signature(X)[3], state_dtype)
 
 
 def _kernel_field(X, weight, bias, z0):
     """f(t, y) = (Linear(y).view(H, C)) @ dX/dt(t) as ONE launch of ``tcde_vector_field_linear``."""
-    kind, _, channels, n_rows = _control_signature(X)
-    hidden = z0.size(-1)
-    code = _lib.dtype_code(z0.dtype)
-    control = X._rows() if kind == _lib.CONTROL_CUBIC else X._derivs
-    _check_linear_problem(control, weight, bias, z0)
-    control = control.detach().reshape(-1, control.size(-2), control.size(-1)).contiguous()
-    w = weight.detach().contiguous()
-    b = bias.detach().contiguous() if bias is not None else torch.zeros(hidden * channels, dtype=z0.dtype,
-                                                                        device=z0.device)
-    where = _host_locator(X, z0.dtype)
-
-    def field(t, y, nudge=0):
-        index, frac = where(t, nudge)
-        yf = y.reshape(-1, hidden)
-        if not yf.is_contiguous():
-            yf = yf.contiguous()
-        out = torch.empty_like(yf)
-        with torch.cuda.device(y.device):
-            _lib.call("tcde_vector_field_linear", _lib.ptr(control), kind, n_rows, _lib.ptr(w), _lib.ptr(b),
-                      _lib.ptr(yf), _lib.ptr(out), yf.size(0), channels, hidden, index, float(frac), code,
-                      _lib.stream_of(yf))
-        return out.view_as(y)
-
-    return field
+    return LinearFieldKernels(X, weight, bias, z0).field()
 
 
-def _kernel_vjp(X, weight, bias, z0, params):
-    """The adjoint stage of the linear field as ONE launch of ``tcde_vector_field_linear_vjp``:
-    ``(t, y, a, scale) -> (f, scale * a^T df/dy, [scale * a^T df/dp for p in params])``, or ``None`` when the
-    kernel is not built for this problem (then autograd serves the backward solve)."""
-    kind, _, channels, n_rows = _control_signature(X)
-    hidden = z0.size(-1)
-    roles = []
-    for p in params:
-        if p is weight:
-            roles.append("w")
-        elif bias is not None and p is bias:
-            roles.append("b")
-        else:
-            return None                       # a parameter that is not the linear map: autograd knows how
-    control_check = X._rows() if kind == _lib.CONTROL_CUBIC else X._derivs
-    _check_linear_problem(control_check, weight, bias, z0)
-    if z0.dtype != torch.float32:
-        return None
-    n_paths = z0.numel() // hidden
-    scratch_bytes = _lib.load().tcde_vector_field_linear_vjp_scratch_bytes(n_paths, channels, hidden)
-    if scratch_bytes < 0:
-        return None
-    code = _lib.dtype_code(z0.dtype)
-    control = X._rows() if kind == _lib.CONTROL_CUBIC else X._derivs
-    control = control.detach().reshape(-1, control.size(-2), control.size(-1)).contiguous()
-    w = weight.detach().contiguous()
-    b = bias.detach().contiguous() if bias is not None else torch.zeros(hidden * channels, dtype=z0.dtype,
-                                                                        device=z0.device)
-    scratch = torch.empty(max(scratch_bytes // 4, 4), dtype=torch.float32, device=z0.device)
-    where = _host_locator(X, z0.dtype)
-    knots = _schedule_knots(X)
-
-    def launch(index, frac, y, a, f_out, vjp_out, gw, gb, f_scale, vjp_scale, grad_scale):
-        with torch.cuda.device(y.device):
-            _lib.call("tcde_vector_field_linear_vjp", _lib.ptr(control), kind, n_rows, _lib.ptr(w), _lib.ptr(b),
-                      _lib.ptr(y), _lib.ptr(a), _lib.ptr(f_out), _lib.ptr(vjp_out), _lib.ptr(gw), _lib.ptr(gb),
-                      _lib.ptr(scratch), y.numel() // hidden, channels, hidden, index, float(frac), float(f_scale),
-                      float(vjp_scale), float(grad_scale), code, _lib.stream_of(y))
-
-    def stage(t, y, a, scale):
-        index, frac = where(t)
-        yf = y.reshape(-1, hidden).contiguous()
-        af = a.reshape(-1, hidden).contiguous()
-        f = torch.empty_like(yf)
-        vjp_y = torch.empty_like(yf)
-        gw = torch.zeros_like(w) if "w" in roles else None
-        gb = torch.zeros_like(b) if "b" in roles else None
-        launch(index, frac, yf, af, f, vjp_y, gw, gb, 1.0, scale, scale)
-        return f.view_as(y), vjp_y.view_as(y), [gw if r == "w" else gb for r in roles]
-
-    def locate_many(times):
-        """Interval index / fraction of a list of stage times, with the casts of ``_host_locator``, in one go."""
-        tt = torch.tensor(times, dtype=torch.float64).to(z0.dtype)
-        frac, index = locate(knots, tt.to(knots.dtype), n_rows)
-        return index.tolist(), frac.tolist()
-
-    regrouped = []            # -W with rows regrouped as (k, c) and columns h: the "weight" of the adjoint state's own CDE
-
-    def segment(t_hi, t_lo, y_hi, a_hi, method, step_size, gw, gb):
-        """One segment [t_hi -> t_lo] of a fixed-step backward solve WITHOUT a launch per stage.  For this linear
-        field d a/ds = a^T df/dz does not involve z, so z(s) and a(s) are two ordinary fused solves (tensor-core
-        kernel, reversed time), each leaving the input of every stage in HBM; one more launch contracts the two
-        trajectories with dX/dt and the Runge-Kutta weights into dL/dW, dL/db.  Returns a(t_lo), or None when the
-        tensor-core kernel or the memory for the two trajectories (2 x stages x paths x 128 bytes) is not available."""
-        lib = _lib.load()
-        yf = y_hi.reshape(-1, hidden).contiguous()
-        af = a_hi.reshape(-1, hidden).contiguous()
-        n_paths = yf.size(0)
-        tt = torch.tensor([t_hi, t_lo], dtype=torch.float64)
-        sched, (_floats, _ints, v) = _schedules.get(tt, knots, n_rows, method, step_size, z0.dtype, z0.device)
-        n_total = sched.n_steps * sched.n_stages
-        scratch_bytes = lib.tcde_linear_field_param_grads_scratch_bytes(n_paths, n_total, channels, hidden)
-        if scratch_bytes < 0:
-            return None
-        need = 2 * n_total * n_paths * hidden * 4
-        with torch.cuda.device(z0.device):
-            free, _total = torch.cuda.mem_get_info()
-            if need + scratch_bytes > 0.7 * free:
-                return None
-            if not regrouped:
-                regrouped.append(w.view(hidden, channels, hidden).permute(2, 1, 0).contiguous()
-                                 .view(hidden * channels, hidden).neg_())
-                regrouped.append(torch.zeros_like(b))
-            z_stages = torch.empty(n_total, n_paths, hidden, dtype=z0.dtype, device=z0.device)
-            a_stages = torch.empty_like(z_stages)
-            ends = torch.empty(2, n_paths, sched.n_out, hidden, dtype=z0.dtype, device=z0.device)
-            try:
-                for which, (start, dump, ww, bb) in enumerate(((yf, z_stages, w, b),
-                                                               (af, a_stages, regrouped[0], regrouped[1]))):
-                    _lib.call("tcde_cdeint_fixed_linear_stages", _lib.ptr(control), kind, n_rows, _lib.ptr(ww),
-                              _lib.ptr(bb), _lib.ptr(start), _lib.ptr(ends[which]), _lib.ptr(dump), n_paths, channels,
-                              hidden, _lib.METHODS[method], sched.n_steps, _lib.ptr(v["step_dt"]),
-                              _lib.ptr(v["stage_index"]), _lib.ptr(v["stage_frac"]), sched.n_out,
-                              _lib.ptr(v["out_step"]), _lib.ptr(v["out_mode"]), _lib.ptr(v["out_slope"]),
-                              float(sched.sign), code, _lib.stream_of(yf))
-            except NotImplementedError:
-                return None
-            rk = {"rk4": (0.125, 0.375, 0.375, 0.125), "midpoint": (0.0, 1.0), "euler": (1.0,)}[method]
-            weights = (sched.step_dt.to(torch.float64).unsqueeze(1) * torch.tensor(rk, dtype=torch.float64)).reshape(-1)
-            weights = weights.to(z0.dtype).to(z0.device)
-            scratch2 = torch.empty(max(scratch_bytes // 4, 4), dtype=torch.float32, device=z0.device)
-            _lib.call("tcde_linear_field_param_grads", _lib.ptr(control), kind, n_rows, _lib.ptr(z_stages),
-                      _lib.ptr(a_stages), _lib.ptr(v["stage_index"]), _lib.ptr(v["stage_frac"]), _lib.ptr(weights),
-                      n_total, _lib.ptr(gw), _lib.ptr(gb), _lib.ptr(scratch2), n_paths, channels, hidden, 1.0, code,
-                      _lib.stream_of(yf))
-        return ends[1][:, -1].reshape(a_hi.shape)
-
-    def adaptive_segment(t_hi, t_lo, y_hi, a_hi, rtol, atol, gw, gb, slots_hint):
-        """One segment [t_hi -> t_lo] of the dopri5 backward solve with the step controller on the device
-        (``tcde_dopri5_linear_paired_attempts``): the state z and the adjoint state a advance as one virtual batch of
-        2 x paths under one controller, every attempt leaves the inputs of its five weighted stages in the slot of the
-        step it would become, and one launch of the parameter-gradient GEMM over the accepted steps' stages adds
-        dL/dW, dL/db into ``gw`` / ``gb``.  Returns a(t_lo), or None (not built for this problem / out of memory / more
-        accepted steps than slots) -- the caller then runs the host-driven backward."""
-        from . import adaptive
-        lib = _lib.load()
-        yf = y_hi.reshape(-1, hidden).contiguous()
-        af = a_hi.reshape(-1, hidden).contiguous()
-        n_paths = yf.size(0)
-        if hidden != 32 or channels != 8 or n_paths % 256 != 0 or n_paths == 0:
-            return None
-        with torch.cuda.device(z0.device):
-            if not regrouped:
-                regrouped.append(w.view(hidden, channels, hidden).permute(2, 1, 0).contiguous()
-                                 .view(hidden * channels, hidden).neg_())
-                regrouped.append(torch.zeros_like(b))
-            w2, b2 = regrouped
-            if not fields:
-                fields.append(_kernel_field(X, w, b, z0))
-                fields.append(_kernel_field(X, w2, b2, z0))
-
-            def field_v(s_time, v):                  # the virtual batch's slope in s = -t (start slope, Hairer's first step)
-                return torch.cat([-fields[0](-s_time, v[:n_paths]), -fields[1](-s_time, v[n_paths:])])
-
-            s0, s1 = -float(t_hi), -float(t_lo)
-            v0 = torch.cat([yf, af])
-            f0 = field_v(s0, v0)
-            dt = adaptive._initial_step(field_v, s0, v0, f0, rtol, atol)
-            # trajectory slots: enough for a few hundred accepted steps, at most a quarter of the free memory; when they are
-            # full the device pauses, the filled slots are contracted into the gradients and the solve goes on
-            free, _total = torch.cuda.mem_get_info()
-            per_slot = 2 * 5 * n_paths * hidden * 4
-            max_slots = int(min(max(16, slots_hint), 256, 0.25 * free // per_slot))
-            if max_slots < 8:
-                return None
-            dev = z0.device
-            state = torch.empty(5, 2 * n_paths, hidden, dtype=torch.float32, device=dev)
-            state[0].copy_(v0)
-            state[2].copy_(f0)
-            grid = lib.tcde_dopri5_linear_grid(2 * n_paths)
-            partials = torch.zeros(2, grid, dtype=torch.float64, device=dev)
-            ctl = adaptive.initial_control(s0, dt, s1, rtol, atol).to(dev)
-            out = torch.empty(2 * n_paths, 2, hidden, dtype=torch.float32, device=dev)
-            out[:, 0].copy_(v0)
-            out_times = torch.tensor([s0, s1], dtype=torch.float64, device=dev)
-            dump_z = torch.empty(max_slots * 5, n_paths, hidden, dtype=torch.float32, device=dev)
-            dump_a = torch.empty_like(dump_z)
-            q_index = torch.zeros(max_slots * 5, dtype=torch.int32, device=dev)
-            q_frac = torch.zeros(max_slots * 5, dtype=torch.float32, device=dev)
-            q_weight = torch.zeros(max_slots * 5, dtype=torch.float32, device=dev)
-            knots_dev = knots.detach().to(device=dev, dtype=torch.float32).contiguous()
-            stream = _lib.stream_of(yf)
-            scratch_cache = {}
-
-            def contract(n_steps):                   # dL/dW, dL/db += the quadrature over the first n_steps slots
-                n_total = 5 * n_steps
-                if n_total <= 0 or (gw is None and gb is None):
-                    return
-                scratch_bytes = lib.tcde_linear_field_param_grads_scratch_bytes(n_paths, n_total, channels, hidden)
-                if scratch_bytes < 0:
-                    raise RuntimeError("dopri5 adjoint: the parameter-gradient kernel is not built for this problem")
-                if scratch_cache.get("n", 0) < scratch_bytes:
-                    scratch_cache["buf"] = torch.empty(max(scratch_bytes // 4, 4), dtype=torch.float32, device=dev)
-                    scratch_cache["n"] = scratch_bytes
-                _lib.call("tcde_linear_field_param_grads", _lib.ptr(control), kind, n_rows, _lib.ptr(dump_z), _lib.ptr(dump_a),
-                          _lib.ptr(q_index), _lib.ptr(q_frac), _lib.ptr(q_weight), n_total, _lib.ptr(gw), _lib.ptr(gb),
-                          _lib.ptr(scratch_cache["buf"]), n_paths, channels, hidden, 1.0, code, stream)
-
-            seq, base, flushes = 0, 0, 0
-            while True:
-                _lib.call("tcde_dopri5_linear_paired_attempts", _lib.ptr(control), kind, n_rows, _lib.ptr(knots_dev), _lib.ptr(w),
-                          _lib.ptr(b), _lib.ptr(w2), _lib.ptr(b2), _lib.ptr(state), _lib.ptr(partials), _lib.ptr(ctl),
-                          _lib.ptr(out), _lib.ptr(out_times), 2, n_paths, channels, hidden, -1.0, _lib.ptr(dump_z),
-                          _lib.ptr(dump_a), _lib.ptr(q_index), _lib.ptr(q_frac), _lib.ptr(q_weight), max_slots, seq,
-                          adaptive._DEVICE_CHUNK, _lib.F32, stream)
-                seq += adaptive._DEVICE_CHUNK
-                last = ctl[(seq - 1) & 1].cpu()
-                if last[adaptive.CTL_DONE] != 0:
-                    contract(int(last[adaptive.CTL_NACC]) - base)
-                    if last[adaptive.CTL_OVERFLOW] == 0:
-                        break
-                    # slots full: the filled ones are contracted; hand the slots back and resume where the device paused
-                    base = int(last[adaptive.CTL_NACC])
-                    flushes += 1
-                    resume = last.clone()
-                    resume[adaptive.CTL_DONE], resume[adaptive.CTL_OVERFLOW] = 0.0, 0.0
-                    resume[adaptive.CTL_BASE] = float(base)
-                    ctl[(seq - 1) & 1].copy_(resume)
-                    continue
-                if not math.isfinite(float(last[adaptive.CTL_DT])) or float(last[adaptive.CTL_DT]) == 0.0 or seq > 10_000_000:
-                    raise RuntimeError("dopri5 adjoint: step size underflow / non-finite error estimate at s = {}".format(
-                        float(last[adaptive.CTL_T])))
-            n_acc = int(last[adaptive.CTL_NACC])
-            stage.adaptive_stats = {"n_accepted": n_acc, "n_rejected": int(last[adaptive.CTL_NREJ]), "launches": seq,
-                                    "slots": max_slots, "flushes": flushes}
-            return out[n_paths:, 1].reshape(a_hi.shape).clone()
-
-    fields = []
-    stage.launch = launch
-    stage.locate_many = locate_many
-    stage.segment = segment
-    stage.adaptive_segment = adaptive_segment
-    stage.adaptive_spec = None
-    stage.roles = roles
-    stage.new_grads = lambda: [torch.zeros_like(w) if r == "w" else torch.zeros_like(b) for r in roles]
-    return stage
+# the one call through which cdeint gets the adjoint stage of a linear field: ``_kernel_vjp(kernels, params)``
+_kernel_vjp = LinearFieldKernels.adjoint_stage
 
 
 def _torch_field(X, func, is_prod, known_control, z0):
@@ -709,10 +301,6 @@ def _torch_field(X, func, is_prod, known_control, z0):
         return (func(ts, y) @ dx.unsqueeze(-1)).squeeze(-1)
 
     return field
-
-
-def _reverse(field):
-    return lambda s, y, nudge=0: -1.0 * field(-s, y)
 
 
 def _time_first_to_reference_layout(out):
@@ -840,11 +428,6 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
         jumps = jumps.detach().cpu().tolist() if isinstance(jumps, torch.Tensor) else list(jumps)
         options["jump_t"] = sorted(-float(v) for v in jumps) if flipped else sorted(float(v) for v in jumps)
 
-    def fast_field():
-        f = _kernel_field(X, field_params[0], field_params[1], z0) if field_params is not None \
-            else _torch_field(X, func, is_prod, sig is not None, z0)
-        return _reverse(f) if flipped else f
-
     def autograd_field():
         f = _torch_field(X, func, is_prod, sig is not None, z0)
         return _reverse(f) if flipped else f
@@ -854,10 +437,9 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     def forward_values(y0):
         """Outputs only, time first, by the fastest route."""
         if method in FIXED_METHODS:
-            if field_params is not None:
+            if kernels is not None:
                 try:
-                    out = _fused_solve(X, field_params[0], field_params[1], y0, t, method, step_size)
-                    return out.movedim(-2, 0)
+                    return kernels.solve(y0, t, method, step_size).movedim(-2, 0)
                 except NotImplementedError:
                     # a shape the fused kernels are not built for (e.g. hidden * channels * hidden beyond the
                     # shared-memory budget of the CUDA-core kernel): this package's own stage loop takes any shape
@@ -866,26 +448,22 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                     and sig[1] == tuple(y0.shape[:-1]):
                 return _generic_solve_kernels(X, func, y0, t, method, step_size, is_prod, use_graph).movedim(-2, 0)
             return _generic_solve(X, func, y0, t, method, step_size, is_prod, sig is not None).movedim(-2, 0)
-        if (field_params is not None and adaptive.device_dopri5_available(y0, sig[2]) and not options.get("jump_t")
+        if (kernels is not None and adaptive.device_dopri5_available(y0, sig[2]) and not options.get("jump_t")
                 and set(options) <= {"first_step", "jump_t"}):
             # config 4's forward pass: the whole adaptive loop on the device, one launch per attempted step
-            kind = sig[0]
-            control = X._rows() if kind == _lib.CONTROL_CUBIC else X._derivs
-            _check_linear_problem(control, field_params[0], field_params[1], y0)
-            control = control.detach().reshape(-1, control.size(-2), control.size(-1)).contiguous()
-            bias = field_params[1]
-            bias = bias.detach().contiguous() if bias is not None else torch.zeros(
-                field_params[0].size(0), dtype=y0.dtype, device=y0.device)
-            knots = X._t.detach().to(device=y0.device, dtype=y0.dtype).contiguous()
-            out, stats = adaptive.odeint_dopri5_device(control, kind, sig[3], knots, field_params[0].detach().contiguous(), bias,
-                                                       fast_field(), y0, times, rtol, atol, -1.0 if flipped else 1.0,
-                                                       options.get("first_step"))
-            cdeint.last_stats = stats
+            out, cdeint.last_stats = kernels.dopri5(y0, times, rtol, atol, -1.0 if flipped else 1.0,
+                                                    options.get("first_step"))
             return out
-        out, solver_obj = adaptive.odeint_dopri5(fast_field(), y0, times, rtol, atol, options)
+        field = kernels.field() if kernels is not None else _torch_field(X, func, is_prod, sig is not None, z0)
+        out, solver_obj = adaptive.odeint_dopri5(_reverse(field) if flipped else field, y0, times, rtol, atol, options)
         cdeint.last_stats = {"n_accepted": solver_obj.n_accepted, "n_rejected": solver_obj.n_rejected,
                              "device_controlled": False}
         return out
+
+    # the routes that call a kernel own the linear-field problem; building it checks dtypes and devices
+    kernels = None
+    if field_params is not None and (adjoint or not wants_grad):
+        kernels = LinearFieldKernels(X, field_params[0], field_params[1], z0)
 
     if not wants_grad:
         with torch.no_grad():
@@ -906,9 +484,9 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
         def fused_vjp(params):
             # decreasing t, gradients with respect to the output times, or parameters that are not the linear map
             # (the control's coefficients or knots in ``adjoint_params``): autograd serves the backward solve
-            if field_params is None or flipped or t_grad is not None:
+            if kernels is None or flipped or t_grad is not None:
                 return None
-            st = _kernel_vjp(X, field_params[0], field_params[1], z0, params)
+            st = _kernel_vjp(kernels, params)
             if (st is not None and a_method not in FIXED_METHODS and adaptive.device_dopri5_available(z0, sig[2])
                     and not kwargs.get("adjoint_options", None)):
                 # dopri5 backward with the controller on the device; the forward pass's step count sizes the trajectory slots
