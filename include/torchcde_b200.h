@@ -47,7 +47,7 @@ enum tcde_status {
 };
 
 enum tcde_control { TCDE_CONTROL_CUBIC = 0, TCDE_CONTROL_LINEAR = 1 };
-enum tcde_method { TCDE_EULER = 0, TCDE_MIDPOINT = 1, TCDE_RK4_38 = 2 };
+enum tcde_method { TCDE_EULER = 0, TCDE_MIDPOINT = 1, TCDE_RK4_38 = 2, TCDE_REVERSIBLE_HEUN = 3 };
 
 /* flag bits written by the builders into *flags (a device int32, may be NULL) */
 #define TCDE_FLAG_NAN_SEEN 1        /* at least one NaN in x */
@@ -193,7 +193,39 @@ TCDE_API int tcde_cdeint_fixed_linear_stages(const void* control, int control_ki
                                     const int32_t* out_step, const int32_t* out_mode, const void* out_slope,
                                     double sign, int dtype, void* stream);
 
-/* ... and the parameter gradients of that whole backward solve in one launch:
+/* torchsde's reversible Heun method with zero diffusion (cdeint(..., backend="torchsde", method="reversible_heun")) for
+ * the same linear field, in ONE launch (the CUDA-core kernel, fp32 or fp64, any shape it is built for):
+ *   z_{n+1} = 2 y_n - z_n + f_n dt_n,  f_{n+1} = f(t_{n+1}, z_{n+1}),  y_{n+1} = y_n + (f_n + f_{n+1}) (0.5 dt_n)
+ * starting from z_0 = y_0, f_0 = f(t_0, y_0).  Schedule (torchcde_b200/schedule.py, build_sde_schedule):
+ *   step_dt[n_steps]; stage_index / stage_frac[n_steps + 1]: the evaluation points t_0 .. t_N;
+ *   out_step[n_out] (-1: output j is y_0); out_weights[2][n_out]: w1 of every output, then w0, and output j is
+ *   w0 y_n + w1 y_{n+1} of its step n (torchsde's linear_interp).
+ * checkpoints (may be NULL): [ceil(n_steps / checkpoint_stride) + 1][3][n_paths][hidden] receives (y, z, f) of every step
+ * that is a multiple of checkpoint_stride and of the last step -- the restart points of the reversible backward. */
+TCDE_API int tcde_cdeint_reversible_heun_linear(const void* control, int control_kind, int64_t n_rows, const void* weight,
+                                       const void* bias, const void* z0, void* out, void* checkpoints,
+                                       int64_t checkpoint_stride, int64_t n_paths, int64_t channels, int64_t hidden,
+                                       int64_t n_steps, const void* step_dt, const int32_t* stage_index,
+                                       const void* stage_frac, int64_t n_out, const int32_t* out_step,
+                                       const void* out_weights, int dtype, void* stream);
+
+/* One checkpoint segment [lo, hi] of the reversible Heun backward (fp32, hidden = 32, channels = 8), in one launch: walks the
+ * steps m = hi - 1 .. lo in reverse, reconstructing z_m, f_m = F(z_m), y_m algebraically from step m + 1 (the state of step lo
+ * is taken from its checkpoint), running the adjoint recurrence of (y, z, f) and adding the output gradients
+ * g[n_paths][n_out][hidden] (inj_range[N + 1][2]: the outputs [first, end) that touch y_m; weight w0 when out_step == m,
+ * 1 when out_step < 0, w1 otherwise).  J_F^T fbar is the same field product with weight_t[(k, c)][h] = weight[(h, c)][k] and
+ * the bias `zeros` (256 zeros).  ckpt_lo / ckpt_hi: [3][n_paths][hidden] (y, z, f) of steps lo and hi; carry [2][n_paths]
+ * [hidden]: (ybar, zbar) of step hi in, of step lo out.  dump_z / dump_a [hi - lo][n_paths][hidden] receive (z_m, fbar_m)
+ * for tcde_linear_field_param_grads (weights 1) to contract into dL/dW, dL/db. */
+TCDE_API int tcde_reversible_heun_linear_backward_segment(
+    const void* control, int control_kind, int64_t n_rows, const void* weight, const void* bias, const void* weight_t,
+    const void* zeros, const void* ckpt_lo, const void* ckpt_hi, void* carry, const void* g, int64_t n_out,
+    const int32_t* out_step, const void* out_weights, const int32_t* inj_range, const void* step_dt,
+    const int32_t* stage_index, const void* stage_frac, int64_t lo, int64_t hi, int64_t n_paths, int64_t channels,
+    int64_t hidden, void* dump_z, void* dump_a, int dtype, void* stream);
+
+/* The parameter gradients of a whole backward solve (the stage trajectories of tcde_cdeint_fixed_linear_stages, or any
+ * other list of (z, a, stage) triples) in one launch:
  *   grad_weight[h*C+c][k] += scale * sum_e sum_p stage_weight[e] * a_stages[e][p][h] * dXdt_e[p][c] * z_stages[e][p][k]
  *   grad_bias[h*C+c]      += scale * sum_e sum_p stage_weight[e] * a_stages[e][p][h] * dXdt_e[p][c]
  * with dXdt_e from the control at (stage_index[e], stage_frac[e]) and stage_weight[e] = step * Runge-Kutta weight

@@ -8,7 +8,9 @@ Drop-in names (reference torchcde/__init__.py:1-9): ``cdeint``, ``CubicSpline``,
 there is no CPU path and no PyTorch-eager fallback.
 
 ``logsig_windows`` / ``logsignature_windows`` (the log-ODE transform) run on a kernel of this package instead of the optional
-``signatory`` dependency.  Not provided (outside the hot path, SURVEY.md section 2): ``TupleControl`` and the torchsde backend.
+``signatory`` dependency.  ``cdeint(..., backend="torchsde", method="reversible_heun")`` is torchsde's reversible Heun
+method with an exact, checkpointed reversible backward (``reversible.py``); the other torchsde methods are not built.
+Not provided (outside the hot path, SURVEY.md section 2): ``TupleControl``.
 """
 from . import misc
 from .coeffs import (hermite_cubic_coefficients_with_backward_differences, linear_interpolation_coeffs,

@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libtcde_b200.so")
 F32, F64 = 0, 1
 CONTROL_CUBIC, CONTROL_LINEAR = 0, 1
 METHODS = {"euler": 0, "midpoint": 1, "rk4": 2}
+REVERSIBLE_HEUN = 3          # tcde_method of torchsde's reversible Heun (tcde_cdeint_reversible_heun_linear)
 STAGES = {"euler": 1, "midpoint": 2, "rk4": 4}
 FLAG_NAN_SEEN, FLAG_NAN_TIME, FLAG_NAN_FIRST_ROW = 1, 2, 4
 
@@ -42,6 +43,10 @@ SIGNATURES = {
                                       _dbl, _dbl, _dbl, _int, _p], _int),
     "tcde_cdeint_fixed_linear_stages": ([_p, _int, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i64, _int, _i64, _p, _p, _p,
                                          _i64, _p, _p, _p, _dbl, _int, _p], _int),
+    "tcde_cdeint_reversible_heun_linear": ([_p, _int, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _i64, _p, _p,
+                                            _p, _i64, _p, _p, _int, _p], _int),
+    "tcde_reversible_heun_linear_backward_segment": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _p,
+                                                      _p, _p, _i64, _i64, _i64, _i64, _i64, _p, _p, _int, _p], _int),
     "tcde_linear_field_param_grads_scratch_bytes": ([_i64, _i64, _i64, _i64], _i64),
     "tcde_linear_field_param_grads": ([_p, _int, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _i64, _i64, _i64, _dbl,
                                        _int, _p], _int),

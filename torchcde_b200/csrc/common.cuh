@@ -107,7 +107,9 @@ struct UmmaArgs {
     int64_t n_rows;
     int control_kind, method, n_stages, n_steps, n_out;
     float sign;
-    float* stage_dump;    // optional [n_steps * n_stages][n_paths][32]: the input of every stage (for the adjoint)
+    float* stage_dump;    // optional [n_steps * n_stages][n_paths][32]: the input of every stage (for the adjoint);
+                          // reversible Heun: the checkpoints [slot][3][n_paths][32] (y, z, f of every ckpt_stride-th step)
+    int ckpt_stride;      // reversible Heun only
 };
 bool solve_tc_supported(int H, int C);
 // tensor-core kernel (solve_tc.cu): Runge-Kutta state in registers; mode 0 = 3xTF32 operand split, mode 1 = 2xFP16 with

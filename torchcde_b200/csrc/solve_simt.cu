@@ -45,6 +45,11 @@ template <typename T> struct SolveArgs {
     // (eval_index, eval_frac) and the kernel returns after the first stage; no schedule is read
     int eval_only, eval_index;
     T eval_frac;
+    // reversible Heun (method TCDE_REVERSIBLE_HEUN): stage_index / stage_frac hold n_steps + 1 evaluation points t_0..t_N,
+    // out_slope holds [2][n_out] interpolation weights (w1 of every output, then w0), and (y, z, f) of every step that is
+    // a multiple of ckpt_stride, and of the last step, go to ckpt[slot][3][n_paths][H] (slot = ceil(step / stride))
+    int ckpt_stride;
+    T* ckpt;
 };
 
 // Shared-memory carve-up (all offsets in elements of T; every region 16-byte aligned):
@@ -75,7 +80,8 @@ template <typename T> static SolveSmem<T> solve_smem_layout(int H, int Cp, int g
     return s;
 }
 
-template <typename T, int ST, int CT>
+// REV: the reversible Heun instantiation (method TCDE_REVERSIBLE_HEUN); the Runge-Kutta instantiations do not contain it
+template <typename T, int ST, int CT, bool REV>
 __global__ void __launch_bounds__(256, (sizeof(T) == 4 && ST * CT >= 64) ? 2 : 1)
 cdeint_simt_kernel(const SolveArgs<T> a, const SolveSmem<T> lay) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -203,7 +209,8 @@ cdeint_simt_kernel(const SolveArgs<T> a, const SolveSmem<T> lay) {
     __syncthreads();
 
     const int n_stages = a.n_stages;
-    const int total = a.eval_only ? 1 : a.n_steps * n_stages;
+    // reversible Heun evaluates once more than it steps: the prologue f(t_0, y_0)
+    const int total = a.eval_only ? 1 : a.n_steps * n_stages + (REV ? 1 : 0);
     const T third = T(1.0 / 3.0);
     int step = 0, sub = 0;
     T dt = a.eval_only ? T(0) : a.step_dt[0];
@@ -324,6 +331,54 @@ cdeint_simt_kernel(const SolveArgs<T> a, const SolveSmem<T> lay) {
                 for (int s = 0; s < ST; ++s) zn[s] = E::add(y[s], E::mul(dt, kv[s]));
                 step_done = true;
             }
+        } else if (REV) {
+            // torchsde's reversible Heun with zero diffusion: evaluation st is f_st = f(t_st, z_st).  Slot 0 keeps f of
+            // the step start, slot 1 the z this evaluation was made at; y stays in registers.
+            //   z_{n+1} = 2 y_n - z_n + f_n dt_n,   y_{n+1} = y_n + (f_n + f_{n+1}) (0.5 dt_n)
+            T zc[ST];
+            if (st == 0) {
+#pragma unroll
+                for (int s = 0; s < ST; ++s) zc[s] = y[s];                  // z_0 = y_0
+            } else {
+                const T half = E::mul(T(0.5), dt);
+#pragma unroll
+                for (int s = 0; s < ST; ++s) {
+                    zc[s] = parked(1, s);
+                    zn[s] = E::add(y[s], E::mul(E::add(parked(0, s), kv[s]), half));
+                }
+                while (jn < a.n_out && a.out_step[jn] == step) {         // torchsde's linear_interp: w0 y_n + w1 y_{n+1}
+                    const T w1 = a.out_slope[jn], w0 = a.out_slope[a.n_out + jn];
+                    T v[ST];
+#pragma unroll
+                    for (int s = 0; s < ST; ++s) v[s] = E::add(E::mul(w0, y[s]), E::mul(w1, zn[s]));
+                    write_out(jn, v);
+                    ++jn;
+                }
+#pragma unroll
+                for (int s = 0; s < ST; ++s) y[s] = zn[s];
+                ++step;
+            }
+            if (a.ckpt && worker && (step % a.ckpt_stride == 0 || step == a.n_steps)) {
+                T* base = a.ckpt + (size_t)((step + a.ckpt_stride - 1) / a.ckpt_stride) * 3 * a.n_paths * H + h;
+#pragma unroll
+                for (int s = 0; s < ST; ++s) {
+                    const int64_t p = path0 + lp0 + s;
+                    if (p < a.n_paths) {
+                        base[p * H] = y[s];
+                        base[(a.n_paths + p) * H] = zc[s];
+                        base[(2 * a.n_paths + p) * H] = kv[s];
+                    }
+                }
+            }
+            if (step < a.n_steps) {
+                dt = a.step_dt[step];
+#pragma unroll
+                for (int s = 0; s < ST; ++s) {
+                    zn[s] = E::add(E::sub(E::mul(T(2), y[s]), zc[s]), E::mul(kv[s], dt));
+                    park(0, s, kv[s]);
+                    park(1, s, zn[s]);
+                }
+            }
         } else {
 #pragma unroll
             for (int s = 0; s < ST; ++s) zn[s] = E::add(y[s], E::mul(dt, kv[s]));
@@ -415,7 +470,7 @@ vector_field_kernel(const T* __restrict__ control, int control_kind, int64_t n_r
 
 template <typename T, int ST, int CT>
 static int launch_solve_ct(SolveArgs<T> a, cudaStream_t stream) {
-    auto kern = cdeint_simt_kernel<T, ST, CT>;
+    auto kern = (a.method == TCDE_REVERSIBLE_HEUN) ? cdeint_simt_kernel<T, ST, CT, true> : cdeint_simt_kernel<T, ST, CT, false>;
     TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     int g_max = 256 / a.H;
     if (g_max < 1) g_max = 1;
@@ -597,6 +652,54 @@ extern "C" int tcde_cdeint_fixed_linear(const void* control, int control_kind, i
     return solve_fixed_linear(control, control_kind, n_rows, weight, bias, z0, out, n_paths, channels, hidden, method,
                               n_steps, step_dt, stage_index, stage_frac, n_out, out_step, out_mode, out_slope, sign, dtype,
                               nullptr, stream);
+}
+
+extern "C" int tcde_cdeint_reversible_heun_linear(const void* control, int control_kind, int64_t n_rows, const void* weight,
+                                                  const void* bias, const void* z0, void* out, void* checkpoints,
+                                                  int64_t checkpoint_stride, int64_t n_paths, int64_t channels,
+                                                  int64_t hidden, int64_t n_steps, const void* step_dt,
+                                                  const int32_t* stage_index, const void* stage_frac, int64_t n_out,
+                                                  const int32_t* out_step, const void* out_weights, int dtype,
+                                                  void* stream) {
+    TCDE_CHECK_ARG(control && weight && bias && z0 && out, "null data pointer");
+    TCDE_CHECK_ARG(step_dt && stage_index && stage_frac && out_step && out_weights, "null schedule pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && n_rows >= 1, "bad sizes");
+    TCDE_CHECK_ARG(n_steps >= 1 && n_out >= 1, "n_steps=%lld n_out=%lld", (long long)n_steps, (long long)n_out);
+    TCDE_CHECK_ARG(checkpoint_stride >= 1 && checkpoint_stride < (1ll << 30), "checkpoint_stride=%lld",
+                   (long long)checkpoint_stride);
+    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    TCDE_CHECK_SUPPORTED(n_steps + 1 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
+    if (n_paths == 0) return TCDE_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (dtype == TCDE_F32) {
+        // the tensor-core kernel wherever the fixed-step solve uses it (same variant switch), the CUDA-core kernel otherwise
+        const bool tc_ok = solve_tc_supported((int)hidden, (int)channels) &&
+                           ((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z0) |
+                             reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(checkpoints)) & 15) == 0;
+        if ((g_solve_variant >= 2) || (g_solve_variant == 0 && tc_ok)) {
+            UmmaArgs u{(const float*)control, (const float*)weight, (const float*)bias, (const float*)z0, (float*)out,
+                       (const float*)step_dt, stage_index, (const float*)stage_frac, out_step, nullptr,
+                       (const float*)out_weights, n_paths, n_rows, control_kind, TCDE_REVERSIBLE_HEUN, 1, (int)n_steps,
+                       (int)n_out, 1.f, (float*)checkpoints, (int)checkpoint_stride};
+            const int mode = (g_solve_variant == 2 || g_solve_variant == 3 || g_solve_variant == 6) ? 0
+                             : (g_solve_variant == 4 || g_solve_variant == 5) ? 1 : TCDE_DEFAULT_TC_MODE;
+            return solve_tc_f32(u, (int)hidden, (int)channels, mode, s);
+        }
+        SolveArgs<float> a{(const float*)control, (const float*)weight, (const float*)bias, (const float*)z0,
+                           (float*)out, (const float*)step_dt, stage_index, (const float*)stage_frac, out_step,
+                           nullptr, (const float*)out_weights, n_paths, n_rows, (int)channels, 0, (int)hidden,
+                           control_kind, TCDE_REVERSIBLE_HEUN, 1, (int)n_steps, (int)n_out, 0, 0, 1.f, 0, 0, 0.f,
+                           (int)checkpoint_stride, (float*)checkpoints};
+        return solve_simt_f32(a, s);
+    }
+    SolveArgs<double> a{(const double*)control, (const double*)weight, (const double*)bias, (const double*)z0,
+                        (double*)out, (const double*)step_dt, stage_index, (const double*)stage_frac, out_step,
+                        nullptr, (const double*)out_weights, n_paths, n_rows, (int)channels, 0, (int)hidden,
+                        control_kind, TCDE_REVERSIBLE_HEUN, 1, (int)n_steps, (int)n_out, 0, 0, 1.0, 0, 0, 0.0,
+                        (int)checkpoint_stride, (double*)checkpoints};
+    return solve_simt_f64(a, s);
 }
 
 extern "C" int tcde_cdeint_fixed_linear_stages(const void* control, int control_kind, int64_t n_rows, const void* weight,

@@ -76,6 +76,47 @@ __device__ __forceinline__ bool rk_combine(const UmmaArgs& a, int sub, float dt,
     return true;
 }
 
+// torchsde's reversible Heun (zero diffusion) on NV state values: the slots y, f (k1) and z (s23) hold y_n, f_n and the z
+// the current evaluation kv = f(t_st, z) was made at.  Evaluation 0 is the prologue f(t_0, y_0); evaluation st > 0 ends
+// step st - 1:  y_{n+1} = y_n + (f_n + f_{n+1}) (0.5 dt_n), outputs w0 y_n + w1 y_{n+1} (out_slope = [w1..., w0...]).
+// ckpt(slot, y, z, f) stores the state of every ckpt_stride-th step and of the last; zin receives the next evaluation's
+// input z_{n+1} = 2 y_n - z_n + f_n dt_n.
+template <int NV, typename Write, typename Ckpt>
+__device__ __forceinline__ void rev_heun_combine(const UmmaArgs& a, int st, int& step, float& dt, float* y, float* f,
+                                                 float* z, const float* kv, float* zin, int& jn, Write write, Ckpt ckpt) {
+    using E = exact<float>;
+    if (st == 0) {
+#pragma unroll
+        for (int h = 0; h < NV; ++h) z[h] = y[h];                       // z_0 = y_0
+    } else {
+        const float half = E::mul(0.5f, dt);
+        float yn[NV];
+#pragma unroll
+        for (int h = 0; h < NV; ++h) yn[h] = E::add(y[h], E::mul(E::add(f[h], kv[h]), half));
+        while (jn < a.n_out && a.out_step[jn] == step) {
+            const float w1 = a.out_slope[jn], w0 = a.out_slope[a.n_out + jn];
+            float v[NV];
+#pragma unroll
+            for (int h = 0; h < NV; ++h) v[h] = E::add(E::mul(w0, y[h]), E::mul(w1, yn[h]));
+            write(jn, v);
+            ++jn;
+        }
+#pragma unroll
+        for (int h = 0; h < NV; ++h) y[h] = yn[h];
+        ++step;
+    }
+    if (step % a.ckpt_stride == 0 || step == a.n_steps) ckpt((step + a.ckpt_stride - 1) / a.ckpt_stride, y, z, kv);
+    if (step < a.n_steps) {
+        dt = a.step_dt[step];
+#pragma unroll
+        for (int h = 0; h < NV; ++h) {
+            zin[h] = E::add(E::sub(E::mul(2.f, y[h]), z[h]), E::mul(kv[h], dt));
+            f[h] = kv[h];
+            z[h] = zin[h];
+        }
+    }
+}
+
 // The outputs that fall on the step just completed (y = its start, zin = its end); write(j, v) stores output j.
 template <int NV, typename Write>
 __device__ __forceinline__ void step_outputs(const UmmaArgs& a, int step, int& jn, int& next_out, const float* y,
@@ -108,7 +149,8 @@ struct Smem {
     static constexpr int total = warps + kWarps * WarpSmem<0>::bytes;
 };
 
-template <bool DUMP>
+// REV: reversible Heun (rev_heun_combine, checkpoints through the stage-dump pointer) instead of the Runge-Kutta methods
+template <bool DUMP, bool REV>
 __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a) {
     using S = Smem;
     using E = exact<float>;
@@ -144,7 +186,7 @@ __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a
         for (int c4 = 0; c4 < 8; ++c4) dst[c4] = make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
     };
     auto dump = [&](int stage_no, const float* z) {
-        if (!DUMP || !live) return;
+        if (!DUMP || REV || !live) return;
         float4* dst = reinterpret_cast<float4*>(a.stage_dump + ((int64_t)stage_no * a.n_paths + path) * kHid);
 #pragma unroll
         for (int c4 = 0; c4 < 8; ++c4) dst[c4] = make_float4(z[4 * c4], z[4 * c4 + 1], z[4 * c4 + 2], z[4 * c4 + 3]);
@@ -169,7 +211,7 @@ __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a
         next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
     }
 
-    const int n_st = a.n_steps * a.n_stages;
+    const int n_st = a.n_steps * a.n_stages + (REV ? 1 : 0);
     float4 raw[6], nxt[6];
     fetch(a.stage_index[0], raw);
     int step = 0, sub = 0;
@@ -195,7 +237,22 @@ __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a
         float kv[kHid];
         warp_field<0>(zin, dx, kv, ws, smem + S::b, beta, inv_w_scale);
 
-        if (rk_combine<kHid>(a, sub, dt, y, k1, s23, kv, zin)) {
+        if (REV) {
+            rev_heun_combine<kHid>(a, st, step, dt, y, k1, s23, kv, zin, jn, write_out,
+                                   [&](int slot, const float* vy, const float* vz, const float* vf) {
+                                       if (!DUMP || !live) return;
+                                       const float* src[3] = {vy, vz, vf};
+#pragma unroll
+                                       for (int w = 0; w < 3; ++w) {
+                                           float4* dst = reinterpret_cast<float4*>(
+                                               a.stage_dump + (((int64_t)slot * 3 + w) * a.n_paths + path) * kHid);
+#pragma unroll
+                                           for (int c4 = 0; c4 < 8; ++c4)
+                                               dst[c4] = make_float4(src[w][4 * c4], src[w][4 * c4 + 1], src[w][4 * c4 + 2],
+                                                                     src[w][4 * c4 + 3]);
+                                       }
+                                   });
+        } else if (rk_combine<kHid>(a, sub, dt, y, k1, s23, kv, zin)) {
             step_outputs<kHid>(a, step, jn, next_out, y, zin, write_out);
 #pragma unroll
             for (int h = 0; h < kHid; ++h) y[h] = zin[h];
@@ -257,9 +314,110 @@ __device__ __forceinline__ void pin(float* d) {
     for (int i = 0; i < kAcc; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// One evaluation of the linear field for the warpgroup's 64 rows: kv = (W zin + b) . dx in the fragment layout above.
+// beta, inv_w_scale: prepare_b<1>'s scales of the tile at b_tile (bias at b_bias).  dx (the lane's two channels of both
+// rows) is scaled in place.  mid() runs halfway through the chunks (the caller's next dX/dt hides behind the MMAs).
+template <typename Mid>
+__device__ __forceinline__ void field(const float* zin, float (*dx)[2], float beta, float inv_w_scale, const float* b_bias,
+                                      uint32_t b_tile, int q, float* kv, Mid mid) {
+    const bool odd = q & 1, upper = q >> 1;
+    // Each row scaled by its own power of two so that max(|z|, bias floor) lands in [2^13, 2^14), split into FP16
+    // hi + lo A fragments [k step][4]; the inverse scales are folded into dX/dt.
+    float rs[2];
+    uint32_t ahi[2][4], alo[2][4];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        float m = beta;
+#pragma unroll
+        for (int h = 0; h < 8; ++h) m = fmaxf(m, fabsf(zin[8 * r + h]));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        const int e = min(max(exponent_of(m), 30), 224);
+        rs[r] = pow2_biased(127 + 13 - (e - 127));
+        const float inv = pow2_biased(127 - 13 + (e - 127)) * inv_w_scale;
+        dx[r][0] = __fmul_rn(dx[r][0], inv);
+        dx[r][1] = __fmul_rn(dx[r][1], inv);
+    }
+#pragma unroll
+    for (int k = 0; k < 2; ++k)
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {                     // register t: row t & 1, columns 16 k + 8 (t >> 1) + 2q, +1
+            const int r = t & 1, v = 8 * r + 4 * k + 2 * (t >> 1);
+            const float s0 = __fmul_rn(zin[v], rs[r]), s1 = __fmul_rn(zin[v + 1], rs[r]);
+            float h0, h1;
+            ahi[k][t] = pack_h2(s0, s1);
+            unpack_h2(ahi[k][t], h0, h1);
+            alo[k][t] = pack_h2(__fsub_rn(s0, h0), __fsub_rn(s1, h1));
+        }
+
+    float acc[2][kAcc];
+    auto issue = [&](int chunk, float* d) {
+#pragma unroll
+        for (int j = 0; j < kN / 8; ++j) {                // bias of columns 8 (4 chunk + j) + 2q, +1 times the row scales
+            const float2 bb = *reinterpret_cast<const float2*>(b_bias + chunk * kN + 8 * j + 2 * q);
+            d[4 * j + 0] = bb.x * rs[0]; d[4 * j + 1] = bb.y * rs[0];
+            d[4 * j + 2] = bb.x * rs[1]; d[4 * j + 3] = bb.y * rs[1];
+        }
+        mma_fence();
+        const uint32_t rows = b_tile + chunk * kN * 128;
+        mma_m64n32k16(d, alo[0], desc_sw128(rows + 0));    // z_lo . W_hi
+        mma_m64n32k16(d, alo[1], desc_sw128(rows + 32));
+        mma_m64n32k16(d, ahi[0], desc_sw128(rows + 64));   // z_hi . W_lo
+        mma_m64n32k16(d, ahi[1], desc_sw128(rows + 96));
+        mma_m64n32k16(d, ahi[0], desc_sw128(rows + 0));    // z_hi . W_hi
+        mma_m64n32k16(d, ahi[1], desc_sw128(rows + 32));
+        mma_commit();
+    };
+    float u_even[2][2];
+    issue(0, acc[0]);
+#pragma unroll
+    for (int c = 0; c < kChunks; ++c) {
+        float* d = acc[c & 1];
+        if (c + 1 < kChunks) {
+            issue(c + 1, acc[(c + 1) & 1]);
+            mma_wait<1>();
+        } else {
+            mma_wait<0>();
+        }
+        pin(d);
+        if (c == kChunks / 2) mid();
+        // partial contraction of the lane's two channels for hidden units 4c + j, rows g and g + 8
+        float p[4][2];
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) p[j][r] = fmaf(d[4 * j + 2 * r + 1], dx[r][1], __fmul_rn(d[4 * j + 2 * r], dx[r][0]));
+        // xor 1: keep the hidden units whose owner has the parity of q (4c + 2 (q & 1) + e)
+        float u[2][2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const float got = __shfl_xor_sync(0xffffffffu, odd ? p[e][r] : p[2 + e][r], 1);
+                u[e][r] = (odd ? p[2 + e][r] : p[e][r]) + got;
+            }
+        if ((c & 1) == 0) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) u_even[e][r] = u[e][r];
+        } else {
+            // xor 2: lanes 0, 1 keep the even chunk's units, lanes 2, 3 the odd chunk's: 8 (c >> 1) + 2q + e
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const float got = __shfl_xor_sync(0xffffffffu, upper ? u_even[e][r] : u[e][r], 2);
+                    kv[8 * r + 2 * (c >> 1) + e] = (upper ? u[e][r] : u_even[e][r]) + got;
+                }
+        }
+    }
+}
+
 }  // namespace wg
 
-template <bool DUMP>
+// REV: reversible Heun (rev_heun_combine, checkpoints through the stage-dump pointer) instead of the Runge-Kutta methods
+template <bool DUMP, bool REV>
 __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const UmmaArgs a) {
     using S = BSmem<1>;
     using E = exact<float>;
@@ -330,8 +488,7 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
 
     const float* b_bias = reinterpret_cast<const float*>(smem + S::bias);
     const uint32_t b_tile = smem_u32(smem + S::tile);
-    const bool odd = q & 1, upper = q >> 1;
-    const int n_st = a.n_steps * a.n_stages;
+    const int n_st = a.n_steps * a.n_stages + (REV ? 1 : 0);
     // dX/dt (interpolation_cubic.py:331-336) of a stage at fraction fr of its interval, channels 2q, 2q + 1 of both rows
     auto slope = [&](const float2 (*raw)[3], float fr, float (*dx)[2]) {
 #pragma unroll
@@ -355,7 +512,7 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
     int step = 0, sub = 0;
     float dt = a.step_dt[0];
     for (int st = 0; st < n_st; ++st) {
-        if (DUMP) {
+        if (DUMP && !REV) {
             store_rows(dump_at, 1, 0, zin);
             dump_at += a.n_paths * kHid;
         }
@@ -364,99 +521,21 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
         float dx_next[2][2];
         if (st + 1 < n_st) fetch(a.stage_index[st + 1], nxt);
 
-        // Each row scaled by its own power of two so that max(|z|, bias floor) lands in [2^13, 2^14), split into FP16
-        // hi + lo A fragments [k step][4]; the inverse scales are folded into dX/dt.
-        float rs[2];
-        uint32_t ahi[2][4], alo[2][4];
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-            float m = beta;
-#pragma unroll
-            for (int h = 0; h < 8; ++h) m = fmaxf(m, fabsf(zin[8 * r + h]));
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
-            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-            const int e = min(max(exponent_of(m), 30), 224);
-            rs[r] = pow2_biased(127 + 13 - (e - 127));
-            const float inv = pow2_biased(127 - 13 + (e - 127)) * inv_w_scale;
-            dx[r][0] = __fmul_rn(dx[r][0], inv);
-            dx[r][1] = __fmul_rn(dx[r][1], inv);
-        }
-#pragma unroll
-        for (int k = 0; k < 2; ++k)
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {                     // register t: row t & 1, columns 16 k + 8 (t >> 1) + 2q, +1
-                const int r = t & 1, v = 8 * r + 4 * k + 2 * (t >> 1);
-                const float s0 = __fmul_rn(zin[v], rs[r]), s1 = __fmul_rn(zin[v + 1], rs[r]);
-                float h0, h1;
-                ahi[k][t] = pack_h2(s0, s1);
-                unpack_h2(ahi[k][t], h0, h1);
-                alo[k][t] = pack_h2(__fsub_rn(s0, h0), __fsub_rn(s1, h1));
-            }
+        float kv[wg::kNV];
+        wg::field(zin, dx, beta, inv_w_scale, b_bias, b_tile, q, kv, [&] {
+            if (st + 1 < n_st) slope(nxt, a.stage_frac[st + 1], dx_next);
+        });
 
-        float acc[2][wg::kAcc];
-        auto issue = [&](int chunk, float* d) {
-#pragma unroll
-            for (int j = 0; j < wg::kN / 8; ++j) {                // bias of columns 8 (4 chunk + j) + 2q, +1 times the row scales
-                const float2 bb = *reinterpret_cast<const float2*>(b_bias + chunk * wg::kN + 8 * j + 2 * q);
-                d[4 * j + 0] = bb.x * rs[0]; d[4 * j + 1] = bb.y * rs[0];
-                d[4 * j + 2] = bb.x * rs[1]; d[4 * j + 3] = bb.y * rs[1];
-            }
-            wg::mma_fence();
-            const uint32_t rows = b_tile + chunk * wg::kN * 128;
-            wg::mma_m64n32k16(d, alo[0], wg::desc_sw128(rows + 0));    // z_lo . W_hi
-            wg::mma_m64n32k16(d, alo[1], wg::desc_sw128(rows + 32));
-            wg::mma_m64n32k16(d, ahi[0], wg::desc_sw128(rows + 64));   // z_hi . W_lo
-            wg::mma_m64n32k16(d, ahi[1], wg::desc_sw128(rows + 96));
-            wg::mma_m64n32k16(d, ahi[0], wg::desc_sw128(rows + 0));    // z_hi . W_hi
-            wg::mma_m64n32k16(d, ahi[1], wg::desc_sw128(rows + 32));
-            wg::mma_commit();
-        };
-        float kv[wg::kNV], u_even[2][2];
-        issue(0, acc[0]);
-#pragma unroll
-        for (int c = 0; c < wg::kChunks; ++c) {
-            float* d = acc[c & 1];
-            if (c + 1 < wg::kChunks) {
-                issue(c + 1, acc[(c + 1) & 1]);
-                wg::mma_wait<1>();
-            } else {
-                wg::mma_wait<0>();
-            }
-            wg::pin(d);
-            if (c == wg::kChunks / 2 && st + 1 < n_st) slope(nxt, a.stage_frac[st + 1], dx_next);
-            // partial contraction of the lane's two channels for hidden units 4c + j, rows g and g + 8
-            float p[4][2];
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-#pragma unroll
-                for (int r = 0; r < 2; ++r) p[j][r] = fmaf(d[4 * j + 2 * r + 1], dx[r][1], __fmul_rn(d[4 * j + 2 * r], dx[r][0]));
-            // xor 1: keep the hidden units whose owner has the parity of q (4c + 2 (q & 1) + e)
-            float u[2][2];
-#pragma unroll
-            for (int e = 0; e < 2; ++e)
-#pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    const float got = __shfl_xor_sync(0xffffffffu, odd ? p[e][r] : p[2 + e][r], 1);
-                    u[e][r] = (odd ? p[2 + e][r] : p[e][r]) + got;
-                }
-            if ((c & 1) == 0) {
-#pragma unroll
-                for (int e = 0; e < 2; ++e)
-#pragma unroll
-                    for (int r = 0; r < 2; ++r) u_even[e][r] = u[e][r];
-            } else {
-                // xor 2: lanes 0, 1 keep the even chunk's units, lanes 2, 3 the odd chunk's: 8 (c >> 1) + 2q + e
-#pragma unroll
-                for (int e = 0; e < 2; ++e)
-#pragma unroll
-                    for (int r = 0; r < 2; ++r) {
-                        const float got = __shfl_xor_sync(0xffffffffu, upper ? u_even[e][r] : u[e][r], 2);
-                        kv[8 * r + 2 * (c >> 1) + e] = (upper ? u[e][r] : u_even[e][r]) + got;
-                    }
-            }
-        }
-
-        if (rk_combine<wg::kNV>(a, sub, dt, y, k1, s23, kv, zin)) {
+        if (REV) {
+            rev_heun_combine<wg::kNV>(a, st, step, dt, y, k1, s23, kv, zin, jn, write_out,
+                                      [&](int slot, const float* vy, const float* vz, const float* vf) {
+                                          if (!DUMP) return;
+                                          float* base = a.stage_dump + (int64_t)slot * 3 * a.n_paths * kHid;
+                                          store_rows(base, 1, 0, vy);
+                                          store_rows(base + a.n_paths * kHid, 1, 0, vz);
+                                          store_rows(base + 2 * a.n_paths * kHid, 1, 0, vf);
+                                      });
+        } else if (rk_combine<wg::kNV>(a, sub, dt, y, k1, s23, kv, zin)) {
             step_outputs<wg::kNV>(a, step, jn, next_out, y, zin, write_out);
 #pragma unroll
             for (int h = 0; h < wg::kNV; ++h) y[h] = zin[h];
@@ -471,12 +550,174 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
     }
 }
 
+
+// ---- the reversible Heun backward: one launch per checkpoint segment ---------------------------------------------------
+//
+// The transpose of rev_heun_combine, run backwards over the steps m = hi - 1 .. lo of one segment in the wgmma fragment
+// layout (one warpgroup per 64 paths, the lane's 16 values as in cdeint_wgmma_kernel).  State per lane: y, z, f of step
+// m + 1 and the adjoints ybar, zbar.  Per step:
+//   ybar_m = ybar + 2 zbar + (output gradients on y_m);   fbar_m = ybar dt_m / 2 + zbar dt_m + ybar_m dt_{m-1} / 2;
+//   z_m = 2 y - z - f dt_m (at m = lo: the checkpoint's z);
+//   f_m = F(z_m) with (W, b) and J_F(z_m)^T fbar_m = sum_c dX_c (W2 fbar_m) with the regrouped W2, both wg::field products
+//   at dX/dt(t_m) from two B tiles;  y_m = y - (f_m + f) dt_m / 2 (at m = lo: the checkpoint's y, f);
+//   zbar_m = J^T fbar_m - zbar;
+// and (z_m, fbar_m) go to the segment's dump, which tcde_linear_field_param_grads contracts into dL/dW, dL/db.
+struct RevBwdArgs {
+    const float* control;
+    const float* weight;          // [256][32]
+    const float* bias;            // [256]
+    const float* weight_t;        // W2[(k, c)][h] = W[(h, c)][k]
+    const float* zeros;           // [256] zeros: W2's bias
+    const float* ckpt_lo;         // [3][n_paths][32]: y, z, f of step lo
+    const float* ckpt_hi;         // ... of step hi
+    float* carry;                 // [2][n_paths][32]: ybar, zbar of step hi in, of step lo out
+    const float* g;               // [n_paths][n_out][32] output gradients
+    const int32_t* out_step;      // [n_out]
+    const float* out_weights;     // [2][n_out]: w1, then w0
+    const int32_t* inj_range;     // [N + 1][2]: the outputs [first, end) that touch y_m
+    const float* step_dt;
+    const int32_t* stage_index;   // [N + 1]
+    const float* stage_frac;
+    float* dump_z;                // [hi - lo][n_paths][32]
+    float* dump_a;
+    int64_t n_paths, n_rows;
+    int control_kind, n_out, lo, hi;
+};
+
+constexpr int kRevTile = (BSmem<1>::bytes + 1023) & ~1023;
+constexpr int kRevSmem = 2 * kRevTile + 1024;
+
+__global__ void __launch_bounds__(wg::kThreads, 2) reversible_backward_kernel(const RevBwdArgs a) {
+    using S = BSmem<1>;
+    using E = exact<float>;
+    constexpr int NV = wg::kNV;
+    extern __shared__ unsigned char smem_unaligned[];
+    unsigned char* smem = smem_unaligned + ((1024u - (smem_u32(smem_unaligned) & 1023u)) & 1023u);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
+    float inv_f, beta_f, inv_g, beta_g;
+    prepare_b<1>(smem, a.weight, a.bias, tid, wg::kThreads, inv_f, beta_f);
+    prepare_b<1>(smem + kRevTile, a.weight_t, a.zeros, tid, wg::kThreads, inv_g, beta_g);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    const float* bias_f = reinterpret_cast<const float*>(smem + S::bias);
+    const float* bias_g = reinterpret_cast<const float*>(smem + kRevTile + S::bias);
+    const uint32_t tile_f = smem_u32(smem + S::tile), tile_g = smem_u32(smem + kRevTile + S::tile);
+
+    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
+    const int row_f2 = (cubic ? 4 * kCh : kCh) / 2;
+    int64_t path[2], lpath[2];
+    bool live[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        path[r] = (int64_t)blockIdx.x * wg::kPaths + 16 * warp + g + 8 * r;
+        live[r] = path[r] < a.n_paths;
+        lpath[r] = live[r] ? path[r] : a.n_paths - 1;
+    }
+    auto load_rows = [&](const float* base, int64_t stride_rows, int64_t row_off, float* v) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const float2* src = reinterpret_cast<const float2*>(base + (lpath[r] * stride_rows + row_off) * kHid) + q;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const float2 t = src[4 * i];
+                v[8 * r + 2 * i] = t.x; v[8 * r + 2 * i + 1] = t.y;
+            }
+        }
+    };
+    auto store_rows = [&](float* base, const float* v) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            if (!live[r]) continue;
+            float2* dst = reinterpret_cast<float2*>(base + path[r] * kHid) + q;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) dst[4 * i] = make_float2(v[8 * r + 2 * i], v[8 * r + 2 * i + 1]);
+        }
+    };
+    // dX/dt of evaluation point m: channels 2q, 2q + 1 of both rows
+    auto slope_at = [&](int m, float (*dx)[2]) {
+        const int interval = a.stage_index[m];
+        const float fr = a.stage_frac[m];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const float2* src = reinterpret_cast<const float2*>(a.control + (lpath[r] * a.n_rows + interval) * (2 * row_f2) +
+                                                                (cubic ? kCh : 0)) + q;
+            const float2 b = __ldg(src);
+            if (cubic) {
+                const float2 c2 = __ldg(src + 4), d3 = __ldg(src + 8);
+                dx[r][0] = E::add(b.x, E::mul(E::add(c2.x, E::mul(d3.x, fr)), fr));
+                dx[r][1] = E::add(b.y, E::mul(E::add(c2.y, E::mul(d3.y, fr)), fr));
+            } else {
+                dx[r][0] = b.x;
+                dx[r][1] = b.y;
+            }
+        }
+    };
+
+    const int64_t plane = a.n_paths;
+    float y[NV], z[NV], f[NV], yb[NV], zb[NV];
+    load_rows(a.ckpt_hi, 1, 0, y);
+    load_rows(a.ckpt_hi + plane * kHid, 1, 0, z);
+    load_rows(a.ckpt_hi + 2 * plane * kHid, 1, 0, f);
+    load_rows(a.carry, 1, 0, yb);
+    load_rows(a.carry + plane * kHid, 1, 0, zb);
+    for (int m = a.hi - 1; m >= a.lo; --m) {
+        const float d = a.step_dt[m], dp = m > 0 ? a.step_dt[m - 1] : 0.f;
+        const float hd = E::mul(0.5f, d), hdp = E::mul(0.5f, dp);
+        float ybm[NV], fb[NV], zm[NV];
+#pragma unroll
+        for (int h = 0; h < NV; ++h) ybm[h] = E::add(yb[h], E::mul(2.f, zb[h]));
+        for (int j = a.inj_range[2 * m]; j < a.inj_range[2 * m + 1]; ++j) {
+            const int os = a.out_step[j];
+            const float w = (os == m) ? a.out_weights[a.n_out + j] : (os < 0 ? 1.f : a.out_weights[j]);
+            float gv[NV];
+            load_rows(a.g, a.n_out, j, gv);
+#pragma unroll
+            for (int h = 0; h < NV; ++h) ybm[h] = fmaf(w, gv[h], ybm[h]);
+        }
+#pragma unroll
+        for (int h = 0; h < NV; ++h) fb[h] = E::add(E::add(E::mul(yb[h], hd), E::mul(zb[h], d)), E::mul(ybm[h], hdp));
+        if (m == a.lo) {
+            load_rows(a.ckpt_lo + plane * kHid, 1, 0, zm);
+        } else {
+#pragma unroll
+            for (int h = 0; h < NV; ++h) zm[h] = E::sub(E::sub(E::mul(2.f, y[h]), z[h]), E::mul(f[h], d));
+        }
+        float dxf[2][2], dxg[2][2];
+        slope_at(m, dxf);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) { dxg[r][0] = dxf[r][0]; dxg[r][1] = dxf[r][1]; }
+        float kf[NV], kg[NV];
+        wg::field(zm, dxf, beta_f, inv_f, bias_f, tile_f, q, kf, [] {});
+        wg::field(fb, dxg, beta_g, inv_g, bias_g, tile_g, q, kg, [] {});
+        store_rows(a.dump_z + (int64_t)(m - a.lo) * plane * kHid, zm);
+        store_rows(a.dump_a + (int64_t)(m - a.lo) * plane * kHid, fb);
+        if (m == a.lo) {
+            load_rows(a.ckpt_lo, 1, 0, y);
+            load_rows(a.ckpt_lo + 2 * plane * kHid, 1, 0, f);
+        } else {
+#pragma unroll
+            for (int h = 0; h < NV; ++h) {
+                y[h] = E::sub(y[h], E::mul(E::add(kf[h], f[h]), hd));
+                f[h] = kf[h];
+            }
+        }
+#pragma unroll
+        for (int h = 0; h < NV; ++h) {
+            z[h] = zm[h];
+            zb[h] = E::sub(kg[h], zb[h]);
+            yb[h] = ybm[h];
+        }
+    }
+    store_rows(a.carry, yb);
+    store_rows(a.carry + plane * kHid, zb);
+}
+
 }  // namespace tc
 
 bool solve_tc_supported(int H, int C) { return H == tc::kHid && C == tc::kCh; }
 
-template <typename Kernel>
-static int launch(Kernel kern, int64_t grid, int threads, int smem, const UmmaArgs& a, cudaStream_t stream) {
+template <typename Kernel, typename Args>
+static int launch(Kernel kern, int64_t grid, int threads, int smem, const Args& a, cudaStream_t stream) {
     TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
     TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     kern<<<(unsigned)grid, threads, smem, stream>>>(a);
@@ -492,12 +733,46 @@ int solve_tc_f32(const UmmaArgs& a, int H, int C, int mode, cudaStream_t stream)
     TCDE_CHECK_SUPPORTED(a.stage_dump == nullptr || (reinterpret_cast<uintptr_t>(a.stage_dump) & 15) == 0,
                          "tensor-core solve: the stage dump must be 16-byte aligned");
     // mode: bit 0 = operand split (0 = 3xTF32, 1 = 2xFP16)
+    const bool rev = (a.method == TCDE_REVERSIBLE_HEUN);
     if (mode & 1)
-        return launch(a.stage_dump ? tc::cdeint_wgmma_kernel<true> : tc::cdeint_wgmma_kernel<false>,
+        return launch(rev ? (a.stage_dump ? tc::cdeint_wgmma_kernel<true, true> : tc::cdeint_wgmma_kernel<false, true>)
+                          : (a.stage_dump ? tc::cdeint_wgmma_kernel<true, false> : tc::cdeint_wgmma_kernel<false, false>),
                       (a.n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths, tc::wg::kThreads, tc::wg::kSmem, a, stream);
-    return launch(a.stage_dump ? tc::cdeint_tc_kernel<true> : tc::cdeint_tc_kernel<false>,
+    return launch(rev ? (a.stage_dump ? tc::cdeint_tc_kernel<true, true> : tc::cdeint_tc_kernel<false, true>)
+                      : (a.stage_dump ? tc::cdeint_tc_kernel<true, false> : tc::cdeint_tc_kernel<false, false>),
                   (a.n_paths + tc::kThreads - 1) / tc::kThreads, tc::kThreads,
                   tc::Smem::total + 128, a, stream);               // slack for the 128-byte alignment of the tiles
 }
 
 }  // namespace tcde
+
+extern "C" int tcde_reversible_heun_linear_backward_segment(
+    const void* control, int control_kind, int64_t n_rows, const void* weight, const void* bias, const void* weight_t,
+    const void* zeros, const void* ckpt_lo, const void* ckpt_hi, void* carry, const void* g, int64_t n_out,
+    const int32_t* out_step, const void* out_weights, const int32_t* inj_range, const void* step_dt,
+    const int32_t* stage_index, const void* stage_frac, int64_t lo, int64_t hi, int64_t n_paths, int64_t channels,
+    int64_t hidden, void* dump_z, void* dump_a, int dtype, void* stream) {
+    using namespace tcde;
+    TCDE_CHECK_ARG(control && weight && bias && weight_t && zeros && ckpt_lo && ckpt_hi && carry && g && dump_z && dump_a,
+                   "null data pointer");
+    TCDE_CHECK_ARG(out_step && out_weights && inj_range && step_dt && stage_index && stage_frac, "null schedule pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_out >= 1 && lo >= 0 && hi > lo && hi < (1ll << 31), "bad sizes");
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && solve_tc_supported((int)hidden, (int)channels),
+                         "the reversible backward kernel is built for fp32, hidden=32, channels=8 (got dtype=%d, "
+                         "hidden=%lld, channels=%lld)", dtype, (long long)hidden, (long long)channels);
+    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(ckpt_lo) |
+                           reinterpret_cast<uintptr_t>(ckpt_hi) | reinterpret_cast<uintptr_t>(carry) |
+                           reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(dump_z) |
+                           reinterpret_cast<uintptr_t>(dump_a)) & 15) == 0,
+                         "reversible backward: buffers must be 16-byte aligned");
+    if (n_paths == 0) return TCDE_OK;
+    tc::RevBwdArgs a{(const float*)control, (const float*)weight, (const float*)bias, (const float*)weight_t,
+                     (const float*)zeros, (const float*)ckpt_lo, (const float*)ckpt_hi, (float*)carry, (const float*)g,
+                     out_step, (const float*)out_weights, inj_range, (const float*)step_dt, stage_index,
+                     (const float*)stage_frac, (float*)dump_z, (float*)dump_a, n_paths, n_rows, control_kind, (int)n_out,
+                     (int)lo, (int)hi};
+    return launch(tc::reversible_backward_kernel, (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths, tc::wg::kThreads,
+                  tc::kRevSmem, a, static_cast<cudaStream_t>(stream));
+}

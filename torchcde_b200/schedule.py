@@ -39,9 +39,10 @@ class Schedule:
         """Pack into two device tensors (one float, one int32) and return them with the views."""
         floats = torch.cat([self.step_dt, self.stage_frac.reshape(-1), self.out_slope]).to(device)
         ints = torch.cat([self.stage_index.reshape(-1), self.out_step, self.out_mode]).to(device)
-        ns, nst, no = self.n_steps, self.n_steps * self.n_stages, self.n_out
+        # (a reversible Heun schedule has one evaluation point more than steps and two output weights per output)
+        ns, nst, no, nw = self.n_steps, self.stage_index.numel(), self.n_out, self.out_slope.numel()
         views = {
-            "step_dt": floats[:ns], "stage_frac": floats[ns:ns + nst], "out_slope": floats[ns + nst:ns + nst + no],
+            "step_dt": floats[:ns], "stage_frac": floats[ns:ns + nst], "out_slope": floats[ns + nst:ns + nst + nw],
             "stage_index": ints[:nst], "out_step": ints[nst:nst + no], "out_mode": ints[nst + no:nst + 2 * no],
         }
         return floats, ints, views
@@ -149,6 +150,67 @@ def build_schedule(t, knots, n_intervals, method, step_size, state_dtype):
     s.out_step, s.out_mode, s.out_slope = out_step, out_mode, out_slope
     s.grid = grid
     s.stage_times = stages
+    return s
+
+
+def build_sde_schedule(t, knots, n_intervals, dt, state_dtype):
+    """The schedule of torchsde's fixed-step ``integrate`` loop with the reversible Heun method, in the table format of
+    ``build_schedule`` (``tcde_cdeint_reversible_heun_linear`` reads it):
+
+      * the grid is made by repeated addition in ``t``'s dtype, ``next_t = min(curr_t + dt, t[-1])``, stepping on across
+        the output times; the last step is clipped and may be very small;
+      * ``stage_index`` / ``stage_frac`` locate the ``N + 1`` evaluation points ``t_0 .. t_N`` (the prologue f(t_0, y_0),
+        then one evaluation at the end of every step), cast to the coefficient dtype like ``_interpret_t``;
+      * output ``j > 0`` is torchsde's ``linear_interp`` between the two grid states that bracket ``t[j]``,
+        ``w0 * y_n + w1 * y_{n+1}`` with ``w0 = (t_{n+1} - t[j]) / dt_n`` and ``w1 = (t[j] - t_n) / dt_n`` formed in ``t``'s
+        dtype; ``out_step[j] = n`` and ``out_slope`` holds ``[w1 of every output, w0 of every output]``; output 0 is
+        ``y_0`` (``out_step = -1``).
+
+    ``t`` must be 1-D and strictly increasing (torchsde integrates forwards only)."""
+    t = t.detach().cpu()
+    knots = knots.detach().cpu()
+    if t.dim() != 1 or t.numel() < 2:
+        raise ValueError("t must be one dimensional with at least two entries.")
+    if not t.is_floating_point():
+        raise ValueError("t must be floating point.")
+    if not bool((t[1:] > t[:-1]).all()):
+        raise ValueError("torchsde backend: t must be strictly increasing")
+    dt = float(dt)
+    if not dt > 0:
+        raise ValueError("torchsde backend: dt must be positive, got {}".format(dt))
+    end = t[-1]
+    grid = [t[0]]
+    curr = t[0]
+    n_out = t.numel()
+    out_step = torch.full((n_out,), -1, dtype=torch.int32)
+    w0 = torch.zeros(n_out, dtype=t.dtype)
+    w1 = torch.zeros(n_out, dtype=t.dtype)
+    for j in range(1, n_out):
+        out_t = t[j]
+        while curr < out_t:
+            curr = min(curr + dt, end)
+            grid.append(curr)
+        t0, t1 = grid[-2], grid[-1]
+        out_step[j] = len(grid) - 2
+        w0[j] = (t1 - out_t) / (t1 - t0)
+        w1[j] = (out_t - t0) / (t1 - t0)
+    grid = torch.stack(grid)
+    frac, index = locate(knots, grid.to(knots.dtype), n_intervals)
+
+    s = Schedule()
+    s.method = "reversible_heun"
+    s.n_steps = grid.numel() - 1
+    s.n_stages = 1
+    s.n_out = n_out
+    s.sign = 1.0
+    s.step_dt = (grid[1:] - grid[:-1]).to(state_dtype).contiguous()
+    s.stage_index = index.to(torch.int32).contiguous()
+    s.stage_frac = frac.to(state_dtype).contiguous()
+    s.out_step = out_step
+    s.out_mode = torch.zeros(n_out, dtype=torch.int32)
+    s.out_slope = torch.cat([w1, w0]).to(state_dtype).contiguous()
+    s.grid = grid
+    s.stage_times = grid
     return s
 
 

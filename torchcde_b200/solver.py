@@ -322,6 +322,11 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     that is exactly one ``nn.Linear`` + ``view``) the solve is one fused CUDA kernel.  Gradients:
     ``adjoint=True`` runs this package's continuous-adjoint backward (fused kernels for the linear
     field), ``adjoint=False`` backpropagates through the differentiable generic stage loop.
+
+    ``backend="torchsde"`` is built for ``method="reversible_heun"`` (torchsde's reversible Heun
+    method with zero diffusion, fixed step ``dt``, default 1e-3; ``z0`` of shape (batch, hidden),
+    increasing ``t``).  ``adjoint=True`` gives the exact gradient of the discrete solve by running it
+    backwards algebraically from checkpoints (``reversible.py``); ``t`` receives no gradient.
     """
     # Reduce the default values for the tolerances because CDEs are difficult to solve with the default high tolerances.
     if 'atol' not in kwargs:
@@ -342,8 +347,10 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     if not isinstance(z0, torch.Tensor):
         raise ValueError("z0 must either a tensor or a tuple/list of tensors.")
     if backend == "torchsde":
-        raise NotImplementedError("torchcde_b200.cdeint: the torchsde backend is out of scope (SURVEY.md section 2, "
-                                  "row 8); use backend='torchdiffeq' semantics with a fixed-step method.")
+        if not isinstance(t, torch.Tensor):
+            t = torch.as_tensor(t)
+        from .reversible import cdeint_reversible        # (reversible.py builds on this module's helpers)
+        return cdeint_reversible(X, func, z0, t, adjoint, kwargs)
     if backend != "torchdiffeq":
         raise ValueError(f"Unrecognised backend={backend}")
 
