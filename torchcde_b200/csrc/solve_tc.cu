@@ -273,20 +273,21 @@ __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a
 // warp w owns rows 16 w + g and 16 w + g + 8 (the rows of its A and accumulator fragments) and, of each of these rows, the
 // hidden units 8 i + 2 q + e (i < 4, e < 2): exactly the columns of the A fragment of the next stage, so the operand is
 // built in registers from the Runge-Kutta state.  Its 16 values of a state vector sit at index 8 r + 2 i + e (r = row).
-// The product runs in chunks of kN = 32 output columns (four hidden units x eight channels): z_lo.W_hi, z_hi.W_lo and
-// z_hi.W_hi (small terms first) are six m64n32k16 wgmmas onto an accumulator that starts at the scaled bias, with A from
+// The product runs in chunks of kN = 64 output columns (eight hidden units x eight channels): z_lo.W_hi, z_hi.W_lo and
+// z_hi.W_hi (small terms first) are six m64n64k16 wgmmas onto an accumulator that starts at the scaled bias, with A from
 // registers and B (prepare_b<1>'s [256 rows][hi 32 | lo 32] halves, 128-byte swizzled) through one shared-memory
 // descriptor per product and k step.  Two accumulators alternate: the chunk after the current one is in flight on the
-// tensor core while the current one is contracted with dX/dt.  A contraction leaves each lane with the partial sums of its
-// two channels; a reduce-scatter over the quad (xor 1 after every chunk, xor 2 after every pair of chunks) hands each lane
-// the sums of the hidden units it owns, added in the order (q, q ^ 1) + (q ^ 2, q ^ 3).
+// tensor core while the current one is contracted with dX/dt.  Chunk c holds hidden units 8c .. 8c + 7, so it reduces on
+// its own: the contraction leaves each lane with the partial sums of its two channels, and a reduce-scatter over the quad
+// (xor 1, then xor 2) hands each lane the sums of its units 8c + 2q + e, added in the order (q, q ^ 1) + (q ^ 2, q ^ 3).
+// N = 64 issues half the wgmmas of N = 32 for the same flops; scripts/wgmma_probe.py measures what that saves.
 
 namespace wg {
 
 constexpr int kThreads = 128;                    // one warpgroup
 constexpr int kPaths = 64;                       // the M of the wgmma tile
 constexpr int kNV = 16;                          // state values per lane: 2 rows x 8 hidden units
-constexpr int kN = 32;                           // output columns per chunk
+constexpr int kN = 64;                           // output columns per chunk: hidden units 8c .. 8c + 7
 constexpr int kChunks = kCols / kN;
 constexpr int kAcc = kN / 2;                     // accumulator registers per chunk
 constexpr int kSmem = BSmem<1>::bytes + 1024;    // slack for the 1024-byte alignment of the swizzled B tile
@@ -296,13 +297,16 @@ __device__ __forceinline__ uint64_t desc_sw128(uint32_t addr) {
     return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 
-__device__ __forceinline__ void mma_m64n32k16(float* d, const uint32_t* a, uint64_t b) {
+__device__ __forceinline__ void mma_m64n64k16(float* d, const uint32_t* a, uint64_t b) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
 }
 __device__ __forceinline__ void mma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -353,22 +357,21 @@ __device__ __forceinline__ void field(const float* zin, float (*dx)[2], float be
     float acc[2][kAcc];
     auto issue = [&](int chunk, float* d) {
 #pragma unroll
-        for (int j = 0; j < kN / 8; ++j) {                // bias of columns 8 (4 chunk + j) + 2q, +1 times the row scales
+        for (int j = 0; j < kN / 8; ++j) {                // bias of columns 8 (8 chunk + j) + 2q, +1 times the row scales
             const float2 bb = *reinterpret_cast<const float2*>(b_bias + chunk * kN + 8 * j + 2 * q);
             d[4 * j + 0] = bb.x * rs[0]; d[4 * j + 1] = bb.y * rs[0];
             d[4 * j + 2] = bb.x * rs[1]; d[4 * j + 3] = bb.y * rs[1];
         }
         mma_fence();
         const uint32_t rows = b_tile + chunk * kN * 128;
-        mma_m64n32k16(d, alo[0], desc_sw128(rows + 0));    // z_lo . W_hi
-        mma_m64n32k16(d, alo[1], desc_sw128(rows + 32));
-        mma_m64n32k16(d, ahi[0], desc_sw128(rows + 64));   // z_hi . W_lo
-        mma_m64n32k16(d, ahi[1], desc_sw128(rows + 96));
-        mma_m64n32k16(d, ahi[0], desc_sw128(rows + 0));    // z_hi . W_hi
-        mma_m64n32k16(d, ahi[1], desc_sw128(rows + 32));
+        mma_m64n64k16(d, alo[0], desc_sw128(rows + 0));    // z_lo . W_hi
+        mma_m64n64k16(d, alo[1], desc_sw128(rows + 32));
+        mma_m64n64k16(d, ahi[0], desc_sw128(rows + 64));   // z_hi . W_lo
+        mma_m64n64k16(d, ahi[1], desc_sw128(rows + 96));
+        mma_m64n64k16(d, ahi[0], desc_sw128(rows + 0));    // z_hi . W_hi
+        mma_m64n64k16(d, ahi[1], desc_sw128(rows + 32));
         mma_commit();
     };
-    float u_even[2][2];
     issue(0, acc[0]);
 #pragma unroll
     for (int c = 0; c < kChunks; ++c) {
@@ -381,36 +384,31 @@ __device__ __forceinline__ void field(const float* zin, float (*dx)[2], float be
         }
         pin(d);
         if (c == kChunks / 2) mid();
-        // partial contraction of the lane's two channels for hidden units 4c + j, rows g and g + 8
-        float p[4][2];
+        // partial contraction of the lane's two channels for hidden units 8c + j, rows g and g + 8
+        float p[8][2];
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
+        for (int j = 0; j < 8; ++j)
 #pragma unroll
             for (int r = 0; r < 2; ++r) p[j][r] = fmaf(d[4 * j + 2 * r + 1], dx[r][1], __fmul_rn(d[4 * j + 2 * r], dx[r][0]));
-        // xor 1: keep the hidden units whose owner has the parity of q (4c + 2 (q & 1) + e)
-        float u[2][2];
+        // xor 1: keep the hidden units j with (j >> 1) & 1 == q & 1, that is 8c + 4h + 2 (q & 1) + e
+        float u[2][2][2];
 #pragma unroll
-        for (int e = 0; e < 2; ++e)
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                const float got = __shfl_xor_sync(0xffffffffu, odd ? p[e][r] : p[2 + e][r], 1);
-                u[e][r] = (odd ? p[2 + e][r] : p[e][r]) + got;
-            }
-        if ((c & 1) == 0) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e)
-#pragma unroll
-                for (int r = 0; r < 2; ++r) u_even[e][r] = u[e][r];
-        } else {
-            // xor 2: lanes 0, 1 keep the even chunk's units, lanes 2, 3 the odd chunk's: 8 (c >> 1) + 2q + e
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
             for (int e = 0; e < 2; ++e)
 #pragma unroll
                 for (int r = 0; r < 2; ++r) {
-                    const float got = __shfl_xor_sync(0xffffffffu, upper ? u_even[e][r] : u[e][r], 2);
-                    kv[8 * r + 2 * (c >> 1) + e] = (upper ? u[e][r] : u_even[e][r]) + got;
+                    const float got = __shfl_xor_sync(0xffffffffu, odd ? p[4 * h + e][r] : p[4 * h + 2 + e][r], 1);
+                    u[h][e][r] = (odd ? p[4 * h + 2 + e][r] : p[4 * h + e][r]) + got;
                 }
-        }
+        // xor 2: lanes 0, 1 keep h = 0, lanes 2, 3 h = 1: the units 8c + 2q + e
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const float got = __shfl_xor_sync(0xffffffffu, upper ? u[0][e][r] : u[1][e][r], 2);
+                kv[8 * r + 2 * c + e] = (upper ? u[1][e][r] : u[0][e][r]) + got;
+            }
     }
 }
 
