@@ -194,9 +194,13 @@ TCDE_API int tcde_cdeint_fixed_linear_stages(const void* control, int control_ki
                                     double sign, int dtype, void* stream);
 
 /* torchsde's reversible Heun method with zero diffusion (cdeint(..., backend="torchsde", method="reversible_heun")) for
- * the same linear field, in ONE launch (the CUDA-core kernel, fp32 or fp64, any shape it is built for):
+ * the same linear field, in ONE launch:
  *   z_{n+1} = 2 y_n - z_n + f_n dt_n,  f_{n+1} = f(t_{n+1}, z_{n+1}),  y_{n+1} = y_n + (f_n + f_{n+1}) (0.5 dt_n)
- * starting from z_0 = y_0, f_0 = f(t_0, y_0).  Schedule (torchcde_b200/schedule.py, build_sde_schedule):
+ * starting from z_0 = y_0, f_0 = f(t_0, y_0).  float32 runs the kernel that tcde_set_solve_variant selects, as
+ * tcde_cdeint_fixed_linear does: by default the tensor-core kernel with the 2xFP16 split (warpgroup MMA) at hidden =
+ * 32, channels = 8 when control, z0, out and checkpoints are 16-byte aligned, else the CUDA-core kernel; variant 3 the
+ * 3xTF32 tensor-core kernel; variant 1 the CUDA-core kernel.  float64 runs the CUDA-core kernel, at any shape whose
+ * weights fit its shared memory.  Schedule (torchcde_b200/schedule.py, build_sde_schedule):
  *   step_dt[n_steps]; stage_index / stage_frac[n_steps + 1]: the evaluation points t_0 .. t_N;
  *   out_step[n_out] (-1: output j is y_0); out_weights[2][n_out]: w1 of every output, then w0, and output j is
  *   w0 y_n + w1 y_{n+1} of its step n (torchsde's linear_interp).
@@ -312,8 +316,8 @@ TCDE_API int tcde_logsignature_windows(const void* x, int64_t n_paths, int64_t l
  * but the CTA-per-path natural-cubic kernel instead of the warp-per-path one.  For tests / benchmarks. */
 TCDE_API int tcde_set_natural_variant(int variant);
 
-/* Which kernel tcde_cdeint_fixed_linear launches for float32: 0 = automatic (the tensor-core kernel
- * where it is built for the shape: hidden = 32, channels = 8; the CUDA-core kernel otherwise),
+/* Which kernel tcde_cdeint_fixed_linear and tcde_cdeint_reversible_heun_linear launch for float32: 0 = automatic
+ * (the tensor-core kernel where it is built for the shape: hidden = 32, channels = 8; the CUDA-core kernel otherwise),
  * 1 = CUDA-core kernel, 3 / 4 = tensor-core kernel (solve_tc.cu) with the 3xTF32 / the 2xFP16 operand split
  * (TCDE_ERR_UNSUPPORTED for other shapes); 2 and 6 are aliases of 3, 5 of 4; bits above 15 are ignored.
  * Process-wide; meant for tests and benchmarks. */

@@ -132,13 +132,32 @@ def cubic_derivative(coeffs, knots, t):
     return b + (c2 + d3 * fr) * fr
 
 
-def linear_cde_field(coeffs, knots, weight, bias):
-    """f(t, z) = (weight z + bias).view(H, C) . dX/dt(t) with a cubic control."""
+def linear_derivative(slopes, knots, t):
+    """dX/dt of a piecewise linear control with per-interval rows ``slopes`` at a 0-dim time: ``_interpret_t``'s
+    interval, so a knot t_n (n > 0) takes the slope of interval n - 1.  Like ``_interpret_t`` (and ``cubic_derivative``)
+    the time is cast to the knots' dtype first: pass the knots in the control's dtype to locate times as it does."""
+    tt = t.to(knots.dtype)
+    i = int(torch.bucketize(tt, knots).sub(1).clamp(0, slopes.size(-2) - 1))
+    return slopes[..., i, :]
+
+
+def _product_field(derivative, weight, bias):
     hidden = weight.size(1)
 
     def f(t, z):
-        dx = cubic_derivative(coeffs, knots, t)
+        dx = derivative(t)
         m = torch.nn.functional.linear(z, weight, bias).view(*z.shape[:-1], hidden, -1)
         return (m @ dx.unsqueeze(-1)).squeeze(-1)
 
     return f
+
+
+def linear_cde_field(coeffs, knots, weight, bias):
+    """f(t, z) = (weight z + bias).view(H, C) . dX/dt(t) with a cubic control."""
+    return _product_field(lambda t: cubic_derivative(coeffs, knots, t), weight, bias)
+
+
+def linear_control_field(slopes, knots, weight, bias):
+    """f(t, z) = (weight z + bias).view(H, C) . dX/dt(t) with a linear control given by its own slopes (the ``_derivs``
+    rows of ``LinearInterpolation``); ``bias`` may be None."""
+    return _product_field(lambda t: linear_derivative(slopes, knots, t), weight, bias)

@@ -9,6 +9,7 @@ import scipy.integrate
 import torch
 
 import torchcde_b200 as cde
+from oracle import cde_oracle as O
 from oracle import reversible_oracle as R
 from torchcde_b200 import schedule
 
@@ -34,7 +35,15 @@ def _linear_cubic_field(hidden, channels, length, gen):
     return R.linear_cde_field(coeffs, knots, weight, bias), (weight, bias, coeffs)
 
 
-@pytest.mark.parametrize("field", ["mlp", "linear_cubic"])
+def _linear_linear_field(hidden, channels, length, gen):
+    slopes = (0.3 * torch.randn(3, length - 1, channels, generator=gen, dtype=D)).requires_grad_(True)
+    knots = torch.arange(length, dtype=D)
+    weight = (torch.randn(hidden * channels, hidden, generator=gen, dtype=D) / math.sqrt(hidden)).requires_grad_(True)
+    bias = (0.1 * torch.randn(hidden * channels, generator=gen, dtype=D)).requires_grad_(True)
+    return R.linear_control_field(slopes, knots, weight, bias), (weight, bias, slopes)
+
+
+@pytest.mark.parametrize("field", ["mlp", "linear_cubic", "linear_linear"])
 @pytest.mark.parametrize("checkpoint_every", [None, 4])
 def test_oracle_backward_is_the_gradient_of_its_forward(field, checkpoint_every):
     gen = torch.Generator().manual_seed(3)
@@ -44,9 +53,10 @@ def test_oracle_backward_is_the_gradient_of_its_forward(field, checkpoint_every)
         ts = torch.tensor([0.0, 0.35, 0.4, 1.3, 2.05], dtype=D)
         dt = 0.07
     else:
-        f, params = _linear_cubic_field(hidden, 3, 6, gen)
+        make = _linear_cubic_field if field == "linear_cubic" else _linear_linear_field
+        f, params = make(hidden, 3, 6, gen)
         ts = torch.tensor([0.0, 1.0, 2.5, 4.6, 5.0], dtype=D)
-        dt = 0.3
+        dt = 0.3 if field == "linear_cubic" else 0.5           # 0.5: every other step ends on a knot
     y0 = torch.randn(3, hidden, generator=gen, dtype=D).requires_grad_(True)
     g = torch.randn(ts.numel(), 3, hidden, generator=gen, dtype=D)
     ys, _ = R.integrate(f, y0, ts, dt)
@@ -54,6 +64,32 @@ def test_oracle_backward_is_the_gradient_of_its_forward(field, checkpoint_every)
     got_y0, got_p = R.reversible_backward(f, params, y0.detach(), ts, dt, g, checkpoint_every)
     for w, gg in zip(want, (got_y0,) + tuple(got_p)):
         assert (gg - w).abs().max() <= 1e-10 * w.abs().max()
+
+
+@pytest.mark.parametrize("uneven", [False, True])
+def test_oracle_linear_control_is_the_pinned_linear_derivative(uneven):
+    """linear_control_field on a control's own slopes against cde_oracle.linear_derivative (pinned to the reference),
+    at every knot, between knots and at both ends: same interval rule, same field."""
+    gen = torch.Generator().manual_seed(9)
+    length, channels, hidden = 7, 3, 4
+    knots = torch.arange(length, dtype=D)
+    if uneven:
+        knots = torch.cat([torch.zeros(1, dtype=D), (0.4 + torch.rand(length - 1, generator=gen, dtype=D)).cumsum(0)])
+    x = torch.randn(2, length, channels, generator=gen, dtype=D)
+    slopes = O.linear_slopes(x, knots)
+    weight = torch.randn(hidden * channels, hidden, generator=gen, dtype=D)
+    bias = torch.randn(hidden * channels, generator=gen, dtype=D)
+    z = torch.randn(2, hidden, generator=gen, dtype=D)
+    f = R.linear_control_field(slopes, knots, weight, bias)
+    mids = (knots[1:] + knots[:-1]) / 2
+    for t in torch.cat([knots, mids, knots[1:] - 1e-9 * (knots[1:] - knots[:-1])]):
+        want_dx = O.linear_derivative(x, knots, t)
+        assert torch.equal(R.linear_derivative(slopes, knots, t), want_dx), float(t)
+        assert torch.equal(f(t, z), O.linear_field(weight, bias, z, want_dx)), float(t)
+    # a knot t_n takes the slope of interval n - 1 (the first knot: interval 0)
+    for n in range(1, length):
+        assert torch.equal(R.linear_derivative(slopes, knots, knots[n]), slopes[:, n - 1])
+    assert torch.equal(R.linear_derivative(slopes, knots, knots[0]), slopes[:, 0])
 
 
 def test_oracle_converges_at_order_two():
