@@ -63,30 +63,85 @@ def test_spline_buffers_are_views_with_reference_names():
     assert [n for n, _ in lin.named_buffers()] == ["_t", "_coeffs", "_derivs"]     # interpolation_linear.py:191-193
 
 
+# the fixed-step schedules of tests/test_gpu_fixed_routes.py on 40 knots: name: (t, step_size, uneven knots)
+FIXED_SCHEDULES = {
+    "F1": ([0.0, 0.5], 1.0, False),                             # one clipped step
+    "F2": (None, None, False),                                  # t = every knot, no step_size
+    "F3": ([0.0, 0.3, 0.35, 0.9, 7.0, 39.0], 1.0, False),       # three outputs inside step 0, outputs on grid points
+    "F4": ([0.0, 9.8], 0.7, False),                             # float32 t: a zero-length last step
+    "F5": ([0.0, 10.0001], 1.0, False),                         # a last step of 1e-4
+    "F6": ([0.0, 7.75, 39.0], 3.0, False),                      # every rk4 stage on a knot
+    "F7": ([0.5, 20.0, 30.1], 2.5, True),                       # uneven knots, steps longer than intervals
+    "F8": ([39.0, 20.5, 3.0, 0.0], 0.5, False),                 # decreasing t
+}
+
+
+def fixed_schedule_knots(uneven, seed=0):
+    """40 float32 knots: 0..39, or widths drawn in [0.6, 1.4)."""
+    if not uneven:
+        return torch.arange(40, dtype=torch.float32)
+    widths = 0.6 + 0.8 * torch.rand(39, generator=torch.Generator().manual_seed(seed), dtype=torch.float64)
+    return torch.cat([torch.zeros(1, dtype=torch.float64), widths.cumsum(0)]).float()
+
+
+_SCHEDULE_CASES = [pytest.param(m, s, None, id="{}-{}".format(m, s)) for m, s in
+                   [("rk4", 1.0), ("rk4", 0.4), ("midpoint", 0.5), ("euler", 0.25), ("rk4", None)]]
+_SCHEDULE_CASES += [pytest.param(m, FIXED_SCHEDULES[n][1], n, id="{}-{}".format(m, n))
+                    for n in FIXED_SCHEDULES for m in ("rk4", "midpoint", "euler")]
+
+
 @pytest.mark.parametrize("dtype_t", [torch.float32, torch.float64])
-@pytest.mark.parametrize("method,step", [("rk4", 1.0), ("rk4", 0.4), ("midpoint", 0.5), ("euler", 0.25), ("rk4", None)])
-def test_schedule_reproduces_the_stage_by_stage_arithmetic(dtype_t, method, step):
+@pytest.mark.parametrize("method,step,sname", _SCHEDULE_CASES)
+def test_schedule_reproduces_the_stage_by_stage_arithmetic(dtype_t, method, step, sname, monkeypatch):
     """Drive the oracle's solver with a recording field and compare every stage's interval and
-    fraction, computed one stage at a time the reference's way, with the batched table."""
-    knots = (torch.rand(12, dtype=torch.float64) + 0.2).cumsum(0).float()
-    lo, hi = float(knots[0]), float(knots[-1])
-    t = torch.tensor([lo, lo + 0.37 * (hi - lo), lo + 0.5 * (hi - lo), hi], dtype=dtype_t)
-    seen = []
+    fraction, computed one stage at a time the reference's way, with the batched table; and every
+    output's step, mode (start / end / interpolated) and slope with where the oracle's ``_between``
+    places it."""
+    if sname is None:
+        knots = (torch.rand(12, dtype=torch.float64) + 0.2).cumsum(0).float()
+        lo, hi = float(knots[0]), float(knots[-1])
+        t = torch.tensor([lo, lo + 0.37 * (hi - lo), lo + 0.5 * (hi - lo), hi], dtype=dtype_t)
+    else:
+        ts, _step, uneven = FIXED_SCHEDULES[sname]
+        knots = fixed_schedule_knots(uneven)
+        t = knots.to(dtype_t) if ts is None else torch.tensor(ts, dtype=dtype_t)
+    n_intervals = knots.numel() - 1
+    n_stages = schedule.N_STAGES[method]
+    seen, placed = [], []
 
     def field(s, y):
-        frac, idx = O.locate(knots, s, 11)
+        frac, idx = O.locate(knots, s, n_intervals)
         seen.append((int(idx), float(frac)))
         return y * 0
 
+    real_between = odeint_port._between
+
+    def between(t0, t1, y0, y1, tj):
+        # called after the stages of the step that ends at t1
+        mode = 0 if tj == t0 else 1 if tj == t1 else 2
+        slope = float(((tj - t0) / (t1 - t0)).to(torch.float32)) if mode == 2 else 0.0
+        placed.append((len(seen) // n_stages - 1, mode, slope))
+        return real_between(t0, t1, y0, y1, tj)
+
+    monkeypatch.setattr(odeint_port, "_between", between)
     options = {} if step is None else {"step_size": step}
     odeint_port.odeint(field, torch.zeros(1), t, method=method, options=options)
-    sched = schedule.build_schedule(t, knots, 11, method, step, torch.float32)
+    sched = schedule.build_schedule(t, knots, n_intervals, method, step, torch.float32)
     flat_idx = sched.stage_index.reshape(-1).tolist()
     flat_frac = sched.stage_frac.reshape(-1).tolist()
-    assert len(seen) == len(flat_idx)
+    assert len(seen) == len(flat_idx) == sched.n_steps * n_stages
     assert [s[0] for s in seen] == flat_idx                 # interval indices: bit exact
     assert [s[1] for s in seen] == flat_frac
-    assert sched.out_step[0] == -1 and sched.n_out == 4
+    assert sched.out_step[0] == -1 and sched.n_out == t.numel()
+    table = list(zip(sched.out_step.tolist(), sched.out_mode.tolist(), sched.out_slope.tolist()))[1:]
+    assert table == placed                                  # output placement: bit exact
+    dts = sched.step_dt.tolist()
+    if sname == "F4" and dtype_t == torch.float32:
+        assert dts[-1] == 0.0 and sched.n_steps == 15       # 14 * 0.7 is 9.8 in float32: the last step has no length
+    if sname == "F5":
+        assert 0 < dts[-1] < 2e-4
+    if sname == "F6" and method == "rk4":
+        assert all(f in (0.0, 1.0) for f in flat_frac)      # every stage on a knot
 
 
 def test_schedule_knot_semantics_and_reversal():

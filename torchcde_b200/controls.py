@@ -70,6 +70,9 @@ def _eval_kernel(control, knots, n_rows, channels, index, frac, kind, derivative
     fr = frac.reshape(-1).to(control.dtype).contiguous()
     n_times = idx.numel()
     out = torch.empty(flat.size(0), n_times, channels, dtype=control.dtype, device=control.device)
+    if out.numel() == 0:
+        # an empty batch has no storage: its null data pointer would be refused as an argument error
+        return out.view(*batch, *tshape, channels)
     with torch.cuda.device(control.device):
         _lib.call("tcde_spline_eval", _lib.ptr(flat), _lib.ptr(knots), _lib.ptr(idx), _lib.ptr(fr), _lib.ptr(out),
                   flat.size(0), n_rows, channels, n_times, kind, int(derivative), code, _lib.stream_of(flat))

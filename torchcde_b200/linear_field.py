@@ -158,7 +158,8 @@ class LinearFieldKernels:
             sched, (_floats, _ints, v) = _schedules.get(t, self.knots, self.n_rows, method, step_size, self.dtype,
                                                         self.device)
             out = torch.empty(zf.size(0), sched.n_out, self.hidden, dtype=self.dtype, device=self.device)
-            self._fixed(sched, v, self.w, self.b, zf, out)
+            if zf.size(0) > 0:            # an empty batch: nothing to launch (its null data pointers would be refused)
+                self._fixed(sched, v, self.w, self.b, zf, out)
         return out.view(*y0.shape[:-1], sched.n_out, self.hidden)
 
     def _fixed(self, sched, v, w, b, z, out, dump=None):
