@@ -193,6 +193,26 @@ TCDE_API int tcde_cdeint_fixed_linear_stages(const void* control, int control_ki
                                     const int32_t* out_step, const int32_t* out_mode, const void* out_slope,
                                     double sign, int dtype, void* stream);
 
+/* The fused fixed-step solve of tcde_cdeint_fixed_linear for the MLP vector field of the reference's examples
+ * (example/time_series_classification.py:20-51, func = Linear(H, W) -> ReLU -> Linear(W, H*C) -> tanh -> view(H, C)):
+ *   f(t, z) = tanh(w2 relu(w1 z + b1) + b2).view(H, C) @ dX/dt(t)
+ * in ONE launch, with the same control, schedule, output and sign arguments.
+ *   w1, b1       Linear(H, W): w1[W][H], b1[W]         (`width` = W; a missing bias is a zero vector)
+ *   w2, b2       Linear(W, H*C): w2[H*C][W], b2[H*C]
+ * float32 runs the kernel that tcde_set_solve_variant selects: by default the tensor-core kernel (2xFP16 warpgroup MMA for
+ * both products, accurate tanhf) at hidden = 32, channels = 8, width = 128 when control, z0 and out are 16-byte aligned,
+ * else the CUDA-core kernel where it beats a stage loop (hidden <= 8 or hidden * channels <= 32; TCDE_ERR_UNSUPPORTED
+ * elsewhere, so that the caller keeps its own loop); variant 1 the CUDA-core kernel at any shape it is built for;
+ * variants 4 / 5 the tensor-core kernel or TCDE_ERR_UNSUPPORTED; variants 2 / 3 / 6 (3xTF32) TCDE_ERR_UNSUPPORTED.
+ * float64 runs the CUDA-core kernel, by default at the same shapes and with variant 1 at any.  The
+ * CUDA-core kernel takes hidden <= 32 and any width (weights in shared memory when they fit, else read from global
+ * memory) and channels whose per-path scratch (C + H values) fits its shared memory; TCDE_ERR_UNSUPPORTED otherwise. */
+TCDE_API int tcde_cdeint_fixed_mlp(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
+                          const void* w2, const void* b2, const void* z0, void* out, int64_t n_paths, int64_t channels,
+                          int64_t hidden, int64_t width, int method, int64_t n_steps, const void* step_dt,
+                          const int32_t* stage_index, const void* stage_frac, int64_t n_out, const int32_t* out_step,
+                          const int32_t* out_mode, const void* out_slope, double sign, int dtype, void* stream);
+
 /* torchsde's reversible Heun method with zero diffusion (cdeint(..., backend="torchsde", method="reversible_heun")) for
  * the same linear field, in ONE launch:
  *   z_{n+1} = 2 y_n - z_n + f_n dt_n,  f_{n+1} = f(t_{n+1}, z_{n+1}),  y_{n+1} = y_n + (f_n + f_{n+1}) (0.5 dt_n)
@@ -316,10 +336,12 @@ TCDE_API int tcde_logsignature_windows(const void* x, int64_t n_paths, int64_t l
  * but the CTA-per-path natural-cubic kernel instead of the warp-per-path one.  For tests / benchmarks. */
 TCDE_API int tcde_set_natural_variant(int variant);
 
-/* Which kernel tcde_cdeint_fixed_linear and tcde_cdeint_reversible_heun_linear launch for float32: 0 = automatic
- * (the tensor-core kernel where it is built for the shape: hidden = 32, channels = 8; the CUDA-core kernel otherwise),
- * 1 = CUDA-core kernel, 3 / 4 = tensor-core kernel (solve_tc.cu) with the 3xTF32 / the 2xFP16 operand split
- * (TCDE_ERR_UNSUPPORTED for other shapes); 2 and 6 are aliases of 3, 5 of 4; bits above 15 are ignored.
+/* Which kernel tcde_cdeint_fixed_linear, tcde_cdeint_reversible_heun_linear and tcde_cdeint_fixed_mlp launch for
+ * float32: 0 = automatic (the tensor-core kernel where it is built for the shape: hidden = 32, channels = 8, and for the
+ * MLP width = 128; the CUDA-core kernel otherwise, for the MLP only at hidden <= 8 or hidden * channels <= 32), 1 =
+ * CUDA-core kernel (for the MLP also in float64 at every shape it is built for), 3 / 4 = tensor-core kernel (solve_tc.cu,
+ * solve_mlp.cu) with the 3xTF32 / the 2xFP16 operand split (TCDE_ERR_UNSUPPORTED for other shapes; the MLP field has
+ * no 3xTF32 kernel); 2 and 6 are aliases of 3, 5 of 4; bits above 15 are ignored.
  * Process-wide; meant for tests and benchmarks. */
 TCDE_API int tcde_set_solve_variant(int variant);
 

@@ -55,6 +55,8 @@ SIGNATURES = {
     "tcde_error_ratio_sumsq": ([_p, _p, _p, _p, _int, _dbl, _dbl, _i64, _int, _p, _p], _int),
     "tcde_cdeint_fixed_linear": ([_p, _int, _i64, _p, _p, _p, _p, _i64, _i64, _i64, _int, _i64, _p, _p, _p, _i64,
                                   _p, _p, _p, _dbl, _int, _p], _int),
+    "tcde_cdeint_fixed_mlp": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _int, _i64, _p, _p, _p,
+                               _i64, _p, _p, _p, _dbl, _int, _p], _int),
     "tcde_dopri5_linear_grid": ([_i64], _int),
     "tcde_dopri5_linear_paired_attempts": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _dbl,
                                             _p, _p, _p, _p, _p, _i64, _i64, _i64, _int, _p], _int),

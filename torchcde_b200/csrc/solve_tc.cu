@@ -13,68 +13,11 @@
 //   * the Runge-Kutta combination in registers, one rounding per operation in the order of oracle/odeint_port.py.
 // The Runge-Kutta state y, k1 and the running k2 + k3 stay in registers for the whole solve.  With a stage dump (the adjoint's
 // stage trajectory) every stage input is also written to HBM.
-#include "tc_common.cuh"
+#include "wg_common.cuh"
 
 namespace tcde {
 
 namespace tc {
-
-// One Runge-Kutta combination on NV state values of the calling thread: kv = the stage's slopes, the next stage input ends
-// up in zin.  Returns true when the stage completed a step.
-template <int NV>
-__device__ __forceinline__ bool rk_combine(const UmmaArgs& a, int sub, float dt, const float* y, float* k1, float* s23,
-                                           const float* kv, float* zin) {
-    using E = exact<float>;
-    const f2 dt2 = pk(dt, dt);
-    if (a.method == TCDE_RK4_38) {
-        const float third = (float)(1.0 / 3.0);
-        const f2 th2 = pk(third, third);
-        if (sub == 0) {
-#pragma unroll
-            for (int h = 0; h < NV; h += 2) {
-                k1[h] = kv[h]; k1[h + 1] = kv[h + 1];
-                upk(add2(pk(y[h], y[h + 1]), mul2(mul2(dt2, pk(kv[h], kv[h + 1])), th2)), zin[h], zin[h + 1]);
-            }
-        } else if (sub == 1) {
-#pragma unroll
-            for (int h = 0; h < NV; h += 2) {
-                s23[h] = kv[h]; s23[h + 1] = kv[h + 1];
-                upk(add2(pk(y[h], y[h + 1]), mul2(dt2, sub2(pk(kv[h], kv[h + 1]), mul2(pk(k1[h], k1[h + 1]), th2)))),
-                    zin[h], zin[h + 1]);
-            }
-        } else if (sub == 2) {
-#pragma unroll
-            for (int h = 0; h < NV; h += 2) {
-                const f2 k2p = pk(s23[h], s23[h + 1]), k3p = pk(kv[h], kv[h + 1]);
-                upk(add2(pk(y[h], y[h + 1]), mul2(dt2, add2(sub2(pk(k1[h], k1[h + 1]), k2p), k3p))), zin[h], zin[h + 1]);
-                upk(add2(k2p, k3p), s23[h], s23[h + 1]);
-            }
-        } else {
-            const f2 three = pk(3.f, 3.f), eighth = pk(0.125f, 0.125f);
-#pragma unroll
-            for (int h = 0; h < NV; h += 2) {
-                const f2 sum = add2(add2(pk(k1[h], k1[h + 1]), mul2(three, pk(s23[h], s23[h + 1]))), pk(kv[h], kv[h + 1]));
-                upk(add2(pk(y[h], y[h + 1]), mul2(mul2(sum, dt2), eighth)), zin[h], zin[h + 1]);
-            }
-            return true;
-        }
-        return false;
-    }
-    if (a.method == TCDE_MIDPOINT) {
-        if (sub == 0) {
-            const float half = E::mul(0.5f, dt);
-#pragma unroll
-            for (int h = 0; h < NV; ++h) zin[h] = E::add(y[h], E::mul(kv[h], half));
-            return false;
-        }
-#pragma unroll
-        for (int h = 0; h < NV; ++h) zin[h] = E::add(y[h], E::mul(dt, kv[h]));
-        return true;
-    }
-#pragma unroll
-    for (int h = 0; h < NV; ++h) zin[h] = E::add(y[h], E::mul(dt, kv[h]));
-    return true;
-}
 
 // torchsde's reversible Heun (zero diffusion) on NV state values: the slots y, f (k1) and z (s23) hold y_n, f_n and the z
 // the current evaluation kv = f(t_st, z) was made at.  Evaluation 0 is the prologue f(t_0, y_0); evaluation st > 0 ends
@@ -114,27 +57,6 @@ __device__ __forceinline__ void rev_heun_combine(const UmmaArgs& a, int st, int&
             f[h] = kv[h];
             z[h] = zin[h];
         }
-    }
-}
-
-// The outputs that fall on the step just completed (y = its start, zin = its end); write(j, v) stores output j.
-template <int NV, typename Write>
-__device__ __forceinline__ void step_outputs(const UmmaArgs& a, int step, int& jn, int& next_out, const float* y,
-                                             const float* zin, Write write) {
-    using E = exact<float>;
-    while (next_out == step) {
-        const int mode = a.out_mode[jn];
-        if (mode == 0) write(jn, y);
-        else if (mode == 1) write(jn, zin);
-        else {
-            const float slope_w = a.out_slope[jn];
-            float v[NV];
-#pragma unroll
-            for (int h = 0; h < NV; ++h) v[h] = E::add(y[h], E::mul(slope_w, E::sub(zin[h], y[h])));
-            write(jn, v);
-        }
-        ++jn;
-        next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
     }
 }
 
@@ -284,47 +206,12 @@ __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a
 
 namespace wg {
 
-constexpr int kThreads = 128;                    // one warpgroup
-constexpr int kPaths = 64;                       // the M of the wgmma tile
-constexpr int kNV = 16;                          // state values per lane: 2 rows x 8 hidden units
-constexpr int kN = 64;                           // output columns per chunk: hidden units 8c .. 8c + 7
-constexpr int kChunks = kCols / kN;
-constexpr int kAcc = kN / 2;                     // accumulator registers per chunk
-constexpr int kSmem = BSmem<1>::bytes + 1024;    // slack for the 1024-byte alignment of the swizzled B tile
-
-// shared-memory matrix descriptor of a K-major, 128-byte-swizzled operand whose 8-row swizzle atoms are 1024 bytes apart
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t addr) {
-    return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
-}
-
-__device__ __forceinline__ void mma_m64n64k16(float* d, const uint32_t* a, uint64_t b) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
-        "%24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
-          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
-          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
-}
-__device__ __forceinline__ void mma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void mma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-template <int N> __device__ __forceinline__ void mma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
-// keeps the compiler from moving reads or writes of an accumulator across the asynchronous MMAs that own it
-__device__ __forceinline__ void pin(float* d) {
-#pragma unroll
-    for (int i = 0; i < kAcc; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-
 // One evaluation of the linear field for the warpgroup's 64 rows: kv = (W zin + b) . dx in the fragment layout above.
 // beta, inv_w_scale: prepare_b<1>'s scales of the tile at b_tile (bias at b_bias).  dx (the lane's two channels of both
 // rows) is scaled in place.  mid() runs halfway through the chunks (the caller's next dX/dt hides behind the MMAs).
 template <typename Mid>
 __device__ __forceinline__ void field(const float* zin, float (*dx)[2], float beta, float inv_w_scale, const float* b_bias,
                                       uint32_t b_tile, int q, float* kv, Mid mid) {
-    const bool odd = q & 1, upper = q >> 1;
     // Each row scaled by its own power of two so that max(|z|, bias floor) lands in [2^13, 2^14), split into FP16
     // hi + lo A fragments [k step][4]; the inverse scales are folded into dX/dt.
     float rs[2];
@@ -390,25 +277,7 @@ __device__ __forceinline__ void field(const float* zin, float (*dx)[2], float be
         for (int j = 0; j < 8; ++j)
 #pragma unroll
             for (int r = 0; r < 2; ++r) p[j][r] = fmaf(d[4 * j + 2 * r + 1], dx[r][1], __fmul_rn(d[4 * j + 2 * r], dx[r][0]));
-        // xor 1: keep the hidden units j with (j >> 1) & 1 == q & 1, that is 8c + 4h + 2 (q & 1) + e
-        float u[2][2][2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int e = 0; e < 2; ++e)
-#pragma unroll
-                for (int r = 0; r < 2; ++r) {
-                    const float got = __shfl_xor_sync(0xffffffffu, odd ? p[4 * h + e][r] : p[4 * h + 2 + e][r], 1);
-                    u[h][e][r] = (odd ? p[4 * h + 2 + e][r] : p[4 * h + e][r]) + got;
-                }
-        // xor 2: lanes 0, 1 keep h = 0, lanes 2, 3 h = 1: the units 8c + 2q + e
-#pragma unroll
-        for (int e = 0; e < 2; ++e)
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                const float got = __shfl_xor_sync(0xffffffffu, upper ? u[0][e][r] : u[1][e][r], 2);
-                kv[8 * r + 2 * c + e] = (upper ? u[1][e][r] : u[0][e][r]) + got;
-            }
+        reduce_chunk(p, c, q, kv);
     }
 }
 

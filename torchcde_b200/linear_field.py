@@ -68,7 +68,8 @@ def linear_field_of(func, z0, channels, times):
     except TypeError:
         known = None
     if known is None:
-        known = _probe(func, lin, z0, channels, times)
+        known = _probe(func, lambda z: torch.nn.functional.linear(z, lin.weight, lin.bias), z0, channels, times,
+                       "a single nn.Linear", "torchcde_b200.LinearVectorField")
         try:
             _recognised[func] = known
         except TypeError:
@@ -76,8 +77,8 @@ def linear_field_of(func, z0, channels, times):
     return (lin.weight, lin.bias) if known else None
 
 
-def _probe(func, lin, z0, channels, times):
-    """Bit-exact comparison of ``func`` with its ``nn.Linear`` on random (non-degenerate) states of z0's own
+def _probe(func, field, z0, channels, times, looks_like, remedy):
+    """Bit-exact comparison of ``func`` with ``field(z).view(..., H, C)`` on random (non-degenerate) states of z0's own
     shape (user modules may hard-code the batch size) at four distinct times, none of them 0 or 1."""
     hidden = z0.size(-1)
     if z0.numel() * channels > (1 << 27):
@@ -94,11 +95,11 @@ def _probe(func, lin, z0, channels, times):
             try:
                 got = func(tp, zp)
             except Exception:
-                warnings.warn("torchcde_b200.cdeint: `func` looks like a single nn.Linear but could not be probed. "
-                              "Falling back to the generic stage loop; use torchcde_b200.LinearVectorField to get the "
-                              "fused kernel.")
+                warnings.warn("torchcde_b200.cdeint: `func` looks like {} but could not be probed. Falling back to the "
+                              "generic stage loop{}.".format(looks_like, "; use {} to get the fused kernel".format(remedy)
+                                                             if remedy else ""))
                 return False
-            want = torch.nn.functional.linear(zp, lin.weight, lin.bias).view(*zp.shape[:-1], hidden, channels)
+            want = field(zp).view(*zp.shape[:-1], hidden, channels)
             if not (isinstance(got, torch.Tensor) and got.shape == want.shape and got.dtype == want.dtype
                     and torch.equal(got, want)):
                 return False

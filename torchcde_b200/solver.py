@@ -16,6 +16,7 @@ import torch
 from . import _lib, adaptive
 from .controls import CubicSpline, _control_signature, _schedule_knots
 from .linear_field import LinearFieldKernels, LinearVectorField, _reverse, linear_field_of  # noqa: F401
+from .mlp_field import MlpFieldKernels, mlp_field_of
 from .schedule import FIXED_METHODS, build_schedule, host_locator
 
 
@@ -451,6 +452,12 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                     # a shape the fused kernels are not built for (e.g. hidden * channels * hidden beyond the
                     # shared-memory budget of the CUDA-core kernel): this package's own stage loop takes any shape
                     pass
+            if mlp is not None:
+                try:
+                    return mlp.solve(y0, t, method, step_size).movedim(-2, 0)
+                except NotImplementedError:
+                    # a shape or solve variant the MLP kernels are not built for: the stage loop below
+                    pass
             if sig is not None and not torch.is_grad_enabled() and y0.is_cuda and y0.dtype in (torch.float32, torch.float64) \
                     and sig[1] == tuple(y0.shape[:-1]):
                 return _generic_solve_kernels(X, func, y0, t, method, step_size, is_prod, use_graph).movedim(-2, 0)
@@ -471,6 +478,13 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     kernels = None
     if field_params is not None and (adjoint or not wants_grad):
         kernels = LinearFieldKernels(X, field_params[0], field_params[1], z0)
+    # the fixed-step forward of the examples' MLP field (no gradient, or the forward pass of adjoint=True) is one launch
+    mlp = None
+    if (field_params is None and sig is not None and not is_prod and method in FIXED_METHODS and times
+            and (adjoint or not wants_grad)):
+        mlp_params = mlp_field_of(func, z0, sig[2], times)
+        if mlp_params is not None:
+            mlp = MlpFieldKernels(X, mlp_params, z0)
 
     if not wants_grad:
         with torch.no_grad():
