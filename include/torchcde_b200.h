@@ -65,7 +65,8 @@ TCDE_API int tcde_device_info(int* sm_count, int* cc_major, int* cc_minor);
  * (interpolation_hermite_cubic_bdiff.py:5-44, after the linear fill at :33).
  * x[n_paths][length][channels] -> coeffs[n_paths][length-1][4*channels].
  * t: length knots, or NULL for the default 0,1,...,length-1 (misc.py:79-80).
- * Bit-identical to the reference's fp32/fp64 result.  Sets TCDE_FLAG_NAN_SEEN if x holds a
+ * Bit-identical to the reference's fp32/fp64 result at any channel count (rows too wide for one shared-memory tile
+ * are split into channel tiles).  Sets TCDE_FLAG_NAN_SEEN if x holds a
  * NaN (the caller then runs tcde_linear_fill and calls again, as the reference does). */
 TCDE_API int tcde_hermite_bdiff_coeffs(const void* x, const void* t, void* coeffs, int64_t n_paths, int64_t length,
                               int64_t channels, int dtype, int32_t* flags, void* stream);
@@ -92,7 +93,7 @@ TCDE_API int tcde_linear_fill(const void* x, const void* t, void* out, int64_t n
  * interpolation_cubic.py:176) over n elements: sets TCDE_FLAG_NAN_SEEN in *flags. */
 TCDE_API int tcde_nan_flag(const void* x, int64_t n, int dtype, int32_t* flags, void* stream);
 
-/* misc.forward_fill along the length dim (misc.py:103-126); leading NaNs stay NaN. */
+/* misc.forward_fill along the length dim (misc.py:103-126); leading NaNs stay NaN.  length >= 1. */
 TCDE_API int tcde_forward_fill(const void* x, void* out, int64_t n_paths, int64_t length, int64_t channels,
                       int dtype, int32_t* flags, void* stream);
 

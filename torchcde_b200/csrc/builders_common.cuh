@@ -33,11 +33,14 @@ static int persistent_grid(const void* kernel, int threads, size_t smem, int64_t
 
 static constexpr size_t kMaxSmem = 200 * 1024;
 
-static int check_shape(const void* x, const void* out, int64_t n_paths, int64_t length, int64_t channels, int dtype) {
+// min_length: 2 knots for every spline builder (misc.py:96-98); 1 for the forward fill, which has no such limit
+static int check_shape(const void* x, const void* out, int64_t n_paths, int64_t length, int64_t channels, int dtype,
+                       int64_t min_length = 2) {
     TCDE_CHECK_ARG(x != nullptr && out != nullptr, "null data pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1, "n_paths=%lld channels=%lld", (long long)n_paths,
                    (long long)channels);
-    TCDE_CHECK_ARG(length >= 2, "length=%lld (need at least 2 knots, misc.py:96-98)", (long long)length);
+    TCDE_CHECK_ARG(length >= min_length, "length=%lld (need at least %lld knots, misc.py:96-98)", (long long)length,
+                   (long long)min_length);
     TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
     TCDE_CHECK_SUPPORTED(length < (1 << 24) && channels < (1 << 20), "length / channels too large");
     return TCDE_OK;

@@ -660,7 +660,7 @@ extern "C" int tcde_linear_fill(const void* x, const void* t, void* out, int64_t
 template <bool RECT>
 static int launch_hold(const void* x, void* out, int64_t n_paths, int64_t length, int64_t channels, int64_t time_index,
                        int dtype, int32_t* flags, void* stream) {
-    int rc = check_shape(x, out, n_paths, length, channels, dtype);
+    int rc = check_shape(x, out, n_paths, length, channels, dtype, RECT ? 2 : 1);
     if (rc != TCDE_OK) return rc;
     if (RECT) TCDE_CHECK_ARG(time_index >= 0 && time_index < channels, "time_index=%lld", (long long)time_index);
     const int64_t n_series = n_paths * channels;

@@ -18,53 +18,66 @@ namespace tcde {
 // ([row][a|b|2c|3d][channel]), and one thread issues a single bulk store of the tile (the
 // tile is a contiguous byte range of the output).  Two output tiles alternate so that the
 // store of tile n overlaps the computation of tile n+1.
+// A row too wide for one tile in shared memory (fp64 channels >= 2,327) is split into channel tiles of at most CW
+// channels: work item = (path, row tile, channel tile), and the tile's four CW-wide parts per row are stored with
+// plain stores (they are not one contiguous byte range of the output; the launcher passes use_bulk = 0).
 template <typename T, bool UNIT>
 __global__ void __launch_bounds__(kThreads)
 hermite_kernel(const T* __restrict__ x, const T* __restrict__ t, T* __restrict__ out, int64_t n_paths, int L, int C,
-               int TR, int tiles_per_path, int use_bulk, int32_t* __restrict__ flags) {
+               int CW, int TR, int tiles_per_path, int use_bulk, int32_t* __restrict__ flags) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     using E = exact<T>;
-    const int row_elems = 4 * C;
     T* ot0 = reinterpret_cast<T*>(smem_raw);
-    T* ot1 = ot0 + (size_t)TR * row_elems;
-    T* xs = ot1 + (size_t)TR * row_elems;
-    T* ts = xs + (size_t)(TR + 2) * C;
+    T* ot1 = ot0 + (size_t)TR * 4 * CW;
+    T* xs = ot1 + (size_t)TR * 4 * CW;
+    T* ts = xs + (size_t)(TR + 2) * CW;
 
     const int tid = threadIdx.x;
-    const int di = kThreads / C, dc = kThreads - di * C;   // (row, channel) advance per thread-stride
-    const int i_first = tid / C, c_first = tid - i_first * C;
-    const int64_t n_items = n_paths * tiles_per_path;
+    const int ctiles = (C + CW - 1) / CW;
+    const int64_t n_items = n_paths * tiles_per_path * ctiles;
     bool saw_nan = false;
     int buf = 0;
 
     for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x, buf ^= 1) {
-        const int64_t p = item / tiles_per_path;
-        const int tile = (int)(item - p * tiles_per_path);
+        const int64_t pt = item / ctiles;
+        const int c0 = (int)(item - pt * ctiles) * CW;
+        const int cw = min(CW, C - c0);                      // channels of this tile (C when the row is not split)
+        const int row_elems = 4 * cw;
+        const int di = kThreads / cw, dc = kThreads - di * cw;   // (row, channel) advance per thread-stride
+        const int64_t p = pt / tiles_per_path;
+        const int tile = (int)(pt - p * tiles_per_path);
         const int r0 = tile * TR;
         const int nr = min(TR, L - 1 - r0);
         if (use_bulk && tid == 0) bulk_wait_read<1>();   // the store that last read ot[buf] has drained
 
         // knot rows r0-1 .. r0+nr ; row -1 does not exist for the first tile
-        const T* xp = x + (p * L + r0 - 1) * C;
-        const int ne = (nr + 2) * C;
-        for (int e = (r0 == 0 ? C : 0) + tid; e < ne; e += kThreads) xs[e] = xp[e];
+        const T* xp = x + (p * L + r0 - 1) * C + c0;
+        const int ne = (nr + 2) * cw;
+        if (cw == C) {
+            for (int e = (r0 == 0 ? C : 0) + tid; e < ne; e += kThreads) xs[e] = xp[e];
+        } else {
+            for (int e = (r0 == 0 ? cw : 0) + tid; e < ne; e += kThreads) {
+                const int row = e / cw;
+                xs[e] = xp[(int64_t)row * C + (e - row * cw)];
+            }
+        }
         if (!UNIT) {
             for (int e = (r0 == 0 ? 1 : 0) + tid; e < nr + 2; e += kThreads) ts[e] = t[r0 - 1 + e];
         }
         __syncthreads();
 
         T* ot = buf ? ot1 : ot0;
-        int i = i_first, c = c_first;
-        for (int e = tid; e < nr * C; e += kThreads) {
-            const T xl = xs[(i + 1) * C + c];
-            const T xh = xs[(i + 2) * C + c];
+        int i = tid / cw, c = tid - (tid / cw) * cw;
+        for (int e = tid; e < nr * cw; e += kThreads) {
+            const T xl = xs[(i + 1) * cw + c];
+            const T xh = xs[(i + 2) * cw + c];
             saw_nan |= is_nan(xl) | is_nan(xh);
             const bool first = (r0 + i == 0);
             T b, two_c, three_d;
             if (UNIT) {
                 // dt == 1 exactly: every division by dt and the 1/dt^2 factor are exact identities
                 const T dn = E::sub(xh, xl);
-                const T dp = first ? dn : E::sub(xl, xs[i * C + c]);
+                const T dp = first ? dn : E::sub(xl, xs[i * cw + c]);
                 const T bend = E::sub(dn, dp);
                 const T inner = E::add(E::sub(E::mul(T(3), bend), dn), dp);
                 two_c = E::mul(T(2), inner);
@@ -73,7 +86,7 @@ hermite_kernel(const T* __restrict__ x, const T* __restrict__ t, T* __restrict__
             } else {
                 const T dt = E::sub(ts[i + 2], ts[i + 1]);
                 const T dn = E::div(E::sub(xh, xl), dt);                       // bdiff.py:39
-                const T dp = first ? dn : E::div(E::sub(xl, xs[i * C + c]), E::sub(ts[i + 1], ts[i]));
+                const T dp = first ? dn : E::div(E::sub(xl, xs[i * cw + c]), E::sub(ts[i + 1], ts[i]));
                 const T inner = E::add(E::sub(E::mul(T(3), E::sub(dn, dp)), dn), dp);
                 two_c = E::div(E::mul(T(2), inner), dt);                        // bdiff.py:17
                 const T inv_sq = E::div(T(1), E::mul(dt, dt));
@@ -87,14 +100,21 @@ hermite_kernel(const T* __restrict__ x, const T* __restrict__ t, T* __restrict__
             for (int k = 0; k < 4; ++k) {
                 const int w = (k + i) & 3;
                 const T v = (w == 0) ? xl : (w == 1) ? b : (w == 2) ? two_c : three_d;
-                row[w * C] = v;
+                row[w * cw] = v;
             }
             i += di;
             c += dc;
-            if (c >= C) { c -= C; ++i; }
+            if (c >= cw) { c -= cw; ++i; }
         }
-        T* gp = out + (p * (int64_t)(L - 1) + r0) * row_elems;
-        if (use_bulk) {
+        T* gp = out + (p * (int64_t)(L - 1) + r0) * 4 * C;
+        if (cw != C) {                                     // one channel tile: rows 4C apart, parts C apart
+            __syncthreads();
+            for (int e = tid; e < nr * row_elems; e += kThreads) {
+                const int r = e / row_elems, rem = e - r * row_elems;
+                const int w = rem / cw;
+                gp[(int64_t)r * 4 * C + (int64_t)w * C + c0 + (rem - w * cw)] = ot[e];
+            }
+        } else if (use_bulk) {
             fence_proxy_async_smem();
             __syncthreads();
             if (tid == 0) {
@@ -229,15 +249,23 @@ static int launch_hermite(const T* x, const T* t, T* out, int64_t n_paths, int L
     int TR = (int)(16384 / row_bytes);
     if (TR < 1) TR = 1;
     if (TR > L - 1) TR = L - 1;
-    const size_t smem = 2 * TR * row_bytes + (size_t)(TR + 2) * C * sizeof(T) + (size_t)(TR + 2) * sizeof(T) + 16;
-    TCDE_CHECK_SUPPORTED(smem <= kMaxSmem, "hermite: channels=%d needs %zu bytes of shared memory (max %zu)", C, smem,
-                         kMaxSmem);
+    auto smem_of = [&](int cw) {
+        return 2 * TR * (size_t)4 * cw * sizeof(T) + (size_t)(TR + 2) * cw * sizeof(T) + (size_t)(TR + 2) * sizeof(T) + 16;
+    };
+    // rows too wide for one tile (TR = 1 then): split the channels into the fewest tiles that fit, of equal width
+    int CW = C;
+    if (smem_of(C) > kMaxSmem) {
+        const int cw_max = (int)((kMaxSmem - smem_of(0)) / (smem_of(1) - smem_of(0)));
+        const int ctiles = (C + cw_max - 1) / cw_max;
+        CW = (C + ctiles - 1) / ctiles;
+    }
+    const size_t smem = smem_of(CW);
     const int tiles = (L - 1 + TR - 1) / TR;
-    const int use_bulk = aligned16(out) ? 1 : 0;
+    const int use_bulk = (CW == C && aligned16(out)) ? 1 : 0;
     auto kern = t ? hermite_kernel<T, false> : hermite_kernel<T, true>;
     TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int grid = persistent_grid((const void*)kern, kThreads, smem, n_paths * tiles);
-    kern<<<grid, kThreads, smem, stream>>>(x, t, out, n_paths, L, C, TR, tiles, use_bulk, flags);
+    const int grid = persistent_grid((const void*)kern, kThreads, smem, n_paths * tiles * ((C + CW - 1) / CW));
+    kern<<<grid, kThreads, smem, stream>>>(x, t, out, n_paths, L, C, CW, TR, tiles, use_bulk, flags);
     TCDE_CHECK_CUDA(cudaGetLastError());
     return TCDE_OK;
 }
