@@ -168,28 +168,46 @@ def solve(field, y0, times, rtol, atol, first_step=None, clip=False, replay=None
     return torch.stack(out), records, first_dt
 
 
+# ---------------------------------------------------------------------------------------------------- the control
+class _Control:
+    """dX/dt of a cubic spline (``control`` = its coefficient rows) or a linear interpolation (``control`` = its knot
+    values) in fp64.  ``time_dtype``: the dtype a stage time is rounded to before the interval lookup (the state's dtype
+    in the reference stack)."""
+
+    def __init__(self, control, knots, kind, time_dtype):
+        self.control = control.double()
+        self.knots = knots.double().to(self.control.device)
+        self.kind, self.time_dtype = kind, time_dtype
+
+    def time(self, t):
+        return float(torch.tensor(float(t), dtype=torch.float64).to(self.time_dtype))
+
+    def _dxdt_at(self, ts):
+        """dX/dt at the fp64 tensor ``ts`` (differentiable in ``ts`` and in the knots)."""
+        if self.kind == "cubic":
+            return cde_oracle.cubic_derivative(self.control, self.knots, ts)
+        return cde_oracle.linear_derivative(self.control, self.knots, ts)
+
+    def dxdt(self, t):
+        return self._dxdt_at(torch.tensor(self.time(t), dtype=torch.float64, device=self.knots.device))
+
+    def locate(self, t):
+        """(interval, fraction) of a stage time with the lookup the field uses."""
+        frac, index = cde_oracle.locate(self.knots.cpu(), self.time(t), self.control.size(-2) - (self.kind == "linear"))
+        return int(index), float(frac)
+
+
 # -------------------------------------------------------------------------------------------- the linear CDE field
-class LinearCDE:
+class LinearCDE(_Control):
     """f(t, z) = Linear(H, H C)(z).view(H, C) @ dX/dt(t) in fp64 for a cubic spline (``control`` = its coefficient
     rows) or a linear interpolation (``control`` = its knot values).  ``time_dtype``: the dtype a stage time is rounded
     to before the interval lookup (the state's dtype in the reference stack)."""
 
     def __init__(self, control, knots, weight, bias, kind, time_dtype=torch.float64):
-        self.control = control.double()
-        self.knots = knots.double().to(self.control.device)
+        super().__init__(control, knots, kind, time_dtype)
         self.weight, self.bias = weight.double(), bias.double()
-        self.kind, self.time_dtype = kind, time_dtype
         self.hidden = self.weight.size(1)
         self.channels = self.weight.size(0) // self.hidden
-
-    def time(self, t):
-        return float(torch.tensor(float(t), dtype=torch.float64).to(self.time_dtype))
-
-    def dxdt(self, t):
-        t = torch.tensor(self.time(t), dtype=torch.float64, device=self.knots.device)
-        if self.kind == "cubic":
-            return cde_oracle.cubic_derivative(self.control, self.knots, t)
-        return cde_oracle.linear_derivative(self.control, self.knots, t)
 
     def __call__(self, t, z):
         return cde_oracle.linear_field(self.weight, self.bias, z, self.dxdt(t))
@@ -204,11 +222,6 @@ class LinearCDE:
             gz, gw, gb = torch.autograd.grad(f, (zz, w, b), a)
         return f.detach(), gz, gw, gb
 
-    def locate(self, t):
-        """(interval, fraction) of a stage time with the lookup the field uses."""
-        frac, index = cde_oracle.locate(self.knots.cpu(), self.time(t), self.control.size(-2) - (self.kind == "linear"))
-        return int(index), float(frac)
-
     def regrouped(self):
         """The adjoint state's own linear CDE: a^T df/dz = -Linear(-W regrouped, 0)(a) @ dX/dt."""
         h, c = self.hidden, self.channels
@@ -216,33 +229,98 @@ class LinearCDE:
         return LinearCDE(self.control, self.knots, w2, torch.zeros_like(self.bias), self.kind, self.time_dtype)
 
 
-# ------------------------------------------------------------------------------------- the adjoint of a linear CDE
-def fixed_adjoint(cde, ys, grad_ys, times, method, step_size):
-    """torchdiffeq ``odeint_adjoint`` for a fixed-grid method: (z, a, dL/dW, dL/db) integrated from t_i back to t_{i-1}
+# ------------------------------------------------------------------------------------------ the CDE of any field
+class FuncCDE(_Control):
+    """f(t, z) = g(t, z) @ dX/dt(t) in fp64 for any fp64 callable ``g(t, z) -> (..., H, C)``, or with ``prod`` the
+    callable's own product f(t, z) = g(t, z, dX/dt(t)).  ``g`` gets the stage time as a 0-dim fp64 tensor holding it
+    rounded to ``time_dtype``, as the package passes it to ``func`` (under a decreasing ``t`` the time of the original
+    frame, as torchdiffeq's reversal ``func(-s)`` does).  ``params``: the fp64 leaf tensors ``g`` reads, created with
+    ``requires_grad``; they are what ``vjp`` and ``fixed_adjoint`` differentiate unless told otherwise."""
+
+    def __init__(self, control, knots, g, kind, time_dtype=torch.float64, params=(), prod=False):
+        super().__init__(control, knots, kind, time_dtype)
+        self.g, self.params, self.prod = g, list(params), prod
+
+    def _field(self, ts, z):
+        dx = self._dxdt_at(ts)
+        if self.prod:
+            return self.g(ts, z, dx)
+        return (self.g(ts, z) @ dx.unsqueeze(-1)).squeeze(-1)
+
+    def __call__(self, t, z):
+        return self._field(torch.tensor(self.time(t), dtype=torch.float64, device=self.knots.device), z)
+
+    def vjp(self, t, z, a, params=None, with_t=False):
+        """(f, a^T df/dz, [a^T df/dp for p in params]) by fp64 autograd; with ``with_t`` also a^T df/dt.  The rounding
+        of the stage time to ``time_dtype`` passes the time gradient through unchanged, like ``t.to(dtype)``."""
+        params = self.params if params is None else list(params)
+        t_ = torch.tensor(float(t), dtype=torch.float64, device=self.knots.device, requires_grad=True)
+        zz = z.detach().clone().requires_grad_(True)
+        wrt = [zz] + params + ([t_] if with_t else [])
+        with torch.enable_grad():
+            f = self._field(t_ + (self.time(t) - float(t)), zz)
+            grads = torch.autograd.grad(f, wrt, a, allow_unused=True)
+        grads = [torch.zeros_like(x) if g is None else g for g, x in zip(grads, wrt)]
+        gz, gp = grads[0], grads[1:1 + len(params)]
+        return (f.detach(), gz, gp, grads[-1]) if with_t else (f.detach(), gz, gp)
+
+
+# ------------------------------------------------------------------------------------------------ the fixed adjoint
+def fixed_adjoint(cde, ys, grad_ys, times, method, step_size, params=None, with_t=False):
+    """torchdiffeq ``odeint_adjoint`` for a fixed-grid method: (z, a, dL/dparams) integrated from t_i back to t_{i-1}
     by ``odeint_port`` (its grid for the reversed segment, its stages), grad_ys[i-1] added at every output time.
-    ``ys``, ``grad_ys``: (len(times), P, H).  Returns (dL/dz0, dL/dW, dL/db)."""
+    ``ys``, ``grad_ys``: (len(times), P, H).
+
+    A ``LinearCDE`` differentiates (W, b) and returns (dL/dz0, dL/dW, dL/db).  A ``FuncCDE`` differentiates ``params``
+    (default: its own list) and returns (dL/dz0, [dL/dp], dL/dt or None).  ``with_t`` (FuncCDE only): the gradients of
+    the output times, as ``odeint_adjoint`` forms them when ``t.requires_grad`` -- the augmented state carries the
+    integral of -a^T df/dt, ``<f(t_i, y_i), dL/dy_i>`` is dL/dt_i and is subtracted from that integral at every output
+    t_i > t_0, and dL/dt_0 is what the integral holds at the end.  Everything is in the frame of ``times`` itself, so a
+    decreasing ``times`` needs no sign flip."""
+    linear = isinstance(cde, LinearCDE)
+    if linear:
+        assert params is None and not with_t
+        params = [cde.weight, cde.bias]
+    elif params is None:
+        params = cde.params
     shape_z = ys[0].shape
     n_z = ys[0].numel()
-    n_w = cde.weight.numel()
+    sizes = [p.numel() for p in params]
+    dev = ys.device
 
-    def unpack(v):
-        return (v[:n_z].view(shape_z), v[n_z:2 * n_z].view(shape_z))
+    def vjp(t, z, a):
+        if linear:
+            f, gz, gw, gb = cde.vjp(t, z, a)
+            return f, gz, [gw, gb], None
+        return cde.vjp(t, z, a, params, with_t) + (() if with_t else (None,))
 
     def aug(t, v):
-        z, a = unpack(v)
-        f, gz, gw, gb = cde.vjp(float(t), z, a)
-        return torch.cat([f.reshape(-1), -gz.reshape(-1), -gw.reshape(-1), -gb.reshape(-1)])
+        z, a = v[:n_z].view(shape_z), v[n_z:2 * n_z].view(shape_z)
+        f, gz, gp, gt = vjp(float(t), z, a)
+        parts = [f, -gz] + [-g for g in gp] + ([-gt] if with_t else [])
+        return torch.cat([x.reshape(-1) for x in parts])
 
     a = grad_ys[-1].double().clone()
-    gw = torch.zeros(n_w, dtype=torch.float64, device=cde.weight.device)
-    gb = torch.zeros(cde.bias.numel(), dtype=torch.float64, device=cde.weight.device)
+    gp = [torch.zeros(n, dtype=torch.float64, device=dev) for n in sizes]
+    a_t = torch.zeros(1, dtype=torch.float64, device=dev)
+    time_grads = [None] * len(times)
     for i in range(len(times) - 1, 0, -1):
-        v0 = torch.cat([ys[i].double().reshape(-1), a.reshape(-1), gw, gb])
+        if with_t:
+            d_cur = (cde(times[i], ys[i].double()) * grad_ys[i].double()).sum().reshape(1)
+            time_grads[i] = d_cur
+            a_t = a_t - d_cur
+        v0 = torch.cat([ys[i].double().reshape(-1), a.reshape(-1)] + gp + ([a_t] if with_t else []))
         seg = torch.tensor([times[i], times[i - 1]], dtype=torch.float64)
         v1 = odeint_port.odeint(aug, v0, seg, method=method, options={"step_size": step_size})[-1]
-        a = unpack(v1)[1] + grad_ys[i - 1].double()
-        gw, gb = v1[2 * n_z:2 * n_z + n_w], v1[2 * n_z + n_w:]
-    return a, gw.view_as(cde.weight), gb
+        a = v1[n_z:2 * n_z].view(shape_z) + grad_ys[i - 1].double()
+        gp = list(torch.split(v1[2 * n_z:2 * n_z + sum(sizes)], sizes))
+        if with_t:
+            a_t = v1[-1:]
+    if linear:
+        return a, gp[0].view_as(cde.weight), gp[1]
+    time_grads[0] = a_t
+    grads_t = torch.cat(time_grads) if with_t else None
+    return a, [g.view_as(p) for g, p in zip(gp, params)], grads_t
 
 
 class PairedSegment:

@@ -4,9 +4,8 @@ fp64 oracle at the schedule, tile and control edges.
 Routes: the wgmma kernel at hidden 32 / channels 8 / width 128 (variant 0), the CUDA-core kernel in fp32 and fp64 (auto
 at 8 / 3 and 5 / 3, variant 1 at 32 / 8 and 16 / 4, where auto leaves the shape to the stage loop), each at widths 128
 and 48.  Schedules: ``test_host_logic.FIXED_SCHEDULES``
-on 40 knots.  Reference: ``odeint_port.odeint`` driving ``MlpCDE`` below -- ``adaptive_oracle.LinearCDE``'s dX/dt and
-stage-time rounding with the MLP in place of the linear map -- in fp64 on fp64 copies of the kernel's own rounded
-inputs.  Bars are fractions of each path's own scale."""
+on 40 knots.  Reference: ``odeint_port.odeint`` driving ``MlpCDE`` below -- ``adaptive_oracle.FuncCDE`` with the MLP as
+its field -- in fp64 on fp64 copies of the kernel's own rounded inputs.  Bars are fractions of each path's own scale."""
 import contextlib
 import functools
 
@@ -79,20 +78,17 @@ def _options(step):
     return {} if step is None else {"step_size": step}
 
 
-class MlpCDE(AO.LinearCDE):
-    """f(t, z) = tanh(W2 relu(W1 z + b1) + b2).view(H, C) @ dX/dt(t) in fp64: LinearCDE's control, dX/dt and stage-time
-    rounding with the MLP in place of the linear map."""
+def MlpCDE(control, knots, w1, b1, w2, b2, kind, time_dtype):
+    """f(t, z) = tanh(W2 relu(W1 z + b1) + b2).view(H, C) @ dX/dt(t) in fp64: ``adaptive_oracle.FuncCDE`` with the MLP
+    as its ``g``."""
+    w1, b1, w2, b2 = (x.double() for x in (w1, b1, w2, b2))
+    hidden = w1.size(1)
 
-    def __init__(self, control, knots, w1, b1, w2, b2, kind, time_dtype):
-        super().__init__(control, knots, w2, b2, kind, time_dtype)
-        self.w1, self.b1 = w1.double(), b1.double()
-        self.hidden = self.w1.size(1)
-        self.channels = self.weight.size(0) // self.hidden
+    def g(t, z):
+        u = torch.relu(z @ w1.T + b1)
+        return torch.tanh(u @ w2.T + b2).view(*z.shape[:-1], hidden, -1)
 
-    def __call__(self, t, z):
-        u = torch.relu(z @ self.w1.T + self.b1)
-        f = torch.tanh(u @ self.weight.T + self.bias).view(*z.shape[:-1], self.hidden, self.channels)
-        return (f @ self.dxdt(t).unsqueeze(-1)).squeeze(-1)
+    return AO.FuncCDE(control, knots, g, kind, time_dtype)
 
 
 class Func(torch.nn.Module):

@@ -228,6 +228,89 @@ def test_paired_adjoint_converges_to_finite_differences(adjoint_problem):
     assert errs[0] < 1e-3 and errs[1] < errs[0] / 10 and errs[2] < errs[1] / 10 and errs[2] < 1e-7, errs
 
 
+# ------------------------------------------------------------------------------------------------------- FuncCDE
+def _linear_func_cde(cde):
+    """The LinearCDE's field as a FuncCDE of an nn.Linear + view, with W and b as its parameters."""
+    lin = torch.nn.Linear(cde.hidden, cde.hidden * cde.channels, dtype=torch.float64)
+    with torch.no_grad():
+        lin.weight.copy_(cde.weight)
+        lin.bias.copy_(cde.bias)
+    h = cde.hidden
+
+    def g(t, z):
+        return lin(z).view(*z.shape[:-1], h, -1)
+
+    return AO.FuncCDE(cde.control, cde.knots, g, cde.kind, cde.time_dtype, params=[lin.weight, lin.bias])
+
+
+@pytest.mark.parametrize("kind", ["cubic", "linear"])
+def test_func_cde_of_a_linear_module_is_the_linear_cde_bit_for_bit(kind):
+    cde, z0 = _cde(kind, seed=4)
+    fc = _linear_func_cde(cde)
+    a = torch.randn(z0.shape, generator=torch.Generator().manual_seed(5), dtype=torch.float64)
+    for t in (0.0, 0.7, 2.0, 3.25, 5.0):
+        with torch.no_grad():
+            assert torch.equal(fc(t, z0), cde(t, z0))
+        f, gz, gw, gb = cde.vjp(t, z0, a)
+        f2, gz2, (gw2, gb2) = fc.vjp(t, z0, a)
+        for got, want in ((f2, f), (gz2, gz), (gw2, gw), (gb2, gb)):
+            assert torch.equal(got, want)
+        assert fc.locate(t) == cde.locate(t)
+
+
+@pytest.mark.parametrize("method", ["rk4", "midpoint", "euler"])
+def test_generalised_fixed_adjoint_on_a_linear_field(adjoint_problem, method):
+    """The parameter-list form of fixed_adjoint on the FuncCDE of a linear module gives LinearCDE's (W, b) form bit for
+    bit."""
+    cde, z0, g, _truth, ys = adjoint_problem
+    gz, gw, gb = AO.fixed_adjoint(cde, ys, g, _TIMES, method, 1 / 4)
+    gz2, (gw2, gb2), gt = AO.fixed_adjoint(_linear_func_cde(cde), ys, g, _TIMES, method, 1 / 4)
+    assert gt is None
+    assert torch.equal(gz2, gz) and torch.equal(gw2, gw) and torch.equal(gb2, gb)
+
+
+@pytest.mark.parametrize("times", [[2.1, 2.45, 2.9], [2.9, 2.45, 2.1]])
+def test_time_channel_of_fixed_adjoint_matches_central_differences(times):
+    """dL/dt from the augmented state (the integral of -a^T df/dt, <f, dL/dy> at every output) for a field that reads
+    ``t`` itself, against central differences of a fine fp64 solve in every output time, on increasing and decreasing
+    t.  The times lie inside one spline interval: across a knot the second derivative of the control jumps, and the fine
+    solve's error would then move with its grid by more than the bar."""
+    cde, z0 = _cde("cubic", seed=6)
+    h = cde.hidden
+    v = torch.randn(h * cde.channels, generator=torch.Generator().manual_seed(7), dtype=torch.float64) / 4
+    w, b = cde.weight.clone().requires_grad_(True), cde.bias.clone().requires_grad_(True)
+
+    def g(t, z):
+        return torch.tanh(torch.nn.functional.linear(z, w, b) + t * v).view(*z.shape[:-1], h, -1)
+
+    fc = AO.FuncCDE(cde.control, cde.knots, g, "cubic", params=[w, b])
+    gy = torch.randn(len(times), *z0.shape, generator=torch.Generator().manual_seed(8), dtype=torch.float64)
+
+    def loss(ts):
+        # 160 rk4 steps per segment, so that every output is a grid point (no interpolation) and the grid moves with t
+        ys, y = [z0], z0
+        with torch.no_grad():
+            for lo, hi in zip(ts[:-1], ts[1:]):
+                grid = torch.linspace(lo, hi, 161, dtype=torch.float64)
+                y = odeint_port.odeint(fc, y, grid, method="rk4")[-1]
+                ys.append(y)
+        ys = torch.stack(ys)
+        return float((ys * gy).sum()), ys
+
+    _, ys = loss(times)
+    _gz, _gp, gt = AO.fixed_adjoint(fc, ys, gy, times, "rk4", 1 / 64, with_t=True)
+    gt = gt.detach()
+    eps = 1e-5
+    fd = []
+    for j in range(len(times)):
+        up, down = list(times), list(times)
+        up[j] += eps
+        down[j] -= eps
+        fd.append((loss(up)[0] - loss(down)[0]) / (2 * eps))
+    fd = torch.tensor(fd, dtype=torch.float64)
+    assert float((gt - fd).abs().max() / fd.abs().max()) < 1e-6, (gt, fd)
+
+
 def test_paired_segment_quadrature_is_the_integral_of_the_parameter_gradient(adjoint_problem):
     """The quadrature over accepted steps equals integrating dL/dW as a third state with the same Runge-Kutta steps
     (g' does not depend on g), so it agrees with a fine fixed-step adjoint of the same segment."""

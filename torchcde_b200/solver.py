@@ -170,7 +170,12 @@ def _generic_solve_kernels(X, func, z0, t, method, step_size, is_prod, use_graph
     user's code).  With ``use_graph`` the whole time loop is captured into a CUDA graph once per (func, X, shapes,
     schedule) and replayed -- for small states the loop is launch-bound (12 launches per stage), which is what a graph
     removes.  The graph reads ``func``'s parameters and X's coefficients from their own storage, so in-place updates of
-    either are seen by a replay; a different ``func`` / ``X`` object captures anew."""
+    either (``optimizer.step()``) are seen by a replay.  The cache key is everything a replay cannot see change: the
+    ``func`` and ``X`` objects, the state's shape, dtype and device, the method, step and output times, the ``training``
+    flag of every submodule of ``func`` (a branch on ``self.training`` is baked into the capture), and the storage address
+    of every parameter and buffer of ``func`` and of every buffer of ``X`` (``p.data = ...``, ``module.double().float()``
+    or ``load_state_dict(..., assign=True)`` give a parameter new storage, which the captured kernels would not read).
+    The cache entry keeps those tensors alive, so no address in a key can be reused while its graph is cached."""
     kind, _, channels, n_rows = _control_signature(X)
     dtype, device = z0.dtype, z0.device
     sched = build_schedule(t, _schedule_knots(X), n_rows, method, step_size, dtype)
@@ -238,7 +243,12 @@ def _generic_solve_kernels(X, func, z0, t, method, step_size, is_prod, use_graph
     zc = z0.detach().contiguous()
     if not use_graph:
         return run(zc)
-    key = (id(func), id(X), tuple(zc.shape), dtype, str(device), method, step_size, tuple(float(v) for v in t.detach().cpu().tolist()))
+    modules = list(func.modules()) if isinstance(func, torch.nn.Module) else []
+    read = [x for m in modules for x in m.parameters(recurse=False)] + \
+        [x for m in modules for x in m.buffers(recurse=False)] + list(X.buffers())
+    key = (id(func), id(X), tuple(zc.shape), dtype, str(device), method, step_size,
+           tuple(float(v) for v in t.detach().cpu().tolist()), tuple(m.training for m in modules),
+           tuple(x.data_ptr() for x in read))
     hit = _graphs.get(key)
     if hit is None:
         static_in = zc.clone()
@@ -250,9 +260,10 @@ def _generic_solve_kernels(X, func, z0, t, method, step_size, is_prod, use_graph
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             static_out = run(static_in)
-        # func / X are kept alive because their ids are the key; ``run`` is kept because its closure owns the device
-        # copies of the schedule and of the control rows whose addresses the captured kernels read
-        hit = (graph, static_in, static_out, func, X, run)
+        # func / X are kept alive because their ids are the key, the tensors in ``read`` because their addresses are;
+        # ``run`` is kept because its closure owns the device copies of the schedule and of the control rows whose
+        # addresses the captured kernels read
+        hit = (graph, static_in, static_out, func, X, run, read)
         if len(_graphs) >= 8:
             _graphs.clear()
         _graphs[key] = hit
@@ -421,8 +432,9 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
         adjoint_params = tuple(kwargs['adjoint_params'])
     else:
         adjoint_params = tuple(func.parameters()) if isinstance(func, torch.nn.Module) else ()
-    differentiable = (z0, t) + tuple(X.buffers()) + (tuple(func.parameters()) if isinstance(func, torch.nn.Module)
-                                                     else ()) + adjoint_params
+    # a user-defined control need not be a module: all it must have is ``derivative``
+    differentiable = (z0, t) + (tuple(X.buffers()) if isinstance(X, torch.nn.Module) else ()) + \
+        (tuple(func.parameters()) if isinstance(func, torch.nn.Module) else ()) + adjoint_params
     wants_grad = torch.is_grad_enabled() and any(isinstance(x, torch.Tensor) and x.requires_grad
                                                  for x in differentiable)
 
@@ -465,10 +477,26 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
         if (kernels is not None and adaptive.device_dopri5_available(y0, sig[2]) and not options.get("jump_t")
                 and set(options) <= {"first_step", "jump_t"}):
             # config 4's forward pass: the whole adaptive loop on the device, one launch per attempted step
-            out, cdeint.last_stats = kernels.dopri5(y0, times, rtol, atol, -1.0 if flipped else 1.0,
-                                                    options.get("first_step"))
-            return out
-        field = kernels.field() if kernels is not None else _torch_field(X, func, is_prod, sig is not None, z0)
+            try:
+                out, cdeint.last_stats = kernels.dopri5(y0, times, rtol, atol, -1.0 if flipped else 1.0,
+                                                        options.get("first_step"))
+                return out
+            except NotImplementedError:
+                # a problem the device controller is not built for (e.g. control rows off a 16-byte boundary): the
+                # host-driven loop below takes it, with the kernel field
+                pass
+
+        field = None
+        if kernels is not None:
+            field = kernels.field()
+            try:
+                # one evaluation before the solve: the kernel field refuses a shape (e.g. hidden > 256) on every call,
+                # so a field that answers here answers every attempt
+                field(-times[0] if flipped else times[0], y0)
+            except NotImplementedError:
+                field = None                                  # the torch-operator field takes any shape
+        if field is None:
+            field = _torch_field(X, func, is_prod, sig is not None, z0)
         out, solver_obj = adaptive.odeint_dopri5(_reverse(field) if flipped else field, y0, times, rtol, atol, options)
         cdeint.last_stats = {"n_accepted": solver_obj.n_accepted, "n_rejected": solver_obj.n_rejected,
                              "device_controlled": False}
