@@ -194,6 +194,34 @@ TCDE_API int tcde_cdeint_fixed_linear_stages(const void* control, int control_ki
                                     const int32_t* out_step, const int32_t* out_mode, const void* out_slope,
                                     double sign, int dtype, void* stream);
 
+/* The backward pass of tcde_cdeint_fixed_linear_stages through its own discrete operations (cdeint(..., adjoint=False) of a
+ * fixed-step solve): the transposed Runge-Kutta recurrence of every step, in reverse, in ONE launch.  For the linear field
+ * F_s(v) = sign (W v + b) . dX(t_s) the Jacobian J_s does not depend on v, so the forward state is never needed:
+ *   rk4       kappa_4 = dt/8 ybar',  kappa_3 = dt (3/8 ybar' + u_4),  kappa_2 = dt (3/8 ybar' - u_4 + u_3),
+ *             kappa_1 = dt (1/8 ybar' + u_4 - u_3/3 + u_2/3),  with u_s = J_s^T kappa_s;
+ *   midpoint  kappa_2 = dt ybar',  kappa_1 = dt/2 u_2;      euler  kappa_1 = dt ybar';
+ *   ybar = ybar' + sum_s u_s,
+ * where ybar' is the cotangent of the step's end state after its output gradients were added.  J_s^T w = sign sum_c
+ * dX_c(t_s) W_c^T w is the field product with weight_t[(k, c)][h] = weight[(h, c)][k] and the bias `zeros` (hidden *
+ * channels zeros).
+ *   grad_out     [n_paths][n_out][hidden] output gradients;  grad_z0 [n_paths][hidden] receives dL/dz0
+ *   kappa_dump   (may be NULL) [n_steps * n_stages][n_paths][hidden] receives kappa of forward stage (i, s) in slot
+ *                i * n_stages + s, the slot of that stage's input in the forward dump; tcde_linear_field_param_grads
+ *                over the two dumps with stage_weight = sign gives dL/dW and dL/db
+ *   step_dt_rev[n_steps], stage_index_rev / stage_frac_rev[n_steps * n_stages]: the forward schedule's arrays reversed
+ *   inj_range[n_steps + 2], inj_out[], inj_weight[]: grid state r (r = 0 the end of the solve, r = n_steps z0) adds
+ *                inj_weight[e] * grad_out[:, inj_out[e]] for e in [inj_range[r], inj_range[r + 1]) -- an output copied from
+ *                a step's start or end lands there with weight 1, one interpolated at slope s lands on the start with
+ *                1 - s and on the end with s
+ * fp32, hidden = 32, channels = 8, 16-byte aligned buffers (TCDE_ERR_UNSUPPORTED otherwise); the field product is the
+ * 2xFP16 warpgroup MMA of the fused solve. */
+TCDE_API int tcde_cdeint_fixed_linear_backward(const void* control, int control_kind, int64_t n_rows, const void* weight_t,
+                                      const void* zeros, const void* grad_out, void* grad_z0, void* kappa_dump,
+                                      int64_t n_paths, int64_t channels, int64_t hidden, int method, int64_t n_steps,
+                                      const void* step_dt_rev, const int32_t* stage_index_rev, const void* stage_frac_rev,
+                                      int64_t n_out, const int32_t* inj_range, const int32_t* inj_out,
+                                      const void* inj_weight, double sign, int dtype, void* stream);
+
 /* The fused fixed-step solve of tcde_cdeint_fixed_linear for the MLP vector field of the reference's examples
  * (example/time_series_classification.py:20-51, func = Linear(H, W) -> ReLU -> Linear(W, H*C) -> tanh -> view(H, C)):
  *   f(t, z) = tanh(w2 relu(w1 z + b1) + b2).view(H, C) @ dX/dt(t)

@@ -43,6 +43,8 @@ SIGNATURES = {
                                       _dbl, _dbl, _dbl, _int, _p], _int),
     "tcde_cdeint_fixed_linear_stages": ([_p, _int, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i64, _int, _i64, _p, _p, _p,
                                          _i64, _p, _p, _p, _dbl, _int, _p], _int),
+    "tcde_cdeint_fixed_linear_backward": ([_p, _int, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i64, _int, _i64, _p, _p, _p,
+                                           _i64, _p, _p, _p, _dbl, _int, _p], _int),
     "tcde_cdeint_reversible_heun_linear": ([_p, _int, _i64, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _i64, _p, _p,
                                             _p, _i64, _p, _p, _int, _p], _int),
     "tcde_reversible_heun_linear_backward_segment": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _p,

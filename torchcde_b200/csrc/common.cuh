@@ -110,6 +110,13 @@ struct UmmaArgs {
     float* stage_dump;    // optional [n_steps * n_stages][n_paths][32]: the input of every stage (for the adjoint);
                           // reversible Heun: the checkpoints [slot][3][n_paths][32] (y, z, f of every ckpt_stride-th step)
     int ckpt_stride;      // reversible Heun only
+    // the Runge-Kutta backward (tcde_cdeint_fixed_linear_backward) only: the schedule arrays above are reversed, out
+    // receives dL/dz0 [n_paths][32] and stage_dump (optional) the cotangent of every stage's slope, in the forward's slots
+    const float* grad_out;       // [n_paths][n_out][32] output gradients
+    const int32_t* inj_range;    // [n_steps + 2]: grid state r (r = 0: the end of the solve) adds the entries
+                                 // inj_range[r] .. inj_range[r + 1] - 1
+    const int32_t* inj_out;      // output index of each entry
+    const float* inj_weight;     // its weight
 };
 bool solve_tc_supported(int H, int C);
 // tensor-core kernel (solve_tc.cu): Runge-Kutta state in registers; mode 0 = 3xTF32 operand split, mode 1 = 2xFP16 with

@@ -283,8 +283,12 @@ __device__ __forceinline__ void field(const float* zin, float (*dx)[2], float be
 
 }  // namespace wg
 
-// REV: reversible Heun (rev_heun_combine, checkpoints through the stage-dump pointer) instead of the Runge-Kutta methods
-template <bool DUMP, bool REV>
+// REV: reversible Heun (rev_heun_combine, checkpoints through the stage-dump pointer) instead of the Runge-Kutta methods.
+// BWD: the Runge-Kutta backward of the linear field (rk_backward_combine) on the host-reversed schedule: the state is the
+// cotangent ybar, the field product runs on the regrouped weight W2[(k, c)][h] = W[(h, c)][k] with a zero bias, so that
+// the stage product is J_s^T kappa_s; the output gradients are added at every grid state (a.inj_*), the stage inputs
+// kappa_s go to the forward's dump slots (last slot first) and dL/dz0 to a.out.
+template <bool DUMP, bool REV, bool BWD = false>
 __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const UmmaArgs a) {
     using S = BSmem<1>;
     using E = exact<float>;
@@ -331,26 +335,51 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
         }
     };
     auto write_out = [&](int j, const float* v) { store_rows(a.out, a.n_out, j, v); };
+    // BWD: v += the output gradients that land on grid state r (counted from the end of the solve)
+    auto inject = [&](int r, float* v) {
+        for (int e = a.inj_range[r]; e < a.inj_range[r + 1]; ++e) {
+            const int j = a.inj_out[e];
+            const float w = a.inj_weight[e];
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                const int64_t lpath = live[rr] ? path[rr] : a.n_paths - 1;
+                const float2* src = reinterpret_cast<const float2*>(a.grad_out + (lpath * a.n_out + j) * kHid) + q;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float2 t = src[4 * i];
+                    v[8 * rr + 2 * i] = E::add(v[8 * rr + 2 * i], E::mul(w, t.x));
+                    v[8 * rr + 2 * i + 1] = E::add(v[8 * rr + 2 * i + 1], E::mul(w, t.y));
+                }
+            }
+        }
+    };
 
     float y[wg::kNV], k1[wg::kNV], s23[wg::kNV], zin[wg::kNV];
+    int jn = 0, next_out = 0;
+    if constexpr (BWD) {
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-        const int64_t lpath = live[r] ? path[r] : a.n_paths - 1;
-        const float2* zp = reinterpret_cast<const float2*>(a.z0 + lpath * kHid) + q;
+        for (int h = 0; h < wg::kNV; ++h) { y[h] = 0.f; k1[h] = 0.f; s23[h] = 0.f; }
+        inject(0, y);
+        rk_backward_first<wg::kNV>(a, a.step_dt[0], y, zin);
+    } else {
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float2 v = zp[4 * i];
-            y[8 * r + 2 * i] = v.x; y[8 * r + 2 * i + 1] = v.y;
+        for (int r = 0; r < 2; ++r) {
+            const int64_t lpath = live[r] ? path[r] : a.n_paths - 1;
+            const float2* zp = reinterpret_cast<const float2*>(a.z0 + lpath * kHid) + q;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const float2 v = zp[4 * i];
+                y[8 * r + 2 * i] = v.x; y[8 * r + 2 * i + 1] = v.y;
+            }
         }
-    }
 #pragma unroll
-    for (int h = 0; h < wg::kNV; ++h) { k1[h] = 0.f; s23[h] = 0.f; zin[h] = y[h]; }
-    int jn = 0;
-    int next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
-    while (jn < a.n_out && next_out < 0) {                    // outputs at the initial time
-        write_out(jn, y);
-        ++jn;
+        for (int h = 0; h < wg::kNV; ++h) { k1[h] = 0.f; s23[h] = 0.f; zin[h] = y[h]; }
         next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
+        while (jn < a.n_out && next_out < 0) {                    // outputs at the initial time
+            write_out(jn, y);
+            ++jn;
+            next_out = (jn < a.n_out) ? a.out_step[jn] : 0x7fffffff;
+        }
     }
 
     const float* b_bias = reinterpret_cast<const float*>(smem + S::bias);
@@ -369,7 +398,8 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
             }
         }
     };
-    float* dump_at = a.stage_dump;                 // stage st's [path][32] block
+    // stage st's [path][32] block (BWD: the forward's slot of stage st, walking down from the last)
+    float* dump_at = BWD ? a.stage_dump + (int64_t)(n_st - 1) * a.n_paths * kHid : a.stage_dump;
     float dx[2][2];
     {
         float2 raw[2][3];
@@ -381,7 +411,8 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
     for (int st = 0; st < n_st; ++st) {
         if (DUMP && !REV) {
             store_rows(dump_at, 1, 0, zin);
-            dump_at += a.n_paths * kHid;
+            if (BWD) dump_at -= a.n_paths * kHid;
+            else dump_at += a.n_paths * kHid;
         }
         // the next stage's spline rows; their latency hides behind the first half of this stage's products
         float2 nxt[2][3];
@@ -402,6 +433,18 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
                                           store_rows(base + a.n_paths * kHid, 1, 0, vz);
                                           store_rows(base + 2 * a.n_paths * kHid, 1, 0, vf);
                                       });
+        } else if constexpr (BWD) {
+            if (rk_backward_combine<wg::kNV>(a, sub, dt, y, k1, s23, kv, zin)) {
+                ++step;
+                sub = 0;
+                inject(step, y);
+                if (step < a.n_steps) {
+                    dt = a.step_dt[step];
+                    rk_backward_first<wg::kNV>(a, dt, y, zin);
+                }
+            } else {
+                ++sub;
+            }
         } else if (rk_combine<wg::kNV>(a, sub, dt, y, k1, s23, kv, zin)) {
             step_outputs<wg::kNV>(a, step, jn, next_out, y, zin, write_out);
 #pragma unroll
@@ -415,6 +458,7 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
 #pragma unroll
         for (int r = 0; r < 2; ++r) { dx[r][0] = dx_next[r][0]; dx[r][1] = dx_next[r][1]; }
     }
+    if constexpr (BWD) store_rows(a.out, 1, 0, y);
 }
 
 
@@ -642,4 +686,35 @@ extern "C" int tcde_reversible_heun_linear_backward_segment(
                      (int)lo, (int)hi};
     return launch(tc::reversible_backward_kernel, (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths, tc::wg::kThreads,
                   tc::kRevSmem, a, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int tcde_cdeint_fixed_linear_backward(
+    const void* control, int control_kind, int64_t n_rows, const void* weight_t, const void* zeros, const void* grad_out,
+    void* grad_z0, void* kappa_dump, int64_t n_paths, int64_t channels, int64_t hidden, int method, int64_t n_steps,
+    const void* step_dt_rev, const int32_t* stage_index_rev, const void* stage_frac_rev, int64_t n_out,
+    const int32_t* inj_range, const int32_t* inj_out, const void* inj_weight, double sign, int dtype, void* stream) {
+    using namespace tcde;
+    TCDE_CHECK_ARG(control && weight_t && zeros && grad_out && grad_z0, "null data pointer");
+    TCDE_CHECK_ARG(step_dt_rev && stage_index_rev && stage_frac_rev && inj_range && inj_out && inj_weight,
+                   "null schedule pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_steps >= 1 && n_out >= 1, "bad sizes");
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
+    TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
+    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && solve_tc_supported((int)hidden, (int)channels),
+                         "the Runge-Kutta backward kernel is built for fp32, hidden=32, channels=8 (got dtype=%d, "
+                         "hidden=%lld, channels=%lld)", dtype, (long long)hidden, (long long)channels);
+    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(grad_out) |
+                           reinterpret_cast<uintptr_t>(grad_z0) | reinterpret_cast<uintptr_t>(kappa_dump)) & 15) == 0,
+                         "Runge-Kutta backward: control, grad_out, grad_z0 and the dump must be 16-byte aligned");
+    if (n_paths == 0) return TCDE_OK;
+    const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
+    UmmaArgs u{(const float*)control, (const float*)weight_t, (const float*)zeros, nullptr, (float*)grad_z0,
+               (const float*)step_dt_rev, stage_index_rev, (const float*)stage_frac_rev, nullptr, nullptr, nullptr,
+               n_paths, n_rows, control_kind, method, n_stages, (int)n_steps, (int)n_out, (float)sign,
+               (float*)kappa_dump, 0, (const float*)grad_out, inj_range, inj_out, (const float*)inj_weight};
+    return launch(kappa_dump ? tc::cdeint_wgmma_kernel<true, false, true> : tc::cdeint_wgmma_kernel<false, false, true>,
+                  (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths, tc::wg::kThreads, tc::wg::kSmem, u,
+                  static_cast<cudaStream_t>(stream));
 }

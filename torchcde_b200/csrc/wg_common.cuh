@@ -65,6 +65,74 @@ __device__ __forceinline__ bool rk_combine(const UmmaArgs& a, int sub, float dt,
     return true;
 }
 
+// The transpose of rk_combine for a field whose Jacobian J_s does not depend on the state (the linear field): the stages of
+// a step in reverse, sub 0 being its last stage.  yb = the cotangent ybar' of the step's end state, su = the sum of the
+// stage products so far, run = rk4's running combination, kv = u_s = J_s^T kappa_s of the stage just evaluated; the next
+// stage's kappa (the cotangent of its slope) ends up in kap.  rk4 (kappa_4 = dt/8 ybar', rk_backward_first):
+//   kappa_3 = dt (3/8 ybar' + u_4),  kappa_2 = dt (3/8 ybar' - u_4 + u_3),  kappa_1 = dt (1/8 ybar' + u_4 - u_3/3 + u_2/3);
+// midpoint: kappa_1 = dt/2 u_2.  Returns true when the stage closed the step: yb then holds ybar' + sum_s u_s, the
+// cotangent of the step's start state.
+template <int NV>
+__device__ __forceinline__ bool rk_backward_combine(const UmmaArgs& a, int sub, float dt, float* yb, float* su, float* run,
+                                                    const float* kv, float* kap) {
+    using E = exact<float>;
+    if (a.method == TCDE_RK4_38) {
+        const float third = (float)(1.0 / 3.0);
+        if (sub == 0) {
+#pragma unroll
+            for (int h = 0; h < NV; ++h) {
+                su[h] = kv[h];
+                run[h] = kv[h];
+                kap[h] = E::mul(dt, E::add(E::mul(0.375f, yb[h]), kv[h]));
+            }
+        } else if (sub == 1) {
+#pragma unroll
+            for (int h = 0; h < NV; ++h) {
+                kap[h] = E::mul(dt, E::add(E::sub(E::mul(0.375f, yb[h]), run[h]), kv[h]));
+                run[h] = E::sub(run[h], E::mul(kv[h], third));
+                su[h] = E::add(su[h], kv[h]);
+            }
+        } else if (sub == 2) {
+#pragma unroll
+            for (int h = 0; h < NV; ++h) {
+                kap[h] = E::mul(dt, E::add(E::add(E::mul(0.125f, yb[h]), run[h]), E::mul(kv[h], third)));
+                su[h] = E::add(su[h], kv[h]);
+            }
+        } else {
+#pragma unroll
+            for (int h = 0; h < NV; ++h) yb[h] = E::add(yb[h], E::add(su[h], kv[h]));
+            return true;
+        }
+        return false;
+    }
+    if (a.method == TCDE_MIDPOINT) {
+        if (sub == 0) {
+            const float half = E::mul(0.5f, dt);
+#pragma unroll
+            for (int h = 0; h < NV; ++h) {
+                su[h] = kv[h];
+                kap[h] = E::mul(half, kv[h]);
+            }
+            return false;
+        }
+#pragma unroll
+        for (int h = 0; h < NV; ++h) yb[h] = E::add(yb[h], E::add(su[h], kv[h]));
+        return true;
+    }
+#pragma unroll
+    for (int h = 0; h < NV; ++h) yb[h] = E::add(yb[h], kv[h]);
+    return true;
+}
+
+// kappa of a step's last stage from the cotangent ybar' of its end state: dt/8 ybar' (rk4), dt ybar' (midpoint, euler)
+template <int NV>
+__device__ __forceinline__ void rk_backward_first(const UmmaArgs& a, float dt, const float* yb, float* kap) {
+    using E = exact<float>;
+    const float c = (a.method == TCDE_RK4_38) ? E::mul(0.125f, dt) : dt;
+#pragma unroll
+    for (int h = 0; h < NV; ++h) kap[h] = E::mul(c, yb[h]);
+}
+
 // The outputs that fall on the step just completed (y = its start, zin = its end); write(j, v) stores output j.
 template <int NV, typename Write>
 __device__ __forceinline__ void step_outputs(const UmmaArgs& a, int step, int& jn, int& next_out, const float* y,

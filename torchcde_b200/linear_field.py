@@ -9,7 +9,7 @@ import torch
 
 from . import _lib, adaptive
 from .controls import _control_signature, _schedule_knots
-from .schedule import ScheduleCache, host_locator, locate
+from .schedule import ScheduleCache, backward_tables, host_locator, locate
 
 _schedules = ScheduleCache()
 
@@ -194,10 +194,16 @@ class LinearFieldKernels:
         return field
 
     @functools.cached_property
+    def transposed_weights(self):
+        """W with rows regrouped as (k, c) and columns h, and a zero bias: the field product with them is J^T w."""
+        h, c = self.hidden, self.channels
+        return self.w.view(h, c, h).permute(2, 1, 0).contiguous().view(h * c, h), torch.zeros_like(self.b)
+
+    @functools.cached_property
     def adjoint_weights(self):
         """-W with rows regrouped as (k, c) and columns h, and a zero bias: the weights of the adjoint state's own CDE."""
-        h, c = self.hidden, self.channels
-        return self.w.view(h, c, h).permute(2, 1, 0).contiguous().view(h * c, h).neg_(), torch.zeros_like(self.b)
+        w2, zeros = self.transposed_weights
+        return w2.neg(), zeros
 
     def param_grad_scratch_bytes(self, n_paths, n_total):
         return _lib.load().tcde_linear_field_param_grads_scratch_bytes(n_paths, n_total, self.channels, self.hidden)
@@ -254,6 +260,120 @@ class LinearFieldKernels:
         if scratch_bytes < 0:
             return None
         return AdjointStage(self, roles, torch.empty(max(scratch_bytes // 4, 4), dtype=torch.float32, device=self.device))
+
+
+class FixedBackprop:
+    """``cdeint(..., adjoint=False)`` of a fixed-step solve of this linear field with gradients for z0, the weight and /
+    or the bias: the exact gradient of the discrete solve in three launches.  The forward is the stage-dump solve
+    (``tcde_cdeint_fixed_linear_stages``: the outputs are those of the same call without gradients, bit for bit); the
+    backward is ONE launch of ``tcde_cdeint_fixed_linear_backward`` (the transposed Runge-Kutta recurrence over every
+    step, the cotangent kappa of every stage dumped in the forward's slot) and ONE launch of
+    ``tcde_linear_field_param_grads`` over the two dumps (neither without a parameter gradient).
+    ``loop(z0)``: the differentiable torch-operator solve of the same problem, which a backward with ``create_graph``
+    differentiates instead (the kernels give no higher-order derivatives)."""
+
+    def __init__(self, kernels, t, method, step_size, loop):
+        self.kernels, self.method, self.loop = kernels, method, loop
+        self.sched, (_floats, _ints, self.views) = _schedules.get(t, kernels.knots, kernels.n_rows, method, step_size,
+                                                                  kernels.dtype, kernels.device)
+
+    def fits(self, n_paths, want_params):
+        """Whether the stage dump, and with parameter gradients the kappa dump and the scratch of the parameter-gradient
+        kernel, fit in 0.7 of the free device memory (the bound of ``AdjointStage.segment``)."""
+        k = self.kernels
+        n_total = self.sched.n_steps * self.sched.n_stages
+        need = n_total * n_paths * k.hidden * 4
+        if want_params:
+            scratch_bytes = k.param_grad_scratch_bytes(n_paths, n_total)
+            if scratch_bytes < 0:
+                return False
+            need = 2 * need + scratch_bytes
+        with torch.cuda.device(k.device):
+            free, _total = torch.cuda.mem_get_info()
+        return need <= 0.7 * free
+
+    def forward(self, z0):
+        """(the outputs ``(..., n_out, H)``, the input of every stage ``[n_steps * n_stages][paths][H]``)."""
+        k, sched = self.kernels, self.sched
+        with torch.cuda.device(k.device):
+            zf = z0.detach().reshape(-1, k.hidden).contiguous()
+            out = torch.empty(*z0.shape[:-1], sched.n_out, k.hidden, dtype=k.dtype, device=k.device)
+            dump = torch.empty(sched.n_steps * sched.n_stages, zf.size(0), k.hidden, dtype=k.dtype, device=k.device)
+            if zf.size(0) > 0:
+                k._fixed(sched, self.views, k.w, k.b, zf, out.view(-1, sched.n_out, k.hidden), dump)
+        return out, dump
+
+    def backward(self, g, dump, want_w, want_b):
+        """(dL/dz0, dL/dW or None, dL/db or None) for output gradients ``g`` ``(..., n_out, H)``."""
+        k, sched = self.kernels, self.sched
+        hidden, dev = k.hidden, k.device
+        n_total = sched.n_steps * sched.n_stages
+        with torch.cuda.device(dev):
+            gf = g.reshape(-1, sched.n_out, hidden)
+            if not gf.is_contiguous() or gf.data_ptr() % 16:
+                gf = gf.clone(memory_format=torch.contiguous_format)
+            n_paths = gf.size(0)
+            gz = torch.empty(n_paths, hidden, dtype=k.dtype, device=dev)
+            kappa = torch.empty_like(dump) if want_w or want_b else None
+            if n_paths > 0:
+                tables = backward_tables(sched)
+                floats = torch.cat([tables["step_dt"], tables["stage_frac"], tables["inj_weight"]]).to(dev)
+                ints = torch.cat([tables["stage_index"], tables["inj_range"], tables["inj_out"]]).to(dev)
+                ns, nr = sched.n_steps, tables["inj_range"].numel()
+                w_t, zeros = k.transposed_weights
+                _lib.call("tcde_cdeint_fixed_linear_backward", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(w_t),
+                          _lib.ptr(zeros), _lib.ptr(gf), _lib.ptr(gz), _lib.ptr(kappa), n_paths, k.channels, hidden,
+                          _lib.METHODS[sched.method], ns, _lib.ptr(floats[:ns]), _lib.ptr(ints[:n_total]),
+                          _lib.ptr(floats[ns:ns + n_total]), sched.n_out, _lib.ptr(ints[n_total:n_total + nr]),
+                          _lib.ptr(ints[n_total + nr:]), _lib.ptr(floats[ns + n_total:]), float(sched.sign), _lib.F32,
+                          _lib.stream_of(gf))
+            gw = torch.zeros_like(k.w) if want_w else None
+            gb = torch.zeros_like(k.b) if want_b else None
+            if (gw is not None or gb is not None) and n_paths > 0:
+                weights = torch.full((n_total,), float(sched.sign), dtype=k.dtype, device=dev)
+                if not k.param_grads(dump, kappa, self.views["stage_index"], self.views["stage_frac"], weights, n_total,
+                                     gw, gb):
+                    raise RuntimeError("cdeint backward: the parameter-gradient kernel is not built for this problem")
+        return gz.view(g.shape[:-2] + (hidden,)), gw, gb
+
+
+class _FixedBackpropFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, route, z0, weight, bias):
+        out, dump = route.forward(z0)
+        ctx.route = route
+        ctx.save_for_backward(z0, weight, bias, dump)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        z0, weight, bias, dump = ctx.saved_tensors
+        _route_needs, want_z, want_w, want_b = ctx.needs_input_grad
+        if torch.is_grad_enabled():
+            # create_graph: differentiate the torch-operator solve of the same problem, whose gradients are themselves
+            # differentiable
+            inputs = [x for x, want in ((z0, want_z), (weight, want_w), (bias, want_b)) if want]
+            got = iter(torch.autograd.grad(ctx.route.loop(z0), inputs, g, create_graph=True, allow_unused=True))
+            return (None,) + tuple(next(got) if want else None for want in (want_z, want_w, want_b))
+        gz, gw, gb = ctx.route.backward(g, dump, want_w, want_b)
+        return None, gz if want_z else None, gw, gb
+
+
+def fixed_backprop(kernels, z0, t, method, step_size, loop):
+    """``cdeint(..., adjoint=False)``'s outputs ``(..., n_out, H)`` on the three-launch route of ``FixedBackprop``, or
+    None when the route does not serve the problem (the caller runs the torch-operator solve)."""
+    k = kernels
+    if k.dtype != torch.float32 or k.hidden != 32 or k.channels != 8:
+        return None
+    route = FixedBackprop(k, t, method, step_size, loop)
+    want_params = any(p is not None and p.requires_grad for p in (k.weight, k.bias))
+    if not route.fits(k.n_paths, want_params):
+        return None
+    try:
+        return _FixedBackpropFn.apply(route, z0, k.weight, k.bias)
+    except NotImplementedError:
+        # the stage-dump solve refuses the problem (the CUDA-core kernel selected, misaligned rows): nothing ran
+        return None
 
 
 class AdjointStage:

@@ -153,6 +153,39 @@ def build_schedule(t, knots, n_intervals, method, step_size, state_dtype):
     return s
 
 
+def backward_tables(sched):
+    """The tables of ``tcde_cdeint_fixed_linear_backward`` for a fixed-step ``sched`` (CPU tensors): the step widths and
+    the stage intervals / fractions in reverse order, and the output gradients every grid state receives, as a list of
+    (output, weight) entries grouped by grid state counted from the end (``inj_range[r] .. inj_range[r + 1] - 1`` belong
+    to grid state ``n_steps - r``).  Output j after step i lands on that step's start (mode 0, or ``out_step = -1``: z0)
+    or end (mode 1) with weight 1, or, interpolated at slope s (mode 2), on the start with ``1 - s`` and on the end with
+    ``s`` -- the derivatives of ``y + s (y1 - y)``, formed in the state dtype."""
+    n_steps = sched.n_steps
+    by_state = [[] for _ in range(n_steps + 1)]
+    one_minus = (1 - sched.out_slope).tolist()
+    slopes = sched.out_slope.tolist()
+    for j, (step, mode) in enumerate(zip(sched.out_step.tolist(), sched.out_mode.tolist())):
+        if step < 0 or mode == 0:
+            by_state[max(step, 0)].append((j, 1.0))
+        elif mode == 1:
+            by_state[step + 1].append((j, 1.0))
+        else:
+            by_state[step].append((j, one_minus[j]))
+            by_state[step + 1].append((j, slopes[j]))
+    entries = [e for state in reversed(by_state) for e in state]
+    inj_range = [0]
+    for state in reversed(by_state):
+        inj_range.append(inj_range[-1] + len(state))
+    return {
+        "step_dt": sched.step_dt.flip(0),
+        "stage_index": sched.stage_index.reshape(-1).flip(0),
+        "stage_frac": sched.stage_frac.reshape(-1).flip(0),
+        "inj_range": torch.tensor(inj_range, dtype=torch.int32),
+        "inj_out": torch.tensor([j for j, _w in entries], dtype=torch.int32),
+        "inj_weight": torch.tensor([w for _j, w in entries], dtype=sched.out_slope.dtype),
+    }
+
+
 def build_sde_schedule(t, knots, n_intervals, dt, state_dtype):
     """The schedule of torchsde's fixed-step ``integrate`` loop with the reversible Heun method, in the table format of
     ``build_schedule`` (``tcde_cdeint_reversible_heun_linear`` reads it):

@@ -15,7 +15,7 @@ import torch
 
 from . import _lib, adaptive
 from .controls import CubicSpline, _control_signature, _schedule_knots
-from .linear_field import LinearFieldKernels, LinearVectorField, _reverse, linear_field_of  # noqa: F401
+from .linear_field import LinearFieldKernels, LinearVectorField, _reverse, fixed_backprop, linear_field_of  # noqa: F401
 from .mlp_field import MlpFieldKernels, mlp_field_of
 from .schedule import FIXED_METHODS, build_schedule, host_locator
 
@@ -333,7 +333,9 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     ``LinearInterpolation`` control and a linear ``func`` (``LinearVectorField`` or any module
     that is exactly one ``nn.Linear`` + ``view``) the solve is one fused CUDA kernel.  Gradients:
     ``adjoint=True`` runs this package's continuous-adjoint backward (fused kernels for the linear
-    field), ``adjoint=False`` backpropagates through the differentiable generic stage loop.
+    field), ``adjoint=False`` backpropagates through the solve: for the linear field at fp32, hidden 32,
+    channels 8 with gradients for z0 / weight / bias in three launches (``linear_field.FixedBackprop``),
+    otherwise through the differentiable generic stage loop.
 
     ``backend="torchsde"`` is built for ``method="reversible_heun"`` (torchsde's reversible Heun
     method with zero diffusion, fixed step ``dt``, default 1e-3; ``z0`` of shape (batch, hidden),
@@ -502,9 +504,17 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                              "device_controlled": False}
         return out
 
+    # adjoint=False with gradients of a fixed-step linear-field solve: the three-launch route of linear_field.FixedBackprop
+    # serves gradients for z0, the weight and the bias of an fp32 problem at hidden 32 / channels 8; a gradient for
+    # anything else (t, the control's knots or coefficients) keeps the torch-operator solve
+    backprop = (field_params is not None and not adjoint and wants_grad and method in FIXED_METHODS
+                and not t.requires_grad and not any(b.requires_grad for b in X.buffers())
+                and z0.dtype == torch.float32 and z0.size(-1) == 32 and sig[2] == 8
+                and all(b.dtype == torch.float32 and b.device == z0.device for b in X.buffers() if b.is_floating_point())
+                and all(p.dtype == torch.float32 and p.device == z0.device for p in field_params if p is not None))
     # the routes that call a kernel own the linear-field problem; building it checks dtypes and devices
     kernels = None
-    if field_params is not None and (adjoint or not wants_grad):
+    if field_params is not None and (adjoint or not wants_grad or backprop):
         kernels = LinearFieldKernels(X, field_params[0], field_params[1], z0)
     # the fixed-step forward of the examples' MLP field (no gradient, or the forward pass of adjoint=True) is one launch
     mlp = None
@@ -549,6 +559,11 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
 
     # adjoint=False: backpropagate through the solver's own operations, like torchdiffeq.odeint
     if method in FIXED_METHODS:
+        if backprop:
+            ys = fixed_backprop(kernels, z0, t, method, step_size,
+                                lambda y0: _generic_solve(X, func, y0, t, method, step_size, is_prod, True))
+            if ys is not None:
+                return ys
         return _generic_solve(X, func, z0, t, method, step_size, is_prod, sig is not None)
     targets = None
     if t.requires_grad:
