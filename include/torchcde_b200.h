@@ -242,6 +242,51 @@ TCDE_API int tcde_cdeint_fixed_mlp(const void* control, int control_kind, int64_
                           const int32_t* stage_index, const void* stage_frac, int64_t n_out, const int32_t* out_step,
                           const int32_t* out_mode, const void* out_slope, double sign, int dtype, void* stream);
 
+/* tcde_cdeint_fixed_mlp that also stores the INPUT of every stage: stage_dump[n_steps * n_stages][n_paths][hidden] (the
+ * forward state of tcde_cdeint_fixed_mlp_backward).  The outputs equal tcde_cdeint_fixed_mlp's bit for bit.  Served by the
+ * tensor-core kernel only: fp32, hidden = 32, channels = 8, width = 128, 16-byte aligned control, z0, out and dump, solve
+ * variant 0, 4 or 5; TCDE_ERR_UNSUPPORTED otherwise. */
+TCDE_API int tcde_cdeint_fixed_mlp_stages(const void* control, int control_kind, int64_t n_rows, const void* w1,
+                                 const void* b1, const void* w2, const void* b2, const void* z0, void* out,
+                                 void* stage_dump, int64_t n_paths, int64_t channels, int64_t hidden, int64_t width,
+                                 int method, int64_t n_steps, const void* step_dt, const int32_t* stage_index,
+                                 const void* stage_frac, int64_t n_out, const int32_t* out_step, const int32_t* out_mode,
+                                 const void* out_slope, double sign, int dtype, void* stream);
+
+/* The backward pass of tcde_cdeint_fixed_mlp_stages through its own discrete operations (cdeint(..., adjoint=False)): the
+ * transposed Runge-Kutta recurrence of tcde_cdeint_fixed_linear_backward (same kappa / ybar formulas, reversed schedule
+ * arrays and output-gradient lists inj_*) in ONE launch, with the stage product of the MLP field at the forward's stage
+ * input z_s (stage_dump, read from the last slot down):
+ *   u_s = J_s^T kappa_s = W1^T (mask . W2^T g),  g[(h, c)] = (1 - y^2)[(h, c)] kappa_s[h] sign dX_c(t_s),
+ *   y = tanh(W2 h + b2),  h = relu(W1 z_s + b1),  mask = (h > 0)
+ * (h and y recomputed by the forward's own code, so the mask and tanh values are the forward's bits).  grad_z0
+ * [n_paths][hidden] receives dL/dz0; kappa_dump (may be NULL) [n_steps * n_stages][n_paths][hidden] receives kappa_s in the
+ * slot of stage s's input in stage_dump, for tcde_mlp_field_param_grads.  Same support as tcde_cdeint_fixed_mlp_stages
+ * (grad_out and grad_z0 16-byte aligned too). */
+TCDE_API int tcde_cdeint_fixed_mlp_backward(const void* control, int control_kind, int64_t n_rows, const void* w1,
+                                   const void* b1, const void* w2, const void* b2, const void* stage_dump,
+                                   const void* grad_out, void* grad_z0, void* kappa_dump, int64_t n_paths, int64_t channels,
+                                   int64_t hidden, int64_t width, int method, int64_t n_steps, const void* step_dt_rev,
+                                   const int32_t* stage_index_rev, const void* stage_frac_rev, int64_t n_out,
+                                   const int32_t* inj_range, const int32_t* inj_out, const void* inj_weight, double sign,
+                                   int dtype, void* stream);
+
+/* The parameter gradients of tcde_cdeint_fixed_mlp_backward from its two dumps (z_stages = the forward's stage inputs,
+ * kappa_stages = the backward's kappa, both [n_stages_total][n_paths][hidden]):
+ *   grad_w2 += scale sum g h^T,  grad_b2 += scale sum g,  grad_w1 += scale sum ubar z^T,  grad_b1 += scale sum ubar
+ * over every (stage, path), with g and ubar = mask . W2^T g recomputed as the backward forms them (dX/dt from the control at
+ * (stage_index[e], stage_frac[e]) times `sign`).  Any gradient pointer may be NULL.  Tensor cores (2xBF16 split), a
+ * fixed-order reduction: two calls give the same bits.  Same support as tcde_cdeint_fixed_mlp_stages; scratch of
+ * tcde_mlp_field_param_grads_scratch_bytes (-1: not built for the shape). */
+TCDE_API int64_t tcde_mlp_field_param_grads_scratch_bytes(int64_t n_paths, int64_t n_stages_total, int64_t channels,
+                                                 int64_t hidden, int64_t width);
+TCDE_API int tcde_mlp_field_param_grads(const void* control, int control_kind, int64_t n_rows, const void* w1,
+                               const void* b1, const void* w2, const void* b2, const void* z_stages,
+                               const void* kappa_stages, const int32_t* stage_index, const void* stage_frac,
+                               int64_t n_stages_total, void* grad_w1, void* grad_b1, void* grad_w2, void* grad_b2,
+                               void* scratch, int64_t n_paths, int64_t channels, int64_t hidden, int64_t width,
+                               double sign, double scale, int dtype, void* stream);
+
 /* torchsde's reversible Heun method with zero diffusion (cdeint(..., backend="torchsde", method="reversible_heun")) for
  * the same linear field, in ONE launch:
  *   z_{n+1} = 2 y_n - z_n + f_n dt_n,  f_{n+1} = f(t_{n+1}, z_{n+1}),  y_{n+1} = y_n + (f_n + f_{n+1}) (0.5 dt_n)

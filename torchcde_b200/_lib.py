@@ -59,6 +59,13 @@ SIGNATURES = {
                                   _p, _p, _p, _dbl, _int, _p], _int),
     "tcde_cdeint_fixed_mlp": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _int, _i64, _p, _p, _p,
                                _i64, _p, _p, _p, _dbl, _int, _p], _int),
+    "tcde_cdeint_fixed_mlp_stages": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _int, _i64, _p,
+                                      _p, _p, _i64, _p, _p, _p, _dbl, _int, _p], _int),
+    "tcde_cdeint_fixed_mlp_backward": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _int,
+                                        _i64, _p, _p, _p, _i64, _p, _p, _p, _dbl, _int, _p], _int),
+    "tcde_mlp_field_param_grads_scratch_bytes": ([_i64, _i64, _i64, _i64, _i64], _i64),
+    "tcde_mlp_field_param_grads": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _i64, _i64,
+                                    _i64, _i64, _dbl, _dbl, _int, _p], _int),
     "tcde_dopri5_linear_grid": ([_i64], _int),
     "tcde_dopri5_linear_paired_attempts": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _dbl,
                                             _p, _p, _p, _p, _p, _i64, _i64, _i64, _int, _p], _int),

@@ -297,20 +297,21 @@ struct Smem {
 };
 constexpr int kSmem = Smem::bytes + 1024;                    // slack for the 1024-byte alignment of the tiles
 
-// max |x| of two arrays over the CTA (all threads call it; contains __syncthreads)
+// max |x| of two arrays over the CTA of NT threads (all threads call it; contains __syncthreads)
+template <int NT>
 __device__ __forceinline__ void cta_max(float* red, int tid, float& a, float& b, float& c, float& d) {
     float v[4] = {a, b, c, d};
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) v[i] = fmaxf(v[i], __shfl_xor_sync(0xffffffffu, v[i], o));
-        if ((tid & 31) == 0) red[i * (kThreads / 32) + (tid >> 5)] = v[i];
+        if ((tid & 31) == 0) red[i * (NT / 32) + (tid >> 5)] = v[i];
     }
     __syncthreads();
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         v[i] = 0.f;
-        for (int w = 0; w < kThreads / 32; ++w) v[i] = fmaxf(v[i], red[i * (kThreads / 32) + w]);
+        for (int w = 0; w < NT / 32; ++w) v[i] = fmaxf(v[i], red[i * (NT / 32) + w]);
     }
     a = v[0]; b = v[1]; c = v[2]; d = v[3];
 }
@@ -343,21 +344,23 @@ struct Scales {
     float inv1, beta1, inv2, beta2;                          // per weight tile: 1 / weight scale, bias floor
 };
 
+// the split weight tiles and scaled biases in shared memory, by a CTA of NT threads
+template <int NT = kThreads>
 __device__ __forceinline__ Scales prepare(unsigned char* smem, const float* w1, const float* b1, const float* w2,
                                           const float* b2, int tid) {
     float* red = reinterpret_cast<float*>(smem + Smem::red);
     float m1 = 0.f, mb1 = 0.f, m2 = 0.f, mb2 = 0.f;
-    for (int e = tid; e < kWidth * kHid; e += kThreads) m1 = fmaxf(m1, fabsf(w1[e]));
-    for (int e = tid; e < kWidth; e += kThreads) mb1 = fmaxf(mb1, fabsf(b1[e]));
-    for (int e = tid; e < kCols * kWidth; e += kThreads) m2 = fmaxf(m2, fabsf(w2[e]));
-    for (int e = tid; e < kCols; e += kThreads) mb2 = fmaxf(mb2, fabsf(b2[e]));
-    cta_max(red, tid, m1, mb1, m2, mb2);
+    for (int e = tid; e < kWidth * kHid; e += NT) m1 = fmaxf(m1, fabsf(w1[e]));
+    for (int e = tid; e < kWidth; e += NT) mb1 = fmaxf(mb1, fabsf(b1[e]));
+    for (int e = tid; e < kCols * kWidth; e += NT) m2 = fmaxf(m2, fabsf(w2[e]));
+    for (int e = tid; e < kCols; e += NT) mb2 = fmaxf(mb2, fabsf(b2[e]));
+    cta_max<NT>(red, tid, m1, mb1, m2, mb2);
     Scales s;
     float s1, s2;
     split_scales(m1, mb1, s1, s.inv1, s.beta1);
     split_scales(m2, mb2, s2, s.inv2, s.beta2);
     __half* t1 = reinterpret_cast<__half*>(smem + Smem::w1);
-    for (int e = tid; e < kWidth * kHid; e += kThreads) {     // [128 rows][hi k 0..31 | lo k 0..31], 16-byte chunks swizzled
+    for (int e = tid; e < kWidth * kHid; e += NT) {     // [128 rows][hi k 0..31 | lo k 0..31], 16-byte chunks swizzled
         const int n = e >> 5, k = e & 31;
         const float w = w1[e] * s1;
         const __half hi = __float2half_rn(w);
@@ -366,7 +369,7 @@ __device__ __forceinline__ Scales prepare(unsigned char* smem, const float* w1, 
         t1[n * 64 + ((((k >> 3) + 4) ^ (n & 7)) << 3) + (k & 7)] = lo;
     }
     __half* t2 = reinterpret_cast<__half*>(smem + Smem::w2);
-    for (int e = tid; e < kCols * kWidth; e += kThreads) {    // region (piece, k block): [256 rows][64 halves], swizzled
+    for (int e = tid; e < kCols * kWidth; e += NT) {    // region (piece, k block): [256 rows][64 halves], swizzled
         const int n = e >> 7, k = e & 127, kb = k >> 6, kk = k & 63;
         const float w = w2[e] * s2;
         const __half hi = __float2half_rn(w);
@@ -377,20 +380,20 @@ __device__ __forceinline__ Scales prepare(unsigned char* smem, const float* w1, 
     }
     float* sb1 = reinterpret_cast<float*>(smem + Smem::b1);
     float* sb2 = reinterpret_cast<float*>(smem + Smem::b2);
-    for (int n = tid; n < kWidth; n += kThreads) sb1[n] = b1[n] * s1;   // powers of two: exact
-    for (int n = tid; n < kCols; n += kThreads) sb2[n] = b2[n] * s2;
+    for (int n = tid; n < kWidth; n += NT) sb1[n] = b1[n] * s1;   // powers of two: exact
+    for (int n = tid; n < kCols; n += NT) sb2[n] = b2[n] * s2;
     return s;
 }
 
-// One evaluation of the MLP field for the warpgroup's 64 rows: kv = tanh(W2 relu(W1 zin + b1) + b2) . dx in the fragment
-// layout; dx: the lane's two channels of both rows, times the sign of the time direction.  mid() runs during the second
-// product (the caller's next dX/dt hides behind the MMAs).
-template <typename Mid>
-__device__ __forceinline__ void field(const float* zin, const float (*dx)[2], const Scales& sc, const float* sb1,
-                                      const float* sb2, uint32_t tile1, uint32_t tile2, int q, float* kv, Mid mid) {
+// Steps 1 and 2 of field for the warpgroup's 64 rows: h = relu(W1 zin + b1), unscaled, into u (column 64 c + 8 j + 2 q + e
+// of row r at u[c][4 j + 2 r + e]), and the second product's row scales rs / inv2 (times 1 / weight scale) and hi / lo A
+// fragments [k step][4].  The backward kernels call it too, so that their ReLU masks and tanh values are the forward's bits.
+__device__ __forceinline__ void hidden_layer(const float* zin, const Scales& sc, const float* sb1, uint32_t tile1, int q,
+                                             float (*u)[wg::kAcc], float* rs, float* inv2, uint32_t (*bhi)[4],
+                                             uint32_t (*blo)[4]) {
     using namespace wg;
     // 1. u = z W1^T + b1, row-scaled: A from the stage input as in wg::field
-    float rs[2], inv[2];
+    float inv[2];
     uint32_t ahi[2][4], alo[2][4];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -409,7 +412,6 @@ __device__ __forceinline__ void field(const float* zin, const float (*dx)[2], co
             const int r = t & 1, v = 8 * r + 4 * k + 2 * (t >> 1);
             split_h2(__fmul_rn(zin[v], rs[r]), __fmul_rn(zin[v + 1], rs[r]), ahi[k][t], alo[k][t]);
         }
-    float u[2][kAcc];                                         // column 64 c + 8 j + 2 q + e of row r at u[c][4 j + 2 r + e]
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
 #pragma unroll
@@ -446,7 +448,6 @@ __device__ __forceinline__ void field(const float* zin, const float (*dx)[2], co
             u[c][i] = h;
             m2[r] = fmaxf(m2[r], h);
         }
-    float inv2[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         m2[r] = fmaxf(m2[r], __shfl_xor_sync(0xffffffffu, m2[r], 1));
@@ -454,7 +455,6 @@ __device__ __forceinline__ void field(const float* zin, const float (*dx)[2], co
         row_scale(m2[r], rs[r], inv2[r]);
         inv2[r] *= sc.inv2;
     }
-    uint32_t bhi[8][4], blo[8][4];
 #pragma unroll
     for (int k = 0; k < 8; ++k)
 #pragma unroll
@@ -463,36 +463,53 @@ __device__ __forceinline__ void field(const float* zin, const float (*dx)[2], co
             split_h2(__fmul_rn(u[c][4 * j + 2 * r], rs[r]), __fmul_rn(u[c][4 * j + 2 * r + 1], rs[r]), bhi[k][t],
                      blo[k][t]);
         }
+}
+
+// Step 3 of field for one chunk (hidden units 8 chunk .. 8 chunk + 7): d = (h W2^T + b2) of the chunk's 64 columns, scaled
+// by the rows' rs and the weight scale, as 24 wgmmas committed as one group (small terms first)
+__device__ __forceinline__ void issue_v(int chunk, float* d, const float* sb2, const float* rs, uint32_t tile2, int q,
+                                        const uint32_t (*bhi)[4], const uint32_t (*blo)[4]) {
+    using namespace wg;
+#pragma unroll
+    for (int j = 0; j < kN / 8; ++j) {
+        const float2 bb = *reinterpret_cast<const float2*>(sb2 + chunk * kN + 8 * j + 2 * q);
+        d[4 * j + 0] = bb.x * rs[0]; d[4 * j + 1] = bb.y * rs[0];
+        d[4 * j + 2] = bb.x * rs[1]; d[4 * j + 3] = bb.y * rs[1];
+    }
+    mma_fence();
+    const uint32_t rows = tile2 + chunk * kN * 128;
+    const uint32_t hi = rows, lo = rows + 2 * kW2Region;      // piece regions; k block kb at + kb * kW2Region
+#pragma unroll
+    for (int k = 0; k < 8; ++k)                                // h_lo . W2_hi
+        mma_m64n64k16(d, blo[k], desc_sw128(hi + (k >> 2) * kW2Region + 32 * (k & 3)));
+#pragma unroll
+    for (int k = 0; k < 8; ++k)                                // h_hi . W2_lo
+        mma_m64n64k16(d, bhi[k], desc_sw128(lo + (k >> 2) * kW2Region + 32 * (k & 3)));
+#pragma unroll
+    for (int k = 0; k < 8; ++k)                                // h_hi . W2_hi
+        mma_m64n64k16(d, bhi[k], desc_sw128(hi + (k >> 2) * kW2Region + 32 * (k & 3)));
+    mma_commit();
+}
+
+// One evaluation of the MLP field for the warpgroup's 64 rows: kv = tanh(W2 relu(W1 zin + b1) + b2) . dx in the fragment
+// layout; dx: the lane's two channels of both rows, times the sign of the time direction.  mid() runs during the second
+// product (the caller's next dX/dt hides behind the MMAs).
+template <typename Mid>
+__device__ __forceinline__ void field(const float* zin, const float (*dx)[2], const Scales& sc, const float* sb1,
+                                      const float* sb2, uint32_t tile1, uint32_t tile2, int q, float* kv, Mid mid) {
+    using namespace wg;
+    float u[2][kAcc], rs[2], inv2[2];
+    uint32_t bhi[8][4], blo[8][4];
+    hidden_layer(zin, sc, sb1, tile1, q, u, rs, inv2, bhi, blo);
 
     // 3. v = h W2^T + b2 in four chunks of 64 columns, 4. tanh, contraction with dX/dt
     float acc[2][kAcc];
-    auto issue = [&](int chunk, float* d) {
-#pragma unroll
-        for (int j = 0; j < kN / 8; ++j) {
-            const float2 bb = *reinterpret_cast<const float2*>(sb2 + chunk * kN + 8 * j + 2 * q);
-            d[4 * j + 0] = bb.x * rs[0]; d[4 * j + 1] = bb.y * rs[0];
-            d[4 * j + 2] = bb.x * rs[1]; d[4 * j + 3] = bb.y * rs[1];
-        }
-        mma_fence();
-        const uint32_t rows = tile2 + chunk * kN * 128;
-        const uint32_t hi = rows, lo = rows + 2 * kW2Region;  // piece regions; k block kb at + kb * kW2Region
-#pragma unroll
-        for (int k = 0; k < 8; ++k)                            // h_lo . W2_hi
-            mma_m64n64k16(d, blo[k], desc_sw128(hi + (k >> 2) * kW2Region + 32 * (k & 3)));
-#pragma unroll
-        for (int k = 0; k < 8; ++k)                            // h_hi . W2_lo
-            mma_m64n64k16(d, bhi[k], desc_sw128(lo + (k >> 2) * kW2Region + 32 * (k & 3)));
-#pragma unroll
-        for (int k = 0; k < 8; ++k)                            // h_hi . W2_hi
-            mma_m64n64k16(d, bhi[k], desc_sw128(hi + (k >> 2) * kW2Region + 32 * (k & 3)));
-        mma_commit();
-    };
-    issue(0, acc[0]);
+    issue_v(0, acc[0], sb2, rs, tile2, q, bhi, blo);
 #pragma unroll
     for (int c = 0; c < kChunks; ++c) {
         float* d = acc[c & 1];
         if (c + 1 < kChunks) {
-            issue(c + 1, acc[(c + 1) & 1]);
+            issue_v(c + 1, acc[(c + 1) & 1], sb2, rs, tile2, q, bhi, blo);
             mma_wait<1>();
         } else {
             mma_wait<0>();
@@ -512,6 +529,8 @@ __device__ __forceinline__ void field(const float* zin, const float (*dx)[2], co
     }
 }
 
+// DUMP: the input of every stage also goes to a.stage_dump[stage][path][32] (the forward state of the backward kernels)
+template <bool DUMP>
 __global__ void __launch_bounds__(kThreads, 1) cdeint_mlp_wgmma_kernel(const UmmaArgs a, const float* w2, const float* b2) {
     using E = exact<float>;
     extern __shared__ unsigned char smem_unaligned[];
@@ -602,7 +621,18 @@ __global__ void __launch_bounds__(kThreads, 1) cdeint_mlp_wgmma_kernel(const Umm
     }
     int step = 0, sub = 0;
     float dt = a.step_dt[0];
+    float* dump_at = a.stage_dump;
     for (int st = 0; st < n_st; ++st) {
+        if (DUMP) {
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                if (!live[r]) continue;
+                float2* dst = reinterpret_cast<float2*>(dump_at + path[r] * kHid) + q;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) dst[4 * i] = make_float2(zin[8 * r + 2 * i], zin[8 * r + 2 * i + 1]);
+            }
+            dump_at += a.n_paths * kHid;
+        }
         float2 nxt[2][3];
         float dx_next[2][2];
         if (st + 1 < n_st) fetch(a.stage_index[st + 1], nxt);
@@ -625,10 +655,647 @@ __global__ void __launch_bounds__(kThreads, 1) cdeint_mlp_wgmma_kernel(const Umm
     }
 }
 
+// ---- the backward of the tensor-core solve (cdeint(..., adjoint=False)): the transposed Runge-Kutta recurrence ---------
+//
+// F_s(z) = tanh(v).view(H, C) dX_s with v = W2 h + b2, h = relu(W1 z + b1), so the stage product is
+//   u_s = J_s^T kappa_s = W1^T (mask . W2^T g),   g[(h, c)] = (1 - y^2)[(h, c)] kappa_s[h] dX_s[c],   mask = (h > 0),
+// evaluated at the forward's stage input z_s (read back from its dump).  hidden_layer and issue_v recompute h and v with
+// the forward's own code, so the mask and tanh values are the forward's bits.  The two transposed products read the
+// forward's K-major tiles as MN-major B operands through ldmatrix.trans and run as warp-level m16n8k16 MMAs on the same
+// fragment layout (2xFP16 split, per-row powers of two, small terms first).  g (256 columns) is too large to keep as A
+// fragments next to h's, so each warp parks its 16 rows of g in shared memory (fp32) and scales them by the exact row
+// max; that tile is why the CTA holds ONE warpgroup: 145 KB of weights + 4 x 16.5 KB of g fit in 227 KB, 8 warps' would not.
+constexpr int kBwdThreads = wg::kThreads;
+constexpr int kGStride = kCols + 8;                          // floats per row of a warp's g tile (rows g, g + 4 8 banks apart)
+struct BwdSmem {
+    static constexpr int g = Smem::bytes;                    // per warp: [16 rows][kGStride] floats
+    static constexpr int bytes = g + (kBwdThreads / 32) * 16 * kGStride * 4;
+};
+constexpr int kBwdSmem = BwdSmem::bytes + 1024;
+
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t* r) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(addr)
+                 : "memory");
+}
+
+// g of one chunk (columns 64 c + 8 j + 2 q + e: unit 8 c + j, channel 2 q + e) from its scaled accumulator d:
+// gc[4 j + 2 r + e] = (1 - y^2) kc[r][j] dx[r][e], kc[r][j] = kappa of unit 8 c + j of row r
+__device__ __forceinline__ void slope_cotangent(const float* d, const float* inv2, const float (*kc)[8], const float (*dx)[2],
+                                                float* gc) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const float y = tanhf(__fmul_rn(d[4 * j + 2 * r + e], inv2[r]));
+                gc[4 * j + 2 * r + e] = __fmul_rn(__fsub_rn(1.f, __fmul_rn(y, y)), __fmul_rn(kc[r][j], dx[r][e]));
+            }
+}
+
+// hd = g W2 (K = 256, N = 128) for the warp's 16 rows: g from the warp's tile gt scaled per row by rsg, W2 from the
+// forward's tile.  hd[j][2 r + e]: column 8 j + 2 q + e of row g + 8 r.
+__device__ __forceinline__ void hdot_product(const float* gt, const float* rsg, uint32_t tile2, int lane, float (*hd)[4]) {
+    const int g = lane >> 2, q = lane & 3;
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) hd[j][i] = 0.f;
+    const int nl = (lane & 7) + 8 * ((lane >> 3) & 1);       // the W2 row (within the k step) this lane addresses
+#pragma unroll 1
+    for (int ks = 0; ks < kCols / 16; ++ks) {
+        uint32_t ahi[4], alo[4];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {                          // register t: row t & 1, columns 16 ks + 8 (t >> 1) + 2 q, +1
+            const int r = t & 1;
+            const float2 v = *reinterpret_cast<const float2*>(gt + (g + 8 * r) * kGStride + 16 * ks + 8 * (t >> 1) + 2 * q);
+            split_h2(__fmul_rn(v.x, rsg[r]), __fmul_rn(v.y, rsg[r]), ahi[t], alo[t]);
+        }
+        const int n = 16 * ks + nl;
+#pragma unroll
+        for (int np = 0; np < 8; ++np) {
+            const int chunk = 2 * np + (lane >> 4);            // W2 columns 8 chunk .. 8 chunk + 7
+            const uint32_t at = tile2 + (chunk >> 3) * kW2Region + n * 128 + (((chunk & 7) ^ (n & 7)) << 4);
+            uint32_t bh[4], bl[4];
+            ldsm_x4_t(at, bh);
+            ldsm_x4_t(at + 2 * kW2Region, bl);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {                      // small terms first
+                mma_f16(hd[2 * np + h], alo, bh[2 * h], bh[2 * h + 1]);
+                mma_f16(hd[2 * np + h], ahi, bl[2 * h], bl[2 * h + 1]);
+                mma_f16(hd[2 * np + h], ahi, bh[2 * h], bh[2 * h + 1]);
+            }
+        }
+    }
+}
+
+// max |x| over each of the lane's two rows, reduced over the quad
+__device__ __forceinline__ void quad_row_max(float* m) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+        m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 1));
+        m[r] = fmaxf(m[r], __shfl_xor_sync(0xffffffffu, m[r], 2));
+    }
+}
+
+// The part of a stage's backward both kernels share: g of every chunk into the warp's tile gt, then ub = mask . (W2^T g)
+// unscaled (ub[j][2 r + e]: hidden unit 8 j + 2 q + e of row r).  kap: the lane's kappa in the state layout.
+__device__ __forceinline__ void stage_ubar(const float* zs, const float* kap, const float (*dx)[2], const Scales& sc,
+                                           const float* sb1, const float* sb2, uint32_t tile1, uint32_t tile2, int lane,
+                                           float* gt, float (*ub)[4]) {
+    using namespace wg;
+    const int g = lane >> 2, q = lane & 3;
+    float u[2][kAcc], rs[2], inv2[2];
+    uint32_t bhi[8][4], blo[8][4];
+    hidden_layer(zs, sc, sb1, tile1, q, u, rs, inv2, bhi, blo);
+    uint32_t mask[2] = {0u, 0u};
+#pragma unroll
+    for (int c = 0; c < 2; ++c)
+#pragma unroll
+        for (int i = 0; i < kAcc; ++i) mask[c] |= (u[c][i] > 0.f ? 1u : 0u) << i;
+    float acc[2][kAcc], gmax[2] = {0.f, 0.f};
+    issue_v(0, acc[0], sb2, rs, tile2, q, bhi, blo);
+#pragma unroll
+    for (int c = 0; c < kChunks; ++c) {
+        float* d = acc[c & 1];
+        if (c + 1 < kChunks) {
+            issue_v(c + 1, acc[(c + 1) & 1], sb2, rs, tile2, q, bhi, blo);
+            mma_wait<1>();
+        } else {
+            mma_wait<0>();
+        }
+        pin(d);
+        float kc[2][8], gc[kAcc];
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) kc[r][j] = __shfl_sync(0xffffffffu, kap[8 * r + 2 * c + (j & 1)], (lane & ~3) | (j >> 1));
+        slope_cotangent(d, inv2, kc, dx, gc);
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                *reinterpret_cast<float2*>(gt + (g + 8 * r) * kGStride + 64 * c + 8 * j + 2 * q) =
+                    make_float2(gc[4 * j + 2 * r], gc[4 * j + 2 * r + 1]);
+                gmax[r] = fmaxf(gmax[r], fmaxf(fabsf(gc[4 * j + 2 * r]), fabsf(gc[4 * j + 2 * r + 1])));
+            }
+    }
+    __syncwarp();
+    quad_row_max(gmax);
+    float rsg[2], invg[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) row_scale(gmax[r], rsg[r], invg[r]);
+    hdot_product(gt, rsg, tile2, lane, ub);
+    __syncwarp();                                              // the tile is rewritten next
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int r = i >> 1;
+            const float v = __fmul_rn(__fmul_rn(ub[j][i], invg[r]), sc.inv2);
+            ub[j][i] = ((mask[j >> 3] >> (4 * (j & 7) + i)) & 1u) ? v : 0.f;
+        }
+}
+
+// kv = W1^T ub (K = 128, N = 32) in the state layout kv[8 r + 2 i + e] (unit 8 i + 2 q + e of row r)
+__device__ __forceinline__ void input_product(const float (*ub)[4], float inv1, uint32_t tile1, int lane, float* kv) {
+    float m[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) m[i >> 1] = fmaxf(m[i >> 1], fabsf(ub[j][i]));
+    quad_row_max(m);
+    float rs[2], inv[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) row_scale(m[r], rs[r], inv[r]);
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[i][e] = 0.f;
+    const int nl = (lane & 7) + 8 * ((lane >> 3) & 1);
+#pragma unroll
+    for (int kk = 0; kk < kWidth / 16; ++kk) {
+        uint32_t ahi[4], alo[4];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {                          // A column 16 kk + 8 (t >> 1) + 2 q = ub tile 2 kk + (t >> 1)
+            const int r = t & 1, j = 2 * kk + (t >> 1);
+            split_h2(__fmul_rn(ub[j][2 * r], rs[r]), __fmul_rn(ub[j][2 * r + 1], rs[r]), ahi[t], alo[t]);
+        }
+        const int n = 16 * kk + nl;                            // W1 row = hidden unit
+#pragma unroll
+        for (int p = 0; p < 2; ++p) {
+            const int chunk = 2 * p + (lane >> 4);
+            uint32_t bh[4], bl[4];
+            ldsm_x4_t(tile1 + n * 128 + ((chunk ^ (n & 7)) << 4), bh);
+            ldsm_x4_t(tile1 + n * 128 + (((chunk + 4) ^ (n & 7)) << 4), bl);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                mma_f16(acc[2 * p + h], alo, bh[2 * h], bh[2 * h + 1]);
+                mma_f16(acc[2 * p + h], ahi, bl[2 * h], bl[2 * h + 1]);
+                mma_f16(acc[2 * p + h], ahi, bh[2 * h], bh[2 * h + 1]);
+            }
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) kv[8 * r + 2 * i + e] = __fmul_rn(__fmul_rn(acc[i][2 * r + e], inv[r]), inv1);
+}
+
+// The lane's rows of the warpgroup's 64 paths, the control reads and dX/dt of cdeint_mlp_wgmma_kernel, for the backward
+// kernels (path0: the first of the 64)
+struct BwdRows {
+    int64_t path[2], lpath[2];
+    bool live[2];
+    const float2* crow;
+    int row1, row_f2;
+    bool cubic;
+    float sign;
+
+    __device__ __forceinline__ BwdRows(const float* control, int control_kind, int64_t n_rows, int64_t n_paths,
+                                       int64_t path0, int warp, int g, int q, float sgn) {
+        cubic = (control_kind == TCDE_CONTROL_CUBIC);
+        row_f2 = (cubic ? 4 * kCh : kCh) / 2;
+        sign = sgn;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            path[r] = path0 + 16 * warp + g + 8 * r;
+            live[r] = path[r] < n_paths;
+            lpath[r] = live[r] ? path[r] : n_paths - 1;
+        }
+        row1 = (int)(lpath[1] - lpath[0]);
+        crow = reinterpret_cast<const float2*>(control + lpath[0] * n_rows * (2 * row_f2) + (cubic ? kCh : 0)) + q;
+    }
+    __device__ __forceinline__ void fetch(int64_t n_rows, int interval, float2 (*raw)[3]) const {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const float2* src = crow + (r * row1 * n_rows + interval) * row_f2;
+            raw[r][0] = __ldg(src);
+            if (cubic) { raw[r][1] = __ldg(src + 4); raw[r][2] = __ldg(src + 8); }
+        }
+    }
+    // dX/dt at fraction fr, channels 2q, 2q + 1 of both rows, times the sign (the forward's slope, bit for bit)
+    __device__ __forceinline__ void slope(const float2 (*raw)[3], float fr, float (*dx)[2]) const {
+        using E = exact<float>;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            if (cubic) {
+                dx[r][0] = E::add(raw[r][0].x, E::mul(E::add(raw[r][1].x, E::mul(raw[r][2].x, fr)), fr));
+                dx[r][1] = E::add(raw[r][0].y, E::mul(E::add(raw[r][1].y, E::mul(raw[r][2].y, fr)), fr));
+            } else {
+                dx[r][0] = raw[r][0].x;
+                dx[r][1] = raw[r][0].y;
+            }
+            dx[r][0] = E::mul(dx[r][0], sign);
+            dx[r][1] = E::mul(dx[r][1], sign);
+        }
+    }
+    // the lane's 16 values of a [path][32] block (dead rows read the last path)
+    __device__ __forceinline__ void load(const float* base, int q, float* v) const {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const float2* src = reinterpret_cast<const float2*>(base + lpath[r] * kHid) + q;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const float2 t = src[4 * i];
+                v[8 * r + 2 * i] = t.x; v[8 * r + 2 * i + 1] = t.y;
+            }
+        }
+    }
+    __device__ __forceinline__ void store(float* base, int q, const float* v) const {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            if (!live[r]) continue;
+            float2* dst = reinterpret_cast<float2*>(base + path[r] * kHid) + q;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) dst[4 * i] = make_float2(v[8 * r + 2 * i], v[8 * r + 2 * i + 1]);
+        }
+    }
+};
+
+// The Runge-Kutta backward of the MLP field on the host-reversed schedule (a.step_dt etc. reversed, as in
+// tcde_cdeint_fixed_linear_backward): the state is the cotangent ybar, the output gradients a.grad_out are added at every
+// grid state (a.inj_*), kappa_s goes to a.stage_dump (when given) in the forward's slot, dL/dz0 to a.out.  z_dump: the
+// forward's stage inputs.
+__global__ void __launch_bounds__(kBwdThreads, 1) cdeint_mlp_backward_kernel(const UmmaArgs a, const float* w2,
+                                                                             const float* b2, const float* z_dump) {
+    using E = exact<float>;
+    extern __shared__ unsigned char smem_unaligned[];
+    unsigned char* smem = smem_unaligned + ((1024u - (smem_u32(smem_unaligned) & 1023u)) & 1023u);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
+    const Scales sc = prepare<kBwdThreads>(smem, a.weight, a.bias, w2, b2, tid);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    const float* sb1 = reinterpret_cast<const float*>(smem + Smem::b1);
+    const float* sb2 = reinterpret_cast<const float*>(smem + Smem::b2);
+    const uint32_t tile1 = smem_u32(smem + Smem::w1), tile2 = smem_u32(smem + Smem::w2);
+    float* gt = reinterpret_cast<float*>(smem + BwdSmem::g) + warp * 16 * kGStride;
+    const BwdRows rows(a.control, a.control_kind, a.n_rows, a.n_paths, (int64_t)blockIdx.x * wg::kPaths, warp, g, q,
+                       a.sign < 0.f ? -1.f : 1.f);
+
+    // v += the output gradients that land on grid state r (counted from the end of the solve)
+    auto inject = [&](int r, float* v) {
+        for (int e = a.inj_range[r]; e < a.inj_range[r + 1]; ++e) {
+            const int j = a.inj_out[e];
+            const float w = a.inj_weight[e];
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                const float2* src = reinterpret_cast<const float2*>(a.grad_out + (rows.lpath[rr] * a.n_out + j) * kHid) + q;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const float2 t = src[4 * i];
+                    v[8 * rr + 2 * i] = E::add(v[8 * rr + 2 * i], E::mul(w, t.x));
+                    v[8 * rr + 2 * i + 1] = E::add(v[8 * rr + 2 * i + 1], E::mul(w, t.y));
+                }
+            }
+        }
+    };
+
+    float yb[wg::kNV], su[wg::kNV], run[wg::kNV], kap[wg::kNV];
+#pragma unroll
+    for (int h = 0; h < wg::kNV; ++h) { yb[h] = 0.f; su[h] = 0.f; run[h] = 0.f; }
+    inject(0, yb);
+    rk_backward_first<wg::kNV>(a, a.step_dt[0], yb, kap);
+
+    const int n_st = a.n_steps * a.n_stages;
+    const int64_t plane = a.n_paths * kHid;
+    const float* z_at = z_dump + (int64_t)(n_st - 1) * plane;     // stage st's forward slot, walking down
+    float* k_at = a.stage_dump ? a.stage_dump + (int64_t)(n_st - 1) * plane : nullptr;
+    float dx[2][2];
+    {
+        float2 raw[2][3];
+        rows.fetch(a.n_rows, a.stage_index[0], raw);
+        rows.slope(raw, a.stage_frac[0], dx);
+    }
+    int step = 0, sub = 0;
+    float dt = a.step_dt[0];
+    for (int st = 0; st < n_st; ++st) {
+        if (k_at) {
+            rows.store(k_at, q, kap);
+            k_at -= plane;
+        }
+        float zs[wg::kNV];
+        rows.load(z_at, q, zs);
+        z_at -= plane;
+        float2 nxt[2][3];
+        if (st + 1 < n_st) rows.fetch(a.n_rows, a.stage_index[st + 1], nxt);
+        float ub[16][4], kv[wg::kNV];
+        stage_ubar(zs, kap, dx, sc, sb1, sb2, tile1, tile2, lane, gt, ub);
+        input_product(ub, sc.inv1, tile1, lane, kv);
+        if (st + 1 < n_st) rows.slope(nxt, a.stage_frac[st + 1], dx);
+        if (rk_backward_combine<wg::kNV>(a, sub, dt, yb, su, run, kv, kap)) {
+            ++step;
+            sub = 0;
+            inject(step, yb);
+            if (step < a.n_steps) {
+                dt = a.step_dt[step];
+                rk_backward_first<wg::kNV>(a, dt, yb, kap);
+            }
+        } else {
+            ++sub;
+        }
+    }
+    rows.store(a.out, q, yb);
+}
+
+// ---- the parameter gradients of the backward: dW2, db2 (blockIdx.y = chunk b < 4) and dW1, db1 (blockIdx.y = 4) --------
+//
+//   dW2 = sum_e g_e h_e^T,  db2 = sum_e g_e,  dW1 = sum_e ub_e z_e^T,  db1 = sum_e ub_e
+// over the items e = (stage, path), with g and ub recomputed from (z_s, kappa_s, dX_s) as the backward kernel forms them
+// (they are far too large to store).  Work item = one stage x 64 paths, dealt to persistent CTAs of one warpgroup; each
+// CTA's y index picks what it accumulates, so its accumulators stay in registers:
+//   * y = b < 4: v of chunk b only (its 64 columns of g need h but one quarter of the second product); g_b and h go to
+//     shared memory and G_b^T [H | 1] (K = 64 items, M = 64, N = 128 + a column of ones for db2) runs as m16n8k16 MMAs;
+//   * y = 4: the whole ub (stage_ubar), then ub^T [z | 1] (M = 128, N = 32 + ones).
+// Operands are split into two BF16 pieces (no scaling; three MMAs, small terms first), each item is accumulated in
+// fresh registers and added to the CTA's running sums in fp32, and the per-CTA sums are added in a fixed order by
+// mlp_param_reduce_kernel: two runs give the same bits.
+constexpr int kPgY = wg::kChunks + 1;
+constexpr int kPgParams = kWidth * kHid + kWidth + kCols * kWidth + kCols;   // [W1 | b1 | W2 | b2]
+constexpr int kOffB1 = kWidth * kHid, kOffW2 = kOffB1 + kWidth, kOffB2 = kOffW2 + kCols * kWidth;
+constexpr int kGS = wg::kN + 4, kHS = kWidth + 4, kZS = kHid + 4;             // padded fp32 staging rows
+struct PgSmem {
+    static constexpr int stage = BwdSmem::g;                 // y < 4: G [64][kGS], H [64][kHS]; y = 4: the g tiles, then
+    static constexpr int h = stage + 64 * kGS * 4;           // per warp ub [16][kHS] and z [16][kZS] in its own tile
+    static constexpr int bytes_b = h + 64 * kHS * 4;
+    static constexpr int bytes = bytes_b > BwdSmem::bytes ? bytes_b : BwdSmem::bytes;
+};
+constexpr int kPgSmem = PgSmem::bytes + 1024;
+
+__device__ __forceinline__ uint32_t pack_bf2(float lo, float hi) {
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
+}
+__device__ __forceinline__ float bf_round(float x) { return __uint_as_float(pack_bf2(x, 0.f) << 16); }
+__device__ __forceinline__ void split_bf2(float v0, float v1, uint32_t& hi, uint32_t& lo) {
+    const float h0 = bf_round(v0), h1 = bf_round(v1);
+    hi = pack_bf2(h0, h1);
+    lo = pack_bf2(__fsub_rn(v0, h0), __fsub_rn(v1, h1));
+}
+__device__ __forceinline__ void mma_bf16(float* c, const uint32_t* a, uint32_t b0, uint32_t b1) {
+    asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+
+// acc[m][t] += sum over the 64 items i of A[i][row] B[i][col] for the warp's MT m-tiles of rows and NT n-tiles of columns
+// (the last n-tile: a column of ones, then zeros).  a(i, row), b(i, col): the staged fp32 values.
+template <int MT, int NT, typename FA, typename FB>
+__device__ __forceinline__ void outer_items(float (*acc)[NT][4], int row0, int lane, FA a, FB b) {
+    const int g = lane >> 2, q = lane & 3;
+    float part[MT][NT][4];
+#pragma unroll
+    for (int m = 0; m < MT; ++m)
+#pragma unroll
+        for (int t = 0; t < NT; ++t)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) part[m][t][i] = 0.f;
+#pragma unroll 1
+    for (int i0 = 0; i0 < 64; i0 += 16) {
+        uint32_t bh[NT][2], bl[NT][2];
+#pragma unroll
+        for (int t = 0; t < NT; ++t)
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {                      // b0 / b1: items i0 + 2 q (+1) + 8 r, column 8 t + g
+                const int i = i0 + 2 * q + 8 * r, col = 8 * t + g;
+                if (t == NT - 1) {
+                    const float one = (g == 0) ? 1.f : 0.f;
+                    bh[t][r] = pack_bf2(one, one);
+                    bl[t][r] = 0u;
+                } else {
+                    split_bf2(b(i, col), b(i + 1, col), bh[t][r], bl[t][r]);
+                }
+            }
+#pragma unroll
+        for (int m = 0; m < MT; ++m) {
+            uint32_t ah[4], al[4];
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {                      // register t: row g + 8 (t & 1), items i0 + 2 q + 8 (t >> 1), +1
+                const int row = row0 + 16 * m + g + 8 * (t & 1), i = i0 + 2 * q + 8 * (t >> 1);
+                split_bf2(a(i, row), a(i + 1, row), ah[t], al[t]);
+            }
+#pragma unroll
+            for (int t = 0; t < NT; ++t) {
+                mma_bf16(part[m][t], al, bh[t][0], bh[t][1]);
+                mma_bf16(part[m][t], ah, bl[t][0], bl[t][1]);
+                mma_bf16(part[m][t], ah, bh[t][0], bh[t][1]);
+            }
+        }
+    }
+#pragma unroll
+    for (int m = 0; m < MT; ++m)
+#pragma unroll
+        for (int t = 0; t < NT; ++t)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) acc[m][t][i] += part[m][t][i];
+}
+
+struct PgArgs {
+    const float* control;
+    const float* w1;
+    const float* b1;
+    const float* w2;
+    const float* b2;
+    const float* z_stages;        // [n_total][n_paths][32]
+    const float* kappa;           // [n_total][n_paths][32]
+    const int32_t* stage_index;   // [n_total] (forward order)
+    const float* stage_frac;
+    float* scratch;               // [gridDim.x][kPgParams]
+    int64_t n_paths, n_rows;
+    int control_kind, n_total;
+    float sign;
+};
+
+__global__ void __launch_bounds__(kBwdThreads, 1) mlp_param_grad_kernel(const PgArgs a) {
+    extern __shared__ unsigned char smem_unaligned[];
+    unsigned char* smem = smem_unaligned + ((1024u - (smem_u32(smem_unaligned) & 1023u)) & 1023u);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
+    const Scales sc = prepare<kBwdThreads>(smem, a.w1, a.b1, a.w2, a.b2, tid);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    const float* sb1 = reinterpret_cast<const float*>(smem + Smem::b1);
+    const float* sb2 = reinterpret_cast<const float*>(smem + Smem::b2);
+    const uint32_t tile1 = smem_u32(smem + Smem::w1), tile2 = smem_u32(smem + Smem::w2);
+    const int b = blockIdx.y;
+    float* gs = reinterpret_cast<float*>(smem + PgSmem::stage);
+    float* hs = reinterpret_cast<float*>(smem + PgSmem::h);
+    float* wt = reinterpret_cast<float*>(smem + BwdSmem::g) + warp * 16 * kGStride;      // y = 4: the warp's g tile
+    float* mine = a.scratch + (size_t)blockIdx.x * kPgParams;
+
+    const int64_t n_tiles = (a.n_paths + wg::kPaths - 1) / wg::kPaths;
+    const int64_t n_items = n_tiles * a.n_total;
+    const int64_t plane = a.n_paths * kHid;
+    if (b < wg::kChunks) {
+        float acc[1][17][4];
+#pragma unroll
+        for (int t = 0; t < 17; ++t)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) acc[0][t][i] = 0.f;
+        for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
+            const int e = (int)(item / n_tiles);
+            const int64_t path0 = (item - (int64_t)e * n_tiles) * wg::kPaths;
+            const BwdRows rows(a.control, a.control_kind, a.n_rows, a.n_paths, path0, warp, g, q, a.sign < 0.f ? -1.f : 1.f);
+            float zs[wg::kNV], dx[2][2], kc[2][8];
+            rows.load(a.z_stages + e * plane, q, zs);
+            {
+                float2 raw[2][3];
+                rows.fetch(a.n_rows, a.stage_index[e], raw);
+                rows.slope(raw, a.stage_frac[e], dx);
+            }
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {                      // kappa of the chunk's units 8 b .. 8 b + 7 (zero on dead rows)
+                const float4* src = reinterpret_cast<const float4*>(a.kappa + e * plane + rows.lpath[r] * kHid + 8 * b);
+                const float4 k0 = src[0], k1 = src[1];
+                const float live = rows.live[r] ? 1.f : 0.f;
+                kc[r][0] = k0.x * live; kc[r][1] = k0.y * live; kc[r][2] = k0.z * live; kc[r][3] = k0.w * live;
+                kc[r][4] = k1.x * live; kc[r][5] = k1.y * live; kc[r][6] = k1.z * live; kc[r][7] = k1.w * live;
+            }
+            float u[2][wg::kAcc], rs[2], inv2[2], d[wg::kAcc], gc[wg::kAcc];
+            uint32_t bhi[8][4], blo[8][4];
+            hidden_layer(zs, sc, sb1, tile1, q, u, rs, inv2, bhi, blo);
+            issue_v(b, d, sb2, rs, tile2, q, bhi, blo);
+            wg::mma_wait<0>();
+            wg::pin(d);
+            slope_cotangent(d, inv2, kc, dx, gc);
+            __syncthreads();                                   // the previous item's outer product is done with the tiles
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int row = 16 * warp + g + 8 * r;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    *reinterpret_cast<float2*>(gs + row * kGS + 8 * j + 2 * q) = make_float2(gc[4 * j + 2 * r], gc[4 * j + 2 * r + 1]);
+#pragma unroll
+                    for (int c = 0; c < 2; ++c)
+                        *reinterpret_cast<float2*>(hs + row * kHS + 64 * c + 8 * j + 2 * q) =
+                            make_float2(u[c][4 * j + 2 * r], u[c][4 * j + 2 * r + 1]);
+                }
+            }
+            __syncthreads();
+            outer_items<1, 17>(acc, 16 * warp, lane, [&](int i, int row) { return gs[i * kGS + row]; },
+                               [&](int i, int col) { return hs[i * kHS + col]; });
+        }
+        // accumulator t: rows n = 16 w + g (+8) of chunk b, columns 8 t + 2 q (+1); t = 16, column 0: db2
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int n = 64 * b + 16 * warp + g + 8 * r;
+#pragma unroll
+            for (int t = 0; t < 16; ++t)
+                *reinterpret_cast<float2*>(mine + kOffW2 + n * kWidth + 8 * t + 2 * q) =
+                    make_float2(acc[0][t][2 * r], acc[0][t][2 * r + 1]);
+            if (q == 0) mine[kOffB2 + n] = acc[0][16][2 * r];
+        }
+        return;
+    }
+    float acc[2][5][4];
+#pragma unroll
+    for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int t = 0; t < 5; ++t)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) acc[m][t][i] = 0.f;
+    for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const int e = (int)(item / n_tiles);
+        const int64_t path0 = (item - (int64_t)e * n_tiles) * wg::kPaths;
+        const BwdRows rows(a.control, a.control_kind, a.n_rows, a.n_paths, path0, warp, g, q, a.sign < 0.f ? -1.f : 1.f);
+        float zs[wg::kNV], kap[wg::kNV], dx[2][2];
+        rows.load(a.z_stages + e * plane, q, zs);
+        rows.load(a.kappa + e * plane, q, kap);
+#pragma unroll
+        for (int h = 0; h < wg::kNV; ++h)
+            if (!rows.live[h >> 3]) kap[h] = 0.f;
+        {
+            float2 raw[2][3];
+            rows.fetch(a.n_rows, a.stage_index[e], raw);
+            rows.slope(raw, a.stage_frac[e], dx);
+        }
+        __syncthreads();                                       // the previous item's outer product is done with the tiles
+        float ub[16][4];
+        stage_ubar(zs, kap, dx, sc, sb1, sb2, tile1, tile2, lane, wt, ub);
+        float* us = wt;                                        // the warp's rows: ub [16][kHS], then z [16][kZS]
+        float* zt = wt + 16 * kHS;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int row = g + 8 * r;
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+                *reinterpret_cast<float2*>(us + row * kHS + 8 * j + 2 * q) = make_float2(ub[j][2 * r], ub[j][2 * r + 1]);
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+                *reinterpret_cast<float2*>(zt + row * kZS + 8 * i + 2 * q) = make_float2(zs[8 * r + 2 * i], zs[8 * r + 2 * i + 1]);
+        }
+        __syncthreads();
+        const float* base = reinterpret_cast<const float*>(smem + BwdSmem::g);
+        outer_items<2, 5>(acc, 32 * warp, lane,
+                          [&](int i, int row) { return base[(i >> 4) * 16 * kGStride + (i & 15) * kHS + row]; },
+                          [&](int i, int col) { return base[(i >> 4) * 16 * kGStride + 16 * kHS + (i & 15) * kZS + col]; });
+    }
+    // accumulator (m, t): rows k = 32 w + 16 m + g (+8), columns 8 t + 2 q (+1); t = 4, column 0: db1
+#pragma unroll
+    for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int k = 32 * warp + 16 * m + g + 8 * r;
+#pragma unroll
+            for (int t = 0; t < 4; ++t)
+                *reinterpret_cast<float2*>(mine + k * kHid + 8 * t + 2 * q) = make_float2(acc[m][t][2 * r], acc[m][t][2 * r + 1]);
+            if (q == 0) mine[kOffB1 + k] = acc[m][4][2 * r];
+        }
+}
+
+// grads += scale * the per-CTA sums, added in CTA order
+__global__ void mlp_param_reduce_kernel(const float* scratch, int n_parts, float scale, float* gw1, float* gb1, float* gw2,
+                                        float* gb2) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= kPgParams) return;
+    float s = 0.f;
+    for (int p = 0; p < n_parts; ++p) s += scratch[(size_t)p * kPgParams + i];
+    s *= scale;
+    if (i < kOffB1) { if (gw1) gw1[i] += s; }
+    else if (i < kOffW2) { if (gb1) gb1[i - kOffB1] += s; }
+    else if (i < kOffB2) { if (gw2) gw2[i - kOffW2] += s; }
+    else if (gb2) gb2[i - kOffB2] += s;
+}
+
 }  // namespace mlp
 }  // namespace tc
 
 static bool mlp_tc_shape(int64_t H, int64_t C, int64_t W) { return H == tc::kHid && C == tc::kCh && W == tc::mlp::kWidth; }
+
+// cdeint_mlp_wgmma_kernel, with a stage dump when u.stage_dump is set
+static int launch_mlp_tc(const UmmaArgs& u, const float* w2, const float* b2, cudaStream_t s) {
+    const int64_t grid = (u.n_paths + tc::mlp::kPaths - 1) / tc::mlp::kPaths;
+    TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
+    auto kern = u.stage_dump ? tc::mlp::cdeint_mlp_wgmma_kernel<true> : tc::mlp::cdeint_mlp_wgmma_kernel<false>;
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::mlp::kSmem));
+    kern<<<(unsigned)grid, tc::mlp::kThreads, tc::mlp::kSmem, s>>>(u, w2, b2);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    return TCDE_OK;
+}
+
+// What the stage-dump solve, its backward and the parameter gradients are built for: fp32 at 32 / 8 / 128 under a solve
+// variant that runs the tensor-core kernel (0, 4, 5)
+static int check_mlp_backprop(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what) {
+    const int variant = current_solve_variant();
+    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && mlp_tc_shape(hidden, channels, width) && (variant == 0 || variant >= 4) &&
+                             variant != 6,
+                         "%s is built for fp32, hidden=32, channels=8, width=128 on the tensor-core kernel (got dtype=%d, "
+                         "%lld, %lld, %lld, solve variant %d)", what, dtype, (long long)hidden, (long long)channels,
+                         (long long)width, variant);
+    return TCDE_OK;
+}
+
+static int64_t mlp_param_grid(int64_t n_paths, int64_t n_total) {
+    const int64_t items = ((n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths) * n_total;
+    int64_t g = sm_count();
+    if (g > items) g = items;
+    return g < 1 ? 1 : g;
+}
 
 // Where automatic selection runs the CUDA-core kernel: the shapes at which it measured faster than cdeint's stage loop on
 // an H100 (DESIGN 4.2): at most 8 hidden units (the HM = 8 instantiation) or one chunk of outputs (H C <= 32).  Elsewhere
@@ -680,14 +1347,7 @@ extern "C" int tcde_cdeint_fixed_mlp(const void* control, int control_kind, int6
                        (const float*)step_dt, stage_index, (const float*)stage_frac, out_step, out_mode,
                        (const float*)out_slope, n_paths, n_rows, control_kind, method, n_stages, (int)n_steps, (int)n_out,
                        (float)sign, nullptr, 0};
-            const int64_t grid = (n_paths + tc::mlp::kPaths - 1) / tc::mlp::kPaths;
-            TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
-            TCDE_CHECK_CUDA(cudaFuncSetAttribute(tc::mlp::cdeint_mlp_wgmma_kernel,
-                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, tc::mlp::kSmem));
-            tc::mlp::cdeint_mlp_wgmma_kernel<<<(unsigned)grid, tc::mlp::kThreads, tc::mlp::kSmem, s>>>(
-                u, (const float*)w2, (const float*)b2);
-            TCDE_CHECK_CUDA(cudaGetLastError());
-            return TCDE_OK;
+            return launch_mlp_tc(u, (const float*)w2, (const float*)b2, s);
         }
         MlpArgs<float> a{(const float*)control, (const float*)w1, (const float*)b1, (const float*)w2, (const float*)b2,
                          (const float*)z0, (float*)out, (const float*)step_dt, stage_index, (const float*)stage_frac,
@@ -706,4 +1366,110 @@ extern "C" int tcde_cdeint_fixed_mlp(const void* control, int control_kind, int6
                       out_step, out_mode, (const double*)out_slope, n_paths, n_rows, (int)channels, (int)hidden,
                       (int)width, control_kind, method, n_stages, (int)n_steps, (int)n_out, sign};
     return solve_mlp_simt(a, s);
+}
+
+extern "C" int tcde_cdeint_fixed_mlp_stages(const void* control, int control_kind, int64_t n_rows, const void* w1,
+                                            const void* b1, const void* w2, const void* b2, const void* z0, void* out,
+                                            void* stage_dump, int64_t n_paths, int64_t channels, int64_t hidden,
+                                            int64_t width, int method, int64_t n_steps, const void* step_dt,
+                                            const int32_t* stage_index, const void* stage_frac, int64_t n_out,
+                                            const int32_t* out_step, const int32_t* out_mode, const void* out_slope,
+                                            double sign, int dtype, void* stream) {
+    TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z0 && out && stage_dump, "null data pointer");
+    TCDE_CHECK_ARG(step_dt && stage_index && stage_frac && out_step && out_mode && out_slope, "null schedule pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_steps >= 1 && n_out >= 1, "bad sizes");
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
+    TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
+    const int rc = check_mlp_backprop(hidden, channels, width, dtype, "the MLP stage-dump solve");
+    if (rc != TCDE_OK) return rc;
+    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z0) |
+                           reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(stage_dump)) & 15) == 0,
+                         "MLP stage-dump solve: control, z0, out and the dump must be 16-byte aligned");
+    if (n_paths == 0) return TCDE_OK;
+    const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
+    UmmaArgs u{(const float*)control, (const float*)w1, (const float*)b1, (const float*)z0, (float*)out,
+               (const float*)step_dt, stage_index, (const float*)stage_frac, out_step, out_mode, (const float*)out_slope,
+               n_paths, n_rows, control_kind, method, n_stages, (int)n_steps, (int)n_out, (float)sign, (float*)stage_dump,
+               0};
+    return launch_mlp_tc(u, (const float*)w2, (const float*)b2, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int tcde_cdeint_fixed_mlp_backward(
+    const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1, const void* w2, const void* b2,
+    const void* stage_dump, const void* grad_out, void* grad_z0, void* kappa_dump, int64_t n_paths, int64_t channels,
+    int64_t hidden, int64_t width, int method, int64_t n_steps, const void* step_dt_rev, const int32_t* stage_index_rev,
+    const void* stage_frac_rev, int64_t n_out, const int32_t* inj_range, const int32_t* inj_out, const void* inj_weight,
+    double sign, int dtype, void* stream) {
+    TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && stage_dump && grad_out && grad_z0, "null data pointer");
+    TCDE_CHECK_ARG(step_dt_rev && stage_index_rev && stage_frac_rev && inj_range && inj_out && inj_weight,
+                   "null schedule pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_steps >= 1 && n_out >= 1, "bad sizes");
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
+    TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
+    const int rc = check_mlp_backprop(hidden, channels, width, dtype, "the MLP Runge-Kutta backward");
+    if (rc != TCDE_OK) return rc;
+    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(stage_dump) |
+                           reinterpret_cast<uintptr_t>(grad_out) | reinterpret_cast<uintptr_t>(grad_z0) |
+                           reinterpret_cast<uintptr_t>(kappa_dump)) & 15) == 0,
+                         "MLP Runge-Kutta backward: control, the dumps, grad_out and grad_z0 must be 16-byte aligned");
+    if (n_paths == 0) return TCDE_OK;
+    const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
+    UmmaArgs u{(const float*)control, (const float*)w1, (const float*)b1, nullptr, (float*)grad_z0,
+               (const float*)step_dt_rev, stage_index_rev, (const float*)stage_frac_rev, nullptr, nullptr, nullptr,
+               n_paths, n_rows, control_kind, method, n_stages, (int)n_steps, (int)n_out, (float)sign,
+               (float*)kappa_dump, 0, (const float*)grad_out, inj_range, inj_out, (const float*)inj_weight};
+    const int64_t grid = (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths;
+    TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(tc::mlp::cdeint_mlp_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         tc::mlp::kBwdSmem));
+    tc::mlp::cdeint_mlp_backward_kernel<<<(unsigned)grid, tc::mlp::kBwdThreads, tc::mlp::kBwdSmem,
+                                          static_cast<cudaStream_t>(stream)>>>(u, (const float*)w2, (const float*)b2,
+                                                                               (const float*)stage_dump);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    return TCDE_OK;
+}
+
+extern "C" int64_t tcde_mlp_field_param_grads_scratch_bytes(int64_t n_paths, int64_t n_stages_total, int64_t channels,
+                                                           int64_t hidden, int64_t width) {
+    if (n_paths < 0 || n_stages_total < 1 || !mlp_tc_shape(hidden, channels, width)) return -1;
+    return mlp_param_grid(n_paths, n_stages_total) * tc::mlp::kPgParams * (int64_t)sizeof(float);
+}
+
+extern "C" int tcde_mlp_field_param_grads(const void* control, int control_kind, int64_t n_rows, const void* w1,
+                                          const void* b1, const void* w2, const void* b2, const void* z_stages,
+                                          const void* kappa_stages, const int32_t* stage_index, const void* stage_frac,
+                                          int64_t n_stages_total, void* grad_w1, void* grad_b1, void* grad_w2,
+                                          void* grad_b2, void* scratch, int64_t n_paths, int64_t channels, int64_t hidden,
+                                          int64_t width, double sign, double scale, int dtype, void* stream) {
+    TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z_stages && kappa_stages && stage_index && stage_frac && scratch,
+                   "null data pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_stages_total >= 1 && n_stages_total < (1ll << 31), "bad sizes");
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    const int rc = check_mlp_backprop(hidden, channels, width, dtype, "the MLP parameter gradients");
+    if (rc != TCDE_OK) return rc;
+    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z_stages) |
+                           reinterpret_cast<uintptr_t>(kappa_stages) | reinterpret_cast<uintptr_t>(scratch)) & 15) == 0,
+                         "MLP parameter gradients: control, the dumps and scratch must be 16-byte aligned");
+    if (n_paths == 0) return TCDE_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    const int64_t grid = mlp_param_grid(n_paths, n_stages_total);
+    tc::mlp::PgArgs a{(const float*)control, (const float*)w1, (const float*)b1, (const float*)w2, (const float*)b2,
+                      (const float*)z_stages, (const float*)kappa_stages, stage_index, (const float*)stage_frac,
+                      (float*)scratch, n_paths, n_rows, control_kind, (int)n_stages_total, (float)sign};
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(tc::mlp::mlp_param_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         tc::mlp::kPgSmem));
+    tc::mlp::mlp_param_grad_kernel<<<dim3((unsigned)grid, tc::mlp::kPgY), tc::mlp::kBwdThreads, tc::mlp::kPgSmem, s>>>(a);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    if (grad_w1 || grad_b1 || grad_w2 || grad_b2) {
+        tc::mlp::mlp_param_reduce_kernel<<<(tc::mlp::kPgParams + 255) / 256, 256, 0, s>>>(
+            (const float*)scratch, (int)grid, (float)scale, (float*)grad_w1, (float*)grad_b1, (float*)grad_w2,
+            (float*)grad_b2);
+        TCDE_CHECK_CUDA(cudaGetLastError());
+    }
+    return TCDE_OK;
 }

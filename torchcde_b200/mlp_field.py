@@ -2,7 +2,8 @@
 
 example/time_series_classification.py:20-51 trains ``func(t, z) = tanh(Linear(W, H*C)(relu(Linear(H, W)(z)))).view(H, C)``.
 ``mlp_field_of`` recognises a user module that computes exactly that (no new class to adopt), and ``cdeint`` then runs
-its fixed-step forward as ONE launch of ``tcde_cdeint_fixed_mlp``."""
+its fixed-step forward as ONE launch of ``tcde_cdeint_fixed_mlp``; ``cdeint(..., adjoint=False)`` with gradients runs
+``MlpBackprop`` (three launches) where it is built for the problem."""
 import math
 import weakref
 
@@ -11,6 +12,7 @@ import torch
 from . import _lib
 from .controls import _control_signature, _schedule_knots
 from .linear_field import _check_linear_problem, _probe, _schedules
+from .schedule import backward_tables
 
 # module -> {training flag: index of the accepted layer ordering, or -1}; kept apart from the linear probe's cache
 _recognised = weakref.WeakKeyDictionary()
@@ -109,3 +111,131 @@ class MlpFieldKernels:
                           sched.n_out, _lib.ptr(v["out_step"]), _lib.ptr(v["out_mode"]), _lib.ptr(v["out_slope"]),
                           float(sched.sign), _lib.dtype_code(self.dtype), _lib.stream_of(zf))
         return out.view(*y0.shape[:-1], sched.n_out, self.hidden)
+
+
+class MlpBackprop:
+    """``cdeint(..., adjoint=False)`` of a fixed-step solve of the MLP field at fp32, hidden 32, channels 8, width 128 with
+    gradients for any of z0, W1, b1, W2, b2: the exact gradient of the discrete solve in three launches, as
+    ``linear_field.FixedBackprop`` does for the linear field.  The forward is the stage-dump solve
+    (``tcde_cdeint_fixed_mlp_stages``: the outputs of the same call without gradients, bit for bit); the backward is ONE
+    launch of ``tcde_cdeint_fixed_mlp_backward`` (the transposed Runge-Kutta recurrence over every step at the dumped stage
+    inputs) and, with parameter gradients, ONE launch of ``tcde_mlp_field_param_grads`` over the two dumps.  ``loop(z0)``:
+    the differentiable torch-operator solve of the same problem, which a backward with ``create_graph`` differentiates."""
+
+    def __init__(self, kernels, t, method, step_size, loop):
+        self.kernels, self.method, self.loop = kernels, method, loop
+        self.sched, (_floats, _ints, self.views) = _schedules.get(t, kernels.knots, kernels.n_rows, method, step_size,
+                                                                  kernels.dtype, kernels.device)
+        self.n_total = self.sched.n_steps * self.sched.n_stages
+
+    def scratch_bytes(self, n_paths):
+        k = self.kernels
+        return _lib.load().tcde_mlp_field_param_grads_scratch_bytes(n_paths, self.n_total, k.channels, k.hidden, k.width)
+
+    def fits(self, n_paths, want_params):
+        """Whether the stage dump, and with parameter gradients the kappa dump and the parameter-gradient scratch, fit in
+        0.7 of the free device memory."""
+        k = self.kernels
+        need = self.n_total * n_paths * k.hidden * 4
+        if want_params:
+            scratch = self.scratch_bytes(n_paths)
+            if scratch < 0:
+                return False
+            need = 2 * need + scratch
+        with torch.cuda.device(k.device):
+            free, _total = torch.cuda.mem_get_info()
+        return need <= 0.7 * free
+
+    def forward(self, z0):
+        """(the outputs ``(..., n_out, H)``, the input of every stage ``[n_steps * n_stages][paths][H]``)."""
+        k, sched, v = self.kernels, self.sched, self.views
+        with torch.cuda.device(k.device):
+            zf = z0.detach().reshape(-1, k.hidden).contiguous()
+            out = torch.empty(zf.size(0), sched.n_out, k.hidden, dtype=k.dtype, device=k.device)
+            dump = torch.empty(self.n_total, zf.size(0), k.hidden, dtype=k.dtype, device=k.device)
+            if zf.size(0) > 0:
+                _lib.call("tcde_cdeint_fixed_mlp_stages", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1),
+                          _lib.ptr(k.b1), _lib.ptr(k.w2), _lib.ptr(k.b2), _lib.ptr(zf), _lib.ptr(out), _lib.ptr(dump),
+                          zf.size(0), k.channels, k.hidden, k.width, _lib.METHODS[sched.method], sched.n_steps,
+                          _lib.ptr(v["step_dt"]), _lib.ptr(v["stage_index"]), _lib.ptr(v["stage_frac"]), sched.n_out,
+                          _lib.ptr(v["out_step"]), _lib.ptr(v["out_mode"]), _lib.ptr(v["out_slope"]), float(sched.sign),
+                          _lib.F32, _lib.stream_of(zf))
+        return out.view(*z0.shape[:-1], sched.n_out, k.hidden), dump
+
+    def backward(self, g, dump, want):
+        """(dL/dz0, [dL/dW1, dL/db1, dL/dW2, dL/db2] with None where ``want`` is False) for output gradients ``g``."""
+        k, sched = self.kernels, self.sched
+        hidden, dev, n_total = k.hidden, k.device, self.n_total
+        with torch.cuda.device(dev):
+            gf = g.reshape(-1, sched.n_out, hidden)
+            if not gf.is_contiguous() or gf.data_ptr() % 16:
+                gf = gf.clone(memory_format=torch.contiguous_format)
+            n_paths = gf.size(0)
+            gz = torch.empty(n_paths, hidden, dtype=k.dtype, device=dev)
+            kappa = torch.empty_like(dump) if any(want) else None
+            grads = [torch.zeros_like(p) if w else None for p, w in zip((k.w1, k.b1, k.w2, k.b2), want)]
+            if n_paths > 0:
+                tables = backward_tables(sched)
+                floats = torch.cat([tables["step_dt"], tables["stage_frac"], tables["inj_weight"]]).to(dev)
+                ints = torch.cat([tables["stage_index"], tables["inj_range"], tables["inj_out"]]).to(dev)
+                ns, nr = sched.n_steps, tables["inj_range"].numel()
+                _lib.call("tcde_cdeint_fixed_mlp_backward", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1),
+                          _lib.ptr(k.b1), _lib.ptr(k.w2), _lib.ptr(k.b2), _lib.ptr(dump), _lib.ptr(gf), _lib.ptr(gz),
+                          _lib.ptr(kappa), n_paths, k.channels, hidden, k.width, _lib.METHODS[sched.method], ns,
+                          _lib.ptr(floats[:ns]), _lib.ptr(ints[:n_total]), _lib.ptr(floats[ns:ns + n_total]), sched.n_out,
+                          _lib.ptr(ints[n_total:n_total + nr]), _lib.ptr(ints[n_total + nr:]),
+                          _lib.ptr(floats[ns + n_total:]), float(sched.sign), _lib.F32, _lib.stream_of(gf))
+                if kappa is not None:
+                    scratch = torch.empty(max(self.scratch_bytes(n_paths) // 4, 4), dtype=torch.float32, device=dev)
+                    _lib.call("tcde_mlp_field_param_grads", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1),
+                              _lib.ptr(k.b1), _lib.ptr(k.w2), _lib.ptr(k.b2), _lib.ptr(dump), _lib.ptr(kappa),
+                              _lib.ptr(self.views["stage_index"]), _lib.ptr(self.views["stage_frac"]), n_total,
+                              *(_lib.ptr(x) for x in grads), _lib.ptr(scratch), n_paths, k.channels, hidden, k.width,
+                              float(sched.sign), 1.0, _lib.F32, _lib.stream_of(gf))
+        return gz.view(g.shape[:-2] + (hidden,)), grads
+
+
+class _MlpBackpropFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, route, z0, *params):
+        out, dump = route.forward(z0)
+        ctx.route = route
+        ctx.save_for_backward(z0, dump, *params)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        z0, dump, *params = ctx.saved_tensors
+        want_z, *want = ctx.needs_input_grad[1:]
+        if torch.is_grad_enabled():
+            # create_graph: differentiate the torch-operator solve of the same problem, whose gradients are themselves
+            # differentiable
+            inputs = [x for x, w in zip([z0] + params, [want_z] + want) if w]
+            got = iter(torch.autograd.grad(ctx.route.loop(z0), inputs, g, create_graph=True, allow_unused=True))
+            return (None,) + tuple(next(got) if w else None for w in [want_z] + want)
+        gz, grads = ctx.route.backward(g, dump, want)
+        return (None, gz if want_z else None) + tuple(grads)
+
+
+def mlp_backprop(X, params, z0, t, method, step_size, loop):
+    """``cdeint(..., adjoint=False)``'s outputs ``(..., n_out, H)`` on the three-launch route of ``MlpBackprop``, or None
+    when the route does not serve the problem (the caller runs the torch-operator solve).  ``params``: (W1, b1, W2, b2)
+    of the recognised field, a bias may be None."""
+    w1 = params[0]
+    if (z0.dtype != torch.float32 or z0.size(-1) != 32 or w1.size(0) != 128
+            or any(p is not None and (p.dtype != torch.float32 or p.device != z0.device) for p in params)):
+        return None
+    k = MlpFieldKernels(X, params, z0)
+    if k.channels != 8 or k.control.dtype != torch.float32 or k.control.device != z0.device:
+        return None
+    route = MlpBackprop(k, t, method, step_size, loop)
+    present = [p for p in params if p is not None]
+    if not route.fits(k.n_paths, any(p.requires_grad for p in present)):
+        return None
+    # a missing bias is the kernels' zero vector, which wants no gradient
+    leaves = [p if p is not None else b for p, b in zip(params, (k.w1, k.b1, k.w2, k.b2))]
+    try:
+        return _MlpBackpropFn.apply(route, z0, *leaves)
+    except NotImplementedError:
+        # the stage-dump solve refuses the problem (solve variant, misaligned rows): nothing ran
+        return None

@@ -16,7 +16,7 @@ import torch
 from . import _lib, adaptive
 from .controls import CubicSpline, _control_signature, _schedule_knots
 from .linear_field import LinearFieldKernels, LinearVectorField, _reverse, fixed_backprop, linear_field_of  # noqa: F401
-from .mlp_field import MlpFieldKernels, mlp_field_of
+from .mlp_field import MlpFieldKernels, mlp_backprop, mlp_field_of
 from .schedule import FIXED_METHODS, build_schedule, host_locator
 
 
@@ -335,7 +335,8 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     ``adjoint=True`` runs this package's continuous-adjoint backward (fused kernels for the linear
     field), ``adjoint=False`` backpropagates through the solve: for the linear field at fp32, hidden 32,
     channels 8 with gradients for z0 / weight / bias in three launches (``linear_field.FixedBackprop``),
-    otherwise through the differentiable generic stage loop.
+    likewise for the examples' MLP field at fp32, hidden 32, channels 8, width 128 with gradients for z0
+    and its two layers (``mlp_field.MlpBackprop``), otherwise through the differentiable generic stage loop.
 
     ``backend="torchsde"`` is built for ``method="reversible_heun"`` (torchsde's reversible Heun
     method with zero diffusion, fixed step ``dt``, default 1e-3; ``z0`` of shape (batch, hidden),
@@ -559,11 +560,20 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
 
     # adjoint=False: backpropagate through the solver's own operations, like torchdiffeq.odeint
     if method in FIXED_METHODS:
+        loop = lambda y0: _generic_solve(X, func, y0, t, method, step_size, is_prod, True)  # noqa: E731
         if backprop:
-            ys = fixed_backprop(kernels, z0, t, method, step_size,
-                                lambda y0: _generic_solve(X, func, y0, t, method, step_size, is_prod, True))
+            ys = fixed_backprop(kernels, z0, t, method, step_size, loop)
             if ys is not None:
                 return ys
+        # the examples' MLP field: the three-launch route of mlp_field.MlpBackprop serves gradients for z0 and the two
+        # layers' weights and biases (fp32, hidden 32, channels 8, width 128); a gradient for t or the control keeps the loop
+        if (field_params is None and sig is not None and not is_prod and times and not t.requires_grad
+                and not any(b.requires_grad for b in X.buffers())):
+            mlp_params = mlp_field_of(func, z0, sig[2], times)
+            if mlp_params is not None:
+                ys = mlp_backprop(X, mlp_params, z0, t, method, step_size, loop)
+                if ys is not None:
+                    return ys
         return _generic_solve(X, func, z0, t, method, step_size, is_prod, sig is not None)
     targets = None
     if t.requires_grad:
