@@ -6,8 +6,9 @@
 //   * cdeint_tc_kernel (3xTF32 split): thread = path, warp = 32 paths, warp-level mma.sync through tc_common.cuh's
 //     warp_field<0>.
 // Each Runge-Kutta stage is
-//   * dX/dt of the stage from the path's spline row (read straight from HBM: b | 2c | 3d of the interval; the next stage's
-//     row is requested before the current stage's products so that its latency hides behind them);
+//   * dX/dt of the stage from the path's spline row (b | 2c | 3d of the interval, from HBM; the next stage's row is
+//     requested before the current stage's products so that its latency hides behind them: into registers in the 3xTF32
+//     kernel, into shared memory by cp.async in the 2xFP16 one);
 //   * the field W z + b as a [paths x 32] . [32 x 256] product on the tensor cores with a two-way operand split
 //     (tc_common.cuh), contracted with dX/dt in registers;
 //   * the Runge-Kutta combination in registers, one rounding per operation in the order of oracle/odeint_port.py.
@@ -197,25 +198,32 @@ __global__ void __launch_bounds__(kThreads, 2) cdeint_tc_kernel(const UmmaArgs a
 // built in registers from the Runge-Kutta state.  Its 16 values of a state vector sit at index 8 r + 2 i + e (r = row).
 // The product runs in chunks of kN = 64 output columns (eight hidden units x eight channels): z_lo.W_hi, z_hi.W_lo and
 // z_hi.W_hi (small terms first) are six m64n64k16 wgmmas onto an accumulator that starts at the scaled bias, with A from
-// registers and B (prepare_b<1>'s [256 rows][hi 32 | lo 32] halves, 128-byte swizzled) through one shared-memory
+// registers and B (prepare_b<1, true>'s [256 rows][hi 32 | lo 32] halves, 128-byte swizzled) through one shared-memory
 // descriptor per product and k step.  Two accumulators alternate: the chunk after the current one is in flight on the
-// tensor core while the current one is contracted with dX/dt.  Chunk c holds hidden units 8c .. 8c + 7, so it reduces on
-// its own: the contraction leaves each lane with the partial sums of its two channels, and a reduce-scatter over the quad
-// (xor 1, then xor 2) hands each lane the sums of its units 8c + 2q + e, added in the order (q, q ^ 1) + (q ^ 2, q ^ 3).
+// tensor core while the current one is contracted with dX/dt.  Chunk c holds hidden units 8c .. 8c + 7 with its rows
+// permuted (field_tile_row) so that accumulator column 8j + 2q + e is unit 8c + 2q + (j >> 2), channel 4e + (j & 3): each
+// lane holds all eight channels of exactly the units 8c + 2q + e it owns, and the contraction closes inside the lane.  The
+// lane gets all eight channels of dX/dt from its quad through a per-warp shared-memory slot once per stage.  The sum is
+// (P_0 + P_1) + (P_2 + P_3) with P_k = the products of channels 2k, 2k + 1, the order in which the quad reduce-scatter of
+// the unpermuted layout (wg::reduce_chunk) added them, so the bits are the same.
 // N = 64 issues half the wgmmas of N = 32 for the same flops; scripts/wgmma_probe.py measures what that saves.
 
 namespace wg {
 
 // One evaluation of the linear field for the warpgroup's 64 rows: kv = (W zin + b) . dx in the fragment layout above.
-// beta, inv_w_scale: prepare_b<1>'s scales of the tile at b_tile (bias at b_bias).  dx (the lane's two channels of both
-// rows) is scaled in place.  mid() runs halfway through the chunks (the caller's next dX/dt hides behind the MMAs).
-template <typename Mid>
-__device__ __forceinline__ void field(const float* zin, float (*dx)[2], float beta, float inv_w_scale, const float* b_bias,
-                                      uint32_t b_tile, int q, float* kv, Mid mid) {
+// beta, inv_w_scale: prepare_b<1, true>'s scales of the tile at b_tile (bias at b_bias).  dx: the lane's two channels of
+// both rows; xch: the warp's kDxSlot bytes of shared memory, through which the quad shares them.  HOLD: all eight
+// channels of both rows stay in registers for the whole evaluation (four 16-byte loads); otherwise they are read again,
+// one float at a time, for each chunk and row, which holds 16 registers fewer (the Runge-Kutta backward and
+// reversible_backward_kernel have no room for them; 16-byte loads there spill).
+template <bool HOLD>
+__device__ __forceinline__ void field(const float* zin, const float (*dx)[2], float beta, float inv_w_scale,
+                                      const float* b_bias, uint32_t b_tile, float* xch, int g, int q, float* kv) {
     // Each row scaled by its own power of two so that max(|z|, bias floor) lands in [2^13, 2^14), split into FP16
-    // hi + lo A fragments [k step][4]; the inverse scales are folded into dX/dt.
+    // hi + lo A fragments [k step][4]; the inverse scales are folded into dX/dt, which goes to the quad's row of xch.
     float rs[2];
     uint32_t ahi[2][4], alo[2][4];
+    __syncwarp();                                         // the previous evaluation's reads of xch are done
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
         float m = beta;
@@ -226,8 +234,8 @@ __device__ __forceinline__ void field(const float* zin, float (*dx)[2], float be
         const int e = min(max(exponent_of(m), 30), 224);
         rs[r] = pow2_biased(127 + 13 - (e - 127));
         const float inv = pow2_biased(127 - 13 + (e - 127)) * inv_w_scale;
-        dx[r][0] = __fmul_rn(dx[r][0], inv);
-        dx[r][1] = __fmul_rn(dx[r][1], inv);
+        *reinterpret_cast<float2*>(xch + (g + 8 * r) * kCh + 2 * q) =
+            make_float2(__fmul_rn(dx[r][0], inv), __fmul_rn(dx[r][1], inv));
     }
 #pragma unroll
     for (int k = 0; k < 2; ++k)
@@ -240,6 +248,19 @@ __device__ __forceinline__ void field(const float* zin, float (*dx)[2], float be
             unpack_h2(ahi[k][t], h0, h1);
             alo[k][t] = pack_h2(__fsub_rn(s0, h0), __fsub_rn(s1, h1));
         }
+    __syncwarp();                                         // xch holds the quad's dX/dt
+    float dxs[2][kCh];                                    // all eight channels of rows g and g + 8
+    auto load_row = [&](int r) {
+        const float4 lo = *reinterpret_cast<const float4*>(xch + (g + 8 * r) * kCh);
+        const float4 hi = *reinterpret_cast<const float4*>(xch + (g + 8 * r) * kCh + 4);
+        dxs[r][0] = lo.x; dxs[r][1] = lo.y; dxs[r][2] = lo.z; dxs[r][3] = lo.w;
+        dxs[r][4] = hi.x; dxs[r][5] = hi.y; dxs[r][6] = hi.z; dxs[r][7] = hi.w;
+    };
+    auto reload_row = [&](int r) {
+#pragma unroll
+        for (int k = 0; k < kCh; ++k) dxs[r][k] = xch[(g + 8 * r) * kCh + k];
+    };
+    if (HOLD) { load_row(0); load_row(1); }
 
     float acc[2][kAcc];
     auto issue = [&](int chunk, float* d) {
@@ -270,14 +291,23 @@ __device__ __forceinline__ void field(const float* zin, float (*dx)[2], float be
             mma_wait<0>();
         }
         pin(d);
-        if (c == kChunks / 2) mid();
-        // partial contraction of the lane's two channels for hidden units 8c + j, rows g and g + 8
-        float p[8][2];
+        // the contraction of the lane's units 8c + 2q + u, rows g and g + 8: d[4 j + 2 r + e] is unit 8c + 2q + (j >> 2),
+        // channel 4e + (j & 3), so channels 2k, 2k + 1 of unit u sit at j = 4u + 2 (k & 1) + {0, 1}, e = k >> 1
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
+        for (int r = 0; r < 2; ++r) {
+            if (!HOLD) reload_row(r);
 #pragma unroll
-            for (int r = 0; r < 2; ++r) p[j][r] = fmaf(d[4 * j + 2 * r + 1], dx[r][1], __fmul_rn(d[4 * j + 2 * r], dx[r][0]));
-        reduce_chunk(p, c, q, kv);
+            for (int u = 0; u < 2; ++u) {
+                float p[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const int j = 4 * u + 2 * (k & 1), e = k >> 1;
+                    p[k] = fmaf(d[4 * (j + 1) + 2 * r + e], dxs[r][2 * k + 1],
+                                __fmul_rn(d[4 * j + 2 * r + e], dxs[r][2 * k]));
+                }
+                kv[8 * r + 2 * c + u] = (p[0] + p[1]) + (p[2] + p[3]);
+            }
+        }
     }
 }
 
@@ -296,7 +326,7 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
     unsigned char* smem = smem_unaligned + ((1024u - (smem_u32(smem_unaligned) & 1023u)) & 1023u);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
     float inv_w_scale, beta;
-    prepare_b<1>(smem, a.weight, a.bias, tid, wg::kThreads, inv_w_scale, beta);
+    prepare_b<1, true>(smem, a.weight, a.bias, tid, wg::kThreads, inv_w_scale, beta);
     if (a.sign < 0.f) inv_w_scale = -inv_w_scale;       // the sign of the time direction: dX/dt is negated exactly either way
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // the tile is read by wgmma (the async proxy)
     __syncthreads();
@@ -316,13 +346,19 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
     const int row1 = (int)((live[1] ? path[1] : a.n_paths - 1) - lpath0);
     const float2* crow = reinterpret_cast<const float2*>(a.control + lpath0 * a.n_rows * (2 * row_f2) + (cubic ? kCh : 0)) + q;
 
-    auto fetch = [&](int interval, float2 (*raw)[3]) {
+    // These pieces travel to shared memory by cp.async, a stage ahead of their use, into one of two per-warp buffers of
+    // [row r][b | 2c | 3d][lane] float2: held in registers across the products they would push the stage over the
+    // register cap.  Each lane reads back only what it copied itself.
+    float2* rows_buf = reinterpret_cast<float2*>(smem + wg::kRows + warp * 2 * wg::kRowSlot) + lane;
+    auto fetch = [&](int interval, int buf) {
+        float2* dst = rows_buf + buf * (wg::kRowSlot / 8);
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
             const float2* src = crow + (r * row1 * a.n_rows + interval) * row_f2;
-            raw[r][0] = __ldg(src);
-            if (cubic) { raw[r][1] = __ldg(src + 4); raw[r][2] = __ldg(src + 8); }
+            cp_async8(dst + 3 * r * 32, src);
+            if (cubic) { cp_async8(dst + (3 * r + 1) * 32, src + 4); cp_async8(dst + (3 * r + 2) * 32, src + 8); }
         }
+        cp_async_commit();
     };
     // the lane's 16 values of a [path][32] row pair: float2 at column 8 i + 2 q of row r
     auto store_rows = [&](float* base, int64_t stride_rows, int64_t row_off, const float* v) {
@@ -384,28 +420,29 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
 
     const float* b_bias = reinterpret_cast<const float*>(smem + S::bias);
     const uint32_t b_tile = smem_u32(smem + S::tile);
+    float* xch = reinterpret_cast<float*>(smem + wg::kXch + warp * wg::kDxSlot);
     const int n_st = a.n_steps * a.n_stages + (REV ? 1 : 0);
-    // dX/dt (interpolation_cubic.py:331-336) of a stage at fraction fr of its interval, channels 2q, 2q + 1 of both rows
-    auto slope = [&](const float2 (*raw)[3], float fr, float (*dx)[2]) {
+    // dX/dt (interpolation_cubic.py:331-336) of a stage at fraction fr of its interval, channels 2q, 2q + 1 of both rows,
+    // from the rows fetched into buffer buf
+    auto slope = [&](int buf, float fr, float (*dx)[2]) {
+        cp_async_wait<0>();
+        const float2* raw = rows_buf + buf * (wg::kRowSlot / 8);
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
+            const float2 b = raw[3 * r * 32];
             if (cubic) {
-                dx[r][0] = E::add(raw[r][0].x, E::mul(E::add(raw[r][1].x, E::mul(raw[r][2].x, fr)), fr));
-                dx[r][1] = E::add(raw[r][0].y, E::mul(E::add(raw[r][1].y, E::mul(raw[r][2].y, fr)), fr));
+                const float2 c2 = raw[(3 * r + 1) * 32], d3 = raw[(3 * r + 2) * 32];
+                dx[r][0] = E::add(b.x, E::mul(E::add(c2.x, E::mul(d3.x, fr)), fr));
+                dx[r][1] = E::add(b.y, E::mul(E::add(c2.y, E::mul(d3.y, fr)), fr));
             } else {
-                dx[r][0] = raw[r][0].x;
-                dx[r][1] = raw[r][0].y;
+                dx[r][0] = b.x;
+                dx[r][1] = b.y;
             }
         }
     };
     // stage st's [path][32] block (BWD: the forward's slot of stage st, walking down from the last)
     float* dump_at = BWD ? a.stage_dump + (int64_t)(n_st - 1) * a.n_paths * kHid : a.stage_dump;
-    float dx[2][2];
-    {
-        float2 raw[2][3];
-        fetch(a.stage_index[0], raw);
-        slope(raw, a.stage_frac[0], dx);
-    }
+    fetch(a.stage_index[0], 0);
     int step = 0, sub = 0;
     float dt = a.step_dt[0];
     for (int st = 0; st < n_st; ++st) {
@@ -414,15 +451,13 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
             if (BWD) dump_at -= a.n_paths * kHid;
             else dump_at += a.n_paths * kHid;
         }
-        // the next stage's spline rows; their latency hides behind the first half of this stage's products
-        float2 nxt[2][3];
-        float dx_next[2][2];
-        if (st + 1 < n_st) fetch(a.stage_index[st + 1], nxt);
+        float dx[2][2];
+        slope(st & 1, a.stage_frac[st], dx);
+        // the next stage's spline rows; their latency hides behind this stage's products
+        if (st + 1 < n_st) fetch(a.stage_index[st + 1], (st + 1) & 1);
 
         float kv[wg::kNV];
-        wg::field(zin, dx, beta, inv_w_scale, b_bias, b_tile, q, kv, [&] {
-            if (st + 1 < n_st) slope(nxt, a.stage_frac[st + 1], dx_next);
-        });
+        wg::field<!BWD>(zin, dx, beta, inv_w_scale, b_bias, b_tile, xch, g, q, kv);
 
         if (REV) {
             rev_heun_combine<wg::kNV>(a, st, step, dt, y, k1, s23, kv, zin, jn, write_out,
@@ -455,8 +490,6 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
         } else {
             ++sub;
         }
-#pragma unroll
-        for (int r = 0; r < 2; ++r) { dx[r][0] = dx_next[r][0]; dx[r][1] = dx_next[r][1]; }
     }
     if constexpr (BWD) store_rows(a.out, 1, 0, y);
 }
@@ -496,7 +529,7 @@ struct RevBwdArgs {
 };
 
 constexpr int kRevTile = (BSmem<1>::bytes + 1023) & ~1023;
-constexpr int kRevSmem = 2 * kRevTile + 1024;
+constexpr int kRevSmem = 2 * kRevTile + 4 * wg::kDxSlot + 1024;     // two B tiles, the warps' dX/dt slots, alignment
 
 __global__ void __launch_bounds__(wg::kThreads, 2) reversible_backward_kernel(const RevBwdArgs a) {
     using S = BSmem<1>;
@@ -506,13 +539,14 @@ __global__ void __launch_bounds__(wg::kThreads, 2) reversible_backward_kernel(co
     unsigned char* smem = smem_unaligned + ((1024u - (smem_u32(smem_unaligned) & 1023u)) & 1023u);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
     float inv_f, beta_f, inv_g, beta_g;
-    prepare_b<1>(smem, a.weight, a.bias, tid, wg::kThreads, inv_f, beta_f);
-    prepare_b<1>(smem + kRevTile, a.weight_t, a.zeros, tid, wg::kThreads, inv_g, beta_g);
+    prepare_b<1, true>(smem, a.weight, a.bias, tid, wg::kThreads, inv_f, beta_f);
+    prepare_b<1, true>(smem + kRevTile, a.weight_t, a.zeros, tid, wg::kThreads, inv_g, beta_g);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncthreads();
     const float* bias_f = reinterpret_cast<const float*>(smem + S::bias);
     const float* bias_g = reinterpret_cast<const float*>(smem + kRevTile + S::bias);
     const uint32_t tile_f = smem_u32(smem + S::tile), tile_g = smem_u32(smem + kRevTile + S::tile);
+    float* xch = reinterpret_cast<float*>(smem + 2 * kRevTile + warp * wg::kDxSlot);
 
     const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
     const int row_f2 = (cubic ? 4 * kCh : kCh) / 2;
@@ -593,13 +627,11 @@ __global__ void __launch_bounds__(wg::kThreads, 2) reversible_backward_kernel(co
 #pragma unroll
             for (int h = 0; h < NV; ++h) zm[h] = E::sub(E::sub(E::mul(2.f, y[h]), z[h]), E::mul(f[h], d));
         }
-        float dxf[2][2], dxg[2][2];
-        slope_at(m, dxf);
-#pragma unroll
-        for (int r = 0; r < 2; ++r) { dxg[r][0] = dxf[r][0]; dxg[r][1] = dxf[r][1]; }
+        float dx[2][2];
+        slope_at(m, dx);
         float kf[NV], kg[NV];
-        wg::field(zm, dxf, beta_f, inv_f, bias_f, tile_f, q, kf, [] {});
-        wg::field(fb, dxg, beta_g, inv_g, bias_g, tile_g, q, kg, [] {});
+        wg::field<false>(zm, dx, beta_f, inv_f, bias_f, tile_f, xch, g, q, kf);
+        wg::field<false>(fb, dx, beta_g, inv_g, bias_g, tile_g, xch, g, q, kg);
         store_rows(a.dump_z + (int64_t)(m - a.lo) * plane * kHid, zm);
         store_rows(a.dump_a + (int64_t)(m - a.lo) * plane * kHid, fb);
         if (m == a.lo) {

@@ -1,6 +1,7 @@
 // The linear vector field of one warp's 32 paths on the tensor cores (warp-level mma.sync, sm_90a), used by the 3xTF32
-// fixed-step solve (solve_tc.cu) and the device-controlled dopri5 attempts (solve_dopri5.cu).  prepare_b<1>'s operand B is
-// also the B of the 2xFP16 fixed-step solve's wgmma (a K-major 128-byte-swizzled tile).
+// fixed-step solve (solve_tc.cu) and the device-controlled dopri5 attempts (solve_dopri5.cu).  prepare_b<1>'s operand B, with
+// its rows permuted (prepare_b<1, true>), is also the B of the 2xFP16 fixed-step solve's wgmma (a K-major 128-byte-swizzled
+// tile).
 //
 // One evaluation is the product D[32 paths x 256] = z[32 x 32] . W^T[32 x 256] + bias followed by the contraction
 // kv[h] = sum_c D[h * 8 + c] dX/dt[c].  fp32 accuracy on the tensor pipe comes from a two-way operand split:
@@ -72,9 +73,18 @@ __device__ __forceinline__ void mma_tf32(float* c, const uint32_t* a, uint32_t b
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
+// Tile row of weight row n = 8h + c in the column-permuted MODE 1 tile of the fused solve (prepare_b<1, true>): within each
+// 64-row chunk i, row 8j + 2q + e holds unit h = 8i + 2q + (j >> 2), channel c = 4e + (j & 3), so that lane q of a
+// wgmma m64n64 accumulator (columns 8j + 2q + e) holds the two whole units 8i + 2q, 8i + 2q + 1 x all eight channels.
+__device__ __forceinline__ int field_tile_row(int n) {
+    const int h = n >> 3, c = n & 7;
+    return 64 * (h >> 3) + 8 * (4 * (h & 1) + (c & 3)) + 2 * ((h >> 1) & 3) + (c >> 2);
+}
+
 // Operand B and the bias of the linear field weight [256][32], bias [256] (called by every thread of the CTA; contains
 // __syncthreads).  MODE 1 returns the scales the rows need through inv_w_scale and beta (2^(ex(max|bias|) - ex(max|W|))).
-template <int MODE>
+// PERM (MODE 1 only): weight row n and its bias go to tile row field_tile_row(n) instead of n.
+template <int MODE, bool PERM = false>
 __device__ __forceinline__ void prepare_b(unsigned char* bsm, const float* weight, const float* bias, int tid, int n_threads,
                                           float& inv_w_scale, float& beta) {
     using S = BSmem<MODE>;
@@ -115,14 +125,14 @@ __device__ __forceinline__ void prepare_b(unsigned char* bsm, const float* weigh
     beta = (bmax > 0.f) ? pow2_biased(min(max(127 + eb - ew, 2), 250)) : 0.f;    // 2^(ex(bmax) - ex(wmax))
     __half* bt = reinterpret_cast<__half*>(bsm + S::tile);
     for (int e = tid; e < kCols * kHid; e += n_threads) {
-        const int n = e >> 5, k = e & 31;
+        const int n = (PERM ? field_tile_row(e >> 5) : e >> 5), k = e & 31;     // n: the tile row (swizzled by n & 7)
         const float w = weight[e] * w_scale;
         const __half hi = __float2half_rn(w);
         const __half lo = __float2half_rn(w - __half2float(hi));
         bt[n * 64 + ((((k >> 3)) ^ (n & 7)) << 3) + (k & 7)] = hi;
         bt[n * 64 + ((((k >> 3) + 4) ^ (n & 7)) << 3) + (k & 7)] = lo;
     }
-    for (int n = tid; n < kCols; n += n_threads) b_bias[n] = bias[n] * w_scale;   // a power of two: exact
+    for (int n = tid; n < kCols; n += n_threads) b_bias[PERM ? field_tile_row(n) : n] = bias[n] * w_scale;   // exact
 }
 
 // Row `row` of the warp's operand tile from z (32 floats).  MODE 1: z times the path's own power of two s, split into

@@ -162,7 +162,11 @@ constexpr int kNV = 16;                          // state values per lane: 2 row
 constexpr int kN = 64;                           // output columns per chunk: hidden units 8c .. 8c + 7
 constexpr int kChunks = kCols / kN;
 constexpr int kAcc = kN / 2;                     // accumulator registers per chunk
-constexpr int kSmem = BSmem<1>::bytes + 1024;    // slack for the 1024-byte alignment of the swizzled B tile
+constexpr int kDxSlot = 16 * kCh * 4;           // per warp: the scaled dX/dt of its 16 rows (solve_tc.cu's wg::field)
+constexpr int kXch = BSmem<1>::bytes;            // the four warps' dX/dt slots, after the B tile and the bias
+constexpr int kRowSlot = 6 * 32 * 8;             // per warp and buffer: spline rows, [2][b | 2c | 3d][32] float2
+constexpr int kRows = kXch + 4 * kDxSlot;        // the four warps' two buffers each
+constexpr int kSmem = kRows + 8 * kRowSlot + 1024;   // slack for the 1024-byte alignment of the swizzled B tile
 
 // shared-memory matrix descriptor of a K-major, 128-byte-swizzled operand whose 8-row swizzle atoms are 1024 bytes apart
 __device__ __forceinline__ uint64_t desc_sw128(uint32_t addr) {
