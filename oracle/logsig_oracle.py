@@ -65,7 +65,24 @@ def lyndon_words(channels, depth):
 
 
 def logsignature(path, depth):
-    """Coefficients of the Lyndon words (by length, then lexicographically) of log(signature)."""
-    path = np.asarray(path, dtype=np.float64)
+    """Coefficients of the Lyndon words (by length, then lexicographically) of log(signature).  A complex ``path`` stays
+    complex (the arithmetic is the same), which is what ``logsignature_jacobian`` differentiates through."""
+    path = np.asarray(path)
+    path = path.astype(np.complex128 if np.iscomplexobj(path) else np.float64)
     log = log_tensor(signature(path, depth), depth)
     return np.array([log[len(w)][w] for w in lyndon_words(path.shape[1], depth)])
+
+
+def logsignature_jacobian(path, depth, h=1e-30):
+    """d logsignature / d path, shape (n_words, length, C), by complex-step differentiation: imag(f(x + i h e_j)) / h.
+    ``logsignature`` is built from +, * and / only, so there is no subtractive cancellation: the result is exact to
+    rounding for any small ``h``."""
+    path = np.asarray(path, dtype=np.float64)
+    length, channels = path.shape
+    cols = []
+    for p in range(length):
+        for c in range(channels):
+            z = path.astype(np.complex128)
+            z[p, c] += 1j * h
+            cols.append(logsignature(z, depth).imag / h)
+    return np.stack(cols, axis=-1).reshape(-1, length, channels)

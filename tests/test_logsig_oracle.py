@@ -57,16 +57,92 @@ def test_window_knots_bookkeeping():
     from torchcde_b200.log_ode import _window_knots
 
     random.seed(1)
+    torch.manual_seed(1)
     for trial in range(300):
         n = random.randint(2, 30)
         dtype = random.choice([torch.float32, torch.float64])
         t = torch.linspace(0, n - 1, n, dtype=dtype) if trial % 3 == 0 else (torch.rand(n, dtype=torch.float64) + 0.05).cumsum(0).to(dtype)
         wl = random.choice([0.5, 1.0, 2.0, float(t[-1] - t[0]) / random.randint(1, 5), random.uniform(0.3, 4.0)])
         ends, positions, extra = _window_knots(t, wl)
-        assert float(ends[0]) == float(t[0]) and float(ends[-1]) == float(t[-1])
+        # the last end is the linspace end clipped to the final time; it can round to just below it, and then it is
+        # within torch.allclose of the final time and still names the last knot (positions[-1] below)
+        last = t[0] + (ends.numel() - 1) * wl
+        assert float(ends[0]) == float(t[0]) and float(ends[-1]) == min(float(last), float(t[-1]))
+        assert torch.allclose(ends[-1], t[-1])
         assert ends.numel() == int(math.ceil(float((t[-1] - t[0]) / wl))) + 1 or ends.numel() == int((((t[-1] - t[0]) / wl).ceil()).item()) + 1
         merged = torch.cat([t] + extra).sort().values if extra else t
         assert all(b > a for a, b in zip(positions[:-1], positions[1:]))
-        assert merged.numel() == n + len(extra)
+        assert merged.numel() == n + len(extra) and positions[-1] == merged.numel() - 1
         for e, p in zip(ends.tolist(), positions):
             assert abs(float(merged[p]) - e) <= 1e-8 + 1e-5 * abs(e)
+
+
+def test_jacobian_matches_central_differences_and_level_one():
+    """The complex-step Jacobian against central differences, and level 1 (the total increment) is exactly -1 at the
+    first point, +1 at the last and 0 in between, channel by channel."""
+    rng = np.random.default_rng(3)
+    for length, channels, depth in ((5, 2, 4), (3, 3, 3), (6, 1, 2), (2, 2, 5)):
+        path = rng.standard_normal((length, channels))
+        jac = O.logsignature_jacobian(path, depth)
+        assert jac.shape == (len(O.lyndon_words(channels, depth)), length, channels)
+        h = 1e-6
+        num = np.zeros_like(jac)
+        for p in range(length):
+            for c in range(channels):
+                e = np.zeros_like(path)
+                e[p, c] = h
+                num[:, p, c] = (O.logsignature(path + e, depth) - O.logsignature(path - e, depth)) / (2 * h)
+        assert np.abs(jac - num).max() <= 1e-7 * max(1.0, np.abs(jac).max()), (length, channels, depth)
+        level_one = np.zeros((channels, length, channels))
+        for c in range(channels):
+            level_one[c, 0, c], level_one[c, -1, c] = -1.0, 1.0
+        assert np.array_equal(jac[:channels], level_one)
+        real = O.logsignature(path, depth)
+        assert np.allclose(O.logsignature(path.astype(complex), depth).real, real, rtol=1e-14, atol=1e-14)
+
+
+def test_jacobian_agrees_with_chen_across_a_split_window():
+    """The signature of a path is the product of the signatures of its two halves (Chen), so perturbing a point of the
+    first half moves the whole path's logsignature as the chain rule through that product says.  The whole path's
+    Jacobian at a point of the first half, pushed through the product by complex step on the first half alone, must
+    agree with the Jacobian of the whole; at the point the halves share, both halves move."""
+    rng = np.random.default_rng(4)
+    depth = 4
+    path = rng.standard_normal((7, 2))
+    words = O.lyndon_words(2, depth)
+    whole = O.logsignature_jacobian(path, depth)
+    second = O.signature(path[3:], depth)
+    h = 1e-30
+    for p in range(3):
+        for c in range(2):
+            z = path[:4].astype(complex)
+            z[p, c] += 1j * h
+            log = O.log_tensor(O._mul(O.signature(z, depth), second, depth), depth)
+            chen = np.array([log[len(w)][w] for w in words]).imag / h
+            assert np.allclose(chen, whole[:, p, c], rtol=1e-12, atol=1e-12), (p, c)
+    # the point shared by the halves: the second half's start moves too
+    z = path.astype(complex)
+    z[3, 0] += 1j * h
+    log = O.log_tensor(O._mul(O.signature(z[:4], depth), O.signature(z[3:], depth), depth), depth)
+    assert np.allclose(np.array([log[len(w)][w] for w in words]).imag / h, whole[:, 3, 0], rtol=1e-12, atol=1e-12)
+
+
+def test_window_positions_match_the_reference_slices():
+    """The window end positions of _window_knots against the lengths of the window slices the reference's own log_ode.py
+    handed to signatory (tests/golden/reference_live.npz, oracle/make_reference_golden.py): random fp32 and fp64 ``t``,
+    and ``t`` with a knot a few ulps either side of torch.allclose's tolerance of a window end, where the comparison has
+    to be made in ``t``'s dtype."""
+    import os
+    import torch
+    from torchcde_b200.log_ode import _window_knots
+
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_live.npz"))
+    count = int(z["logsig_spy__count"])
+    assert count >= 300
+    for i in range(count):
+        key = "logsig_spy__{}__".format(i)
+        t = torch.from_numpy(z[key + "t"])
+        lengths = z[key + "lengths"].tolist()
+        _, positions, extra = _window_knots(t, float(z[key + "window"]))
+        assert [b - a + 1 for a, b in zip(positions[:-1], positions[1:])] == lengths, (i, t.dtype)
+        assert positions[0] == 0 and positions[-1] == t.numel() + len(extra) - 1
