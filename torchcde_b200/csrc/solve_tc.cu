@@ -215,10 +215,11 @@ namespace wg {
 // both rows; xch: the warp's kDxSlot bytes of shared memory, through which the quad shares them.  HOLD: all eight
 // channels of both rows stay in registers for the whole evaluation (four 16-byte loads); otherwise they are read again,
 // one float at a time, for each chunk and row, which holds 16 registers fewer (the Runge-Kutta backward and
-// reversible_backward_kernel have no room for them; 16-byte loads there spill).
+// reversible_backward_kernel have no room for them; 16-byte loads there spill).  b_desc = desc_sw128 of the tile: each
+// wgmma's descriptor is b_desc plus a constant.
 template <bool HOLD>
 __device__ __forceinline__ void field(const float* zin, const float (*dx)[2], float beta, float inv_w_scale,
-                                      const float* b_bias, uint32_t b_tile, float* xch, int g, int q, float* kv) {
+                                      const float* b_bias, uint64_t b_desc, float* xch, int g, int q, float* kv) {
     // Each row scaled by its own power of two so that max(|z|, bias floor) lands in [2^13, 2^14), split into FP16
     // hi + lo A fragments [k step][4]; the inverse scales are folded into dX/dt, which goes to the quad's row of xch.
     float rs[2];
@@ -271,13 +272,13 @@ __device__ __forceinline__ void field(const float* zin, const float (*dx)[2], fl
             d[4 * j + 2] = bb.x * rs[1]; d[4 * j + 3] = bb.y * rs[1];
         }
         mma_fence();
-        const uint32_t rows = b_tile + chunk * kN * 128;
-        mma_m64n64k16(d, alo[0], desc_sw128(rows + 0));    // z_lo . W_hi
-        mma_m64n64k16(d, alo[1], desc_sw128(rows + 32));
-        mma_m64n64k16(d, ahi[0], desc_sw128(rows + 64));   // z_hi . W_lo
-        mma_m64n64k16(d, ahi[1], desc_sw128(rows + 96));
-        mma_m64n64k16(d, ahi[0], desc_sw128(rows + 0));    // z_hi . W_hi
-        mma_m64n64k16(d, ahi[1], desc_sw128(rows + 32));
+        const uint32_t rows = chunk * kN * 128;
+        mma_m64n64k16(d, alo[0], desc_add(b_desc, rows + 0));    // z_lo . W_hi
+        mma_m64n64k16(d, alo[1], desc_add(b_desc, rows + 32));
+        mma_m64n64k16(d, ahi[0], desc_add(b_desc, rows + 64));   // z_hi . W_lo
+        mma_m64n64k16(d, ahi[1], desc_add(b_desc, rows + 96));
+        mma_m64n64k16(d, ahi[0], desc_add(b_desc, rows + 0));    // z_hi . W_hi
+        mma_m64n64k16(d, ahi[1], desc_add(b_desc, rows + 32));
         mma_commit();
     };
     issue(0, acc[0]);
@@ -348,15 +349,28 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
 
     // These pieces travel to shared memory by cp.async, a stage ahead of their use, into one of two per-warp buffers of
     // [row r][b | 2c | 3d][lane] float2: held in registers across the products they would push the stage over the
-    // register cap.  Each lane reads back only what it copied itself.
-    float2* rows_buf = reinterpret_cast<float2*>(smem + wg::kRows + warp * 2 * wg::kRowSlot) + lane;
+    // register cap.  Each lane reads back only what it copied itself.  The lane's two source rows and its buffer address
+    // are kept in its fetch slot (wg::kFetch) and read back once per stage: at the register cap the compiler would
+    // otherwise recompute them from the lane's paths every stage, about 60 integer instructions.
+    {
+        const float2* src1 = crow + (int64_t)row1 * a.n_rows * row_f2;
+        reinterpret_cast<ulonglong2*>(smem + wg::kFetch)[tid] =
+            make_ulonglong2(reinterpret_cast<uint64_t>(crow), reinterpret_cast<uint64_t>(src1));
+        reinterpret_cast<uint32_t*>(smem + wg::kFetch + wg::kThreads * 16)[tid] =
+            smem_u32(smem + wg::kRows + warp * 2 * wg::kRowSlot + lane * 8);
+    }
+    const ulonglong2* fetch_src = reinterpret_cast<const ulonglong2*>(smem + wg::kFetch) + tid;
+    const uint32_t* fetch_dst = reinterpret_cast<const uint32_t*>(smem + wg::kFetch + wg::kThreads * 16) + tid;
+    const int row_bytes = row_f2 * 8;
     auto fetch = [&](int interval, int buf) {
-        float2* dst = rows_buf + buf * (wg::kRowSlot / 8);
+        const ulonglong2 base = *fetch_src;
+        const uint32_t dst = *fetch_dst + buf * wg::kRowSlot;
+        const int64_t off = (int64_t)interval * row_bytes;
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
-            const float2* src = crow + (r * row1 * a.n_rows + interval) * row_f2;
-            cp_async8(dst + 3 * r * 32, src);
-            if (cubic) { cp_async8(dst + (3 * r + 1) * 32, src + 4); cp_async8(dst + (3 * r + 2) * 32, src + 8); }
+            const char* src = reinterpret_cast<const char*>(r ? base.y : base.x) + off;
+            wg::cp_async8(dst + 3 * r * 256, src);
+            if (cubic) { wg::cp_async8(dst + (3 * r + 1) * 256, src + 32); wg::cp_async8(dst + (3 * r + 2) * 256, src + 64); }
         }
         cp_async_commit();
     };
@@ -419,19 +433,19 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
     }
 
     const float* b_bias = reinterpret_cast<const float*>(smem + S::bias);
-    const uint32_t b_tile = smem_u32(smem + S::tile);
+    const uint64_t b_desc = wg::desc_sw128(smem_u32(smem + S::tile));
     float* xch = reinterpret_cast<float*>(smem + wg::kXch + warp * wg::kDxSlot);
     const int n_st = a.n_steps * a.n_stages + (REV ? 1 : 0);
     // dX/dt (interpolation_cubic.py:331-336) of a stage at fraction fr of its interval, channels 2q, 2q + 1 of both rows,
     // from the rows fetched into buffer buf
     auto slope = [&](int buf, float fr, float (*dx)[2]) {
         cp_async_wait<0>();
-        const float2* raw = rows_buf + buf * (wg::kRowSlot / 8);
+        const uint32_t raw = *fetch_dst + buf * wg::kRowSlot;
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
-            const float2 b = raw[3 * r * 32];
+            const float2 b = wg::lds_f2(raw + 3 * r * 256);
             if (cubic) {
-                const float2 c2 = raw[(3 * r + 1) * 32], d3 = raw[(3 * r + 2) * 32];
+                const float2 c2 = wg::lds_f2(raw + (3 * r + 1) * 256), d3 = wg::lds_f2(raw + (3 * r + 2) * 256);
                 dx[r][0] = E::add(b.x, E::mul(E::add(c2.x, E::mul(d3.x, fr)), fr));
                 dx[r][1] = E::add(b.y, E::mul(E::add(c2.y, E::mul(d3.y, fr)), fr));
             } else {
@@ -457,7 +471,7 @@ __global__ void __launch_bounds__(wg::kThreads, 3) cdeint_wgmma_kernel(const Umm
         if (st + 1 < n_st) fetch(a.stage_index[st + 1], (st + 1) & 1);
 
         float kv[wg::kNV];
-        wg::field<!BWD>(zin, dx, beta, inv_w_scale, b_bias, b_tile, xch, g, q, kv);
+        wg::field<!BWD>(zin, dx, beta, inv_w_scale, b_bias, b_desc, xch, g, q, kv);
 
         if (REV) {
             rev_heun_combine<wg::kNV>(a, st, step, dt, y, k1, s23, kv, zin, jn, write_out,
@@ -545,7 +559,8 @@ __global__ void __launch_bounds__(wg::kThreads, 2) reversible_backward_kernel(co
     __syncthreads();
     const float* bias_f = reinterpret_cast<const float*>(smem + S::bias);
     const float* bias_g = reinterpret_cast<const float*>(smem + kRevTile + S::bias);
-    const uint32_t tile_f = smem_u32(smem + S::tile), tile_g = smem_u32(smem + kRevTile + S::tile);
+    const uint64_t desc_f = wg::desc_sw128(smem_u32(smem + S::tile));
+    const uint64_t desc_g = wg::desc_sw128(smem_u32(smem + kRevTile + S::tile));
     float* xch = reinterpret_cast<float*>(smem + 2 * kRevTile + warp * wg::kDxSlot);
 
     const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
@@ -630,8 +645,8 @@ __global__ void __launch_bounds__(wg::kThreads, 2) reversible_backward_kernel(co
         float dx[2][2];
         slope_at(m, dx);
         float kf[NV], kg[NV];
-        wg::field<false>(zm, dx, beta_f, inv_f, bias_f, tile_f, xch, g, q, kf);
-        wg::field<false>(fb, dx, beta_g, inv_g, bias_g, tile_g, xch, g, q, kg);
+        wg::field<false>(zm, dx, beta_f, inv_f, bias_f, desc_f, xch, g, q, kf);
+        wg::field<false>(fb, dx, beta_g, inv_g, bias_g, desc_g, xch, g, q, kg);
         store_rows(a.dump_z + (int64_t)(m - a.lo) * plane * kHid, zm);
         store_rows(a.dump_a + (int64_t)(m - a.lo) * plane * kHid, fb);
         if (m == a.lo) {

@@ -166,12 +166,16 @@ constexpr int kDxSlot = 16 * kCh * 4;           // per warp: the scaled dX/dt of
 constexpr int kXch = BSmem<1>::bytes;            // the four warps' dX/dt slots, after the B tile and the bias
 constexpr int kRowSlot = 6 * 32 * 8;             // per warp and buffer: spline rows, [2][b | 2c | 3d][32] float2
 constexpr int kRows = kXch + 4 * kDxSlot;        // the four warps' two buffers each
-constexpr int kSmem = kRows + 8 * kRowSlot + 1024;   // slack for the 1024-byte alignment of the swizzled B tile
+constexpr int kFetch = kRows + 8 * kRowSlot;     // per thread: its two spline-row sources (16 bytes), then its buffer
+constexpr int kSmem = kFetch + kThreads * 20 + 1024;   // slack for the 1024-byte alignment of the swizzled B tile
 
 // shared-memory matrix descriptor of a K-major, 128-byte-swizzled operand whose 8-row swizzle atoms are 1024 bytes apart
 __device__ __forceinline__ uint64_t desc_sw128(uint32_t addr) {
     return (uint64_t)((addr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
+// desc_sw128(addr + off) from base = desc_sw128(addr), for a shared-memory address addr + off below 2^18 (every shared
+// address is) and off a multiple of 16: the start-address field (bits 0-13) is then (addr + off) >> 4, with no carry
+__device__ __forceinline__ uint64_t desc_add(uint64_t base, uint32_t off) { return base + (off >> 4); }
 
 __device__ __forceinline__ void mma_m64n64k16(float* d, const uint32_t* a, uint64_t b) {
     asm volatile(
@@ -184,6 +188,15 @@ __device__ __forceinline__ void mma_m64n64k16(float* d, const uint32_t* a, uint6
           "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
           "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+}
+// cp.async of 8 bytes to the shared address s; an 8-byte load from one
+__device__ __forceinline__ void cp_async8(uint32_t s, const void* gmem) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(s), "l"(gmem) : "memory");
+}
+__device__ __forceinline__ float2 lds_f2(uint32_t s) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(s) : "memory");
+    return v;
 }
 __device__ __forceinline__ void mma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void mma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
