@@ -244,8 +244,11 @@ TCDE_API int tcde_cdeint_fixed_mlp(const void* control, int control_kind, int64_
 
 /* tcde_cdeint_fixed_mlp that also stores the INPUT of every stage: stage_dump[n_steps * n_stages][n_paths][hidden] (the
  * forward state of tcde_cdeint_fixed_mlp_backward).  The outputs equal tcde_cdeint_fixed_mlp's bit for bit.  Served by the
- * tensor-core kernel only: fp32, hidden = 32, channels = 8, width = 128, 16-byte aligned control, z0, out and dump, solve
- * variant 0, 4 or 5; TCDE_ERR_UNSUPPORTED otherwise. */
+ * tensor-core kernel at fp32, hidden = 32, channels = 8, width = 128 with 16-byte aligned control, z0, out and dump under
+ * solve variant 0, 4 or 5, and by the CUDA-core kernel (fp32 or fp64, any alignment) at hidden <= 8 under solve variant
+ * 0 or 1, and under variant 1 also at hidden * channels <= 32 (the other shapes where tcde_cdeint_fixed_mlp runs it by
+ * default; by default they are refused because the backward there is slower than a stage loop); TCDE_ERR_UNSUPPORTED
+ * otherwise. */
 TCDE_API int tcde_cdeint_fixed_mlp_stages(const void* control, int control_kind, int64_t n_rows, const void* w1,
                                  const void* b1, const void* w2, const void* b2, const void* z0, void* out,
                                  void* stage_dump, int64_t n_paths, int64_t channels, int64_t hidden, int64_t width,
@@ -262,7 +265,7 @@ TCDE_API int tcde_cdeint_fixed_mlp_stages(const void* control, int control_kind,
  * (h and y recomputed by the forward's own code, so the mask and tanh values are the forward's bits).  grad_z0
  * [n_paths][hidden] receives dL/dz0; kappa_dump (may be NULL) [n_steps * n_stages][n_paths][hidden] receives kappa_s in the
  * slot of stage s's input in stage_dump, for tcde_mlp_field_param_grads.  Same support as tcde_cdeint_fixed_mlp_stages
- * (grad_out and grad_z0 16-byte aligned too). */
+ * (on the tensor-core kernel, grad_out and grad_z0 16-byte aligned too). */
 TCDE_API int tcde_cdeint_fixed_mlp_backward(const void* control, int control_kind, int64_t n_rows, const void* w1,
                                    const void* b1, const void* w2, const void* b2, const void* stage_dump,
                                    const void* grad_out, void* grad_z0, void* kappa_dump, int64_t n_paths, int64_t channels,
@@ -275,9 +278,11 @@ TCDE_API int tcde_cdeint_fixed_mlp_backward(const void* control, int control_kin
  * kappa_stages = the backward's kappa, both [n_stages_total][n_paths][hidden]):
  *   grad_w2 += scale sum g h^T,  grad_b2 += scale sum g,  grad_w1 += scale sum ubar z^T,  grad_b1 += scale sum ubar
  * over every (stage, path), with g and ubar = mask . W2^T g recomputed as the backward forms them (dX/dt from the control at
- * (stage_index[e], stage_frac[e]) times `sign`).  Any gradient pointer may be NULL.  Tensor cores (2xBF16 split), a
- * fixed-order reduction: two calls give the same bits.  Same support as tcde_cdeint_fixed_mlp_stages; scratch of
- * tcde_mlp_field_param_grads_scratch_bytes (-1: not built for the shape). */
+ * (stage_index[e], stage_frac[e]) times `sign`).  Any gradient pointer may be NULL.  Tensor cores (2xBF16 split) at
+ * 32 / 8 / 128, the CUDA cores at the CUDA-core shapes; a fixed-order reduction: two calls give the same bits.  Same
+ * support as tcde_cdeint_fixed_mlp_stages, except that a CUDA-core width whose staging does not fit shared memory is
+ * refused; scratch of tcde_mlp_field_param_grads_scratch_bytes (-1: not built for the shape; it has no dtype argument, so
+ * at the CUDA-core shapes it is the size for 8-byte elements). */
 TCDE_API int64_t tcde_mlp_field_param_grads_scratch_bytes(int64_t n_paths, int64_t n_stages_total, int64_t channels,
                                                  int64_t hidden, int64_t width);
 TCDE_API int tcde_mlp_field_param_grads(const void* control, int control_kind, int64_t n_rows, const void* w1,

@@ -1,5 +1,6 @@
-"""Time one training step (forward + ``out[:, -1].sum().backward()``) of cdeint at config 3 (length 256, channels 8, hidden
-32) with the examples' MLP field (width 128, cubic control, rk4, step 1) on three routes, alternated in one process:
+"""Time one training step (forward + ``out[:, -1].sum().backward()``) of cdeint at length 256 with the examples' MLP field
+(by default config 3: channels 8, hidden 32, width 128; cubic control, rk4, step 1) on three routes, alternated in one
+process:
 
   * ``backprop``: adjoint=False on the three-launch discrete backward (stage-dump solve, tcde_cdeint_fixed_mlp_backward,
     tcde_mlp_field_param_grads);
@@ -11,7 +12,8 @@ Each step is bracketed by device synchronisations; medians over the repetitions,
 route, and each route's dL/dz0 and dL/dW2 against the backprop route's on the same batch.  The card's name, power limit
 and SM clock are read in the same run.  ``--profile DIR``: instead, one step of each route under torch.profiler, the
 per-kernel CUDA times written to DIR/mlp_backprop_kernels.txt.
-usage: python scripts/mlp_backprop_bench.py [--batch 65536] [--reps 3] [--profile DIR]"""
+usage: python scripts/mlp_backprop_bench.py [--batch 65536] [--reps 3] [--hidden 32] [--channels 8] [--width 128]
+                                           [--profile DIR]"""
 import argparse
 import json
 import math
@@ -96,8 +98,13 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=65536)
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--hidden", type=int, default=32)
+    ap.add_argument("--channels", type=int, default=8)
+    ap.add_argument("--width", type=int, default=128)
     ap.add_argument("--profile", default=None)
     args = ap.parse_args()
+    global C, H, W
+    C, H, W = args.channels, args.hidden, args.width
     info = card()
     full = problem(args.batch)
     if args.profile:
@@ -149,7 +156,7 @@ def main():
             "sequences_per_s": batch / statistics.median(times[name]), "peak_gib": peak[name] / 2 ** 30,
             "dl_dz0_vs_backprop": rel(gz, ref[0], True), "dl_dw2_vs_backprop": rel(gw, ref[1], False),
             "gpu": info.get("name"), "power_limit": info.get("power.limit"), "sm_clock": info.get("clocks.sm"),
-            "max_sm_clock": info.get("clocks.max.sm")}), flush=True)
+            "max_sm_clock": info.get("clocks.max.sm"), "hidden": H, "channels": C, "width": W}), flush=True)
 
 
 if __name__ == "__main__":

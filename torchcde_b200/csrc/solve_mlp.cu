@@ -4,8 +4,9 @@
 // controls, Runge-Kutta methods and outputs of tcde_cdeint_fixed_linear.  Two kernels:
 //   * cdeint_mlp_wgmma_kernel (fp32, H = 32, C = 8, W = 128): the 2xFP16 split of cdeint_wgmma_kernel for both products,
 //     two warpgroups per CTA sharing one copy of the split weights;
-//   * cdeint_mlp_simt_kernel<T, HM> (fp32 / fp64, H <= HM, any C and W): one thread per path on the CUDA cores; the fp64
-//     instantiation is the reference solve of the parity tests.
+//   * cdeint_mlp_simt_kernel<T, HM, DUMP> (fp32 / fp64, H <= HM, any C and W): one thread per path on the CUDA cores; the
+//     fp64 instantiation is the reference solve of the parity tests.
+// Each has a stage-dump variant, a Runge-Kutta backward and a parameter-gradient kernel for cdeint(..., adjoint=False).
 #include "wg_common.cuh"
 
 namespace tcde {
@@ -53,7 +54,8 @@ template <typename T> struct MlpSimtLayout {
     bool staged;
 };
 
-template <typename T> static MlpSimtLayout<T> mlp_simt_layout(int H, int C, int W, bool stage) {
+template <typename T> static MlpSimtLayout<T> mlp_simt_layout(int H, int C, int W, bool stage,
+                                                                int nt = kMlpSimtThreads) {
     MlpSimtLayout<T> l;
     l.Hp = (H + 3) / 4 * 4;
     l.Nq = (H * C + kMlpChunk - 1) / kMlpChunk * kMlpChunk;
@@ -68,13 +70,80 @@ template <typename T> static MlpSimtLayout<T> mlp_simt_layout(int H, int C, int 
     } else {
         l.w1 = l.w2t = l.b1 = l.b2 = 0;
     }
-    l.cols = off; off += (size_t)(C + H) * kMlpSimtThreads;       // per thread: dX/dt [C], slopes [H]
+    l.cols = off; off += (size_t)(C + H) * nt;                    // per thread: dX/dt [C], slopes [H]
     l.total = off * sizeof(T);
     return l;
 }
 
-template <typename T, int HM>
-__global__ void __launch_bounds__(kMlpSimtThreads) cdeint_mlp_simt_kernel(const MlpArgs<T> a, const MlpSimtLayout<T> lay) {
+// The field evaluation that the forward and the backward kernels share, so that the backward's dX/dt, ReLU masks and tanh
+// values are the forward's bits.  Macros rather than __forceinline__ functions: the forward kernel expands them in place,
+// token for token the code it had before the backward kernels existed, so its instructions are unchanged (as functions,
+// the same code came out with a different register allocation).  They read the caller's a, lay, smem, tid, nt, crow,
+// cubic, zin and H, C, W, HC, Hp, Nq, and the types E and P4.
+//
+// The weights in shared memory as W1 [W][Hp] and W2^T [W][Nq] (zero padded), by the CTA's nt threads (tid: this one)
+#define TCDE_MLP_STAGE_WEIGHTS()                                                                                       \
+    for (int e = tid; e < W * Hp; e += nt) {                                                                           \
+        const int w = e / Hp, k = e - w * Hp;                                                                          \
+        smem[lay.w1 + e] = k < H ? a.w1[(size_t)w * H + k] : T(0);                                                     \
+    }                                                                                                                  \
+    for (int e = tid; e < W * Nq; e += nt) {                                                                           \
+        const int w = e / Nq, n = e - w * Nq;                                                                          \
+        smem[lay.w2t + e] = n < HC ? a.w2[(size_t)n * W + w] : T(0);                                                   \
+    }                                                                                                                  \
+    for (int e = tid; e < W; e += nt) smem[lay.b1 + e] = a.b1[e];                                                      \
+    for (int e = tid; e < Nq; e += nt) smem[lay.b2 + e] = e < HC ? a.b2[e] : T(0);
+
+// dX/dt at (interval, fr) (interpolation_cubic.py:331-336), times the sign of the time direction, into dxs[c * nt]
+#define TCDE_MLP_SLOPE(interval, frac)                                                                                 \
+    const T* r = crow + (int64_t)(interval) * (cubic ? 4 * C : C);                                                     \
+    const T fr = (frac);                                                                                               \
+    for (int c = 0; c < C; ++c) {                                                                                      \
+        const T v = cubic ? E::add(r[c], E::mul(E::add(r[C + c], E::mul(r[2 * C + c], fr)), fr)) : r[c];             \
+        dxs[(size_t)c * nt] = a.sign < T(0) ? -v : v;                                                                  \
+    }
+
+// u = the pre-activation W1[w] . z + b1[w] of hidden unit w
+#define TCDE_MLP_PRE(u, w)                                                                                             \
+    T u;                                                                                                               \
+    if (lay.staged) {                                                                                                  \
+        u = smem[lay.b1 + w];                                                                                          \
+        const T* wr = smem + lay.w1 + (size_t)w * Hp;                                                                  \
+        _Pragma("unroll") for (int k4 = 0; k4 < HM / 4; ++k4) {                                                        \
+            if (4 * k4 < Hp) {                                                                                         \
+                const P4 w4 = *reinterpret_cast<const P4*>(wr + 4 * k4);                                               \
+                _Pragma("unroll") for (int i = 0; i < 4; ++i) u = fma(w4.v[i], zin[4 * k4 + i], u);                    \
+            }                                                                                                          \
+        }                                                                                                              \
+    } else {                                                                                                           \
+        u = __ldg(a.b1 + w);                                                                                           \
+        const T* wr = a.w1 + (size_t)w * H;                                                                            \
+        _Pragma("unroll") for (int k = 0; k < HM; ++k) if (k < H) u = fma(__ldg(wr + k), zin[k], u);                  \
+    }
+
+// acc [NT] = W2 relu(W1 z + b1) + b2 for the outputs n0 .. n0 + NT - 1
+#define TCDE_MLP_CHUNK(acc, n0)                                                                                        \
+    _Pragma("unroll") for (int j = 0; j < kMlpChunk; ++j)                                                              \
+        acc[j] = lay.staged ? smem[lay.b2 + n0 + j] : (n0 + j < HC ? __ldg(a.b2 + n0 + j) : T(0));                     \
+    for (int w = 0; w < W; ++w) {                                                                                      \
+        TCDE_MLP_PRE(u, w)                                                                                             \
+        u = u > T(0) ? u : T(0);                                                                                       \
+        if (lay.staged) {                                                                                              \
+            const T* wc = smem + lay.w2t + (size_t)w * Nq + n0;                                                        \
+            _Pragma("unroll") for (int j4 = 0; j4 < kMlpChunk / 4; ++j4) {                                             \
+                const P4 w4 = *reinterpret_cast<const P4*>(wc + 4 * j4);                                               \
+                _Pragma("unroll") for (int i = 0; i < 4; ++i) acc[4 * j4 + i] = fma(w4.v[i], u, acc[4 * j4 + i]);      \
+            }                                                                                                          \
+        } else {                                                                                                       \
+            _Pragma("unroll") for (int j = 0; j < kMlpChunk; ++j)                                                      \
+                if (n0 + j < HC) acc[j] = fma(__ldg(a.w2 + (size_t)(n0 + j) * W + w), u, acc[j]);                      \
+        }                                                                                                              \
+    }
+
+// DUMP: the input of every stage also goes to stage_dump[stage][path][H] (the forward state of the backward kernels)
+template <typename T, int HM, bool DUMP>
+__global__ void __launch_bounds__(kMlpSimtThreads) cdeint_mlp_simt_kernel(const MlpArgs<T> a, const MlpSimtLayout<T> lay,
+                                                                          T* stage_dump) {
     using E = exact<T>;
     using P4 = Pack<T, 4>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -82,16 +151,7 @@ __global__ void __launch_bounds__(kMlpSimtThreads) cdeint_mlp_simt_kernel(const 
     const int tid = threadIdx.x, nt = blockDim.x;
     const int H = a.H, C = a.C, W = a.W, HC = a.H * a.C, Hp = lay.Hp, Nq = lay.Nq;
     if (lay.staged) {
-        for (int e = tid; e < W * Hp; e += nt) {
-            const int w = e / Hp, k = e - w * Hp;
-            smem[lay.w1 + e] = k < H ? a.w1[(size_t)w * H + k] : T(0);
-        }
-        for (int e = tid; e < W * Nq; e += nt) {
-            const int w = e / Nq, n = e - w * Nq;
-            smem[lay.w2t + e] = n < HC ? a.w2[(size_t)n * W + w] : T(0);
-        }
-        for (int e = tid; e < W; e += nt) smem[lay.b1 + e] = a.b1[e];
-        for (int e = tid; e < Nq; e += nt) smem[lay.b2 + e] = e < HC ? a.b2[e] : T(0);
+        TCDE_MLP_STAGE_WEIGHTS()
         __syncthreads();
     }
     T* dxs = smem + lay.cols + tid;                                // dxs[c * nt]: dX/dt channel c
@@ -123,57 +183,20 @@ __global__ void __launch_bounds__(kMlpSimtThreads) cdeint_mlp_simt_kernel(const 
     int step = 0, sub = 0;
     T dt = a.step_dt[0];
     for (int st = 0; st < total; ++st) {
+        if (DUMP && live) {
+            T* dst = stage_dump + ((int64_t)st * a.n_paths + path) * H;
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) dst[h] = zin[h];
+        }
         // dX/dt of this stage (interpolation_cubic.py:331-336), times the sign of the time direction
         {
-            const T* r = crow + (int64_t)a.stage_index[st] * (cubic ? 4 * C : C);
-            const T fr = a.stage_frac[st];
-            for (int c = 0; c < C; ++c) {
-                const T v = cubic ? E::add(r[c], E::mul(E::add(r[C + c], E::mul(r[2 * C + c], fr)), fr)) : r[c];
-                dxs[(size_t)c * nt] = a.sign < T(0) ? -v : v;
-            }
+            TCDE_MLP_SLOPE(a.stage_index[st], a.stage_frac[st])
             for (int h = 0; h < H; ++h) kvs[(size_t)h * nt] = T(0);
         }
         for (int n0 = 0; n0 < HC; n0 += kMlpChunk) {
             T acc[kMlpChunk];
-#pragma unroll
-            for (int j = 0; j < kMlpChunk; ++j)
-                acc[j] = lay.staged ? smem[lay.b2 + n0 + j] : (n0 + j < HC ? __ldg(a.b2 + n0 + j) : T(0));
-            for (int w = 0; w < W; ++w) {
-                // hidden unit w: relu(W1[w] . z + b1[w])
-                T u;
-                if (lay.staged) {
-                    u = smem[lay.b1 + w];
-                    const T* wr = smem + lay.w1 + (size_t)w * Hp;
-#pragma unroll
-                    for (int k4 = 0; k4 < HM / 4; ++k4) {
-                        if (4 * k4 < Hp) {
-                            const P4 w4 = *reinterpret_cast<const P4*>(wr + 4 * k4);
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) u = fma(w4.v[i], zin[4 * k4 + i], u);
-                        }
-                    }
-                } else {
-                    u = __ldg(a.b1 + w);
-                    const T* wr = a.w1 + (size_t)w * H;
-#pragma unroll
-                    for (int k = 0; k < HM; ++k)
-                        if (k < H) u = fma(__ldg(wr + k), zin[k], u);
-                }
-                u = u > T(0) ? u : T(0);
-                if (lay.staged) {
-                    const T* wc = smem + lay.w2t + (size_t)w * Nq + n0;
-#pragma unroll
-                    for (int j4 = 0; j4 < kMlpChunk / 4; ++j4) {
-                        const P4 w4 = *reinterpret_cast<const P4*>(wc + 4 * j4);
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) acc[4 * j4 + i] = fma(w4.v[i], u, acc[4 * j4 + i]);
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < kMlpChunk; ++j)
-                        if (n0 + j < HC) acc[j] = fma(__ldg(a.w2 + (size_t)(n0 + j) * W + w), u, acc[j]);
-                }
-            }
+            TCDE_MLP_CHUNK(acc, n0)
             // tanh, times dX/dt, into the slopes: output n = h C + c
             int h = n0 / C, c = n0 - h * C;
 #pragma unroll
@@ -241,27 +264,365 @@ __global__ void __launch_bounds__(kMlpSimtThreads) cdeint_mlp_simt_kernel(const 
     }
 }
 
+// The layout of a CUDA-core kernel: the weights staged when everything fits in kMax bytes, else read from global memory
+constexpr size_t kMlpSimtMaxSmem = 200 * 1024;
+template <typename T> static int mlp_simt_pick_layout(int H, int C, int W, MlpSimtLayout<T>& lay) {
+    lay = mlp_simt_layout<T>(H, C, W, true);
+    if (lay.total > kMlpSimtMaxSmem) lay = mlp_simt_layout<T>(H, C, W, false);
+    TCDE_CHECK_SUPPORTED(lay.total <= kMlpSimtMaxSmem, "MLP solve: hidden=%d channels=%d do not fit the CUDA-core "
+                         "kernel's shared memory", H, C);
+    return TCDE_OK;
+}
+
 template <typename T, int HM>
-static int launch_mlp_simt(const MlpArgs<T>& a, cudaStream_t stream) {
-    auto kern = cdeint_mlp_simt_kernel<T, HM>;
-    constexpr size_t kMax = 200 * 1024;
-    MlpSimtLayout<T> lay = mlp_simt_layout<T>(a.H, a.C, a.W, true);
-    if (lay.total > kMax) lay = mlp_simt_layout<T>(a.H, a.C, a.W, false);
-    TCDE_CHECK_SUPPORTED(lay.total <= kMax, "MLP solve: hidden=%d channels=%d do not fit the CUDA-core kernel's shared "
-                         "memory", a.H, a.C);
+static int launch_mlp_simt(const MlpArgs<T>& a, T* stage_dump, cudaStream_t stream) {
+    auto kern = stage_dump ? cdeint_mlp_simt_kernel<T, HM, true> : cdeint_mlp_simt_kernel<T, HM, false>;
+    MlpSimtLayout<T> lay;
+    const int rc = mlp_simt_pick_layout<T>(a.H, a.C, a.W, lay);
+    if (rc != TCDE_OK) return rc;
     TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
     const int64_t ctas = (a.n_paths + kMlpSimtThreads - 1) / kMlpSimtThreads;
     TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
-    kern<<<(unsigned)ctas, kMlpSimtThreads, lay.total, stream>>>(a, lay);
+    kern<<<(unsigned)ctas, kMlpSimtThreads, lay.total, stream>>>(a, lay, stage_dump);
     TCDE_CHECK_CUDA(cudaGetLastError());
     return TCDE_OK;
 }
 
 template <typename T>
-static int solve_mlp_simt(const MlpArgs<T>& a, cudaStream_t stream) {
+static int solve_mlp_simt(const MlpArgs<T>& a, cudaStream_t stream, T* stage_dump = nullptr) {
     TCDE_CHECK_SUPPORTED(a.H <= 32, "MLP solve: hidden=%d > 32 is not built for the CUDA-core kernel", a.H);
-    if (a.H <= 8) return launch_mlp_simt<T, 8>(a, stream);
-    return launch_mlp_simt<T, 32>(a, stream);
+    if (a.H <= 8) return launch_mlp_simt<T, 8>(a, stage_dump, stream);
+    return launch_mlp_simt<T, 32>(a, stage_dump, stream);
+}
+
+// ---- the backward of the CUDA-core solve (cdeint(..., adjoint=False)): one thread per path ---------------------------
+//
+// The transposed Runge-Kutta recurrence of cdeint_mlp_backward_kernel (rk_backward_combine, the host-reversed tables, the
+// same output-gradient injection), with the stage product at the forward's stage input z_s (read back from its dump)
+//   u_s = W1^T (mask . W2^T g),   g[(h, c)] = (1 - y^2)[(h, c)] kappa_s[h] dX_s[c],   mask = (W1 z_s + b1 > 0)
+// formed chunk by chunk: TCDE_MLP_CHUNK recomputes the chunk's v = W2 h + b2 (the forward's bits, so y = tanh(v) and the ReLU
+// mask are the forward's), g of its NT outputs stays in registers, and a second pass over the hidden units recomputes
+// each pre-activation for its mask and adds W1[w] (mask_w W2[chunk, w] . g) to u.  u is linear in g, so nothing of
+// width W is kept per thread.  dX/dt and kappa sit in the thread's column of shared memory, as the forward's dX/dt and
+// slopes do (their index runs with the output n = h C + c).
+
+// For every chunk: chunk(n0, g) with g [NT] (zero past H C), then unit(w, pre_w, W2[n0 .., w] . g) for every hidden unit
+template <typename T, int HM, typename Chunk, typename Unit>
+__device__ __forceinline__ void mlp_vjp(const MlpArgs<T>& a, const MlpSimtLayout<T>& lay, const T* smem, const T* zin,
+                                        const T* dxs, const T* kvs, int nt, Chunk chunk, Unit unit) {
+    using E = exact<T>;
+    using P4 = Pack<T, 4>;
+    const int H = a.H, C = a.C, W = a.W, HC = a.H * a.C, Hp = lay.Hp, Nq = lay.Nq;
+    for (int n0 = 0; n0 < HC; n0 += kMlpChunk) {
+        T gc[kMlpChunk];
+        TCDE_MLP_CHUNK(gc, n0)
+        int h = n0 / C, c = n0 - h * C;
+#pragma unroll
+        for (int j = 0; j < kMlpChunk; ++j) {
+            if (n0 + j < HC) {
+                const T y = tanh_of(gc[j]);
+                gc[j] = E::mul(E::sub(T(1), E::mul(y, y)), E::mul(kvs[(size_t)h * nt], dxs[(size_t)c * nt]));
+                if (++c == C) { c = 0; ++h; }
+            } else {
+                gc[j] = T(0);
+            }
+        }
+        chunk(n0, gc);
+        for (int w = 0; w < W; ++w) {
+            TCDE_MLP_PRE(pre, w)
+            T sv = T(0);
+            if (lay.staged) {
+                const T* wc = smem + lay.w2t + (size_t)w * Nq + n0;
+#pragma unroll
+                for (int j4 = 0; j4 < kMlpChunk / 4; ++j4) {
+                    const P4 w4 = *reinterpret_cast<const P4*>(wc + 4 * j4);
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) sv = fma(w4.v[i], gc[4 * j4 + i], sv);
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < kMlpChunk; ++j)
+                    if (n0 + j < HC) sv = fma(__ldg(a.w2 + (size_t)(n0 + j) * W + w), gc[j], sv);
+            }
+            unit(n0, w, pre, sv);
+        }
+    }
+}
+
+template <typename T> struct MlpSimtBwd {
+    const T* z_dump;              // the forward's stage inputs [n_total][n_paths][H]
+    T* kappa_dump;                // kappa_s in the same slots (may be null)
+    const T* grad_out;            // [n_paths][n_out][H]
+    const int32_t* inj_range;
+    const int32_t* inj_out;
+    const T* inj_weight;
+};
+
+// a.step_dt, a.stage_index, a.stage_frac: the host-reversed tables; a.out: dL/dz0 [n_paths][H]
+template <typename T, int HM>
+__global__ void __launch_bounds__(kMlpSimtThreads) cdeint_mlp_simt_backward_kernel(const MlpArgs<T> a,
+                                                                                   const MlpSimtLayout<T> lay,
+                                                                                   const MlpSimtBwd<T> b) {
+    using E = exact<T>;
+    using P4 = Pack<T, 4>;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    T* smem = reinterpret_cast<T*>(smem_raw);
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const int H = a.H, C = a.C, W = a.W, HC = a.H * a.C, Hp = lay.Hp, Nq = lay.Nq;
+    if (lay.staged) {
+        TCDE_MLP_STAGE_WEIGHTS()
+        __syncthreads();
+    }
+    T* dxs = smem + lay.cols + tid;
+    T* kvs = dxs + (size_t)C * nt;                                 // kvs[h * nt]: kappa of hidden unit h
+    const int64_t path = (int64_t)blockIdx.x * nt + tid;
+    const bool live = path < a.n_paths;
+    const int64_t lp = live ? path : a.n_paths - 1;
+    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
+    const T* crow = a.control + lp * a.n_rows * (cubic ? 4 * C : C) + (cubic ? C : 0);
+
+    // v += the output gradients that land on grid state r (counted from the end of the solve)
+    auto inject = [&](int r, T* v) {
+        for (int e = b.inj_range[r]; e < b.inj_range[r + 1]; ++e) {
+            const T wt = b.inj_weight[e];
+            const T* src = b.grad_out + (lp * a.n_out + b.inj_out[e]) * H;
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) v[h] = E::add(v[h], E::mul(wt, src[h]));
+        }
+    };
+
+    T yb[HM], su[HM], run[HM], kap[HM];
+#pragma unroll
+    for (int h = 0; h < HM; ++h) { yb[h] = T(0); su[h] = T(0); run[h] = T(0); }
+    inject(0, yb);
+    tc::rk_backward_first<HM>(a, a.step_dt[0], yb, kap);
+
+    const int n_st = a.n_steps * a.n_stages;
+    const int64_t plane = a.n_paths * H;
+    const T* z_at = b.z_dump + (int64_t)(n_st - 1) * plane + lp * H;     // stage st's forward slot, walking down
+    T* k_at = b.kappa_dump ? b.kappa_dump + (int64_t)(n_st - 1) * plane + lp * H : nullptr;
+    int step = 0, sub = 0;
+    T dt = a.step_dt[0];
+    for (int st = 0; st < n_st; ++st) {
+        T zs[HM], kv[HM];
+#pragma unroll
+        for (int h = 0; h < HM; ++h) {
+            zs[h] = (h < H) ? z_at[h] : T(0);
+            kv[h] = T(0);
+            if (h < H) {
+                kvs[(size_t)h * nt] = kap[h];
+                if (k_at && live) k_at[h] = kap[h];
+            }
+        }
+        z_at -= plane;
+        if (k_at) k_at -= plane;
+        {
+            TCDE_MLP_SLOPE(a.stage_index[st], a.stage_frac[st])
+        }
+        mlp_vjp<T, HM>(a, lay, smem, zs, dxs, kvs, nt, [](int, const T*) {}, [&](int, int w, T pre, T sv) {
+            if (!(pre > T(0))) return;
+            if (lay.staged) {
+                const T* wr = smem + lay.w1 + (size_t)w * lay.Hp;
+#pragma unroll
+                for (int k4 = 0; k4 < HM / 4; ++k4) {
+                    if (4 * k4 < lay.Hp) {
+                        const P4 w4 = *reinterpret_cast<const P4*>(wr + 4 * k4);
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) kv[4 * k4 + i] = fma(w4.v[i], sv, kv[4 * k4 + i]);
+                    }
+                }
+            } else {
+                const T* wr = a.w1 + (size_t)w * H;
+#pragma unroll
+                for (int k = 0; k < HM; ++k)
+                    if (k < H) kv[k] = fma(__ldg(wr + k), sv, kv[k]);
+            }
+        });
+        if (tc::rk_backward_combine<HM>(a, sub, dt, yb, su, run, kv, kap)) {
+            ++step;
+            sub = 0;
+            inject(step, yb);
+            if (step < a.n_steps) {
+                dt = a.step_dt[step];
+                tc::rk_backward_first<HM>(a, dt, yb, kap);
+            }
+        } else {
+            ++sub;
+        }
+    }
+    if (live) {
+#pragma unroll
+        for (int h = 0; h < HM; ++h)
+            if (h < H) a.out[path * H + h] = yb[h];
+    }
+}
+
+template <typename T, int HM>
+static int launch_mlp_simt_backward(const MlpArgs<T>& a, const MlpSimtBwd<T>& b, cudaStream_t stream) {
+    auto kern = cdeint_mlp_simt_backward_kernel<T, HM>;
+    MlpSimtLayout<T> lay;
+    const int rc = mlp_simt_pick_layout<T>(a.H, a.C, a.W, lay);
+    if (rc != TCDE_OK) return rc;
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
+    const int64_t ctas = (a.n_paths + kMlpSimtThreads - 1) / kMlpSimtThreads;
+    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
+    kern<<<(unsigned)ctas, kMlpSimtThreads, lay.total, stream>>>(a, lay, b);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    return TCDE_OK;
+}
+
+// ---- the parameter gradients of the CUDA-core backward ---------------------------------------------------------------
+//
+//   dW2 = sum_e g_e h_e^T,  db2 = sum_e g_e,  dW1 = sum_e ub_e z_e^T,  db1 = sum_e ub_e
+// over the items e = (stage, path).  A block is one stage x NI paths, one thread per item, dealt to a persistent grid.
+// Each thread recomputes its g and ub with mlp_vjp (the backward's code on the dumped z_s and kappa_s) and stages g [HC],
+// h [W], ub [W] and z [H] in shared memory, item-minor; the CTA then adds the block's items, in order, to the running
+// sums of the parameter entries each thread owns (entry p, p + NI, ...), kept in the CTA's row of the scratch.
+// mlp_simt_param_reduce_kernel adds the rows in CTA order: two runs give the same bits.
+struct MlpSimtPg {
+    int ni;                        // items per block = threads per CTA
+    int rs;                        // staging row stride in elements (ni + 1)
+    size_t g, h, ub, z;            // staging offsets in elements of T: g [HC][rs], h [W][rs], ub [W][rs], z [H][rs]
+    size_t total;                  // bytes of dynamic shared memory
+};
+constexpr int kMlpPgCtasPerSm = 4;
+
+// the per-CTA parameter vector [W1 | b1 | W2 | b2]
+static int64_t mlp_simt_n_params(int64_t H, int64_t C, int64_t W) { return W * H + W + H * C * W + H * C; }
+
+// The staging of ni items after the weights and the per-thread columns of lay (lay built for ni threads)
+template <typename T> static MlpSimtPg mlp_simt_pg_layout(const MlpSimtLayout<T>& lay, int H, int C, int W, int ni) {
+    MlpSimtPg p;
+    p.ni = ni;
+    p.rs = ni + 1;
+    size_t off = lay.total / sizeof(T);
+    p.g = off; off += (size_t)H * C * p.rs;
+    p.h = off; off += (size_t)W * p.rs;
+    p.ub = off; off += (size_t)W * p.rs;
+    p.z = off; off += (size_t)H * p.rs;
+    p.total = off * sizeof(T);
+    return p;
+}
+
+// The widest block (128, 64 or 32 items) whose staging fits, with the weights staged if they fit too; false if none does
+template <typename T>
+static bool mlp_simt_pg_pick(int H, int C, int W, MlpSimtLayout<T>& lay, MlpSimtPg& pg) {
+    for (int ni = kMlpSimtThreads; ni >= 32; ni /= 2) {
+        for (int stage = 1; stage >= 0; --stage) {
+            lay = mlp_simt_layout<T>(H, C, W, stage != 0, ni);
+            pg = mlp_simt_pg_layout<T>(lay, H, C, W, ni);
+            if (pg.total <= kMlpSimtMaxSmem) return true;
+        }
+    }
+    return false;
+}
+
+template <typename T> struct MlpSimtPgArgs {
+    const T* z_stages;            // [n_total][n_paths][H]
+    const T* kappa;               // [n_total][n_paths][H]
+    T* scratch;                   // [gridDim.x][n_params]
+    int64_t n_params;
+    int n_total;                  // stages of the solve
+};
+
+// a.stage_index, a.stage_frac: the forward's tables
+template <typename T, int HM>
+__global__ void __launch_bounds__(kMlpSimtThreads) mlp_simt_param_grad_kernel(const MlpArgs<T> a,
+                                                                              const MlpSimtLayout<T> lay,
+                                                                              const MlpSimtPg pg,
+                                                                              const MlpSimtPgArgs<T> p) {
+    using E = exact<T>;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    T* smem = reinterpret_cast<T*>(smem_raw);
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const int H = a.H, C = a.C, W = a.W, HC = a.H * a.C, Hp = lay.Hp, Nq = lay.Nq, rs = pg.rs;
+    if (lay.staged) {
+        TCDE_MLP_STAGE_WEIGHTS()
+    }
+    T* dxs = smem + lay.cols + tid;
+    T* kvs = dxs + (size_t)C * nt;
+    T* gs = smem + pg.g + tid;                                     // this item's column of each staging array
+    T* hs = smem + pg.h + tid;
+    T* us = smem + pg.ub + tid;
+    T* zt = smem + pg.z + tid;
+    T* mine = p.scratch + (int64_t)blockIdx.x * p.n_params;
+    for (int64_t e = tid; e < p.n_params; e += nt) mine[e] = T(0);
+    __syncthreads();
+    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
+    const int64_t n_tiles = (a.n_paths + nt - 1) / nt;
+    const int64_t n_blocks = n_tiles * p.n_total;
+    const int64_t plane = a.n_paths * H;
+    const int64_t o_b1 = (int64_t)W * H, o_w2 = o_b1 + W, o_b2 = o_w2 + (int64_t)HC * W;
+    for (int64_t blk = blockIdx.x; blk < n_blocks; blk += gridDim.x) {
+        const int st = (int)(blk / n_tiles);
+        const int64_t path = (blk - (int64_t)st * n_tiles) * nt + tid;
+        const bool live = path < a.n_paths;
+        const int64_t lp = live ? path : a.n_paths - 1;
+        T zs[HM];
+        const T* zp = p.z_stages + st * plane + lp * H;
+        const T* kp = p.kappa + st * plane + lp * H;
+#pragma unroll
+        for (int h = 0; h < HM; ++h) {
+            zs[h] = (h < H) ? zp[h] : T(0);
+            if (h < H) {
+                kvs[(size_t)h * nt] = live ? kp[h] : T(0);         // a dead item adds zero
+                zt[(size_t)h * rs] = zs[h];
+            }
+        }
+        const T* crow = a.control + lp * a.n_rows * (cubic ? 4 * C : C) + (cubic ? C : 0);
+        {
+            TCDE_MLP_SLOPE(a.stage_index[st], a.stage_frac[st])
+        }
+        mlp_vjp<T, HM>(a, lay, smem, zs, dxs, kvs, nt,
+                       [&](int n0, const T* g) {
+#pragma unroll
+                           for (int j = 0; j < kMlpChunk; ++j)
+                               if (n0 + j < HC) gs[(size_t)(n0 + j) * rs] = g[j];
+                       },
+                       [&](int n0, int w, T pre, T sv) {
+                           const T m = pre > T(0) ? sv : T(0);
+                           if (n0 == 0) {
+                               hs[(size_t)w * rs] = pre > T(0) ? pre : T(0);
+                               us[(size_t)w * rs] = m;
+                           } else {
+                               us[(size_t)w * rs] += m;
+                           }
+                       });
+        __syncthreads();
+        // the block's items, in order, into the entries this thread owns
+        for (int64_t e = tid; e < p.n_params; e += nt) {
+            const T* x;
+            const T* y = nullptr;
+            if (e < o_b1) { x = smem + pg.ub + (size_t)(e / H) * rs; y = smem + pg.z + (size_t)(e % H) * rs; }
+            else if (e < o_w2) { x = smem + pg.ub + (size_t)(e - o_b1) * rs; }
+            else if (e < o_b2) { x = smem + pg.g + (size_t)((e - o_w2) / W) * rs; y = smem + pg.h + (size_t)((e - o_w2) % W) * rs; }
+            else { x = smem + pg.g + (size_t)(e - o_b2) * rs; }
+            T s = mine[e];
+            if (y) {
+                for (int i = 0; i < nt; ++i) s = fma(x[i], y[i], s);
+            } else {
+                for (int i = 0; i < nt; ++i) s += x[i];
+            }
+            mine[e] = s;
+        }
+        __syncthreads();                                           // the staging is rewritten next
+    }
+}
+
+// grads += scale * the per-CTA sums, added in CTA order
+template <typename T>
+__global__ void mlp_simt_param_reduce_kernel(const T* scratch, int n_parts, int64_t n_params, int64_t o_b1, int64_t o_w2,
+                                             int64_t o_b2, T scale, T* gw1, T* gb1, T* gw2, T* gb2) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_params) return;
+    T s = T(0);
+    for (int q = 0; q < n_parts; ++q) s += scratch[(int64_t)q * n_params + i];
+    s *= scale;
+    if (i < o_b1) { if (gw1) gw1[i] += s; }
+    else if (i < o_w2) { if (gb1) gb1[i - o_b1] += s; }
+    else if (i < o_b2) { if (gw2) gw2[i - o_w2] += s; }
+    else if (gb2) gb2[i - o_b2] += s;
 }
 
 // ---- tensor cores: 2xFP16 wgmma, H = 32, C = 8, W = 128 --------------------------------------------------------------
@@ -1278,6 +1639,12 @@ static int launch_mlp_tc(const UmmaArgs& u, const float* w2, const float* b2, cu
     return TCDE_OK;
 }
 
+// Where automatic selection runs the CUDA-core kernel: the shapes at which it measured faster than cdeint's stage loop on
+// an H100 (DESIGN 4.2): at most 8 hidden units (the HM = 8 instantiation) or one chunk of outputs (H C <= 32).  Elsewhere
+// it recomputes the first product per chunk of 32 outputs and runs at low occupancy, and was 1.3-4.5x (fp32) and up to
+// 13.6x (fp64) slower than the loop, so automatic selection refuses the shape and the caller keeps its stage loop.
+static bool mlp_simt_preferred(int64_t H, int64_t C) { return H <= 8 || H * C <= kMlpChunk; }
+
 // What the stage-dump solve, its backward and the parameter gradients are built for: fp32 at 32 / 8 / 128 under a solve
 // variant that runs the tensor-core kernel (0, 4, 5)
 static int check_mlp_backprop(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what) {
@@ -1290,6 +1657,104 @@ static int check_mlp_backprop(int64_t hidden, int64_t channels, int64_t width, i
     return TCDE_OK;
 }
 
+// Which kernels the stage-dump solve, its backward and the parameter gradients run: the CUDA-core ones (*simt = true) at
+// shapes where the CUDA-core forward runs by default (mlp_simt_preferred; fp32 or fp64, solve variant 0 or 1), the
+// tensor-core ones at fp32 32 / 8 / 128 under variant 0, 4 or 5 (check_mlp_backprop); TCDE_ERR_UNSUPPORTED otherwise.
+// Variant 1 serves only the shapes mlp_simt_preferred admits, so that elsewhere the caller keeps its own loop.  By default
+// the CUDA-core route also needs hidden <= 8 (the HM = 8 instantiations): at hidden 32, channels 1 a training step on it
+// measured slower per sequence than the torch-operator loop on an H100 (DESIGN 4.2), so variant 1 alone runs HM = 32.
+static int mlp_backprop_route(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what, bool* simt) {
+    TCDE_CHECK_ARG(channels >= 1 && hidden >= 1 && width >= 1, "bad sizes");
+    TCDE_CHECK_SUPPORTED(width < (1 << 20) && channels < (1 << 20) && hidden * channels < (1 << 20), "MLP too wide");
+    *simt = mlp_simt_preferred(hidden, channels);
+    if (!*simt) return check_mlp_backprop(hidden, channels, width, dtype, what);
+    const int variant = current_solve_variant();
+    TCDE_CHECK_SUPPORTED(hidden <= 8 || variant == 1, "%s: at hidden=%lld the CUDA-core route is slower than the stage "
+                         "loop; automatic selection does not run it (variant 1 forces it)", what, (long long)hidden);
+    TCDE_CHECK_SUPPORTED((dtype == TCDE_F32 || dtype == TCDE_F64) && variant <= 1 && width >= 1 && width < (1 << 20),
+                         "%s on the CUDA cores is built for fp32 / fp64 under solve variant 0 or 1 (got dtype=%d, "
+                         "width %lld, solve variant %d)", what, dtype, (long long)width, variant);
+    return TCDE_OK;
+}
+
+template <typename T>
+static MlpArgs<T> mlp_simt_args(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
+                                const void* w2, const void* b2, const void* z0, void* out, int64_t n_paths,
+                                int64_t channels, int64_t hidden, int64_t width, int method, int64_t n_steps,
+                                const void* step_dt, const int32_t* stage_index, const void* stage_frac, int64_t n_out,
+                                const int32_t* out_step, const int32_t* out_mode, const void* out_slope, double sign) {
+    const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
+    return MlpArgs<T>{(const T*)control, (const T*)w1, (const T*)b1, (const T*)w2, (const T*)b2, (const T*)z0, (T*)out,
+                      (const T*)step_dt, stage_index, (const T*)stage_frac, out_step, out_mode, (const T*)out_slope,
+                      n_paths, n_rows, (int)channels, (int)hidden, (int)width, control_kind, method, n_stages,
+                      (int)n_steps, (int)n_out, (T)sign};
+}
+
+template <typename T>
+static int mlp_simt_backward(const MlpArgs<T>& a, const MlpSimtBwd<T>& b, cudaStream_t s) {
+    if (a.H <= 8) return launch_mlp_simt_backward<T, 8>(a, b, s);
+    return launch_mlp_simt_backward<T, 32>(a, b, s);
+}
+
+// the persistent grid of mlp_simt_param_grad_kernel (independent of the dtype: the scratch size has no dtype)
+static int64_t mlp_simt_param_grid(int64_t n_paths, int64_t n_total, int ni) {
+    const int64_t blocks = ((n_paths + ni - 1) / ni) * n_total;
+    int64_t g = (int64_t)sm_count() * kMlpPgCtasPerSm;
+    if (g > blocks) g = blocks;
+    return g < 1 ? 1 : g;
+}
+
+// the items per block of the parameter gradients at this shape (sized for 8-byte elements, so that both dtypes use the
+// same grid and scratch), or 0 if no block fits in shared memory
+static int mlp_simt_param_items(int64_t H, int64_t C, int64_t W) {
+    MlpSimtLayout<double> lay;
+    MlpSimtPg pg;
+    return mlp_simt_pg_pick<double>((int)H, (int)C, (int)W, lay, pg) ? pg.ni : 0;
+}
+
+template <typename T, int HM>
+static int launch_mlp_simt_param_grads(const MlpArgs<T>& a, const MlpSimtPgArgs<T>& p, int64_t grid, int ni,
+                                       cudaStream_t s) {
+    auto kern = mlp_simt_param_grad_kernel<T, HM>;
+    MlpSimtLayout<T> lay;
+    MlpSimtPg pg;
+    // the same block width as the scratch was sized for; fp32 may then also stage the weights
+    lay = mlp_simt_layout<T>(a.H, a.C, a.W, true, ni);
+    pg = mlp_simt_pg_layout<T>(lay, a.H, a.C, a.W, ni);
+    if (pg.total > kMlpSimtMaxSmem) {
+        lay = mlp_simt_layout<T>(a.H, a.C, a.W, false, ni);
+        pg = mlp_simt_pg_layout<T>(lay, a.H, a.C, a.W, ni);
+    }
+    TCDE_CHECK_SUPPORTED(pg.total <= kMlpSimtMaxSmem, "MLP parameter gradients: the shape does not fit");
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pg.total));
+    kern<<<(unsigned)grid, ni, pg.total, s>>>(a, lay, pg, p);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    return TCDE_OK;
+}
+
+template <typename T>
+static int mlp_simt_param_grads(const MlpArgs<T>& a, const T* z_stages, const T* kappa, int64_t n_total, void* grad_w1,
+                                void* grad_b1, void* grad_w2, void* grad_b2, void* scratch, double scale,
+                                cudaStream_t s) {
+    const int ni = mlp_simt_param_items(a.H, a.C, a.W);
+    TCDE_CHECK_SUPPORTED(ni > 0, "MLP parameter gradients: hidden=%d channels=%d width=%d do not fit the CUDA-core "
+                         "kernel's shared memory", a.H, a.C, a.W);
+    const int64_t grid = mlp_simt_param_grid(a.n_paths, n_total, ni);
+    const int64_t n_params = mlp_simt_n_params(a.H, a.C, a.W);
+    const MlpSimtPgArgs<T> p{z_stages, kappa, (T*)scratch, n_params, (int)n_total};
+    const int rc = a.H <= 8 ? launch_mlp_simt_param_grads<T, 8>(a, p, grid, ni, s)
+                            : launch_mlp_simt_param_grads<T, 32>(a, p, grid, ni, s);
+    if (rc != TCDE_OK) return rc;
+    if (grad_w1 || grad_b1 || grad_w2 || grad_b2) {
+        const int64_t o_b1 = (int64_t)a.W * a.H, o_w2 = o_b1 + a.W, o_b2 = o_w2 + (int64_t)a.H * a.C * a.W;
+        mlp_simt_param_reduce_kernel<T><<<(unsigned)((n_params + 255) / 256), 256, 0, s>>>(
+            (const T*)scratch, (int)grid, n_params, o_b1, o_w2, o_b2, (T)scale, (T*)grad_w1, (T*)grad_b1, (T*)grad_w2,
+            (T*)grad_b2);
+        TCDE_CHECK_CUDA(cudaGetLastError());
+    }
+    return TCDE_OK;
+}
+
 static int64_t mlp_param_grid(int64_t n_paths, int64_t n_total) {
     const int64_t items = ((n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths) * n_total;
     int64_t g = sm_count();
@@ -1297,11 +1762,6 @@ static int64_t mlp_param_grid(int64_t n_paths, int64_t n_total) {
     return g < 1 ? 1 : g;
 }
 
-// Where automatic selection runs the CUDA-core kernel: the shapes at which it measured faster than cdeint's stage loop on
-// an H100 (DESIGN 4.2): at most 8 hidden units (the HM = 8 instantiation) or one chunk of outputs (H C <= 32).  Elsewhere
-// it recomputes the first product per chunk of 32 outputs and runs at low occupancy, and was 1.3-4.5x (fp32) and up to
-// 13.6x (fp64) slower than the loop, so automatic selection refuses the shape and the caller keeps its stage loop.
-static bool mlp_simt_preferred(int64_t H, int64_t C) { return H <= 8 || H * C <= kMlpChunk; }
 
 }  // namespace tcde
 
@@ -1382,8 +1842,23 @@ extern "C" int tcde_cdeint_fixed_mlp_stages(const void* control, int control_kin
                    control_kind);
     TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
     TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
-    const int rc = check_mlp_backprop(hidden, channels, width, dtype, "the MLP stage-dump solve");
+    bool simt;
+    const int rc = mlp_backprop_route(hidden, channels, width, dtype, "the MLP stage-dump solve", &simt);
     if (rc != TCDE_OK) return rc;
+    if (simt) {
+        TCDE_CHECK_SUPPORTED(n_paths * hidden * n_steps * 4 < (1ll << 62), "stage dump too large");
+        if (n_paths == 0) return TCDE_OK;
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        if (dtype == TCDE_F32)
+            return solve_mlp_simt(mlp_simt_args<float>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths,
+                                                       channels, hidden, width, method, n_steps, step_dt, stage_index,
+                                                       stage_frac, n_out, out_step, out_mode, out_slope, sign),
+                                  s, (float*)stage_dump);
+        return solve_mlp_simt(mlp_simt_args<double>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths,
+                                                    channels, hidden, width, method, n_steps, step_dt, stage_index,
+                                                    stage_frac, n_out, out_step, out_mode, out_slope, sign),
+                              s, (double*)stage_dump);
+    }
     TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z0) |
                            reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(stage_dump)) & 15) == 0,
                          "MLP stage-dump solve: control, z0, out and the dump must be 16-byte aligned");
@@ -1410,8 +1885,28 @@ extern "C" int tcde_cdeint_fixed_mlp_backward(
                    control_kind);
     TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
     TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
-    const int rc = check_mlp_backprop(hidden, channels, width, dtype, "the MLP Runge-Kutta backward");
+    bool simt;
+    const int rc = mlp_backprop_route(hidden, channels, width, dtype, "the MLP Runge-Kutta backward", &simt);
     if (rc != TCDE_OK) return rc;
+    if (simt) {
+        if (n_paths == 0) return TCDE_OK;
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        if (dtype == TCDE_F32)
+            return mlp_simt_backward(
+                mlp_simt_args<float>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, grad_z0, n_paths, channels,
+                                     hidden, width, method, n_steps, step_dt_rev, stage_index_rev, stage_frac_rev, n_out,
+                                     nullptr, nullptr, nullptr, sign),
+                MlpSimtBwd<float>{(const float*)stage_dump, (float*)kappa_dump, (const float*)grad_out, inj_range,
+                                  inj_out, (const float*)inj_weight},
+                s);
+        return mlp_simt_backward(
+            mlp_simt_args<double>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, grad_z0, n_paths, channels,
+                                  hidden, width, method, n_steps, step_dt_rev, stage_index_rev, stage_frac_rev, n_out,
+                                  nullptr, nullptr, nullptr, sign),
+            MlpSimtBwd<double>{(const double*)stage_dump, (double*)kappa_dump, (const double*)grad_out, inj_range,
+                               inj_out, (const double*)inj_weight},
+            s);
+    }
     TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(stage_dump) |
                            reinterpret_cast<uintptr_t>(grad_out) | reinterpret_cast<uintptr_t>(grad_z0) |
                            reinterpret_cast<uintptr_t>(kappa_dump)) & 15) == 0,
@@ -1435,7 +1930,15 @@ extern "C" int tcde_cdeint_fixed_mlp_backward(
 
 extern "C" int64_t tcde_mlp_field_param_grads_scratch_bytes(int64_t n_paths, int64_t n_stages_total, int64_t channels,
                                                            int64_t hidden, int64_t width) {
-    if (n_paths < 0 || n_stages_total < 1 || !mlp_tc_shape(hidden, channels, width)) return -1;
+    if (n_paths < 0 || n_stages_total < 1 || hidden < 1 || channels < 1 || width < 1) return -1;
+    if (width >= (1 << 20) || channels >= (1 << 20) || hidden * channels >= (1 << 20)) return -1;
+    if (mlp_simt_preferred(hidden, channels)) {               // the CUDA-core kernel, sized for 8-byte elements
+        const int ni = mlp_simt_param_items(hidden, channels, width);
+        if (ni == 0) return -1;
+        return mlp_simt_param_grid(n_paths, n_stages_total, ni) * mlp_simt_n_params(hidden, channels, width) *
+               (int64_t)sizeof(double);
+    }
+    if (!mlp_tc_shape(hidden, channels, width)) return -1;
     return mlp_param_grid(n_paths, n_stages_total) * tc::mlp::kPgParams * (int64_t)sizeof(float);
 }
 
@@ -1450,8 +1953,27 @@ extern "C" int tcde_mlp_field_param_grads(const void* control, int control_kind,
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_stages_total >= 1 && n_stages_total < (1ll << 31), "bad sizes");
     TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
                    control_kind);
-    const int rc = check_mlp_backprop(hidden, channels, width, dtype, "the MLP parameter gradients");
+    bool simt;
+    const int rc = mlp_backprop_route(hidden, channels, width, dtype, "the MLP parameter gradients", &simt);
     if (rc != TCDE_OK) return rc;
+    if (simt) {
+        if (n_paths == 0) return TCDE_OK;
+        cudaStream_t s = static_cast<cudaStream_t>(stream);
+        // the forward's stage tables; the solve's method and steps do not matter here
+        if (dtype == TCDE_F32)
+            return mlp_simt_param_grads(
+                mlp_simt_args<float>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths, channels,
+                                     hidden, width, TCDE_EULER, 1, nullptr, stage_index, stage_frac, 1, nullptr, nullptr,
+                                     nullptr, sign),
+                (const float*)z_stages, (const float*)kappa_stages, n_stages_total, grad_w1, grad_b1, grad_w2, grad_b2,
+                scratch, scale, s);
+        return mlp_simt_param_grads(
+            mlp_simt_args<double>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths, channels,
+                                  hidden, width, TCDE_EULER, 1, nullptr, stage_index, stage_frac, 1, nullptr, nullptr,
+                                  nullptr, sign),
+            (const double*)z_stages, (const double*)kappa_stages, n_stages_total, grad_w1, grad_b1, grad_w2, grad_b2,
+            scratch, scale, s);
+    }
     TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z_stages) |
                            reinterpret_cast<uintptr_t>(kappa_stages) | reinterpret_cast<uintptr_t>(scratch)) & 15) == 0,
                          "MLP parameter gradients: control, the dumps and scratch must be 16-byte aligned");

@@ -71,31 +71,30 @@ __device__ __forceinline__ bool rk_combine(const UmmaArgs& a, int sub, float dt,
 // stage's kappa (the cotangent of its slope) ends up in kap.  rk4 (kappa_4 = dt/8 ybar', rk_backward_first):
 //   kappa_3 = dt (3/8 ybar' + u_4),  kappa_2 = dt (3/8 ybar' - u_4 + u_3),  kappa_1 = dt (1/8 ybar' + u_4 - u_3/3 + u_2/3);
 // midpoint: kappa_1 = dt/2 u_2.  Returns true when the stage closed the step: yb then holds ybar' + sum_s u_s, the
-// cotangent of the step's start state.
-template <int NV>
-__device__ __forceinline__ bool rk_backward_combine(const UmmaArgs& a, int sub, float dt, float* yb, float* su, float* run,
-                                                    const float* kv, float* kap) {
-    using E = exact<float>;
+// cotangent of the step's start state.  T: float (the tensor-core kernels) or double; A: any argument struct with `method`.
+template <int NV, typename A, typename T>
+__device__ __forceinline__ bool rk_backward_combine(const A& a, int sub, T dt, T* yb, T* su, T* run, const T* kv, T* kap) {
+    using E = exact<T>;
     if (a.method == TCDE_RK4_38) {
-        const float third = (float)(1.0 / 3.0);
+        const T third = (T)(1.0 / 3.0);
         if (sub == 0) {
 #pragma unroll
             for (int h = 0; h < NV; ++h) {
                 su[h] = kv[h];
                 run[h] = kv[h];
-                kap[h] = E::mul(dt, E::add(E::mul(0.375f, yb[h]), kv[h]));
+                kap[h] = E::mul(dt, E::add(E::mul(T(0.375), yb[h]), kv[h]));
             }
         } else if (sub == 1) {
 #pragma unroll
             for (int h = 0; h < NV; ++h) {
-                kap[h] = E::mul(dt, E::add(E::sub(E::mul(0.375f, yb[h]), run[h]), kv[h]));
+                kap[h] = E::mul(dt, E::add(E::sub(E::mul(T(0.375), yb[h]), run[h]), kv[h]));
                 run[h] = E::sub(run[h], E::mul(kv[h], third));
                 su[h] = E::add(su[h], kv[h]);
             }
         } else if (sub == 2) {
 #pragma unroll
             for (int h = 0; h < NV; ++h) {
-                kap[h] = E::mul(dt, E::add(E::add(E::mul(0.125f, yb[h]), run[h]), E::mul(kv[h], third)));
+                kap[h] = E::mul(dt, E::add(E::add(E::mul(T(0.125), yb[h]), run[h]), E::mul(kv[h], third)));
                 su[h] = E::add(su[h], kv[h]);
             }
         } else {
@@ -107,7 +106,7 @@ __device__ __forceinline__ bool rk_backward_combine(const UmmaArgs& a, int sub, 
     }
     if (a.method == TCDE_MIDPOINT) {
         if (sub == 0) {
-            const float half = E::mul(0.5f, dt);
+            const T half = E::mul(T(0.5), dt);
 #pragma unroll
             for (int h = 0; h < NV; ++h) {
                 su[h] = kv[h];
@@ -125,10 +124,10 @@ __device__ __forceinline__ bool rk_backward_combine(const UmmaArgs& a, int sub, 
 }
 
 // kappa of a step's last stage from the cotangent ybar' of its end state: dt/8 ybar' (rk4), dt ybar' (midpoint, euler)
-template <int NV>
-__device__ __forceinline__ void rk_backward_first(const UmmaArgs& a, float dt, const float* yb, float* kap) {
-    using E = exact<float>;
-    const float c = (a.method == TCDE_RK4_38) ? E::mul(0.125f, dt) : dt;
+template <int NV, typename A, typename T>
+__device__ __forceinline__ void rk_backward_first(const A& a, T dt, const T* yb, T* kap) {
+    using E = exact<T>;
+    const T c = (a.method == TCDE_RK4_38) ? E::mul(T(0.125), dt) : dt;
 #pragma unroll
     for (int h = 0; h < NV; ++h) kap[h] = E::mul(c, yb[h]);
 }

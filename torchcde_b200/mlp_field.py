@@ -114,9 +114,11 @@ class MlpFieldKernels:
 
 
 class MlpBackprop:
-    """``cdeint(..., adjoint=False)`` of a fixed-step solve of the MLP field at fp32, hidden 32, channels 8, width 128 with
-    gradients for any of z0, W1, b1, W2, b2: the exact gradient of the discrete solve in three launches, as
-    ``linear_field.FixedBackprop`` does for the linear field.  The forward is the stage-dump solve
+    """``cdeint(..., adjoint=False)`` of a fixed-step solve of the MLP field with gradients for any of z0, W1, b1, W2, b2:
+    the exact gradient of the discrete solve in three launches, as
+    ``linear_field.FixedBackprop`` does for the linear field, on the tensor cores at fp32 32 / 8 / 128 and on the CUDA
+    cores (fp32, fp64) where the CUDA-core forward runs by default; the C dispatch owns that policy.  The forward is the
+    stage-dump solve
     (``tcde_cdeint_fixed_mlp_stages``: the outputs of the same call without gradients, bit for bit); the backward is ONE
     launch of ``tcde_cdeint_fixed_mlp_backward`` (the transposed Runge-Kutta recurrence over every step at the dumped stage
     inputs) and, with parameter gradients, ONE launch of ``tcde_mlp_field_param_grads`` over the two dumps.  ``loop(z0)``:
@@ -136,7 +138,7 @@ class MlpBackprop:
         """Whether the stage dump, and with parameter gradients the kappa dump and the parameter-gradient scratch, fit in
         0.7 of the free device memory."""
         k = self.kernels
-        need = self.n_total * n_paths * k.hidden * 4
+        need = self.n_total * n_paths * k.hidden * torch.empty(0, dtype=k.dtype).element_size()
         if want_params:
             scratch = self.scratch_bytes(n_paths)
             if scratch < 0:
@@ -159,7 +161,7 @@ class MlpBackprop:
                           zf.size(0), k.channels, k.hidden, k.width, _lib.METHODS[sched.method], sched.n_steps,
                           _lib.ptr(v["step_dt"]), _lib.ptr(v["stage_index"]), _lib.ptr(v["stage_frac"]), sched.n_out,
                           _lib.ptr(v["out_step"]), _lib.ptr(v["out_mode"]), _lib.ptr(v["out_slope"]), float(sched.sign),
-                          _lib.F32, _lib.stream_of(zf))
+                          _lib.dtype_code(k.dtype), _lib.stream_of(zf))
         return out.view(*z0.shape[:-1], sched.n_out, k.hidden), dump
 
     def backward(self, g, dump, want):
@@ -184,14 +186,15 @@ class MlpBackprop:
                           _lib.ptr(kappa), n_paths, k.channels, hidden, k.width, _lib.METHODS[sched.method], ns,
                           _lib.ptr(floats[:ns]), _lib.ptr(ints[:n_total]), _lib.ptr(floats[ns:ns + n_total]), sched.n_out,
                           _lib.ptr(ints[n_total:n_total + nr]), _lib.ptr(ints[n_total + nr:]),
-                          _lib.ptr(floats[ns + n_total:]), float(sched.sign), _lib.F32, _lib.stream_of(gf))
+                          _lib.ptr(floats[ns + n_total:]), float(sched.sign), _lib.dtype_code(k.dtype),
+                          _lib.stream_of(gf))
                 if kappa is not None:
                     scratch = torch.empty(max(self.scratch_bytes(n_paths) // 4, 4), dtype=torch.float32, device=dev)
                     _lib.call("tcde_mlp_field_param_grads", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1),
                               _lib.ptr(k.b1), _lib.ptr(k.w2), _lib.ptr(k.b2), _lib.ptr(dump), _lib.ptr(kappa),
                               _lib.ptr(self.views["stage_index"]), _lib.ptr(self.views["stage_frac"]), n_total,
                               *(_lib.ptr(x) for x in grads), _lib.ptr(scratch), n_paths, k.channels, hidden, k.width,
-                              float(sched.sign), 1.0, _lib.F32, _lib.stream_of(gf))
+                              float(sched.sign), 1.0, _lib.dtype_code(k.dtype), _lib.stream_of(gf))
         return gz.view(g.shape[:-2] + (hidden,)), grads
 
 
@@ -220,13 +223,13 @@ class _MlpBackpropFn(torch.autograd.Function):
 def mlp_backprop(X, params, z0, t, method, step_size, loop):
     """``cdeint(..., adjoint=False)``'s outputs ``(..., n_out, H)`` on the three-launch route of ``MlpBackprop``, or None
     when the route does not serve the problem (the caller runs the torch-operator solve).  ``params``: (W1, b1, W2, b2)
-    of the recognised field, a bias may be None."""
-    w1 = params[0]
-    if (z0.dtype != torch.float32 or z0.size(-1) != 32 or w1.size(0) != 128
-            or any(p is not None and (p.dtype != torch.float32 or p.device != z0.device) for p in params)):
+    of the recognised field, a bias may be None.  Which shapes, dtypes and solve variants are served is the C dispatch's
+    call: a refusal (``TCDE_ERR_UNSUPPORTED``, as a -1 scratch size or NotImplementedError) keeps the loop."""
+    if (z0.dtype not in (torch.float32, torch.float64) or not z0.is_cuda
+            or any(p is not None and (p.dtype != z0.dtype or p.device != z0.device) for p in params)):
         return None
     k = MlpFieldKernels(X, params, z0)
-    if k.channels != 8 or k.control.dtype != torch.float32 or k.control.device != z0.device:
+    if k.control.dtype != z0.dtype or k.control.device != z0.device:
         return None
     route = MlpBackprop(k, t, method, step_size, loop)
     present = [p for p in params if p is not None]
@@ -237,5 +240,5 @@ def mlp_backprop(X, params, z0, t, method, step_size, loop):
     try:
         return _MlpBackpropFn.apply(route, z0, *leaves)
     except NotImplementedError:
-        # the stage-dump solve refuses the problem (solve variant, misaligned rows): nothing ran
+        # the stage-dump solve refuses the problem (shape, solve variant, misaligned rows): nothing ran
         return None

@@ -566,7 +566,7 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
             if ys is not None:
                 return ys
         # the examples' MLP field: the three-launch route of mlp_field.MlpBackprop serves gradients for z0 and the two
-        # layers' weights and biases (fp32, hidden 32, channels 8, width 128); a gradient for t or the control keeps the loop
+        # layers' weights and biases where its kernels are built for the shape; a gradient for t or the control keeps the loop
         if (field_params is None and sig is not None and not is_prod and times and not t.requires_grad
                 and not any(b.requires_grad for b in X.buffers())):
             mlp_params = mlp_field_of(func, z0, sig[2], times)
