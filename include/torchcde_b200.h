@@ -292,6 +292,37 @@ TCDE_API int tcde_mlp_field_param_grads(const void* control, int control_kind, i
                                void* scratch, int64_t n_paths, int64_t channels, int64_t hidden, int64_t width,
                                double sign, double scale, int dtype, void* stream);
 
+/* One evaluation of the MLP vector field of tcde_cdeint_fixed_mlp at one time, for an adaptive driver (the counterpart of
+ * tcde_vector_field_linear):
+ *   out[p][h] = sum_c tanh(w2 relu(w1 z[p] + b1) + b2)[h*C+c] * dXdt[p][c]
+ * with dXdt from the control at (index, frac), in the CUDA-core solve's arithmetic.  Built where the CUDA-core kernels
+ * of tcde_cdeint_fixed_mlp_stages run (fp32 or fp64; hidden <= 8, and under solve variant 1 also hidden * channels <= 32;
+ * widths whose parameter-gradient staging fits shared memory).  By default served only at fp32 with hidden * channels
+ * <= 32 and width <= 128, where an adjoint=True training step on them measured faster than autograd per stage; solve
+ * variant 1 forces the rest.  TCDE_ERR_UNSUPPORTED elsewhere, the tensor-core shape fp32 32 / 8 / 128 included, so that
+ * the caller keeps its torch-operator field. */
+TCDE_API int tcde_vector_field_mlp(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
+                          const void* w2, const void* b2, const void* z, void* out, int64_t n_paths, int64_t channels,
+                          int64_t hidden, int64_t width, int32_t index, double frac, int dtype, void* stream);
+
+/* The same evaluation together with its vector-Jacobian products -- one stage of the adjoint backward solve, with the
+ * scale convention of tcde_vector_field_linear_vjp:
+ *   f_out      = f_scale * f                        vjp_z_out = vjp_scale * a^T df/dz
+ *   grad_w1 += grad_scale * sum_p a^T df/dw1, and likewise grad_b1, grad_w2, grad_b2 (each may be NULL)
+ * At most three launches: the field and a^T df/dz in one pass (f_out equals tcde_vector_field_mlp's out bit for bit at
+ * f_scale = 1), then, with a parameter gradient, the parameter-gradient kernel of tcde_mlp_field_param_grads over this
+ * one stage and its fixed-order reduction (two calls give the same bits).  scratch: 16-byte aligned device buffer of
+ * tcde_vector_field_mlp_vjp_scratch_bytes(...) bytes (-1: the shape is not served at fp32; the query has no dtype, the
+ * size fits both, and a call with n_paths = 0 gives the verdict for a dtype).  Same support as tcde_vector_field_mlp. */
+TCDE_API int64_t tcde_vector_field_mlp_vjp_scratch_bytes(int64_t n_paths, int64_t channels, int64_t hidden,
+                                                int64_t width);
+TCDE_API int tcde_vector_field_mlp_vjp(const void* control, int control_kind, int64_t n_rows, const void* w1,
+                              const void* b1, const void* w2, const void* b2, const void* z, const void* a, void* f_out,
+                              void* vjp_z_out, void* grad_w1, void* grad_b1, void* grad_w2, void* grad_b2, void* scratch,
+                              int64_t n_paths, int64_t channels, int64_t hidden, int64_t width, int32_t index,
+                              double frac, double f_scale, double vjp_scale, double grad_scale, int dtype,
+                              void* stream);
+
 /* torchsde's reversible Heun method with zero diffusion (cdeint(..., backend="torchsde", method="reversible_heun")) for
  * the same linear field, in ONE launch:
  *   z_{n+1} = 2 y_n - z_n + f_n dt_n,  f_{n+1} = f(t_{n+1}, z_{n+1}),  y_{n+1} = y_n + (f_n + f_{n+1}) (0.5 dt_n)

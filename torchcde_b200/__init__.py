@@ -8,8 +8,11 @@ Drop-in names (reference torchcde/__init__.py:1-9): ``cdeint``, ``CubicSpline``,
 there is no CPU path and no PyTorch-eager fallback.
 
 ``logsig_windows`` / ``logsignature_windows`` (the log-ODE transform) run on a kernel of this package instead of the optional
-``signatory`` dependency.  ``cdeint(..., backend="torchsde", method="reversible_heun")`` is torchsde's reversible Heun
-method with an exact, checkpointed reversible backward (``reversible.py``); the other torchsde methods are not built.
+``signatory`` dependency.  ``cdeint``'s default call on the examples' MLP field (``Linear -> ReLU -> Linear -> tanh``;
+dopri5 with ``adjoint=True``) evaluates the field in one launch and each adjoint stage in one call
+(fp32, hidden * channels <= 32, width <= 128).
+``cdeint(..., backend="torchsde", method="reversible_heun")`` is torchsde's reversible Heun method with an exact,
+checkpointed reversible backward (``reversible.py``); the other torchsde methods are not built.
 Not provided (outside the hot path, SURVEY.md section 2): ``TupleControl``.
 """
 from . import misc

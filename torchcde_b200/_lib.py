@@ -66,6 +66,11 @@ SIGNATURES = {
     "tcde_mlp_field_param_grads_scratch_bytes": ([_i64, _i64, _i64, _i64, _i64], _i64),
     "tcde_mlp_field_param_grads": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _i64, _i64,
                                     _i64, _i64, _dbl, _dbl, _int, _p], _int),
+    "tcde_vector_field_mlp": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _i32, _dbl, _int, _p],
+                              _int),
+    "tcde_vector_field_mlp_vjp_scratch_bytes": ([_i64, _i64, _i64, _i64], _i64),
+    "tcde_vector_field_mlp_vjp": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64,
+                                   _i64, _i32, _dbl, _dbl, _dbl, _dbl, _int, _p], _int),
     "tcde_dopri5_linear_grid": ([_i64], _int),
     "tcde_dopri5_linear_paired_attempts": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _dbl,
                                             _p, _p, _p, _p, _p, _i64, _i64, _i64, _int, _p], _int),

@@ -21,7 +21,9 @@ The backward pass of ``adjoint=True`` for the flagship linear field (fp32, hidde
 through autograd: a fixed-step backward solve is three launches per segment (``_fused_fixed_backward`` ->
 ``linear_field.AdjointStage.segment``), an adaptive one gets the field and its vector-Jacobian products from one launch
 per evaluation (``tcde_vector_field_linear_vjp``); the stage combinations and the error ratio of a dopri5
-attempt are single launches too (``tcde_linear_combination`` / ``tcde_error_ratio_sumsq``).
+attempt are single launches too (``tcde_linear_combination`` / ``tcde_error_ratio_sumsq``).  The examples' MLP field
+gets the same per-evaluation layer at its CUDA-core shapes (``mlp_field.MlpAdjointStage``, one call of
+``tcde_vector_field_mlp_vjp`` per stage, for dopri5 and the fixed-step methods alike).
 """
 import ctypes
 import math
@@ -485,8 +487,7 @@ def _fused_fixed_backward(stage, times, ys, grad_ys, method, step_size):
     gradients -- whose slopes do not depend on themselves -- are accumulated in place by the kernel with the
     stage's weight, instead of being carried through ``torch.cat`` as 8,448 extra state components."""
     grads = stage.new_grads()
-    gw = next((g for g, r in zip(grads, stage.roles) if r == "w"), None)
-    gb = next((g for g, r in zip(grads, stage.roles) if r == "b"), None)
+    unweighted = [None] * len(grads)
     shape = ys[0].shape
     U = torch.empty((2,) + tuple(shape), dtype=ys.dtype, device=ys.device)
     V = torch.empty_like(U)
@@ -495,14 +496,12 @@ def _fused_fixed_backward(stage, times, ys, grad_ys, method, step_size):
 
     def field(idx, frac, state, out, weight):
         # d(z, a)/ds = (-f, +a^T df/dz), d(grad)/ds = +a^T df/dp  (s = -t), the latter times the stage weight
-        if weight == 0.0:
-            stage.launch(idx, frac, state[0], state[1], out[0], out[1], None, None, -1.0, 1.0, 0.0)
-        else:
-            stage.launch(idx, frac, state[0], state[1], out[0], out[1], gw, gb, -1.0, 1.0, weight)
+        stage.launch(idx, frac, state[0], state[1], out[0], out[1], *(unweighted if weight == 0.0 else grads),
+                     f_scale=-1.0, vjp_scale=1.0, grad_scale=weight)
 
     for i in range(len(times) - 1, 0, -1):
         # whole segment in three launches (two tensor-core solves that keep their stage inputs + one contraction)
-        a_lo = stage.segment(times[i], times[i - 1], ys[i], a_y, method, step_size, gw, gb)
+        a_lo = stage.segment(times[i], times[i - 1], ys[i], a_y, method, step_size, *grads)
         if a_lo is not None:
             a_y = a_lo + grad_ys[i - 1]
             continue

@@ -7,6 +7,8 @@
 //   * cdeint_mlp_simt_kernel<T, HM, DUMP> (fp32 / fp64, H <= HM, any C and W): one thread per path on the CUDA cores; the
 //     fp64 instantiation is the reference solve of the parity tests.
 // Each has a stage-dump variant, a Runge-Kutta backward and a parameter-gradient kernel for cdeint(..., adjoint=False).
+#include <type_traits>
+
 #include "wg_common.cuh"
 
 namespace tcde {
@@ -54,8 +56,9 @@ template <typename T> struct MlpSimtLayout {
     bool staged;
 };
 
+// extra: more values per thread after the slopes (tcde_vector_field_mlp_vjp keeps f there, H of them)
 template <typename T> static MlpSimtLayout<T> mlp_simt_layout(int H, int C, int W, bool stage,
-                                                                int nt = kMlpSimtThreads) {
+                                                                int nt = kMlpSimtThreads, int extra = 0) {
     MlpSimtLayout<T> l;
     l.Hp = (H + 3) / 4 * 4;
     l.Nq = (H * C + kMlpChunk - 1) / kMlpChunk * kMlpChunk;
@@ -70,7 +73,7 @@ template <typename T> static MlpSimtLayout<T> mlp_simt_layout(int H, int C, int 
     } else {
         l.w1 = l.w2t = l.b1 = l.b2 = 0;
     }
-    l.cols = off; off += (size_t)(C + H) * nt;                    // per thread: dX/dt [C], slopes [H]
+    l.cols = off; off += (size_t)(C + H + extra) * nt;            // per thread: dX/dt [C], slopes [H], extra
     l.total = off * sizeof(T);
     return l;
 }
@@ -266,9 +269,9 @@ __global__ void __launch_bounds__(kMlpSimtThreads) cdeint_mlp_simt_kernel(const 
 
 // The layout of a CUDA-core kernel: the weights staged when everything fits in kMax bytes, else read from global memory
 constexpr size_t kMlpSimtMaxSmem = 200 * 1024;
-template <typename T> static int mlp_simt_pick_layout(int H, int C, int W, MlpSimtLayout<T>& lay) {
-    lay = mlp_simt_layout<T>(H, C, W, true);
-    if (lay.total > kMlpSimtMaxSmem) lay = mlp_simt_layout<T>(H, C, W, false);
+template <typename T> static int mlp_simt_pick_layout(int H, int C, int W, MlpSimtLayout<T>& lay, int extra = 0) {
+    lay = mlp_simt_layout<T>(H, C, W, true, kMlpSimtThreads, extra);
+    if (lay.total > kMlpSimtMaxSmem) lay = mlp_simt_layout<T>(H, C, W, false, kMlpSimtThreads, extra);
     TCDE_CHECK_SUPPORTED(lay.total <= kMlpSimtMaxSmem, "MLP solve: hidden=%d channels=%d do not fit the CUDA-core "
                          "kernel's shared memory", H, C);
     return TCDE_OK;
@@ -306,10 +309,16 @@ static int solve_mlp_simt(const MlpArgs<T>& a, cudaStream_t stream, T* stage_dum
 // width W is kept per thread.  dX/dt and kappa sit in the thread's column of shared memory, as the forward's dX/dt and
 // slopes do (their index runs with the output n = h C + c).
 
-// For every chunk: chunk(n0, g) with g [NT] (zero past H C), then unit(w, pre_w, W2[n0 .., w] . g) for every hidden unit
-template <typename T, int HM, typename Chunk, typename Unit>
-__device__ __forceinline__ void mlp_vjp(const MlpArgs<T>& a, const MlpSimtLayout<T>& lay, const T* smem, const T* zin,
-                                        const T* dxs, const T* kvs, int nt, Chunk chunk, Unit unit) {
+struct MlpIgnore {
+    template <typename... Args> __device__ __forceinline__ void operator()(Args...) const {}
+};
+
+// For every chunk: chunk(n0, g) with g [NT] (zero past H C), then unit(w, pre_w, W2[n0 .., w] . g) for every hidden unit;
+// tanh_out(h, c, y) sees every output's tanh value as g is formed (tcde_vector_field_mlp_vjp forms f from them)
+template <typename T, int HM, typename Chunk, typename Unit, typename Tanh = MlpIgnore, typename Z = const T*>
+__device__ __forceinline__ void mlp_vjp(const MlpArgs<T>& a, const MlpSimtLayout<T>& lay, const T* smem, Z zin,
+                                        const T* dxs, const T* kvs, int nt, Chunk chunk, Unit unit,
+                                        Tanh tanh_out = Tanh()) {
     using E = exact<T>;
     using P4 = Pack<T, 4>;
     const int H = a.H, C = a.C, W = a.W, HC = a.H * a.C, Hp = lay.Hp, Nq = lay.Nq;
@@ -321,6 +330,7 @@ __device__ __forceinline__ void mlp_vjp(const MlpArgs<T>& a, const MlpSimtLayout
         for (int j = 0; j < kMlpChunk; ++j) {
             if (n0 + j < HC) {
                 const T y = tanh_of(gc[j]);
+                tanh_out(h, c, y);
                 gc[j] = E::mul(E::sub(T(1), E::mul(y, y)), E::mul(kvs[(size_t)h * nt], dxs[(size_t)c * nt]));
                 if (++c == C) { c = 0; ++h; }
             } else {
@@ -623,6 +633,143 @@ __global__ void mlp_simt_param_reduce_kernel(const T* scratch, int n_parts, int6
     else if (i < o_w2) { if (gb1) gb1[i - o_b1] += s; }
     else if (i < o_b2) { if (gw2) gw2[i - o_w2] += s; }
     else if (gb2) gb2[i - o_b2] += s;
+}
+
+// ---- one evaluation of the field, and one adjoint stage, on the CUDA cores (tcde_vector_field_mlp[_vjp]) --------------
+//
+// One thread per path at one time (index, frac), with the forward's code: f[h] = sum_c tanh(v[(h, c)]) dX_c in increasing
+// c, accumulated in the thread's column of shared memory.  With VJP the same pass through mlp_vjp (kappa = the cotangent
+// a, in the slope column) also gives f from its tanh values, and a^T df/dz = W1^T (mask . W2^T g) as the Runge-Kutta
+// backward forms u_s.  The parameter part is mlp_simt_param_grad_kernel over this one stage, which reads the stage's
+// (index, frac) from the device: block 0's thread 0 stores them into q_index / q_frac.
+template <typename T> struct MlpFieldEval {
+    const T* adj;                 // the cotangent a [n_paths][H] (VJP)
+    T* vjp_out;                   // vjp_scale a^T df/dz [n_paths][H] (VJP)
+    int32_t* q_index;             // where the stage's interval index and fraction go (VJP, may be null)
+    T* q_frac;
+    int32_t index;
+    T frac, f_scale, vjp_scale;
+};
+
+// The per-thread values after the slopes: f [H], and with VJP in fp64 at HM = 32 also the a^T df/dz accumulator [H] and z
+// zero padded to Hp (held in registers there beside the chunk, they spill; the first product reads z up to Hp)
+template <typename T, int HM, bool VJP> __host__ __device__ constexpr bool mlp_field_kv_shared() {
+    return VJP && sizeof(T) == 8 && HM == 32;
+}
+static int mlp_field_extra_shared(int H) { return 2 * H + (H + 3) / 4 * 4; }
+template <typename T, int HM, bool VJP> static int mlp_field_extra(int H) {
+    return !VJP ? 0 : mlp_field_kv_shared<T, HM, VJP>() ? mlp_field_extra_shared(H) : H;
+}
+
+// a.z0: z [n_paths][H]; a.out: f_scale f [n_paths][H]; a.sign = 1
+template <typename T, int HM, bool VJP>
+__global__ void __launch_bounds__(kMlpSimtThreads) mlp_field_kernel(const MlpArgs<T> a, const MlpSimtLayout<T> lay,
+                                                                    const MlpFieldEval<T> e) {
+    constexpr bool kKvShared = mlp_field_kv_shared<T, HM, VJP>();
+    using E = exact<T>;
+    using P4 = Pack<T, 4>;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    T* smem = reinterpret_cast<T*>(smem_raw);
+    const int tid = threadIdx.x, nt = blockDim.x;
+    const int H = a.H, C = a.C, W = a.W, HC = a.H * a.C, Hp = lay.Hp, Nq = lay.Nq;
+    if (lay.staged) {
+        TCDE_MLP_STAGE_WEIGHTS()
+        __syncthreads();
+    }
+    T* dxs = smem + lay.cols + tid;
+    T* kvs = dxs + (size_t)C * nt;                                 // kvs[h * nt]: a of hidden unit h (VJP)
+    T* fs = kvs + (size_t)(VJP ? H : 0) * nt;                      // fs[h * nt]: f of hidden unit h
+    T* kvx = fs + (size_t)H * nt;                                  // kvx[k * nt]: a^T df/dz_k (kKvShared)
+    T* zx = kvx + (size_t)H * nt;                                  // zx[k * nt]: z_k, zero for k >= H (kKvShared)
+    const int64_t path = (int64_t)blockIdx.x * nt + tid;
+    const bool live = path < a.n_paths;
+    const int64_t lp = live ? path : a.n_paths - 1;
+    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
+    const T* crow = a.control + lp * a.n_rows * (cubic ? 4 * C : C) + (cubic ? C : 0);
+    if (VJP && e.q_index && blockIdx.x == 0 && tid == 0) {
+        *e.q_index = e.index;
+        *e.q_frac = e.frac;
+    }
+    T zin[HM];
+#pragma unroll
+    for (int h = 0; h < HM; ++h) {
+        zin[h] = (h < H) ? a.z0[lp * H + h] : T(0);
+        if (h < H) {
+            fs[(size_t)h * nt] = T(0);
+            if (VJP) kvs[(size_t)h * nt] = e.adj[lp * H + h];
+        }
+    }
+    {
+        TCDE_MLP_SLOPE(e.index, e.frac)
+    }
+    if (!VJP) {
+        for (int n0 = 0; n0 < HC; n0 += kMlpChunk) {
+            T acc[kMlpChunk];
+            TCDE_MLP_CHUNK(acc, n0)
+            int h = n0 / C, c = n0 - h * C;
+#pragma unroll
+            for (int j = 0; j < kMlpChunk; ++j) {
+                if (n0 + j < HC) {
+                    fs[(size_t)h * nt] = fma(tanh_of(acc[j]), dxs[(size_t)c * nt], fs[(size_t)h * nt]);
+                    if (++c == C) { c = 0; ++h; }
+                }
+            }
+        }
+    } else {
+        T kv[HM];
+#pragma unroll
+        for (int h = 0; h < HM; ++h) {
+            kv[h] = T(0);
+            if (kKvShared && h < H) kvx[(size_t)h * nt] = T(0);
+            if (kKvShared && h < Hp) zx[(size_t)h * nt] = zin[h];           // zin is zero past H
+        }
+        struct Column {                                            // z read from the thread's column (kKvShared)
+            const T* p;
+            int nt;
+            __device__ __forceinline__ T operator[](int k) const { return p[(size_t)k * nt]; }
+        };
+        using Z = std::conditional_t<kKvShared, Column, const T*>;
+        Z zarg;
+        if constexpr (kKvShared) zarg = Column{zx, nt};
+        else zarg = zin;
+        mlp_vjp<T, HM>(
+            a, lay, smem, zarg, dxs, kvs, nt, [](int, const T*) {},
+            [&](int, int w, T pre, T sv) {
+                if (!(pre > T(0))) return;
+                auto add = [&](int k, T wv) {
+                    if constexpr (kKvShared) kvx[(size_t)k * nt] = fma(wv, sv, kvx[(size_t)k * nt]);
+                    else kv[k] = fma(wv, sv, kv[k]);
+                };
+                if (lay.staged) {
+                    const T* wr = smem + lay.w1 + (size_t)w * lay.Hp;
+#pragma unroll
+                    for (int k4 = 0; k4 < HM / 4; ++k4) {
+                        if (4 * k4 < lay.Hp) {
+                            const P4 w4 = *reinterpret_cast<const P4*>(wr + 4 * k4);
+#pragma unroll
+                            for (int i = 0; i < 4; ++i)
+                                if (!kKvShared || 4 * k4 + i < H) add(4 * k4 + i, w4.v[i]);
+                        }
+                    }
+                } else {
+                    const T* wr = a.w1 + (size_t)w * H;
+#pragma unroll
+                    for (int k = 0; k < HM; ++k)
+                        if (k < H) add(k, __ldg(wr + k));
+                }
+            },
+            [&](int h, int c, T y) { fs[(size_t)h * nt] = fma(y, dxs[(size_t)c * nt], fs[(size_t)h * nt]); });
+        if (live) {
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) e.vjp_out[path * H + h] = E::mul(e.vjp_scale, kKvShared ? kvx[(size_t)h * nt] : kv[h]);
+        }
+    }
+    if (live) {
+#pragma unroll
+        for (int h = 0; h < HM; ++h)
+            if (h < H) a.out[path * H + h] = VJP ? E::mul(e.f_scale, fs[(size_t)h * nt]) : fs[(size_t)h * nt];
+    }
 }
 
 // ---- tensor cores: 2xFP16 wgmma, H = 32, C = 8, W = 128 --------------------------------------------------------------
@@ -1755,6 +1902,75 @@ static int mlp_simt_param_grads(const MlpArgs<T>& a, const T* z_stages, const T*
     return TCDE_OK;
 }
 
+// The shapes tcde_vector_field_mlp[_vjp] are built for: those where mlp_backprop_route runs the CUDA cores, the
+// parameter-gradient staging included, so that a stage the scratch query admits runs every call.  By default they serve
+// only fp32 with hidden * channels <= 32 (one chunk of outputs: the first product is formed once per pass) and width <=
+// 128, where an adjoint=True training step on them measured faster than autograd per stage on an H100 (DESIGN 8);
+// fp64, channels 14 and width 366 at hidden 8 measured 0.13-0.83x of autograd's speed, so automatic selection refuses
+// them and solve variant 1 forces them (as it does for the HM = 32 kernels)
+static int mlp_field_route(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what) {
+    bool simt;
+    const int rc = mlp_backprop_route(hidden, channels, width, dtype, what, &simt);
+    if (rc != TCDE_OK) return rc;
+    TCDE_CHECK_SUPPORTED(simt, "%s is built for the CUDA-core shapes (hidden <= 8, or hidden * channels <= 32 under solve "
+                         "variant 1; got %lld, %lld, %lld)", what, (long long)hidden, (long long)channels,
+                         (long long)width);
+    TCDE_CHECK_SUPPORTED(current_solve_variant() == 1 || (dtype == TCDE_F32 && hidden * channels <= kMlpChunk &&
+                                                          width <= 128),
+                         "%s: at dtype=%d hidden=%lld channels=%lld width=%lld it is slower than autograd per stage; "
+                         "automatic selection does not run it (variant 1 forces it)", what, dtype, (long long)hidden,
+                         (long long)channels, (long long)width);
+    // the largest field layout: fp64, unstaged, with the HM = 32 vjp's shared columns past hidden 8
+    const int extra = hidden > 8 ? mlp_field_extra_shared((int)hidden) : (int)hidden;
+    TCDE_CHECK_SUPPORTED(mlp_simt_param_items(hidden, channels, width) > 0 &&
+                             mlp_simt_layout<double>((int)hidden, (int)channels, (int)width, false, kMlpSimtThreads,
+                                                     extra).total <= kMlpSimtMaxSmem,
+                         "%s: hidden=%lld channels=%lld width=%lld do not fit the CUDA-core kernels' shared memory", what,
+                         (long long)hidden, (long long)channels, (long long)width);
+    return TCDE_OK;
+}
+
+// the parameter-gradient scratch of tcde_vector_field_mlp_vjp starts after the stage's (index, frac)
+constexpr int64_t kMlpFieldScratchHead = 16;
+
+template <typename T, int HM, bool VJP>
+static int launch_mlp_field(const MlpArgs<T>& a, const MlpFieldEval<T>& e, cudaStream_t s) {
+    auto kern = mlp_field_kernel<T, HM, VJP>;
+    MlpSimtLayout<T> lay;
+    const int rc = mlp_simt_pick_layout<T>(a.H, a.C, a.W, lay, mlp_field_extra<T, HM, VJP>(a.H));
+    if (rc != TCDE_OK) return rc;
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
+    const int64_t ctas = (a.n_paths + kMlpSimtThreads - 1) / kMlpSimtThreads;
+    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
+    kern<<<(unsigned)ctas, kMlpSimtThreads, lay.total, s>>>(a, lay, e);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    return TCDE_OK;
+}
+
+// One field evaluation (no cotangent) or one adjoint stage: at most three launches (the field kernel, then with a
+// parameter gradient mlp_simt_param_grad_kernel over this one stage and mlp_simt_param_reduce_kernel)
+template <typename T>
+static int mlp_field_eval(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
+                          const void* w2, const void* b2, const void* z, void* f_out, int64_t n_paths, int64_t channels,
+                          int64_t hidden, int64_t width, int32_t index, double frac, const void* adj, void* vjp_out,
+                          void* grad_w1, void* grad_b1, void* grad_w2, void* grad_b2, void* scratch, double f_scale,
+                          double vjp_scale, double grad_scale, cudaStream_t s) {
+    const bool vjp = adj != nullptr;
+    const bool grads = grad_w1 || grad_b1 || grad_w2 || grad_b2;
+    int32_t* q_index = grads ? static_cast<int32_t*>(scratch) : nullptr;
+    T* q_frac = grads ? reinterpret_cast<T*>(static_cast<char*>(scratch) + 8) : nullptr;
+    const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, z, f_out, n_paths, channels,
+                                          hidden, width, TCDE_EULER, 1, nullptr, q_index, q_frac, 1, nullptr, nullptr,
+                                          nullptr, 1.0);
+    const MlpFieldEval<T> e{(const T*)adj, (T*)vjp_out, q_index, q_frac, index, (T)frac, (T)f_scale, (T)vjp_scale};
+    int rc;
+    if (!vjp) rc = hidden <= 8 ? launch_mlp_field<T, 8, false>(a, e, s) : launch_mlp_field<T, 32, false>(a, e, s);
+    else rc = hidden <= 8 ? launch_mlp_field<T, 8, true>(a, e, s) : launch_mlp_field<T, 32, true>(a, e, s);
+    if (rc != TCDE_OK || !grads) return rc;
+    return mlp_simt_param_grads(a, (const T*)z, (const T*)adj, 1, grad_w1, grad_b1, grad_w2, grad_b2,
+                                static_cast<char*>(scratch) + kMlpFieldScratchHead, grad_scale, s);
+}
+
 static int64_t mlp_param_grid(int64_t n_paths, int64_t n_total) {
     const int64_t items = ((n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths) * n_total;
     int64_t g = sm_count();
@@ -1994,4 +2210,59 @@ extern "C" int tcde_mlp_field_param_grads(const void* control, int control_kind,
         TCDE_CHECK_CUDA(cudaGetLastError());
     }
     return TCDE_OK;
+}
+
+extern "C" int tcde_vector_field_mlp(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
+                                     const void* w2, const void* b2, const void* z, void* out, int64_t n_paths,
+                                     int64_t channels, int64_t hidden, int64_t width, int32_t index, double frac,
+                                     int dtype, void* stream) {
+    TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z && out, "null data pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1, "bad sizes");
+    TCDE_CHECK_ARG(index >= 0 && index < n_rows, "index=%d outside [0, %lld)", index, (long long)n_rows);
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    const int rc = mlp_field_route(hidden, channels, width, dtype, "the MLP field evaluation");
+    if (rc != TCDE_OK) return rc;
+    if (n_paths == 0) return TCDE_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (dtype == TCDE_F32)
+        return mlp_field_eval<float>(control, control_kind, n_rows, w1, b1, w2, b2, z, out, n_paths, channels, hidden,
+                                     width, index, frac, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                     1.0, 1.0, 1.0, s);
+    return mlp_field_eval<double>(control, control_kind, n_rows, w1, b1, w2, b2, z, out, n_paths, channels, hidden, width,
+                                  index, frac, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 1.0, 1.0,
+                                  1.0, s);
+}
+
+extern "C" int64_t tcde_vector_field_mlp_vjp_scratch_bytes(int64_t n_paths, int64_t channels, int64_t hidden,
+                                                           int64_t width) {
+    if (n_paths < 0 || hidden < 1 || channels < 1 || width < 1) return -1;
+    if (mlp_field_route(hidden, channels, width, TCDE_F32, "the MLP adjoint stage") != TCDE_OK) return -1;
+    return kMlpFieldScratchHead + mlp_simt_param_grid(n_paths, 1, mlp_simt_param_items(hidden, channels, width)) *
+                                      mlp_simt_n_params(hidden, channels, width) * (int64_t)sizeof(double);
+}
+
+extern "C" int tcde_vector_field_mlp_vjp(const void* control, int control_kind, int64_t n_rows, const void* w1,
+                                         const void* b1, const void* w2, const void* b2, const void* z, const void* a,
+                                         void* f_out, void* vjp_z_out, void* grad_w1, void* grad_b1, void* grad_w2,
+                                         void* grad_b2, void* scratch, int64_t n_paths, int64_t channels, int64_t hidden,
+                                         int64_t width, int32_t index, double frac, double f_scale, double vjp_scale,
+                                         double grad_scale, int dtype, void* stream) {
+    TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z && a && f_out && vjp_z_out && scratch, "null data pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1, "bad sizes");
+    TCDE_CHECK_ARG(index >= 0 && index < n_rows, "index=%d outside [0, %lld)", index, (long long)n_rows);
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    TCDE_CHECK_ARG((reinterpret_cast<uintptr_t>(scratch) & 15) == 0, "scratch must be 16-byte aligned");
+    const int rc = mlp_field_route(hidden, channels, width, dtype, "the MLP adjoint stage");
+    if (rc != TCDE_OK) return rc;
+    if (n_paths == 0) return TCDE_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (dtype == TCDE_F32)
+        return mlp_field_eval<float>(control, control_kind, n_rows, w1, b1, w2, b2, z, f_out, n_paths, channels, hidden,
+                                     width, index, frac, a, vjp_z_out, grad_w1, grad_b1, grad_w2, grad_b2, scratch,
+                                     f_scale, vjp_scale, grad_scale, s);
+    return mlp_field_eval<double>(control, control_kind, n_rows, w1, b1, w2, b2, z, f_out, n_paths, channels, hidden,
+                                  width, index, frac, a, vjp_z_out, grad_w1, grad_b1, grad_w2, grad_b2, scratch, f_scale,
+                                  vjp_scale, grad_scale, s);
 }

@@ -392,8 +392,16 @@ class AdjointStage:
         k = self.kernels
         return [torch.zeros_like(k.w) if r == "w" else torch.zeros_like(k.b) for r in self.roles]
 
-    def launch(self, index, frac, y, a, f_out, vjp_out, gw, gb, f_scale, vjp_scale, grad_scale):
+    def _by_role(self, grads):
+        """(dL/dW, dL/db) out of one tensor (or None) per parameter in the order of ``params``."""
+        gw = next((g for g, r in zip(grads, self.roles) if r == "w"), None)
+        gb = next((g for g, r in zip(grads, self.roles) if r == "b"), None)
+        return gw, gb
+
+    def launch(self, index, frac, y, a, f_out, vjp_out, *grads, f_scale, vjp_scale, grad_scale):
+        """``grads``: one tensor (or None) per parameter, in the order of ``params``, += grad_scale * a^T df/dp."""
         k = self.kernels
+        gw, gb = self._by_role(grads)
         with torch.cuda.device(y.device):
             _lib.call("tcde_vector_field_linear_vjp", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w),
                       _lib.ptr(k.b), _lib.ptr(y), _lib.ptr(a), _lib.ptr(f_out), _lib.ptr(vjp_out), _lib.ptr(gw),
@@ -407,10 +415,9 @@ class AdjointStage:
         af = a.reshape(-1, k.hidden).contiguous()
         f = torch.empty_like(yf)
         vjp_y = torch.empty_like(yf)
-        gw = torch.zeros_like(k.w) if "w" in self.roles else None
-        gb = torch.zeros_like(k.b) if "b" in self.roles else None
-        self.launch(index, frac, yf, af, f, vjp_y, gw, gb, 1.0, scale, scale)
-        return f.view_as(y), vjp_y.view_as(y), [gw if r == "w" else gb for r in self.roles]
+        grads = self.new_grads()
+        self.launch(index, frac, yf, af, f, vjp_y, *grads, f_scale=1.0, vjp_scale=scale, grad_scale=scale)
+        return f.view_as(y), vjp_y.view_as(y), grads
 
     def locate_many(self, times):
         """Interval index / fraction of a list of stage times, with the casts of ``schedule.host_locator``, in one go."""
@@ -419,13 +426,15 @@ class AdjointStage:
         frac, index = locate(k.knots, tt.to(k.knots.dtype), k.n_rows)
         return index.tolist(), frac.tolist()
 
-    def segment(self, t_hi, t_lo, y_hi, a_hi, method, step_size, gw, gb):
+    def segment(self, t_hi, t_lo, y_hi, a_hi, method, step_size, *grads):
         """One segment [t_hi -> t_lo] of a fixed-step backward solve WITHOUT a launch per stage.  For this linear
         field d a/ds = a^T df/dz does not involve z, so z(s) and a(s) are two ordinary fused solves (tensor-core
         kernel, reversed time), each leaving the input of every stage in HBM; one more launch contracts the two
         trajectories with dX/dt and the Runge-Kutta weights into dL/dW, dL/db.  Returns a(t_lo), or None when the
-        tensor-core kernel or the memory for the two trajectories (2 x stages x paths x 128 bytes) is not available."""
+        tensor-core kernel or the memory for the two trajectories (2 x stages x paths x 128 bytes) is not available.
+        ``grads``: one tensor per parameter, in the order of ``params``."""
         k = self.kernels
+        gw, gb = self._by_role(grads)
         hidden, dtype, dev = k.hidden, k.dtype, k.device
         yf = y_hi.reshape(-1, hidden).contiguous()
         af = a_hi.reshape(-1, hidden).contiguous()

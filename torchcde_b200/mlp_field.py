@@ -3,7 +3,10 @@
 example/time_series_classification.py:20-51 trains ``func(t, z) = tanh(Linear(W, H*C)(relu(Linear(H, W)(z)))).view(H, C)``.
 ``mlp_field_of`` recognises a user module that computes exactly that (no new class to adopt), and ``cdeint`` then runs
 its fixed-step forward as ONE launch of ``tcde_cdeint_fixed_mlp``; ``cdeint(..., adjoint=False)`` with gradients runs
-``MlpBackprop`` (three launches) where it is built for the problem."""
+``MlpBackprop`` (three launches) where it is built for the problem.  At the CUDA-core shapes ``MlpFieldKernels.field`` and
+``MlpAdjointStage`` give the host-driven dopri5 one launch per field evaluation and the ``adjoint=True`` backward one
+launch per stage (``tcde_vector_field_mlp`` / ``tcde_vector_field_mlp_vjp``)."""
+import functools
 import math
 import weakref
 
@@ -11,8 +14,8 @@ import torch
 
 from . import _lib
 from .controls import _control_signature, _schedule_knots
-from .linear_field import _check_linear_problem, _probe, _schedules
-from .schedule import backward_tables
+from .linear_field import AdjointStage, _check_linear_problem, _probe, _schedules
+from .schedule import backward_tables, host_locator
 
 # module -> {training flag: index of the accepted layer ordering, or -1}; kept apart from the linear probe's cache
 _recognised = weakref.WeakKeyDictionary()
@@ -85,6 +88,7 @@ class MlpFieldKernels:
         self.hidden, self.width = z0.size(-1), w1.size(0)
         self.n_paths = math.prod(z0.shape[:-1])
         self.dtype, self.device = z0.dtype, z0.device
+        self.params = params                   # the parameters themselves, to recognise them in adjoint_params
         control = X._rows() if self.kind == _lib.CONTROL_CUBIC else X._derivs
         _check_linear_problem(control, w1, b1, z0)
         _check_linear_problem(control, w2, b2, z0)
@@ -111,6 +115,114 @@ class MlpFieldKernels:
                           sched.n_out, _lib.ptr(v["out_step"]), _lib.ptr(v["out_mode"]), _lib.ptr(v["out_slope"]),
                           float(sched.sign), _lib.dtype_code(self.dtype), _lib.stream_of(zf))
         return out.view(*y0.shape[:-1], sched.n_out, self.hidden)
+
+    @functools.cached_property
+    def where(self):
+        """``(t, nudge) -> (interval index, fraction)`` of a stage time: ``schedule.host_locator``."""
+        return host_locator(self.knots, self.n_rows, self.dtype)
+
+    def field(self):
+        """f(t, y) = tanh(W2 relu(W1 y + b1) + b2).view(H, C) @ dX/dt(t) as ONE launch of ``tcde_vector_field_mlp``.
+        Raises NotImplementedError, on every call, for a shape, dtype or solve variant the kernel is not built for."""
+        hidden = self.hidden
+        code = _lib.dtype_code(self.dtype)
+
+        def field(t, y, nudge=0):
+            index, frac = self.where(t, nudge)
+            yf = y.reshape(-1, hidden).contiguous()
+            out = torch.empty_like(yf)
+            if yf.size(0) == 0:           # an empty batch: nothing to launch (its null data pointers would be refused)
+                return out.view_as(y)
+            with torch.cuda.device(y.device):
+                _lib.call("tcde_vector_field_mlp", _lib.ptr(self.control), self.kind, self.n_rows, _lib.ptr(self.w1),
+                          _lib.ptr(self.b1), _lib.ptr(self.w2), _lib.ptr(self.b2), _lib.ptr(yf), _lib.ptr(out), yf.size(0),
+                          self.channels, hidden, self.width, index, float(frac), code, _lib.stream_of(yf))
+            return out.view_as(y)
+
+        return field
+
+    def adjoint_stage(self, params):
+        """The adjoint stage of this problem for ``params``, or None when the kernel is not built for it (then autograd
+        serves the backward solve): every parameter must be W1, b1, W2 or b2, and the shape one the CUDA-core kernels
+        serve (the scratch query answers -1 elsewhere, the tensor-core shape included)."""
+        roles = []
+        for p in params:
+            role = next((i for i, q in enumerate(self.params) if q is not None and p is q), None)
+            if role is None:
+                return None                       # a parameter that is not the MLP's: autograd knows how
+            roles.append(role)
+        if self.dtype not in (torch.float32, torch.float64):
+            return None
+        scratch_bytes = _lib.load().tcde_vector_field_mlp_vjp_scratch_bytes(self.n_paths, self.channels, self.hidden,
+                                                                             self.width)
+        if scratch_bytes < 0:
+            return None
+        # one scratch per backward: the stage's launches reuse it
+        scratch = torch.empty(max(scratch_bytes // 4, 4), dtype=torch.float32, device=self.device)
+        # the scratch query has no dtype: the dispatch's verdict on this dtype and solve variant comes from a call with
+        # no paths, which validates the problem and launches nothing (the scratch stands in for the per-path buffers,
+        # the control's among them, which is empty for an empty batch)
+        s = _lib.ptr(scratch)
+        try:
+            with torch.cuda.device(self.device):
+                _lib.call("tcde_vector_field_mlp_vjp", s, self.kind, self.n_rows, _lib.ptr(self.w1),
+                          _lib.ptr(self.b1), _lib.ptr(self.w2), _lib.ptr(self.b2), s, s, s, s, None, None, None, None, s,
+                          0, self.channels, self.hidden, self.width, 0, 0.0, 1.0, 1.0, 1.0, _lib.dtype_code(self.dtype),
+                          _lib.stream_of(scratch))
+        except NotImplementedError:
+            return None
+        return MlpAdjointStage(self, roles, scratch)
+
+
+class MlpAdjointStage:
+    """The adjoint stage of the MLP field: ``stage(t, y, a, scale) -> (f, scale * a^T df/dy, [scale * a^T df/dp for p in
+    params])`` as ONE call of ``tcde_vector_field_mlp_vjp`` (at most three launches), with what ``adaptive._Adjoint`` and
+    ``adaptive._fused_fixed_backward`` use of ``linear_field.AdjointStage``; it has no whole-segment route and no
+    device-controlled dopri5 backward.  ``roles``: the index in (W1, b1, W2, b2) of each parameter."""
+
+    adaptive_spec = None
+
+    def __init__(self, kernels, roles, scratch):
+        self.kernels, self.roles, self.scratch = kernels, roles, scratch
+
+    def _tensors(self):
+        k = self.kernels
+        return k.w1, k.b1, k.w2, k.b2
+
+    def new_grads(self):
+        return [torch.zeros_like(self._tensors()[r]) for r in self.roles]
+
+    def launch(self, index, frac, y, a, f_out, vjp_out, *grads, f_scale, vjp_scale, grad_scale):
+        """``grads``: one tensor (or None) per parameter, in the order of ``params``, += grad_scale * a^T df/dp."""
+        k = self.kernels
+        slots = [None] * 4
+        for r, g in zip(self.roles, grads):
+            slots[r] = g
+        if y.numel() == 0:
+            return
+        with torch.cuda.device(y.device):
+            _lib.call("tcde_vector_field_mlp_vjp", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1), _lib.ptr(k.b1),
+                      _lib.ptr(k.w2), _lib.ptr(k.b2), _lib.ptr(y), _lib.ptr(a), _lib.ptr(f_out), _lib.ptr(vjp_out),
+                      *(_lib.ptr(g) for g in slots), _lib.ptr(self.scratch), y.numel() // k.hidden, k.channels,
+                      k.hidden, k.width, index, float(frac), float(f_scale), float(vjp_scale), float(grad_scale),
+                      _lib.dtype_code(k.dtype), _lib.stream_of(y))
+
+    def __call__(self, t, y, a, scale):
+        k = self.kernels
+        index, frac = k.where(t)
+        yf = y.reshape(-1, k.hidden).contiguous()
+        af = a.reshape(-1, k.hidden).contiguous()
+        f = torch.empty_like(yf)
+        vjp_y = torch.empty_like(yf)
+        grads = self.new_grads()
+        self.launch(index, frac, yf, af, f, vjp_y, *grads, f_scale=1.0, vjp_scale=scale, grad_scale=scale)
+        return f.view_as(y), vjp_y.view_as(y), grads
+
+    locate_many = AdjointStage.locate_many
+
+    def segment(self, *args):
+        """No whole-segment backward for this field: the fixed-step backward runs stage by stage."""
+        return None
 
 
 class MlpBackprop:

@@ -285,6 +285,8 @@ def _kernel_field(X, weight, bias, z0):
 
 # the one call through which cdeint gets the adjoint stage of a linear field: ``_kernel_vjp(kernels, params)``
 _kernel_vjp = LinearFieldKernels.adjoint_stage
+# and of the examples' MLP field: ``_mlp_vjp(mlp, params)``
+_mlp_vjp = MlpFieldKernels.adjoint_stage
 
 
 def _torch_field(X, func, is_prod, known_control, z0):
@@ -331,12 +333,17 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     Supported in this round: ``backend="torchdiffeq"`` semantics with the fixed-step methods
     ``euler``, ``midpoint`` and ``rk4`` (torchdiffeq's 3/8 rule).  With a ``CubicSpline`` or
     ``LinearInterpolation`` control and a linear ``func`` (``LinearVectorField`` or any module
-    that is exactly one ``nn.Linear`` + ``view``) the solve is one fused CUDA kernel.  Gradients:
+    that is exactly one ``nn.Linear`` + ``view``) the solve is one fused CUDA kernel, and likewise
+    for the examples' MLP field (``Linear -> ReLU -> Linear -> tanh``).  The default ``dopri5`` runs
+    this package's own adaptive driver; its field is one launch per evaluation for both fields where
+    their kernels serve the shape (the MLP's: fp32, hidden * channels <= 32, width <= 128).  Gradients:
     ``adjoint=True`` runs this package's continuous-adjoint backward (fused kernels for the linear
-    field), ``adjoint=False`` backpropagates through the solve: for the linear field at fp32, hidden 32,
-    channels 8 with gradients for z0 / weight / bias in three launches (``linear_field.FixedBackprop``),
-    likewise for the examples' MLP field at fp32, hidden 32, channels 8, width 128 with gradients for z0
-    and its two layers (``mlp_field.MlpBackprop``), otherwise through the differentiable generic stage loop.
+    field, and one call per stage for the MLP field at the same shapes as its dopri5 field, with
+    dopri5 or a fixed-step method), ``adjoint=False`` backpropagates through the solve: for the
+    linear field at fp32, hidden 32, channels 8 with gradients for z0 / weight / bias in three
+    launches (``linear_field.FixedBackprop``), likewise for the examples' MLP field at fp32, hidden
+    32, channels 8, width 128 with gradients for z0 and its two layers (``mlp_field.MlpBackprop``),
+    otherwise through the differentiable generic stage loop.
 
     ``backend="torchsde"`` is built for ``method="reversible_heun"`` (torchsde's reversible Heun
     method with zero diffusion, fixed step ``dt``, default 1e-3; ``z0`` of shape (batch, hidden),
@@ -490,11 +497,12 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                 pass
 
         field = None
-        if kernels is not None:
-            field = kernels.field()
+        owner = kernels if kernels is not None else mlp
+        if owner is not None:
+            field = owner.field()
             try:
-                # one evaluation before the solve: the kernel field refuses a shape (e.g. hidden > 256) on every call,
-                # so a field that answers here answers every attempt
+                # one evaluation before the solve: the kernel field refuses a shape (e.g. hidden > 256, or the MLP's
+                # tensor-core shape) on every call, so a field that answers here answers every attempt
                 field(-times[0] if flipped else times[0], y0)
             except NotImplementedError:
                 field = None                                  # the torch-operator field takes any shape
@@ -517,9 +525,10 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     kernels = None
     if field_params is not None and (adjoint or not wants_grad or backprop):
         kernels = LinearFieldKernels(X, field_params[0], field_params[1], z0)
-    # the fixed-step forward of the examples' MLP field (no gradient, or the forward pass of adjoint=True) is one launch
+    # the examples' MLP field (no gradient, or adjoint=True): the fixed-step forward is one launch, a dopri5 field
+    # evaluation and an adjoint stage one call each where its CUDA-core kernels serve the shape
     mlp = None
-    if (field_params is None and sig is not None and not is_prod and method in FIXED_METHODS and times
+    if (field_params is None and sig is not None and not is_prod and times
             and (adjoint or not wants_grad)):
         mlp_params = mlp_field_of(func, z0, sig[2], times)
         if mlp_params is not None:
@@ -542,10 +551,12 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
         t_grad = t if t.requires_grad else None
 
         def fused_vjp(params):
-            # decreasing t, gradients with respect to the output times, or parameters that are not the linear map
+            # decreasing t, gradients with respect to the output times, or parameters that are not the field's own
             # (the control's coefficients or knots in ``adjoint_params``): autograd serves the backward solve
-            if kernels is None or flipped or t_grad is not None:
+            if flipped or t_grad is not None:
                 return None
+            if kernels is None:
+                return _mlp_vjp(mlp, params) if mlp is not None else None
             st = _kernel_vjp(kernels, params)
             if (st is not None and a_method not in FIXED_METHODS and adaptive.device_dopri5_available(z0, sig[2])
                     and not kwargs.get("adjoint_options", None)):
