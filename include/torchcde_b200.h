@@ -358,6 +358,40 @@ TCDE_API int tcde_reversible_heun_linear_backward_segment(
     const int32_t* stage_index, const void* stage_frac, int64_t lo, int64_t hi, int64_t n_paths, int64_t channels,
     int64_t hidden, void* dump_z, void* dump_a, int dtype, void* stream);
 
+/* torchsde's reversible Heun method (as tcde_cdeint_reversible_heun_linear: the same step, schedule, output weights and
+ * checkpoint layout) for the MLP vector field of tcde_cdeint_fixed_mlp, in ONE launch on the CUDA cores (one thread per
+ * path, the field in the arithmetic of the fixed-step CUDA-core solve; fp32 or fp64):
+ *   z_{n+1} = 2 y_n - z_n + f_n dt_n,  f_{n+1} = F(t_{n+1}, z_{n+1}),  y_{n+1} = y_n + (f_n + f_{n+1}) (0.5 dt_n)
+ * from z_0 = y_0, f_0 = F(t_0, y_0), one rounding per operation.  checkpoints (may be NULL):
+ * [ceil(n_steps / checkpoint_stride) + 1][3][n_paths][hidden] receives (y, z, f) of every step that is a multiple of
+ * checkpoint_stride and of the last step.  Served at the CUDA-core shapes of tcde_cdeint_fixed_mlp_stages: by default
+ * hidden <= 8 with hidden * channels <= 32 (fp32 and fp64; where a training step on it measured faster than per-step
+ * autograd), under solve variant 1 every hidden * channels <= 32 or hidden <= 8; widths whose parameter-gradient staging
+ * fits shared memory.  TCDE_ERR_UNSUPPORTED elsewhere (the tensor-core shape 32 / 8 / 128 and solve variant 4 included),
+ * so that the caller keeps its own solve. */
+TCDE_API int tcde_cdeint_reversible_heun_mlp(const void* control, int control_kind, int64_t n_rows, const void* w1,
+                                    const void* b1, const void* w2, const void* b2, const void* z0, void* out,
+                                    void* checkpoints, int64_t checkpoint_stride, int64_t n_paths, int64_t channels,
+                                    int64_t hidden, int64_t width, int64_t n_steps, const void* step_dt,
+                                    const int32_t* stage_index, const void* stage_frac, int64_t n_out,
+                                    const int32_t* out_step, const void* out_weights, int dtype, void* stream);
+
+/* One checkpoint segment [lo, hi] of the reversible Heun backward of tcde_cdeint_reversible_heun_mlp, in one launch (one
+ * thread per path): the recurrence of tcde_reversible_heun_linear_backward_segment (same ckpt_lo / ckpt_hi, carry, g,
+ * out_step, out_weights, inj_range and schedule arrays) with one pass of the field's vector-Jacobian product per step at
+ * the reconstructed z_m, which gives f_m = F(z_m) (the forward's bits) and J_F(z_m)^T fbar_m together.  When hi == n_steps
+ * the launch first closes step N: ybar_N = the output gradients on y_N, fbar_N = ybar_N dt_{N-1} / 2, zbar_N =
+ * J_F(z_N)^T fbar_N (carry is not read).  dump_z / dump_a [hi - lo + (hi == n_steps)][n_paths][hidden] receive (z_m,
+ * fbar_m) in slot m - lo, step N in the last slot: tcde_mlp_field_param_grads over them (stage_index / stage_frac offset
+ * by lo, n_stages_total = the dump's length, sign and scale 1) adds dL/dW1, db1, dW2, db2.  Same support as
+ * tcde_cdeint_reversible_heun_mlp. */
+TCDE_API int tcde_reversible_heun_mlp_backward_segment(
+    const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1, const void* w2, const void* b2,
+    const void* ckpt_lo, const void* ckpt_hi, void* carry, const void* g, int64_t n_out, const int32_t* out_step,
+    const void* out_weights, const int32_t* inj_range, int64_t n_steps, const void* step_dt, const int32_t* stage_index,
+    const void* stage_frac, int64_t lo, int64_t hi, int64_t n_paths, int64_t channels, int64_t hidden, int64_t width,
+    void* dump_z, void* dump_a, int dtype, void* stream);
+
 /* The parameter gradients of a whole backward solve (the stage trajectories of tcde_cdeint_fixed_linear_stages, or any
  * other list of (z, a, stage) triples) in one launch:
  *   grad_weight[h*C+c][k] += scale * sum_e sum_p stage_weight[e] * a_stages[e][p][h] * dXdt_e[p][c] * z_stages[e][p][k]

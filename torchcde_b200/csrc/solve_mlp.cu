@@ -772,6 +772,329 @@ __global__ void __launch_bounds__(kMlpSimtThreads) mlp_field_kernel(const MlpArg
     }
 }
 
+// ---- torchsde's reversible Heun (cdeint(..., backend="torchsde")) on the CUDA cores: one thread per path ---------------
+//
+// The forward (tcde_cdeint_reversible_heun_mlp) evaluates the field at z_0 = y_0 and then once per step, with the forward's
+// own TCDE_MLP_CHUNK into the slope column:
+//   z_{n+1} = 2 y_n - z_n + f_n dt_n,  f_{n+1} = F(t_{n+1}, z_{n+1}),  y_{n+1} = y_n + (f_n + f_{n+1}) (0.5 dt_n)
+// rounded once per operation in the order of the linear field's kernel (solve_simt.cu), with its output weights and its
+// checkpoint layout.  The segment backward (tcde_reversible_heun_mlp_backward_segment) is the recurrence of
+// reversible_backward_kernel (solve_tc.cu) with one mlp_vjp pass per step at the reconstructed z_m: its tanh hook gives
+// f_m = F(z_m) (the forward's bits) and its units J^T fbar_m.
+// y, z, f (and in the backward ybar, zbar, z_m, J^T fbar) are register arrays, or where those would spill (fp64 forward at
+// HM = 32, every HM = 32 backward) the thread's columns of shared memory after the slopes.
+template <typename T, int HM> __host__ __device__ constexpr bool mlp_rev_fwd_shared() { return sizeof(T) == 8 && HM == 32; }
+template <int HM> __host__ __device__ constexpr bool mlp_rev_bwd_shared() { return HM == 32; }
+// the backward at HM = 32 runs 64 threads per CTA, so that its columns fit shared memory in fp64
+template <int HM> __host__ __device__ constexpr int mlp_rev_bwd_threads() { return HM == 32 ? 64 : kMlpSimtThreads; }
+// per-thread values after the slopes: forward y [H], z [Hp], f [H]; backward f_m [H], then y, z, f, ybar, zbar,
+// J^T fbar [H] and z_m [Hp] (z and z_m are read up to Hp by the first product)
+template <typename T, int HM> static int mlp_rev_fwd_extra(int H) {
+    return mlp_rev_fwd_shared<T, HM>() ? 2 * H + (H + 3) / 4 * 4 : 0;
+}
+template <int HM> static int mlp_rev_bwd_extra(int H) { return mlp_rev_bwd_shared<HM>() ? 7 * H + (H + 3) / 4 * 4 : H; }
+
+template <typename T, int HM, bool SHARED, int NT> struct MlpRevVec {          // HM registers, zero past H
+    T v[HM];
+    __device__ __forceinline__ void bind(T*) {}
+    __device__ __forceinline__ T& operator[](int k) { return v[k]; }
+    __device__ __forceinline__ const T* arg() const { return v; }
+};
+// the thread's column of shared memory for a CTA of NT threads (a compile-time stride: immediate address offsets)
+template <typename T, int HM, int NT> struct MlpRevVec<T, HM, true, NT> {
+    T* p;
+    __device__ __forceinline__ void bind(T* col) { p = col; }
+    __device__ __forceinline__ T& operator[](int k) const { return p[k * NT]; }
+    __device__ __forceinline__ MlpRevVec arg() const { return *this; }
+};
+
+// a.out_slope: the output weights [2][n_out] (w1, then w0); a.stage_index / a.stage_frac: the N + 1 evaluation points;
+// ckpt (may be null): [ceil(N / ckpt_stride) + 1][3][n_paths][H]
+template <typename T, int HM>
+__global__ void __launch_bounds__(kMlpSimtThreads, 1) cdeint_mlp_rev_kernel(const MlpArgs<T> a, const MlpSimtLayout<T> lay,
+                                                                         T* ckpt, int ckpt_stride) {
+    constexpr bool kShared = mlp_rev_fwd_shared<T, HM>();
+    using E = exact<T>;
+    using P4 = Pack<T, 4>;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    T* smem = reinterpret_cast<T*>(smem_raw);
+    const int tid = threadIdx.x;
+    constexpr int nt = kMlpSimtThreads;
+    const int H = a.H, C = a.C, W = a.W, HC = a.H * a.C, Hp = lay.Hp, Nq = lay.Nq;
+    if (lay.staged) {
+        TCDE_MLP_STAGE_WEIGHTS()
+        __syncthreads();
+    }
+    T* dxs = smem + lay.cols + tid;
+    T* kvs = dxs + (size_t)C * nt;                                 // kvs[h * nt]: F(z_st) of hidden unit h
+    const int64_t path = (int64_t)blockIdx.x * nt + tid;
+    const bool live = path < a.n_paths;
+    const int64_t lp = live ? path : a.n_paths - 1;
+    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
+    const T* crow = a.control + lp * a.n_rows * (cubic ? 4 * C : C) + (cubic ? C : 0);
+    MlpRevVec<T, HM, kShared, nt> y, zin, f;                          // zin: z_st, the input of evaluation st
+    y.bind(kvs + (size_t)H * nt);
+    zin.bind(kvs + (size_t)2 * H * nt);
+    f.bind(kvs + (size_t)(2 * H + Hp) * nt);
+#pragma unroll
+    for (int h = 0; h < HM; ++h) {
+        const T v = (h < H) ? a.z0[lp * H + h] : T(0);
+        if (!kShared || h < H) { y[h] = v; f[h] = T(0); }
+        if (!kShared || h < Hp) zin[h] = v;
+    }
+    int jn = 0;
+    while (jn < a.n_out && a.out_step[jn] < 0) {                   // outputs at t_0: y_0 itself
+        if (live) {
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) a.out[(path * a.n_out + jn) * H + h] = y[h];
+        }
+        ++jn;
+    }
+    for (int st = 0; st <= a.n_steps; ++st) {
+        {
+            TCDE_MLP_SLOPE(a.stage_index[st], a.stage_frac[st])
+            for (int h = 0; h < H; ++h) kvs[(size_t)h * nt] = T(0);
+        }
+        for (int n0 = 0; n0 < HC; n0 += kMlpChunk) {
+            T acc[kMlpChunk];
+            TCDE_MLP_CHUNK(acc, n0)
+            int h = n0 / C, c = n0 - h * C;
+#pragma unroll
+            for (int j = 0; j < kMlpChunk; ++j) {
+                if (n0 + j < HC) {
+                    kvs[(size_t)h * nt] = fma(tanh_of(acc[j]), dxs[(size_t)c * nt], kvs[(size_t)h * nt]);
+                    if (++c == C) { c = 0; ++h; }
+                }
+            }
+        }
+        if (st > 0) {
+            // step n = st - 1 ends: y_{n+1}, and the outputs w0 y_n + w1 y_{n+1} of this step (torchsde's linear_interp)
+            const T half = E::mul(T(0.5), a.step_dt[st - 1]);
+            while (jn < a.n_out && a.out_step[jn] == st - 1) {
+                const T w1 = a.out_slope[jn], w0 = a.out_slope[a.n_out + jn];
+                if (live) {
+#pragma unroll
+                    for (int h = 0; h < HM; ++h)
+                        if (h < H)
+                            a.out[(path * a.n_out + jn) * H + h] =
+                                E::add(E::mul(w0, y[h]), E::mul(w1, E::add(y[h], E::mul(E::add(f[h], kvs[(size_t)h * nt]),
+                                                                                         half))));
+                }
+                ++jn;
+            }
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) y[h] = E::add(y[h], E::mul(E::add(f[h], kvs[(size_t)h * nt]), half));
+        }
+#pragma unroll
+        for (int h = 0; h < HM; ++h)
+            if (h < H) f[h] = kvs[(size_t)h * nt];
+        if (ckpt && live && (st % ckpt_stride == 0 || st == a.n_steps)) {
+            T* base = ckpt + (int64_t)((st + ckpt_stride - 1) / ckpt_stride) * 3 * a.n_paths * H + path * H;
+#pragma unroll
+            for (int h = 0; h < HM; ++h) {
+                if (h < H) {
+                    base[h] = y[h];
+                    base[a.n_paths * H + h] = zin[h];
+                    base[2 * a.n_paths * H + h] = f[h];
+                }
+            }
+        }
+        if (st < a.n_steps) {
+            const T dt = a.step_dt[st];
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) zin[h] = E::add(E::sub(E::mul(T(2), y[h]), zin[h]), E::mul(f[h], dt));
+        }
+    }
+}
+
+template <typename T> struct MlpRevBwd {
+    const T* ckpt_lo;             // [3][n_paths][H]: y, z, f of step lo
+    const T* ckpt_hi;             // ... of step hi
+    T* carry;                     // [2][n_paths][H]: ybar, zbar of step hi in (not read when hi = N), of step lo out
+    const T* g;                   // [n_paths][n_out][H] output gradients
+    const int32_t* inj_range;     // [N + 1][2]: the outputs [first, end) whose gradient lands on y_m
+    T* dump_z;                    // [hi - lo, + 1 when hi = N][n_paths][H]: z_m, in slot m - lo
+    T* dump_a;                    // ... fbar_m
+    int lo, hi;
+};
+
+// a.step_dt [N], a.stage_index / a.stage_frac [N + 1], a.out_step [n_out], a.out_slope [2][n_out] (w1, then w0)
+template <typename T, int HM>
+__global__ void __launch_bounds__(kMlpSimtThreads, 1) mlp_rev_backward_kernel(const MlpArgs<T> a, const MlpSimtLayout<T> lay,
+                                                                           const MlpRevBwd<T> b) {
+    constexpr bool kShared = mlp_rev_bwd_shared<HM>();
+    using E = exact<T>;
+    using P4 = Pack<T, 4>;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    T* smem = reinterpret_cast<T*>(smem_raw);
+    const int tid = threadIdx.x;
+    constexpr int nt = mlp_rev_bwd_threads<HM>();
+    const int H = a.H, C = a.C, Hp = lay.Hp;
+    if (lay.staged) {
+        const int W = a.W, HC = a.H * a.C, Nq = lay.Nq;
+        TCDE_MLP_STAGE_WEIGHTS()
+        __syncthreads();
+    }
+    T* dxs = smem + lay.cols + tid;
+    T* kvs = dxs + (size_t)C * nt;                                 // kvs[h * nt]: fbar_m, the cotangent of mlp_vjp
+    T* fs = kvs + (size_t)H * nt;                                  // fs[h * nt]: f_m = F(z_m) from its tanh values
+    const int64_t path = (int64_t)blockIdx.x * nt + tid;
+    const bool live = path < a.n_paths;
+    const int64_t lp = live ? path : a.n_paths - 1;
+    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
+    const T* crow = a.control + lp * a.n_rows * (cubic ? 4 * C : C) + (cubic ? C : 0);
+    MlpRevVec<T, HM, kShared, nt> y, z, f, yb, zb, kv, zm;             // kv: J^T fbar_m; zm: z_m
+    {
+        T* col = fs + (size_t)H * nt;
+        const size_t step = (size_t)H * nt;
+        y.bind(col);
+        z.bind(col + step);
+        f.bind(col + 2 * step);
+        yb.bind(col + 3 * step);
+        zb.bind(col + 4 * step);
+        kv.bind(col + 5 * step);
+        zm.bind(col + 6 * step);
+    }
+#pragma unroll
+    for (int h = 0; h < HM; ++h) {
+        if (!kShared || h < H) { y[h] = T(0); z[h] = T(0); f[h] = T(0); yb[h] = T(0); zb[h] = T(0); kv[h] = T(0); }
+        if (!kShared || h < Hp) zm[h] = T(0);
+    }
+    const int64_t plane = a.n_paths * H;
+    auto load = [&](auto& v, const T* base) {
+#pragma unroll
+        for (int h = 0; h < HM; ++h)
+            if (h < H) v[h] = base[lp * H + h];
+    };
+    auto store = [&](T* base, auto& v) {
+        if (!live) return;
+#pragma unroll
+        for (int h = 0; h < HM; ++h)
+            if (h < H) base[path * H + h] = v[h];
+    };
+    auto store_fbar = [&](T* base) {
+        if (!live) return;
+        for (int h = 0; h < H; ++h) base[path * H + h] = kvs[(size_t)h * nt];
+    };
+    // v += the output gradients that land on y_m: weight w0 when the output's step is m, 1 at t_0, w1 otherwise
+    auto inject = [&](int m, auto& v) {
+        for (int j = b.inj_range[2 * m]; j < b.inj_range[2 * m + 1]; ++j) {
+            const int os = a.out_step[j];
+            const T w = (os == m) ? a.out_slope[a.n_out + j] : (os < 0 ? T(1) : a.out_slope[j]);
+            const T* src = b.g + (lp * a.n_out + j) * H;
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) v[h] = fma(w, src[h], v[h]);
+        }
+    };
+    // one pass at evaluation point m: fs = F(z_m), kv = J_F(z_m)^T fbar (fbar in kvs)
+    auto vjp = [&](int m) {
+#pragma unroll
+        for (int h = 0; h < HM; ++h) {
+            if (h < H) {
+                fs[(size_t)h * nt] = T(0);
+                kv[h] = T(0);
+            }
+        }
+        {
+            TCDE_MLP_SLOPE(a.stage_index[m], a.stage_frac[m])
+        }
+        mlp_vjp<T, HM>(
+            a, lay, smem, zm.arg(), dxs, kvs, nt, [](int, const T*) {},
+            [&](int, int w, T pre, T sv) {
+                if (!(pre > T(0))) return;
+                if (lay.staged) {
+                    const T* wr = smem + lay.w1 + (size_t)w * lay.Hp;
+#pragma unroll
+                    for (int k4 = 0; k4 < HM / 4; ++k4) {
+                        if (4 * k4 < lay.Hp) {
+                            const P4 w4 = *reinterpret_cast<const P4*>(wr + 4 * k4);
+#pragma unroll
+                            for (int i = 0; i < 4; ++i)
+                                if (!kShared || 4 * k4 + i < H) kv[4 * k4 + i] = fma(w4.v[i], sv, kv[4 * k4 + i]);
+                        }
+                    }
+                } else {
+                    const T* wr = a.w1 + (size_t)w * H;
+#pragma unroll
+                    for (int k = 0; k < HM; ++k)
+                        if (k < H) kv[k] = fma(__ldg(wr + k), sv, kv[k]);
+                }
+            },
+            [&](int h, int c, T yv) { fs[(size_t)h * nt] = fma(yv, dxs[(size_t)c * nt], fs[(size_t)h * nt]); });
+    };
+
+    load(y, b.ckpt_hi);
+    load(z, b.ckpt_hi + plane);
+    load(f, b.ckpt_hi + 2 * plane);
+    const bool close = b.hi == a.n_steps;
+    if (!close) {
+        load(yb, b.carry);
+        load(zb, b.carry + plane);
+    }
+    // m = N (when hi = N) closes the solve: ybar_N = its output gradients, fbar_N = ybar_N dt_{N-1} / 2, z_N from the
+    // checkpoint, zbar_N = J^T fbar_N; it is dumped in the last slot
+    for (int m = close ? b.hi : b.hi - 1; m >= b.lo; --m) {
+        const bool last = m == a.n_steps;
+        const T d = last ? T(0) : a.step_dt[m], dp = m > 0 ? a.step_dt[m - 1] : T(0);
+        const T hd = E::mul(T(0.5), d), hdp = E::mul(T(0.5), dp);
+        // ybar_m = ybar + 2 zbar + (output gradients on y_m);  fbar_m = ybar dt_m / 2 + zbar dt_m + ybar_m dt_{m-1} / 2
+        if (!last) {
+#pragma unroll
+            for (int h = 0; h < HM; ++h) {
+                if (h < H) {
+                    kvs[(size_t)h * nt] = E::add(E::mul(yb[h], hd), E::mul(zb[h], d));
+                    yb[h] = E::add(yb[h], E::mul(T(2), zb[h]));
+                }
+            }
+        }
+        inject(m, yb);
+#pragma unroll
+        for (int h = 0; h < HM; ++h) {
+            if (h < H) kvs[(size_t)h * nt] = last ? E::mul(yb[h], hdp) : E::add(kvs[(size_t)h * nt], E::mul(yb[h], hdp));
+        }
+        if (last) {
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) zm[h] = z[h];
+        } else if (m == b.lo) {
+            load(zm, b.ckpt_lo + plane);
+        } else {
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) zm[h] = E::sub(E::sub(E::mul(T(2), y[h]), z[h]), E::mul(f[h], d));
+        }
+        vjp(m);
+        store(b.dump_z + (int64_t)(m - b.lo) * plane, zm);
+        store_fbar(b.dump_a + (int64_t)(m - b.lo) * plane);
+        if (m == b.lo) {
+            load(y, b.ckpt_lo);
+            load(f, b.ckpt_lo + 2 * plane);
+        } else if (!last) {
+#pragma unroll
+            for (int h = 0; h < HM; ++h) {
+                if (h < H) {
+                    y[h] = E::sub(y[h], E::mul(E::add(fs[(size_t)h * nt], f[h]), hd));
+                    f[h] = fs[(size_t)h * nt];
+                }
+            }
+        }
+        // zbar_m = J^T fbar_m - zbar (zbar = 0 before step N)
+#pragma unroll
+        for (int h = 0; h < HM; ++h) {
+            if (h < H) {
+                z[h] = zm[h];
+                zb[h] = E::sub(kv[h], zb[h]);
+            }
+        }
+    }
+    store(b.carry, yb);
+    store(b.carry + plane, zb);
+}
+
 // ---- tensor cores: 2xFP16 wgmma, H = 32, C = 8, W = 128 --------------------------------------------------------------
 //
 // Each warpgroup owns 64 paths in cdeint_wgmma_kernel's fragment layout (lane (g, q) of warp w: rows 16 w + g and
@@ -1971,6 +2294,101 @@ static int mlp_field_eval(const void* control, int control_kind, int64_t n_rows,
                                 static_cast<char*>(scratch) + kMlpFieldScratchHead, grad_scale, s);
 }
 
+// The layouts of the reversible Heun forward and segment backward at the HM the dispatch picks for H: the weights staged
+// when everything fits, else read from global memory; false if neither fits
+template <typename T, int HM> static bool mlp_rev_fwd_layout(int H, int C, int W, MlpSimtLayout<T>& lay) {
+    for (int stage = 1; stage >= 0; --stage) {
+        lay = mlp_simt_layout<T>(H, C, W, stage != 0, kMlpSimtThreads, mlp_rev_fwd_extra<T, HM>(H));
+        if (lay.total <= kMlpSimtMaxSmem) return true;
+    }
+    return false;
+}
+template <typename T, int HM> static bool mlp_rev_bwd_layout(int H, int C, int W, MlpSimtLayout<T>& lay) {
+    for (int stage = 1; stage >= 0; --stage) {
+        lay = mlp_simt_layout<T>(H, C, W, stage != 0, mlp_rev_bwd_threads<HM>(), mlp_rev_bwd_extra<HM>(H));
+        if (lay.total <= kMlpSimtMaxSmem) return true;
+    }
+    return false;
+}
+
+// Where tcde_cdeint_reversible_heun_mlp and tcde_reversible_heun_mlp_backward_segment run: the CUDA-core route of
+// mlp_backprop_route (hidden <= 8 by default; variant 4 and the tensor-core shape refused), by default only at hidden *
+// channels <= 32 (one chunk of outputs), fp32 and fp64, at widths where the parameter-gradient staging and both kernels'
+// columns fit shared memory.  A training step on it measured faster than the torch-operator forward and per-step autograd
+// it replaces at (8, 3, 128) fp32 and fp64 and at (5, 3, 37) on an H100, but 7.7x slower at (8, 14, 128) (four chunks:
+// the backward recomputes the first product per chunk, and its parameter gradients stage 112 outputs per item), so
+// automatic selection refuses more than one chunk of outputs and solve variant 1 forces every shape the kernels are built
+// for (DESIGN, "torchsde backend").  TCDE_ERR_UNSUPPORTED elsewhere, so that the caller keeps the torch-operator route.
+static int mlp_reversible_route(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what) {
+    bool simt;
+    const int rc = mlp_backprop_route(hidden, channels, width, dtype, what, &simt);
+    if (rc != TCDE_OK) return rc;
+    TCDE_CHECK_SUPPORTED(simt, "%s is built for the CUDA-core shapes (hidden <= 8, or hidden * channels <= 32 under solve "
+                         "variant 1; got %lld, %lld, %lld)", what, (long long)hidden, (long long)channels,
+                         (long long)width);
+    TCDE_CHECK_SUPPORTED(current_solve_variant() == 1 || hidden * channels <= kMlpChunk,
+                         "%s: at hidden=%lld channels=%lld the backward is slower than per-step autograd; automatic "
+                         "selection does not run it (variant 1 forces it)", what, (long long)hidden, (long long)channels);
+    const int H = (int)hidden, C = (int)channels, W = (int)width;
+    MlpSimtLayout<double> fwd, bwd;                 // the larger element size bounds both dtypes
+    const bool fits = H <= 8 ? mlp_rev_fwd_layout<double, 8>(H, C, W, fwd) && mlp_rev_bwd_layout<double, 8>(H, C, W, bwd)
+                             : mlp_rev_fwd_layout<double, 32>(H, C, W, fwd) && mlp_rev_bwd_layout<double, 32>(H, C, W, bwd);
+    TCDE_CHECK_SUPPORTED(fits && mlp_simt_param_items(hidden, channels, width) > 0,
+                         "%s: hidden=%lld channels=%lld width=%lld do not fit the CUDA-core kernels' shared memory", what,
+                         (long long)hidden, (long long)channels, (long long)width);
+    return TCDE_OK;
+}
+
+template <typename T, int HM>
+static int launch_mlp_rev(const MlpArgs<T>& a, T* ckpt, int ckpt_stride, cudaStream_t s) {
+    auto kern = cdeint_mlp_rev_kernel<T, HM>;
+    MlpSimtLayout<T> lay;
+    const bool fits = mlp_rev_fwd_layout<T, HM>(a.H, a.C, a.W, lay);
+    TCDE_CHECK_SUPPORTED(fits, "MLP reversible Heun: the shape does not fit");
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
+    const int64_t ctas = (a.n_paths + kMlpSimtThreads - 1) / kMlpSimtThreads;
+    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
+    kern<<<(unsigned)ctas, kMlpSimtThreads, lay.total, s>>>(a, lay, ckpt, ckpt_stride);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    return TCDE_OK;
+}
+
+template <typename T, int HM>
+static int launch_mlp_rev_backward(const MlpArgs<T>& a, const MlpRevBwd<T>& b, cudaStream_t s) {
+    auto kern = mlp_rev_backward_kernel<T, HM>;
+    constexpr int nt = mlp_rev_bwd_threads<HM>();
+    MlpSimtLayout<T> lay;
+    const bool fits = mlp_rev_bwd_layout<T, HM>(a.H, a.C, a.W, lay);
+    TCDE_CHECK_SUPPORTED(fits, "MLP reversible backward: the shape does not fit");
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
+    const int64_t ctas = (a.n_paths + nt - 1) / nt;
+    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
+    kern<<<(unsigned)ctas, nt, lay.total, s>>>(a, lay, b);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    return TCDE_OK;
+}
+
+template <typename T>
+static MlpArgs<T> mlp_rev_args(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
+                               const void* w2, const void* b2, const void* z0, void* out, int64_t n_paths,
+                               int64_t channels, int64_t hidden, int64_t width, int64_t n_steps, const void* step_dt,
+                               const int32_t* stage_index, const void* stage_frac, int64_t n_out, const int32_t* out_step,
+                               const void* out_weights) {
+    return mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths, channels, hidden, width,
+                            TCDE_REVERSIBLE_HEUN, n_steps, step_dt, stage_index, stage_frac, n_out, out_step, nullptr,
+                            out_weights, 1.0);
+}
+
+template <typename T>
+static int mlp_rev_forward(const MlpArgs<T>& a, void* ckpt, int ckpt_stride, cudaStream_t s) {
+    return a.H <= 8 ? launch_mlp_rev<T, 8>(a, (T*)ckpt, ckpt_stride, s) : launch_mlp_rev<T, 32>(a, (T*)ckpt, ckpt_stride, s);
+}
+
+template <typename T>
+static int mlp_rev_backward(const MlpArgs<T>& a, const MlpRevBwd<T>& b, cudaStream_t s) {
+    return a.H <= 8 ? launch_mlp_rev_backward<T, 8>(a, b, s) : launch_mlp_rev_backward<T, 32>(a, b, s);
+}
+
 static int64_t mlp_param_grid(int64_t n_paths, int64_t n_total) {
     const int64_t items = ((n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths) * n_total;
     int64_t g = sm_count();
@@ -2265,4 +2683,70 @@ extern "C" int tcde_vector_field_mlp_vjp(const void* control, int control_kind, 
     return mlp_field_eval<double>(control, control_kind, n_rows, w1, b1, w2, b2, z, f_out, n_paths, channels, hidden,
                                   width, index, frac, a, vjp_z_out, grad_w1, grad_b1, grad_w2, grad_b2, scratch, f_scale,
                                   vjp_scale, grad_scale, s);
+}
+
+extern "C" int tcde_cdeint_reversible_heun_mlp(const void* control, int control_kind, int64_t n_rows, const void* w1,
+                                               const void* b1, const void* w2, const void* b2, const void* z0, void* out,
+                                               void* checkpoints, int64_t checkpoint_stride, int64_t n_paths,
+                                               int64_t channels, int64_t hidden, int64_t width, int64_t n_steps,
+                                               const void* step_dt, const int32_t* stage_index, const void* stage_frac,
+                                               int64_t n_out, const int32_t* out_step, const void* out_weights, int dtype,
+                                               void* stream) {
+    TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z0 && out, "null data pointer");
+    TCDE_CHECK_ARG(step_dt && stage_index && stage_frac && out_step && out_weights, "null schedule pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1, "bad sizes");
+    TCDE_CHECK_ARG(n_steps >= 1 && n_out >= 1, "n_steps=%lld n_out=%lld", (long long)n_steps, (long long)n_out);
+    TCDE_CHECK_ARG(checkpoint_stride >= 1 && checkpoint_stride < (1ll << 30), "checkpoint_stride=%lld",
+                   (long long)checkpoint_stride);
+    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    TCDE_CHECK_SUPPORTED(n_steps + 1 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
+    const int rc = mlp_reversible_route(hidden, channels, width, dtype, "the MLP reversible Heun solve");
+    if (rc != TCDE_OK) return rc;
+    if (n_paths == 0) return TCDE_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (dtype == TCDE_F32)
+        return mlp_rev_forward(mlp_rev_args<float>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths,
+                                                   channels, hidden, width, n_steps, step_dt, stage_index, stage_frac,
+                                                   n_out, out_step, out_weights),
+                               checkpoints, (int)checkpoint_stride, s);
+    return mlp_rev_forward(mlp_rev_args<double>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths, channels,
+                                                hidden, width, n_steps, step_dt, stage_index, stage_frac, n_out, out_step,
+                                                out_weights),
+                           checkpoints, (int)checkpoint_stride, s);
+}
+
+extern "C" int tcde_reversible_heun_mlp_backward_segment(
+    const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1, const void* w2, const void* b2,
+    const void* ckpt_lo, const void* ckpt_hi, void* carry, const void* g, int64_t n_out, const int32_t* out_step,
+    const void* out_weights, const int32_t* inj_range, int64_t n_steps, const void* step_dt, const int32_t* stage_index,
+    const void* stage_frac, int64_t lo, int64_t hi, int64_t n_paths, int64_t channels, int64_t hidden, int64_t width,
+    void* dump_z, void* dump_a, int dtype, void* stream) {
+    TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && ckpt_lo && ckpt_hi && carry && g && dump_z && dump_a,
+                   "null data pointer");
+    TCDE_CHECK_ARG(out_step && out_weights && inj_range && step_dt && stage_index && stage_frac, "null schedule pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1 && n_out >= 1, "bad sizes");
+    TCDE_CHECK_ARG(lo >= 0 && hi > lo && hi <= n_steps && n_steps + 1 < (1ll << 31), "lo=%lld hi=%lld n_steps=%lld",
+                   (long long)lo, (long long)hi, (long long)n_steps);
+    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    const int rc = mlp_reversible_route(hidden, channels, width, dtype, "the MLP reversible backward");
+    if (rc != TCDE_OK) return rc;
+    if (n_paths == 0) return TCDE_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (dtype == TCDE_F32)
+        return mlp_rev_backward(
+            mlp_rev_args<float>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths, channels,
+                                hidden, width, n_steps, step_dt, stage_index, stage_frac, n_out, out_step, out_weights),
+            MlpRevBwd<float>{(const float*)ckpt_lo, (const float*)ckpt_hi, (float*)carry, (const float*)g, inj_range,
+                             (float*)dump_z, (float*)dump_a, (int)lo, (int)hi},
+            s);
+    return mlp_rev_backward(
+        mlp_rev_args<double>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths, channels, hidden,
+                             width, n_steps, step_dt, stage_index, stage_frac, n_out, out_step, out_weights),
+        MlpRevBwd<double>{(const double*)ckpt_lo, (const double*)ckpt_hi, (double*)carry, (const double*)g, inj_range,
+                          (double*)dump_z, (double*)dump_a, (int)lo, (int)hi},
+        s);
 }

@@ -223,6 +223,67 @@ class LinearFieldKernels:
                   _lib.dtype_code(self.dtype), _lib.stream_of(z_stages))
         return True
 
+    # ---- torchsde's reversible Heun (reversible._Problem): the forward, the segment backward, the parameter gradients ----
+    @property
+    def field_params(self):
+        return self.weight, self.bias
+
+    @property
+    def field_tensors(self):
+        return self.w, self.b
+
+    @property
+    def reversible_backward_served(self):
+        """The segment kernel is built for fp32 at hidden 32, channels 8."""
+        return self.dtype == torch.float32 and self.hidden == 32 and self.channels == 8
+
+    def reversible_forward(self, sched, v, z0, out, ckpt, stride):
+        """ONE launch of ``tcde_cdeint_reversible_heun_linear`` on ``build_sde_schedule``'s tables (device views ``v``)."""
+        _lib.call("tcde_cdeint_reversible_heun_linear", _lib.ptr(self.control), self.kind, self.n_rows, _lib.ptr(self.w),
+                  _lib.ptr(self.b), _lib.ptr(z0), _lib.ptr(out), _lib.ptr(ckpt), stride, z0.size(0), self.channels,
+                  self.hidden, sched.n_steps, _lib.ptr(v["step_dt"]), _lib.ptr(v["stage_index"]), _lib.ptr(v["stage_frac"]),
+                  sched.n_out, _lib.ptr(v["out_step"]), _lib.ptr(v["out_slope"]), _lib.dtype_code(self.dtype),
+                  _lib.stream_of(z0))
+
+    def reversible_segment(self, bw, lo, hi, ck_lo, ck_hi):
+        """ONE launch of ``tcde_reversible_heun_linear_backward_segment`` over steps [lo, hi]; the segment that ends at
+        step N first closes it (ybar_N from the outputs, zbar_N = J_F(z_N)^T fbar_N and its parameter gradients by one
+        launch of ``tcde_vector_field_linear_vjp``).  Returns the number of dumped steps."""
+        p, v = bw.problem, bw.views
+        n_steps, n_paths = p.sched.n_steps, bw.g.size(0)
+        gw, gb = bw.grads
+        if hi == n_steps:
+            first, end, weights = p._injection(n_steps)
+            bw.carry[0].zero_()
+            for j, w in zip(range(first, end), weights):
+                bw.carry[0].add_(bw.g[:, j], alpha=w)
+            fbar = bw.carry[0] * (0.5 * p.dts[n_steps - 1])
+            z_n = bw.last[1].contiguous()
+            f_tmp = torch.empty_like(z_n)
+            scratch_bytes = _lib.load().tcde_vector_field_linear_vjp_scratch_bytes(n_paths, self.channels, self.hidden)
+            scratch = torch.empty(max(scratch_bytes // 4, 4), dtype=torch.float32, device=self.device)
+            _lib.call("tcde_vector_field_linear_vjp", _lib.ptr(self.control), self.kind, self.n_rows, _lib.ptr(self.w),
+                      _lib.ptr(self.b), _lib.ptr(z_n), _lib.ptr(fbar), _lib.ptr(f_tmp), _lib.ptr(bw.carry[1]),
+                      _lib.ptr(gw), _lib.ptr(gb), _lib.ptr(scratch), n_paths, self.channels, self.hidden,
+                      p.index[n_steps], float(p.frac_state[n_steps]), 1.0, 1.0, 1.0, _lib.F32, bw.stream)
+        w_t, zeros = self.transposed_weights
+        _lib.call("tcde_reversible_heun_linear_backward_segment", _lib.ptr(self.control), self.kind, self.n_rows,
+                  _lib.ptr(self.w), _lib.ptr(self.b), _lib.ptr(w_t), _lib.ptr(zeros), _lib.ptr(ck_lo), _lib.ptr(ck_hi),
+                  _lib.ptr(bw.carry), _lib.ptr(bw.g), p.n_out, _lib.ptr(v["out_step"]), _lib.ptr(v["out_slope"]),
+                  _lib.ptr(bw.inj), _lib.ptr(v["step_dt"]), _lib.ptr(v["stage_index"]), _lib.ptr(v["stage_frac"]), lo, hi,
+                  n_paths, self.channels, self.hidden, _lib.ptr(bw.dump_z), _lib.ptr(bw.dump_a), _lib.F32, bw.stream)
+        return hi - lo
+
+    def reversible_param_grads(self, bw, lo, n):
+        """dL/dW, dL/db += the segment's dump of ``n`` steps from ``lo`` (``param_grads`` with weights 1)."""
+        gw, gb = bw.grads
+        if getattr(bw, "ones", None) is None:
+            bw.ones = torch.ones(bw.dump_z.size(0), dtype=torch.float32, device=self.device)
+        v = bw.views
+        if not self.param_grads(bw.dump_z, bw.dump_a, v["stage_index"][lo:lo + n], v["stage_frac"][lo:lo + n], bw.ones,
+                                n, gw, gb):
+            raise RuntimeError("reversible backward: the parameter-gradient kernel is not built for this problem")
+
     def dopri5(self, y0, times, rtol, atol, sign, first_step=None):
         """The same algorithm as ``adaptive.Dopri5.integrate`` with accept / reject, the step-size rule and the dense
         output on the device (``tcde_dopri5_linear_attempts``: one launch per attempted step, no host read per attempt).

@@ -5,7 +5,8 @@ example/time_series_classification.py:20-51 trains ``func(t, z) = tanh(Linear(W,
 its fixed-step forward as ONE launch of ``tcde_cdeint_fixed_mlp``; ``cdeint(..., adjoint=False)`` with gradients runs
 ``MlpBackprop`` (three launches) where it is built for the problem.  At the CUDA-core shapes ``MlpFieldKernels.field`` and
 ``MlpAdjointStage`` give the host-driven dopri5 one launch per field evaluation and the ``adjoint=True`` backward one
-launch per stage (``tcde_vector_field_mlp`` / ``tcde_vector_field_mlp_vjp``)."""
+launch per stage (``tcde_vector_field_mlp`` / ``tcde_vector_field_mlp_vjp``).  Under ``backend="torchsde"``
+(``reversible.py``) ``MlpFieldKernels`` supplies the reversible Heun forward and its segment backward on the CUDA cores."""
 import functools
 import math
 import weakref
@@ -140,6 +141,55 @@ class MlpFieldKernels:
             return out.view_as(y)
 
         return field
+
+    # ---- torchsde's reversible Heun (reversible._Problem): the forward, the segment backward, the parameter gradients ----
+    # Which shapes, dtypes and solve variants they serve is the C dispatch's call; where it admits the forward it serves the
+    # backward.  A missing bias is the kernels' zero vector, which takes no gradient.
+    reversible_backward_served = True
+
+    @property
+    def field_params(self):
+        return self.params
+
+    @property
+    def field_tensors(self):
+        return self.w1, self.b1, self.w2, self.b2
+
+    def reversible_forward(self, sched, v, z0, out, ckpt, stride):
+        """ONE launch of ``tcde_cdeint_reversible_heun_mlp``; NotImplementedError where it is not built."""
+        _lib.call("tcde_cdeint_reversible_heun_mlp", _lib.ptr(self.control), self.kind, self.n_rows, _lib.ptr(self.w1),
+                  _lib.ptr(self.b1), _lib.ptr(self.w2), _lib.ptr(self.b2), _lib.ptr(z0), _lib.ptr(out), _lib.ptr(ckpt),
+                  stride, z0.size(0), self.channels, self.hidden, self.width, sched.n_steps, _lib.ptr(v["step_dt"]),
+                  _lib.ptr(v["stage_index"]), _lib.ptr(v["stage_frac"]), sched.n_out, _lib.ptr(v["out_step"]),
+                  _lib.ptr(v["out_slope"]), _lib.dtype_code(self.dtype), _lib.stream_of(z0))
+
+    def reversible_segment(self, bw, lo, hi, ck_lo, ck_hi):
+        """ONE launch of ``tcde_reversible_heun_mlp_backward_segment`` over steps [lo, hi] (the segment that ends at step N
+        also closes it and dumps it last).  Returns the number of dumped steps."""
+        p, v = bw.problem, bw.views
+        n_steps = p.sched.n_steps
+        _lib.call("tcde_reversible_heun_mlp_backward_segment", _lib.ptr(self.control), self.kind, self.n_rows,
+                  _lib.ptr(self.w1), _lib.ptr(self.b1), _lib.ptr(self.w2), _lib.ptr(self.b2), _lib.ptr(ck_lo),
+                  _lib.ptr(ck_hi), _lib.ptr(bw.carry), _lib.ptr(bw.g), p.n_out, _lib.ptr(v["out_step"]),
+                  _lib.ptr(v["out_slope"]), _lib.ptr(bw.inj), n_steps, _lib.ptr(v["step_dt"]), _lib.ptr(v["stage_index"]),
+                  _lib.ptr(v["stage_frac"]), lo, hi, bw.g.size(0), self.channels, self.hidden, self.width,
+                  _lib.ptr(bw.dump_z), _lib.ptr(bw.dump_a), _lib.dtype_code(self.dtype), bw.stream)
+        return hi - lo + (1 if hi == n_steps else 0)
+
+    def reversible_param_grads(self, bw, lo, n):
+        """dW1, db1, dW2, db2 += the segment's dump of ``n`` steps from ``lo``: ONE call of ``tcde_mlp_field_param_grads``
+        (its kernel and its fixed-order reduction)."""
+        n_paths = bw.g.size(0)
+        if getattr(bw, "scratch", None) is None:
+            nbytes = _lib.load().tcde_mlp_field_param_grads_scratch_bytes(n_paths, bw.dump_z.size(0), self.channels,
+                                                                           self.hidden, self.width)
+            bw.scratch = torch.empty(max(nbytes // 4, 4), dtype=torch.float32, device=self.device)
+        v = bw.views
+        _lib.call("tcde_mlp_field_param_grads", _lib.ptr(self.control), self.kind, self.n_rows, _lib.ptr(self.w1),
+                  _lib.ptr(self.b1), _lib.ptr(self.w2), _lib.ptr(self.b2), _lib.ptr(bw.dump_z), _lib.ptr(bw.dump_a),
+                  _lib.ptr(v["stage_index"][lo:]), _lib.ptr(v["stage_frac"][lo:]), n, *(_lib.ptr(g) for g in bw.grads),
+                  _lib.ptr(bw.scratch), n_paths, self.channels, self.hidden, self.width, 1.0, 1.0,
+                  _lib.dtype_code(self.dtype), bw.stream)
 
     def adjoint_stage(self, params):
         """The adjoint stage of this problem for ``params``, or None when the kernel is not built for it (then autograd

@@ -6,9 +6,10 @@ in ``t``'s dtype, last step clipped, outputs by linear interpolation between the
 
     z_{n+1} = 2 y_n - z_n + f_n dt_n,   f_{n+1} = f(t_{n+1}, z_{n+1}),   y_{n+1} = y_n + (f_n + f_{n+1}) (0.5 dt_n)
 
-from ``z_0 = y_0``, ``f_0 = f(t_0, y_0)``: one evaluation of the vector field per step.  For the README's linear field on
-a built-in control the whole solve is one launch of ``tcde_cdeint_reversible_heun_linear``; any other ``func`` runs as
-torch operators (differentiable, which is what ``adjoint=False`` backpropagates through).
+from ``z_0 = y_0``, ``f_0 = f(t_0, y_0)``: one evaluation of the vector field per step.  On a built-in control the whole
+solve is one launch of the kernel owner's forward: ``tcde_cdeint_reversible_heun_linear`` for the README's linear field,
+``tcde_cdeint_reversible_heun_mlp`` for the examples' MLP field where the C dispatch serves its shape; any other ``func``
+runs as torch operators (differentiable, which is what ``adjoint=False`` backpropagates through).
 
 Backward (``adjoint=True``).  The gradient of the discrete forward solve, found by running the step backwards
 algebraically -- ``z_n = 2 y_{n+1} - z_{n+1} - f_{n+1} dt_n``, ``f_n = F(n, z_n)``, ``y_n = y_{n+1} - (f_n + f_{n+1})
@@ -16,11 +17,15 @@ dt_n / 2`` -- while the adjoints of (y, z, f) run the transposed recurrence.  In
 backward dynamics amplify rounding), so the forward keeps ``(y, z, f)`` every ``CHECKPOINT_STRIDE`` steps and at the
 end, and each segment of the backward restarts from its saved end state; that is a deliberate departure from torchsde,
 which reconstructs the whole solve from the final state.  The memory is the checkpoints plus O(1) states, independent of
-the number of output times.  For the linear field in fp32 (hidden 32, channels 8) with parameters that are only its
-weight and bias, a segment is ONE launch of ``tcde_reversible_heun_linear_backward_segment`` (the two field products of a
-step on the tensor cores, the recurrence in registers, (z_m, fbar_m) dumped) and one launch of
-``tcde_linear_field_param_grads`` over that dump.  Otherwise each step is one ``torch.autograd.grad`` of ``F``, which
-covers any ``func``, control coefficients in ``adjoint_params`` and fp64.
+the number of output times.  Where the kernels solved the forward and every parameter is one of the field's own, the
+kernel owner (``LinearFieldKernels`` or ``MlpFieldKernels``) runs each segment as one segment launch ((z_m, fbar_m)
+dumped) and one parameter-gradient launch over that dump: for the linear field in fp32 (hidden 32, channels 8)
+``tcde_reversible_heun_linear_backward_segment`` (the two field products of a step on the tensor cores; step N closed by
+``tcde_vector_field_linear_vjp``) and ``tcde_linear_field_param_grads``; for the MLP field
+``tcde_reversible_heun_mlp_backward_segment`` (one vector-Jacobian pass per step on the CUDA cores, step N closed in the
+same launch) and ``tcde_mlp_field_param_grads``.  Otherwise each step is one ``torch.autograd.grad`` of ``F``, which
+covers any ``func``, control coefficients in ``adjoint_params`` and the linear field in fp64; an MLP field whose
+parameters the kernels do not serve also keeps the torch-operator forward.
 
 ``t`` is a constant here: it receives no gradient.
 
@@ -30,12 +35,14 @@ checkpoints of 3 states per 16 steps (about 125 GB at 65,536 paths x 32 hidden).
 refuses a checkpoint buffer that does not fit in the free device memory, with a message that says so.
 """
 import bisect
+import types
 
 import torch
 
 from . import _lib
 from .controls import _control_signature, _schedule_knots
 from .linear_field import LinearFieldKernels, linear_field_of
+from .mlp_field import MlpFieldKernels, mlp_field_of
 from .schedule import build_sde_schedule, locate
 from .solver import _derivative_at, _shape_error_forward, _shape_error_prod
 
@@ -71,8 +78,20 @@ def _check_arguments(z0, t, kwargs):
     return DEFAULT_DT if dt is None else float(dt)
 
 
+def _roles(field_params, params):
+    """The index in ``field_params`` (a missing bias is None) of every parameter, or None when one is not the field's."""
+    roles = []
+    for p in params:
+        role = next((i for i, q in enumerate(field_params) if q is not None and p is q), None)
+        if role is None:
+            return None
+        roles.append(role)
+    return roles
+
+
 class _Problem:
-    """One reversible Heun problem: the schedule, the torch-operator field and, for the linear field, the kernels."""
+    """One reversible Heun problem: the schedule, the torch-operator field and, for the linear or the MLP field, the
+    kernel owner (``LinearFieldKernels`` or ``MlpFieldKernels``)."""
 
     def __init__(self, X, func, z0, t, dt, kernels, params):
         self.X, self.func, self.kernels, self.params = X, func, kernels, params
@@ -136,9 +155,9 @@ class _Problem:
                 ckpts[n + 1] = (y, z, f)
         return torch.stack(outs, dim=-2), ckpts
 
-    # ---- the linear field's kernel ------------------------------------------------------------------------------------
+    # ---- the kernels of the linear or the MLP field ------------------------------------------------------------------
     def kernel_forward(self, y0, keep_checkpoints):
-        """ONE launch of ``tcde_cdeint_reversible_heun_linear``; the same return values as ``torch_forward``."""
+        """ONE launch of the kernel owner's solve (``reversible_forward``); the same return values as ``torch_forward``."""
         k, s = self.kernels, self.sched
         n_paths, hidden = y0.size(0), k.hidden
         n_slots = -(-s.n_steps // CHECKPOINT_STRIDE) + 1
@@ -148,7 +167,7 @@ class _Problem:
             out = torch.empty(n_paths, s.n_out, hidden, dtype=k.dtype, device=k.device)
             ck = None
             if keep_checkpoints:
-                need = n_slots * 3 * n_paths * hidden * k.w.element_size()
+                need = n_slots * 3 * n_paths * hidden * zf.element_size()
                 free, _total = torch.cuda.mem_get_info()
                 if need > free:
                     raise RuntimeError(
@@ -156,11 +175,7 @@ class _Problem:
                         "({} states of {} paths every {} steps), more than the {:.1f} GiB free; use a larger dt."
                         .format(s.n_steps, need / 2 ** 30, 3 * n_slots, n_paths, CHECKPOINT_STRIDE, free / 2 ** 30))
                 ck = torch.empty(n_slots, 3, n_paths, hidden, dtype=k.dtype, device=k.device)
-            _lib.call("tcde_cdeint_reversible_heun_linear", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w),
-                      _lib.ptr(k.b), _lib.ptr(zf), _lib.ptr(out), _lib.ptr(ck), CHECKPOINT_STRIDE, n_paths, k.channels,
-                      hidden, s.n_steps, _lib.ptr(v["step_dt"]), _lib.ptr(v["stage_index"]), _lib.ptr(v["stage_frac"]),
-                      s.n_out, _lib.ptr(v["out_step"]), _lib.ptr(v["out_slope"]), _lib.dtype_code(k.dtype),
-                      _lib.stream_of(zf))
+            k.reversible_forward(s, v, zf, out, ck, CHECKPOINT_STRIDE)
         ckpts = {}
         if keep_checkpoints:
             ckpts["slots"], ckpts["views"] = ck, v
@@ -174,26 +189,19 @@ class _Problem:
             try:
                 return self.kernel_forward(y0, keep_checkpoints)
             except NotImplementedError:
-                # a shape beyond the CUDA-core kernel's shared memory: the torch-operator solve takes any shape
+                # a shape the kernels are not built for: the torch-operator solve takes any shape
                 self.kernels = None
         return self.torch_forward(y0, keep_checkpoints)
 
     # ---- the backward -------------------------------------------------------------------------------------------------
     def fused_roles(self, ckpts):
-        """"w" / "b" for every parameter when the segment kernel serves the backward (the linear field in fp32 at hidden 32,
-        channels 8, solved by the kernel, every parameter its weight or bias), else None."""
+        """The index of every parameter in the kernel owner's ``field_params`` when its segment kernel serves the backward
+        (the field solved by the kernel, ``reversible_backward_served``, every parameter one of the field's own), else
+        None."""
         k = self.kernels
-        if k is None or "slots" not in ckpts or k.dtype != torch.float32 or k.hidden != 32 or k.channels != 8:
+        if k is None or "slots" not in ckpts or not k.reversible_backward_served:
             return None
-        roles = []
-        for p in self.params:
-            if p is k.weight:
-                roles.append("w")
-            elif k.bias is not None and p is k.bias:
-                roles.append("b")
-            else:
-                return None
-        return roles
+        return _roles(k.field_params, self.params)
 
     def _injection(self, m):
         """The outputs [first, end) whose gradient lands on y_m, and their weights."""
@@ -204,57 +212,35 @@ class _Problem:
         return first, end, weights
 
     def fused_backward(self, ckpts, g, roles):
-        """The backward with one launch of ``tcde_reversible_heun_linear_backward_segment`` per checkpoint segment and one
-        launch of ``tcde_linear_field_param_grads`` over its (z, fbar) dump; step N is closed by one launch of
-        ``tcde_vector_field_linear_vjp``."""
+        """The backward with the kernel owner's launches: per checkpoint segment, last first, ``reversible_segment`` (the
+        recurrence over the segment, (ybar, zbar) carried between launches, (z_m, fbar_m) dumped; the segment that ends at
+        step N also closes it) and ``reversible_param_grads`` over that dump."""
         k, s = self.kernels, self.sched
-        n_steps, n_paths, hidden, channels, dev = s.n_steps, g.size(0), k.hidden, k.channels, k.device
-        grads = [torch.zeros_like(k.w) if r == "w" else torch.zeros_like(k.b) for r in roles]
-        gw = grads[roles.index("w")] if "w" in roles else None
-        gb = grads[roles.index("b")] if "b" in roles else None
-        ck, v = ckpts["slots"], ckpts["views"]
-        stream = _lib.stream_of(g)
+        n_steps, n_paths, dev = s.n_steps, g.size(0), k.device
+        tensors = k.field_tensors
+        grads = [torch.zeros_like(tensors[r]) for r in roles]
+        by_role = [None] * len(tensors)
+        for r, acc in zip(roles, grads):
+            if by_role[r] is None:
+                by_role[r] = acc
+        ck = ckpts["slots"]
         with torch.cuda.device(dev):
             ranges = []
             for m in range(n_steps + 1):
                 first, end, _w = self._injection(m)
                 ranges += [first, end]
-            inj = torch.tensor(ranges, dtype=torch.int32).to(dev)
-            w_t = k.w.view(hidden, channels, hidden).permute(2, 1, 0).contiguous().view(hidden * channels, hidden)
-            zeros = torch.zeros_like(k.b)
-            carry = torch.empty(2, n_paths, hidden, dtype=torch.float32, device=dev)
-            # step N: ybar_N from the outputs, zbar_N = J_F(z_N)^T fbar_N (and its parameter gradients)
-            first, end, weights = self._injection(n_steps)
-            carry[0].zero_()
-            for j, w in zip(range(first, end), weights):
-                carry[0].add_(g[:, j], alpha=w)
-            fbar = carry[0] * (0.5 * self.dts[n_steps - 1])
-            z_n = ckpts[n_steps][1].contiguous()
-            f_tmp = torch.empty_like(z_n)
-            scratch_bytes = _lib.load().tcde_vector_field_linear_vjp_scratch_bytes(n_paths, channels, hidden)
-            scratch = torch.empty(max(scratch_bytes // 4, 4), dtype=torch.float32, device=dev)
-            _lib.call("tcde_vector_field_linear_vjp", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w), _lib.ptr(k.b),
-                      _lib.ptr(z_n), _lib.ptr(fbar), _lib.ptr(f_tmp), _lib.ptr(carry[1]), _lib.ptr(gw), _lib.ptr(gb),
-                      _lib.ptr(scratch), n_paths, channels, hidden, self.index[n_steps],
-                      float(self.frac_state[n_steps]), 1.0, 1.0, 1.0, _lib.F32, stream)
-            dump_z = torch.empty(CHECKPOINT_STRIDE, n_paths, hidden, dtype=torch.float32, device=dev)
-            dump_a = torch.empty_like(dump_z)
-            ones = torch.ones(CHECKPOINT_STRIDE, dtype=torch.float32, device=dev)
+            dump_z = torch.empty(CHECKPOINT_STRIDE + 1, n_paths, k.hidden, dtype=k.dtype, device=dev)
+            bw = types.SimpleNamespace(
+                problem=self, views=ckpts["views"], inj=torch.tensor(ranges, dtype=torch.int32).to(dev),
+                carry=torch.empty(2, n_paths, k.hidden, dtype=k.dtype, device=dev), g=g, last=ck[-1], dump_z=dump_z,
+                dump_a=torch.empty_like(dump_z), grads=by_role, stream=_lib.stream_of(g))
             for slot in range(ck.size(0) - 2, -1, -1):
                 lo = slot * CHECKPOINT_STRIDE
                 hi = min(lo + CHECKPOINT_STRIDE, n_steps)
-                _lib.call("tcde_reversible_heun_linear_backward_segment", _lib.ptr(k.control), k.kind, k.n_rows,
-                          _lib.ptr(k.w), _lib.ptr(k.b), _lib.ptr(w_t), _lib.ptr(zeros), _lib.ptr(ck[slot]),
-                          _lib.ptr(ck[slot + 1]), _lib.ptr(carry), _lib.ptr(g), s.n_out, _lib.ptr(v["out_step"]),
-                          _lib.ptr(v["out_slope"]), _lib.ptr(inj), _lib.ptr(v["step_dt"]), _lib.ptr(v["stage_index"]),
-                          _lib.ptr(v["stage_frac"]), lo, hi, n_paths, channels, hidden, _lib.ptr(dump_z),
-                          _lib.ptr(dump_a), _lib.F32, stream)
-                if gw is not None or gb is not None:
-                    if not k.param_grads(dump_z, dump_a, v["stage_index"][lo:hi], v["stage_frac"][lo:hi], ones, hi - lo,
-                                         gw, gb):
-                        raise RuntimeError("reversible backward: the parameter-gradient kernel is not built for this "
-                                           "problem")
-            return carry[0] + carry[1], grads
+                n_dump = k.reversible_segment(bw, lo, hi, ck[slot], ck[slot + 1])
+                if any(acc is not None for acc in by_role):
+                    k.reversible_param_grads(bw, lo, n_dump)
+            return bw.carry[0] + bw.carry[1], grads
 
     def autograd_vjp(self, n, z, a, grads):
         with torch.enable_grad():
@@ -323,6 +309,22 @@ class _ReversibleAdjoint(torch.autograd.Function):
         return (None, gy0) + tuple(gparams)
 
 
+def _mlp_kernels(X, mlp_params, z0, params):
+    """``MlpFieldKernels`` of the recognised MLP field, or None when its kernels cannot serve the problem: a dtype other
+    than fp32 / fp64, a parameter or the control on another dtype or device, or (``params`` not None: the adjoint
+    backward) a parameter that is not the MLP's own.  Shapes are the C dispatch's call, at the first launch."""
+    if z0.dtype not in (torch.float32, torch.float64):
+        return None
+    if any(p is not None and (p.dtype != z0.dtype or p.device != z0.device) for p in mlp_params):
+        return None
+    if params is not None and _roles(mlp_params, params) is None:
+        return None
+    try:
+        return MlpFieldKernels(X, mlp_params, z0)
+    except RuntimeError:
+        return None                      # the control's dtype or device: the torch operators report it as today
+
+
 def cdeint_reversible(X, func, z0, t, adjoint, kwargs):
     """``cdeint(..., backend="torchsde")``; ``kwargs`` as ``cdeint`` received them (tolerances injected)."""
     dt = _check_arguments(z0, t, kwargs)
@@ -350,17 +352,23 @@ def cdeint_reversible(X, func, z0, t, adjoint, kwargs):
     differentiable = (z0,) + tuple(X.buffers()) + (tuple(func.parameters()) if isinstance(func, torch.nn.Module)
                                                     else ()) + params
     wants_grad = torch.is_grad_enabled() and any(isinstance(x, torch.Tensor) and x.requires_grad for x in differentiable)
+    grad_params = tuple(p for p in params if isinstance(p, torch.Tensor) and p.requires_grad)
 
     kernels = None
     if field_params is not None and (adjoint or not wants_grad) and z0.dtype in (torch.float32, torch.float64):
         kernels = LinearFieldKernels(X, field_params[0], field_params[1], z0)
+    elif sig is not None and not is_prod and (adjoint or not wants_grad):
+        # the examples' MLP field: its kernels serve the forward and, for its own parameters, the backward; anything else
+        # keeps the torch-operator forward and the per-step autograd backward
+        mlp_params = mlp_field_of(func, z0, sig[2], times)
+        if mlp_params is not None:
+            kernels = _mlp_kernels(X, mlp_params, z0, grad_params if wants_grad else None)
     problem = _Problem(X, func, z0, t, dt, kernels, params)
     if not wants_grad:
         with torch.no_grad():
             return problem.forward(z0)[0]
     if adjoint:
-        params = tuple(p for p in params if isinstance(p, torch.Tensor) and p.requires_grad)
-        problem.params = params
-        return _ReversibleAdjoint.apply(problem, z0, *params)
+        problem.params = grad_params
+        return _ReversibleAdjoint.apply(problem, z0, *grad_params)
     problem.kernels = None
     return problem.torch_forward(z0, keep_checkpoints=False)[0]
