@@ -419,6 +419,33 @@ TCDE_API int tcde_linear_combination(void* out, const void* base, const void* co
 TCDE_API int tcde_field_contract(const void* field, const void* dx, void* out, int64_t n_paths, int64_t hidden, int64_t channels,
                         int64_t dx_stride, double scale, int dtype, void* stream);
 
+/* Grouped forms of tcde_spline_eval and tcde_field_contract for the members of a TupleControl (misc.py:129-166) and a
+ * tuple state (solver.py:131-133): one launch serves every member, each with its own sizes and pointers, and every
+ * output element is bit-equal to the single-member entry's on that member alone.  `members` is a HOST array read at
+ * launch; up to 16 members go in one launch, a longer list is launched in chunks of 16.  A member with no output
+ * elements may carry NULL pointers.  All members share `dtype` (and, for the evaluation, `derivative`). */
+typedef struct tcde_spline_member {
+    const void* control;       /* as tcde_spline_eval: rows [n_paths][n_rows][4C] (cubic) or [n_paths][n_rows][C] (linear) */
+    const void* knot_t;        /* linear: knots [n_rows] (NULL = 0, 1, 2, ...); unused for cubic */
+    const int32_t* index;      /* [n_times] interval index of every query, located on the host from THIS member's knots */
+    const void* frac;          /* [n_times] */
+    void* out;                 /* [n_paths][n_times][channels] */
+    int64_t n_paths, n_rows, channels, n_times;
+    int32_t control_kind, reserved;
+} tcde_spline_member;
+TCDE_API int tcde_spline_eval_grouped(const tcde_spline_member* members, int n_members, int derivative, int dtype,
+                                      void* stream);
+
+typedef struct tcde_contract_member {
+    const void* field;         /* [n_paths][hidden][channels] contiguous */
+    const void* dx;            /* dx[p * dx_stride + c] */
+    void* out;                 /* [n_paths][hidden] */
+    int64_t n_paths, hidden, channels, dx_stride;
+} tcde_contract_member;
+/* out_k = scale * field_k @ dx_k for every member k, as tcde_field_contract computes it */
+TCDE_API int tcde_field_contract_grouped(const tcde_contract_member* members, int n_members, double scale, int dtype,
+                                         void* stream);
+
 /* The error ratio of one attempted step (rk_common._compute_error_ratio, restated): with
  * err = sum_j coefs[j] * terms[j] and tol = atol + rtol * max(|y0|, |y1|), partials[c] receives the sum over
  * CTA c's elements of (err / tol)^2; the RMS norm is sqrt(sum(partials) / n).  partials: device double

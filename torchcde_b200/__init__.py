@@ -3,7 +3,7 @@
 Drop-in names (reference torchcde/__init__.py:1-9): ``cdeint``, ``CubicSpline``,
 ``LinearInterpolation``, ``natural_cubic_coeffs``, ``natural_cubic_spline_coeffs``,
 ``linear_interpolation_coeffs``, ``hermite_cubic_coefficients_with_backward_differences``,
-``InterpolationBase``.  The arithmetic lives in hand-written CUDA behind the C ABI of
+``InterpolationBase``, ``TupleControl``.  The arithmetic lives in hand-written CUDA behind the C ABI of
 ``include/torchcde_b200.h``; this package is the thin Python host layer.  CUDA tensors only:
 there is no CPU path and no PyTorch-eager fallback.
 
@@ -13,12 +13,13 @@ dopri5 with ``adjoint=True``) evaluates the field in one launch and each adjoint
 (fp32, hidden * channels <= 32, width <= 128).
 ``cdeint(..., backend="torchsde", method="reversible_heun")`` is torchsde's reversible Heun method with an exact,
 checkpointed reversible backward (``reversible.py``); the other torchsde methods are not built.
-Not provided (outside the hot path, SURVEY.md section 2): ``TupleControl``.
+``TupleControl`` drives one CDE with several controls; ``cdeint`` takes the matching tuple state, packs its members
+into one buffer and serves every member's dX/dt and ``f_i @ dX_i`` with one grouped launch each (``tuple_solver.py``).
 """
 from . import misc
 from .coeffs import (hermite_cubic_coefficients_with_backward_differences, linear_interpolation_coeffs,
                      natural_cubic_coeffs, natural_cubic_spline_coeffs)
-from .controls import CubicSpline, InterpolationBase, LinearInterpolation, NaturalCubicSpline
+from .controls import CubicSpline, InterpolationBase, LinearInterpolation, NaturalCubicSpline, TupleControl
 from .log_ode import logsig_windows, logsignature_windows
 from .solver import LinearVectorField, cdeint
 
@@ -28,4 +29,5 @@ __all__ = [
     "InterpolationBase", "natural_cubic_spline_coeffs", "natural_cubic_coeffs", "CubicSpline",
     "linear_interpolation_coeffs", "LinearInterpolation", "hermite_cubic_coefficients_with_backward_differences",
     "logsignature_windows", "logsig_windows", "cdeint", "LinearVectorField", "NaturalCubicSpline", "misc",
+    "TupleControl",
 ]

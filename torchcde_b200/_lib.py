@@ -21,6 +21,18 @@ FLAG_NAN_SEEN, FLAG_NAN_TIME, FLAG_NAN_FIRST_ROW = 1, 2, 4
 
 _p, _i64, _i32, _int, _dbl = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int32, ctypes.c_int, ctypes.c_double
 
+
+class SplineMember(ctypes.Structure):
+    """``tcde_spline_member``: one member of ``tcde_spline_eval_grouped``."""
+    _fields_ = [("control", _p), ("knot_t", _p), ("index", _p), ("frac", _p), ("out", _p), ("n_paths", _i64),
+                ("n_rows", _i64), ("channels", _i64), ("n_times", _i64), ("control_kind", _i32), ("reserved", _i32)]
+
+
+class ContractMember(ctypes.Structure):
+    """``tcde_contract_member``: one member of ``tcde_field_contract_grouped``."""
+    _fields_ = [("field", _p), ("dx", _p), ("out", _p), ("n_paths", _i64), ("hidden", _i64), ("channels", _i64),
+                ("dx_stride", _i64)]
+
 # name -> argtypes; must list every entry point the header declares (tests/test_abi.py checks)
 SIGNATURES = {
     "tcde_abi_version": ([], _int),
@@ -28,6 +40,8 @@ SIGNATURES = {
     "tcde_device_info": ([_p, _p, _p], _int),
     "tcde_hermite_bdiff_coeffs": ([_p, _p, _p, _i64, _i64, _i64, _int, _p, _p], _int),
     "tcde_field_contract": ([_p, _p, _p, _i64, _i64, _i64, _i64, ctypes.c_double, _int, _p], _int),
+    "tcde_spline_eval_grouped": ([ctypes.POINTER(SplineMember), _int, _int, _int, _p], _int),
+    "tcde_field_contract_grouped": ([ctypes.POINTER(ContractMember), _int, _dbl, _int, _p], _int),
     "tcde_hermite_bdiff_coeffs_series": ([_p, _p, _p, _i64, _i64, _i64, _int, _p, _p], _int),
     "tcde_linear_fill": ([_p, _p, _p, _i64, _i64, _i64, _int, _p, _p], _int),
     "tcde_nan_flag": ([_p, _i64, _int, _p, _p], _int),

@@ -57,6 +57,32 @@ def _rms(x):
     return float(x.detach().pow(2).mean().sqrt())
 
 
+# The error norm of a tuple state (TupleControl).  torchdiffeq flattens a tuple ``y0`` into one vector and, unless told
+# otherwise, measures its adaptive steps with the *mixed* norm: the largest of the members' RMS norms, for the error ratio
+# and for the initial step alike (_impl/misc.py ``_mixed_norm`` -- recalled, not verified: torchdiffeq is not installed
+# here, see DESIGN.md section 3).  This switch is the one place that choice is made; "rms" would measure the packed state
+# as one tensor.
+TUPLE_NORM = "mixed"
+
+
+class MixedNorm:
+    """max over the segments of a packed vector (``sizes`` elements each, end to end) of each segment's RMS; a segment
+    without elements contributes nothing."""
+
+    def __init__(self, sizes):
+        self.sizes = [int(n) for n in sizes]
+        self.offsets = [sum(self.sizes[:i]) for i in range(len(self.sizes))]
+
+    def __call__(self, x):
+        flat = x.detach().reshape(-1)
+        return max((_rms(flat[o:o + n]) for o, n in zip(self.offsets, self.sizes) if n), default=0.0)
+
+
+def tuple_norm(sizes):
+    """The norm of a packed tuple state whose members have ``sizes`` elements (see ``TUPLE_NORM``)."""
+    return MixedNorm(sizes) if TUPLE_NORM == "mixed" else _rms
+
+
 def _kernels_apply(*tensors):
     """The single-launch kernels serve plain CUDA float tensors of one shape outside autograd; anything else
     (CPU tensors, states that are being differentiated with adjoint=False) keeps the torch operators."""
@@ -103,6 +129,28 @@ def _error_ratio(y0, y1, ks, weights, dt, atol, rtol, norm):
     launch of ``tcde_error_ratio_sumsq`` plus the sum of its per-CTA partials (the one host read per attempt)."""
     pairs = [(k, w * dt) for k, w in zip(ks, weights) if w != 0.0]
     terms = [k for k, _ in pairs]
+    if isinstance(norm, MixedNorm) and terms and len(terms) <= 7 and _kernels_apply(y0, y1, *terms):
+        # one tcde_error_ratio_sumsq per member range of the packed state, one host read for all of them
+        lib, size = _lib.load(), y0.element_size()
+        segs = [(o, n) for o, n in zip(norm.offsets, norm.sizes) if n]
+        n_parts = [lib.tcde_error_ratio_partials(n) for _, n in segs]
+        partials = torch.empty(sum(n_parts), dtype=torch.float64, device=y0.device)
+        coefs = [c for _, c in pairs]
+        at = 0
+        with torch.cuda.device(y0.device):
+            for (o, n), m in zip(segs, n_parts):
+                _, cf, n_terms = _term_arrays(terms, coefs)
+                ptrs = (ctypes.c_void_p * n_terms)(*[k.data_ptr() + o * size for k in terms])
+                _lib.call("tcde_error_ratio_sumsq", ctypes.c_void_p(y0.data_ptr() + o * size),
+                          ctypes.c_void_p(y1.data_ptr() + o * size), ptrs, cf, n_terms, float(atol), float(rtol), n,
+                          _lib.dtype_code(y0.dtype), ctypes.c_void_p(partials.data_ptr() + at * 8), _lib.stream_of(y0))
+                at += m
+        sums = partials.cpu().tolist()
+        ratios, at = [], 0
+        for (_, n), m in zip(segs, n_parts):
+            ratios.append(math.sqrt(math.fsum(sums[at:at + m]) / n))
+            at += m
+        return max(ratios, default=0.0)
     if norm is _rms and terms and len(terms) <= 7 and _kernels_apply(y0, y1, *terms):
         n_part = _lib.load().tcde_error_ratio_partials(y0.numel())
         partials = torch.empty(n_part, dtype=torch.float64, device=y0.device)
@@ -116,14 +164,14 @@ def _error_ratio(y0, y1, ks, weights, dt, atol, rtol, norm):
     return norm(err / tol)
 
 
-def _initial_step(field, t0, y0, f0, rtol, atol):
+def _initial_step(field, t0, y0, f0, rtol, atol, norm=_rms):
     """Hairer's starting step (torchdiffeq ``_select_initial_step`` with order - 1 = 4)."""
     scale = atol + y0.abs() * rtol
-    d0 = _rms(y0 / scale)
-    d1 = _rms(f0 / scale)
+    d0 = norm(y0 / scale)
+    d1 = norm(f0 / scale)
     h0 = 1e-6 if (d0 < 1e-5 or d1 < 1e-5) else 0.01 * d0 / d1
     f1 = field(t0 + h0, y0 + h0 * f0)
-    d2 = _rms((f1 - f0) / scale) / h0
+    d2 = norm((f1 - f0) / scale) / h0
     if d1 <= 1e-15 and d2 <= 1e-15:
         h1 = max(1e-6, h0 * 1e-3)
     else:
@@ -172,7 +220,7 @@ class Dopri5:
         y0 = self.y0
         f0 = self.field(t0, y0)
         dt = self.first_step if self.first_step is not None else _initial_step(self.field, t0, y0, f0, self.rtol,
-                                                                               self.atol)
+                                                                               self.atol, self.norm)
         t_lo, t_hi = t0, t0
         coeff = None
         jumps = [v for v in self.jump_t if v > t0]
@@ -222,14 +270,14 @@ class Dopri5:
         return total
 
 
-def odeint_dopri5(field, y0, times, rtol, atol, options=None, targets=None):
-    """``times``: increasing Python floats.  Returns (len(times), *y0.shape)."""
+def odeint_dopri5(field, y0, times, rtol, atol, options=None, targets=None, norm=None):
+    """``times``: increasing Python floats.  Returns (len(times), *y0.shape).  ``norm``: the error norm (default RMS)."""
     options = dict(options or {})
     jump_t = options.pop("jump_t", None)
     if isinstance(jump_t, torch.Tensor):
         jump_t = jump_t.detach().cpu().tolist()
     solver = Dopri5(field, y0, rtol, atol, first_step=options.pop("first_step", None),
-                    max_num_steps=options.pop("max_num_steps", 2 ** 31 - 1), jump_t=jump_t)
+                    max_num_steps=options.pop("max_num_steps", 2 ** 31 - 1), norm=norm, jump_t=jump_t)
     if options:
         raise NotImplementedError("dopri5: unsupported options {}".format(sorted(options)))
     out = solver.integrate(list(times), targets)

@@ -220,3 +220,55 @@ class LinearInterpolation(InterpolationBase):
 
     def derivative(self, t):
         return self._eval(t, True)
+
+
+class TupleControl(torch.nn.Module):
+    """Several controls over one interval, for a CDE with a tuple state (misc.py:129-166): ``interval``,
+    ``evaluate(t)`` and ``derivative(t)`` answer with a tuple of the members' answers, and ``grid_points`` is the grid
+    the members share.  The members sit in a ``ModuleList`` named ``controls``, so ``state_dict`` keys are the
+    reference's.  A member is any object with ``interval``, ``grid_points`` and ``derivative`` (when one is not a module the
+    members are kept in a plain tuple instead).  ``cdeint`` evaluates
+    the members that are this package's own controls together, in one launch (``tcde_spline_eval_grouped``)."""
+
+    def __init__(self, *controls):
+        super(TupleControl, self).__init__()
+
+        if len(controls) == 0:
+            raise ValueError("Expected one or more controls to batch together.")
+
+        self._interval = controls[0].interval
+        grid_points = controls[0].grid_points
+        same_grid_points = True
+        for control in controls[1:]:
+            if (control.interval != self._interval).any():
+                raise ValueError("Can only batch togehter controls over the same interval.")
+            # (grids of different lengths are different grids; the reference's elementwise ``!=`` would not broadcast)
+            other = control.grid_points
+            if same_grid_points and (other.shape != grid_points.shape or (other != grid_points).any()):
+                same_grid_points = False
+
+        if same_grid_points:
+            self._grid_points = grid_points
+        else:
+            self._grid_points = None
+
+        if all(isinstance(control, torch.nn.Module) for control in controls):
+            self.controls = torch.nn.ModuleList(controls)
+        else:
+            self.controls = tuple(controls)        # a member that is not a module has no state to register
+
+    @property
+    def interval(self):
+        return self._interval
+
+    @property
+    def grid_points(self):
+        if self._grid_points is None:
+            raise RuntimeError("Batch of controls have different grid points.")
+        return self._grid_points
+
+    def evaluate(self, t):
+        return tuple(control.evaluate(t) for control in self.controls)
+
+    def derivative(self, t):
+        return tuple(control.derivative(t) for control in self.controls)

@@ -3,7 +3,7 @@
 // that the results are bit-identical to the reference's chain of torch ops.  The interval
 // index and fraction of every query come from the host (torchcde_b200/schedule.py runs the
 // reference's own bucketize arithmetic, which is what makes the indices bit-exact).
-#include "common.cuh"
+#include "spline_point.cuh"
 
 namespace tcde {
 
@@ -12,35 +12,13 @@ __global__ void __launch_bounds__(256)
 spline_eval_kernel(const T* __restrict__ control, const T* __restrict__ knot_t, const int32_t* __restrict__ index,
                    const T* __restrict__ frac, T* __restrict__ out, int64_t total, int64_t n_rows, int C,
                    int64_t n_times, int cubic, int derivative) {
-    using E = exact<T>;
     const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (e >= total) return;
     const int c = (int)(e % C);
     const int64_t pj = e / C;
     const int64_t j = pj % n_times;
     const int64_t p = pj / n_times;
-    const int idx = index[j];
-    const T f = frac[j];
-    T v;
-    if (cubic) {
-        const T* r = control + (p * n_rows + idx) * 4 * C + c;
-        const T b = r[C], two_c = r[2 * C], three_d = r[3 * C];
-        if (derivative) {
-            v = E::add(b, E::mul(E::add(two_c, E::mul(three_d, f)), f));
-        } else {
-            T inner = E::add(E::mul(T(0.5), two_c), E::div(E::mul(three_d, f), T(3)));
-            inner = E::add(b, E::mul(inner, f));
-            v = E::add(r[0], E::mul(inner, f));
-        }
-    } else {
-        const T* r = control + (p * n_rows + idx) * C + c;
-        const T lo = r[0], hi = r[C];
-        const T t0 = knot_t ? knot_t[idx] : T(idx), t1 = knot_t ? knot_t[idx + 1] : T(idx + 1);
-        const T width = E::sub(t1, t0);
-        if (derivative) v = E::div(E::sub(hi, lo), width);
-        else v = E::add(lo, E::div(E::mul(f, E::sub(hi, lo)), width));
-    }
-    out[e] = v;
+    out[e] = spline_point(control, knot_t, p, n_rows, C, c, index[j], frac[j], cubic, derivative);
 }
 
 }  // namespace tcde

@@ -1,4 +1,5 @@
-"""The reference's ``torchcde.misc`` names that sit on the hot path (misc.py:70-126)."""
+"""The reference's ``torchcde.misc`` names (misc.py:70-166)."""
 from .coeffs import forward_fill, validate_input_path
+from .controls import TupleControl
 
-__all__ = ["forward_fill", "validate_input_path"]
+__all__ = ["forward_fill", "validate_input_path", "TupleControl"]

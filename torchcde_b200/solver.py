@@ -317,6 +317,40 @@ def _torch_field(X, func, is_prod, known_control, z0):
     return field
 
 
+def _warn_control_gradients(X, adjoint, kwargs):
+    """The reference's warning (solver.py:198-213) when the control needs a gradient the adjoint will not give it."""
+    if not (adjoint and 'adjoint_params' not in kwargs):
+        return
+    for buffer in X.buffers():
+        if buffer.requires_grad:
+            warnings.warn("One of the inputs to the control path X requires gradients but "
+                          "`kwargs['adjoint_params']` has not been passed. This is probably a mistake: these "
+                          "inputs will not receive a gradient when using the adjoint method. Either have the input "
+                          "not require gradients (if that was unintended), or include it (and every other "
+                          "parameter needing gradients) in `adjoint_params`. For example:\n"
+                          "```\n"
+                          "coeffs = ...\n"
+                          "func = ...\n"
+                          "X = CubicSpline(coeffs)\n"
+                          "adjoint_params = tuple(func.parameters()) + (coeffs,)\n"
+                          "cdeint(X=X, func=func, ..., adjoint_params=adjoint_params)\n"
+                          "```")
+
+
+def _oriented_times(times, method, options):
+    """A decreasing ``t`` is solved as the increasing ``-t`` (torchdiffeq's reversal); ``options["jump_t"]`` follows."""
+    flipped = len(times) > 1 and times[0] > times[1]
+    if flipped:
+        times = [-v for v in times]
+    if any(b <= a for a, b in zip(times[:-1], times[1:])):
+        raise ValueError("t must be strictly increasing or decreasing")
+    if method == "dopri5" and options.get("jump_t", None) is not None:
+        jumps = options["jump_t"]
+        jumps = jumps.detach().cpu().tolist() if isinstance(jumps, torch.Tensor) else list(jumps)
+        options["jump_t"] = sorted(-float(v) for v in jumps) if flipped else sorted(float(v) for v in jumps)
+    return times, flipped
+
+
 def _time_first_to_reference_layout(out):
     dims = range(1, out.dim() - 1)
     return out.permute(*dims, 0, -1)
@@ -363,11 +397,12 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
 
     if not hasattr(X, 'derivative'):
         raise ValueError("X must have a 'derivative' method.")
-    if isinstance(z0, (tuple, list)):
-        raise NotImplementedError("torchcde_b200.cdeint: tuple / list states (TupleControl) are outside the fused hot "
-                                  "path; pass a single tensor state.")
-    if not isinstance(z0, torch.Tensor):
+    is_tuple = isinstance(z0, (tuple, list))
+    if not is_tuple and not isinstance(z0, torch.Tensor):
         raise ValueError("z0 must either a tensor or a tuple/list of tensors.")
+    if backend == "torchsde" and is_tuple:
+        raise NotImplementedError("torchcde_b200.cdeint: backend='torchsde' is built for a single tensor state; a tuple / "
+                                  "list state (TupleControl) runs with backend='torchdiffeq'.")
     if backend == "torchsde":
         if not isinstance(t, torch.Tensor):
             t = torch.as_tensor(t)
@@ -396,21 +431,14 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     # schedule -- grid, interval index of every stage -- is host arithmetic, like torchdiffeq's own grid construction)
     times = [float(v) for v in t.detach().cpu().tolist()]
 
-    if adjoint and 'adjoint_params' not in kwargs:
-        for buffer in X.buffers():
-            if buffer.requires_grad:
-                warnings.warn("One of the inputs to the control path X requires gradients but "
-                              "`kwargs['adjoint_params']` has not been passed. This is probably a mistake: these "
-                              "inputs will not receive a gradient when using the adjoint method. Either have the input "
-                              "not require gradients (if that was unintended), or include it (and every other "
-                              "parameter needing gradients) in `adjoint_params`. For example:\n"
-                              "```\n"
-                              "coeffs = ...\n"
-                              "func = ...\n"
-                              "X = CubicSpline(coeffs)\n"
-                              "adjoint_params = tuple(func.parameters()) + (coeffs,)\n"
-                              "cdeint(X=X, func=func, ..., adjoint_params=adjoint_params)\n"
-                              "```")
+    if is_tuple:
+        # one CDE driven by several controls (TupleControl): the members packed into one state (tuple_solver.py)
+        from .tuple_solver import cdeint_tuple
+        _warn_control_gradients(X, adjoint, kwargs)
+        times, flipped = _oriented_times(times, method, options)
+        return cdeint_tuple(X, func, z0, t, adjoint, kwargs, method, step_size, use_graph, options, times, flipped,
+                            is_prod)
+    _warn_control_gradients(X, adjoint, kwargs)
 
     # ---- what kind of problem is this? -----------------------------------------------------------
     field_params = None
@@ -448,15 +476,7 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     wants_grad = torch.is_grad_enabled() and any(isinstance(x, torch.Tensor) and x.requires_grad
                                                  for x in differentiable)
 
-    flipped = len(times) > 1 and times[0] > times[1]
-    if flipped:
-        times = [-v for v in times]
-    if any(b <= a for a, b in zip(times[:-1], times[1:])):
-        raise ValueError("t must be strictly increasing or decreasing")
-    if method == "dopri5" and options.get("jump_t", None) is not None:
-        jumps = options["jump_t"]
-        jumps = jumps.detach().cpu().tolist() if isinstance(jumps, torch.Tensor) else list(jumps)
-        options["jump_t"] = sorted(-float(v) for v in jumps) if flipped else sorted(float(v) for v in jumps)
+    times, flipped = _oriented_times(times, method, options)
 
     def autograd_field():
         f = _torch_field(X, func, is_prod, sig is not None, z0)
