@@ -492,6 +492,43 @@ TCDE_API int tcde_dopri5_linear_paired_attempts(const void* control, int control
                                        int32_t* q_index, void* q_frac, void* q_weight, int64_t max_slots, int64_t first_seq,
                                        int64_t n_launches, int dtype, void* stream);
 
+/* The forward pass of cdeint(adjoint=False) with dopri5 for the linear field when gradients are wanted: the attempts of
+ * tcde_dopri5_linear_attempts (same outputs, same accepted and rejected steps, bit for bit) that also record what the
+ * backward pass needs.  Every attempt writes into slot [accepted steps so far - ctl field 16] (a rejected attempt is
+ * overwritten by the next one):
+ *   rec_step  double [max_slots][2]: (t, dt) of the step
+ *   rec_index int32 / rec_frac float [max_slots][6]: spline interval and fraction of stages 2..7 (stage 7 at t + dt)
+ *   rec_z     float  [max_slots][6][n_paths][32]: the inputs of stages 2..7, the last one being the step's result; may be NULL
+ *             (no parameter gradient wanted)
+ * When the slots are full the solve pauses as in tcde_dopri5_linear_paired_attempts (done = 1, field 15 = 1): the caller
+ * keeps the filled record, passes fresh storage, sets field 16 to the number of accepted steps, clears fields 6 and 15 of
+ * the slot just read and enqueues more launches.  Same support as tcde_dopri5_linear_attempts; rec_z 16-byte aligned. */
+TCDE_API int tcde_dopri5_linear_record_attempts(const void* control, int control_kind, int64_t n_rows, const void* knots,
+                                       const void* weight, const void* bias, void* state, void* partials, void* ctl, void* out,
+                                       const void* out_times, int64_t n_out, int64_t n_paths, int64_t channels, int64_t hidden,
+                                       double sign, void* rec_z, void* rec_step, int32_t* rec_index, void* rec_frac,
+                                       int64_t max_slots, int64_t first_seq, int64_t n_launches, int dtype, void* stream);
+
+/* The backward pass of that record over n_steps accepted steps, last to first, in ONE launch: the transposed
+ * Dormand-Prince recurrence of the linear field (J^T by the field product on weight_t = W.view(H,C,H).permute(2,1,0)
+ * .reshape(H*C,H) with a zero bias).
+ *   grad_out  float [n_paths][n_out][32]: dL/d(outputs)
+ *   carry     float [2][n_paths][32]: in, the cotangent of the state after the last step and the cotangent still pending on
+ *             that step's last evaluation (zero for the last step of the solve); out, the same at the first step's start
+ *             (the second is the cotangent of the start slope f(t0, z0), whose J^T and parameter gradients are the caller's)
+ *   kappa     float [n_steps][6][n_paths][32] or NULL: the cotangent of every evaluation, in the item of its input in rec_z,
+ *             for tcde_linear_field_param_grads with item weight = sign
+ *   coef      float [n_steps][36]: (float)(beta[s][j] * dt) of the Dormand-Prince tableau, rows s = 0..5, zero padded
+ *   stage_index / stage_frac [n_steps][6]: the record's
+ *   inj_range int32 [n_steps + 1], inj_out int32 [n_inj], inj_w float [n_inj][8]: the outputs step n emits and their
+ *             weights on (y_n, y_{n+1}, k1, k3, k4, k5, k6, k7) -- the transposed dense output with y_mid folded in
+ * Same support as tcde_dopri5_linear_attempts; control, grad_out, carry and kappa 16-byte aligned. */
+TCDE_API int tcde_dopri5_linear_backward(const void* control, int control_kind, int64_t n_rows, const void* weight_t,
+                                const void* zeros, const void* grad_out, void* carry, void* kappa, const void* coef,
+                                const int32_t* stage_index, const void* stage_frac, const int32_t* inj_range,
+                                const int32_t* inj_out, const void* inj_w, int64_t n_out, int64_t n_steps, int64_t n_paths,
+                                int64_t channels, int64_t hidden, double sign, int dtype, void* stream);
+
 /* Logsignatures of windows of piecewise-linear paths -- replaces the per-window call of the optional third-party package
  * at torchcde/log_ode.py:56-58 (``signatory.Logsignature(depth)``, default "words" basis).  x [n_paths][length][channels]
  * (NaN free); window w spans the points window_index[w] .. window_index[w + 1] (device int32 [n_windows + 1]); words: device

@@ -94,6 +94,10 @@ SIGNATURES = {
                                             _p, _p, _p, _p, _p, _i64, _i64, _i64, _int, _p], _int),
     "tcde_dopri5_linear_attempts": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _dbl, _i64, _i64,
                                      _int, _p], _int),
+    "tcde_dopri5_linear_record_attempts": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _dbl,
+                                            _p, _p, _p, _p, _i64, _i64, _i64, _int, _p], _int),
+    "tcde_dopri5_linear_backward": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64, _i64, _i64, _i64,
+                                     _dbl, _int, _p], _int),
     "tcde_logsignature_max_terms": ([], _i64),
     "tcde_logsignature_windows": ([_p, _i64, _i64, _i64, _p, _i64, _int, _p, _i64, _p, _int, _p], _int),
     "tcde_set_solve_variant": ([_int], _int),

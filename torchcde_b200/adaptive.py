@@ -202,7 +202,7 @@ class Dopri5:
         # no step may straddle one, and the slope is re-evaluated just after it
         self.jump_t = sorted(float(v) for v in jump_t) if jump_t is not None else []
 
-    def _attempt(self, t0, dt, y0, f0):
+    def _stages(self, t0, dt, y0, f0):
         ks = [f0]
         y1 = y0
         for alpha, beta in zip(_ALPHA, _BETA):
@@ -210,17 +210,27 @@ class Dopri5:
             y1 = _combine(y0, ks, beta, dt)
             ks.append(self.field(ti, y1))
         # the last beta row equals the solution weights (FSAL): y1 is the 5th-order solution
+        return y1, ks
+
+    def _attempt(self, t0, dt, y0, f0):
+        y1, ks = self._stages(t0, dt, y0, f0)
         return y1, ks, _error_ratio(y0, y1, ks, _C_ERROR, dt, self.atol, self.rtol, self.norm)
 
-    def integrate(self, times, targets=None):
+    def integrate(self, times, targets=None, steps=None):
         """``targets``: optional 1-D tensor holding the same output times; when given, the dense output is evaluated at
-        the tensor entries so that autograd sees the dependence on the requested times (adjoint=False)."""
+        the tensor entries so that autograd sees the dependence on the requested times (adjoint=False).  ``steps``: the
+        accepted steps ``[(t, dt), ...]`` of an earlier solve of the same problem (``cdeint.last_stats["steps"]``); the
+        solve then takes exactly those steps, without the controller -- a replay of that discrete solve."""
         out = [self.y0]
         t0 = times[0]
         y0 = self.y0
         f0 = self.field(t0, y0)
-        dt = self.first_step if self.first_step is not None else _initial_step(self.field, t0, y0, f0, self.rtol,
-                                                                               self.atol, self.norm)
+        if steps is not None:
+            steps = list(steps)
+            dt = steps[0][1] if steps else 0.0
+        else:
+            dt = self.first_step if self.first_step is not None else _initial_step(self.field, t0, y0, f0, self.rtol,
+                                                                                   self.atol, self.norm)
         t_lo, t_hi = t0, t0
         coeff = None
         jumps = [v for v in self.jump_t if v > t0]
@@ -230,10 +240,17 @@ class Dopri5:
                 if tries >= self.max_num_steps:
                     raise RuntimeError("max_num_steps exceeded ({}>={})".format(tries, self.max_num_steps))
                 step = dt
-                on_jump = bool(jumps) and t_hi < jumps[0] < t_hi + dt
+                if steps is not None:
+                    if self.n_accepted == len(steps):
+                        raise RuntimeError("dopri5 replay: the recorded steps end at t = {}".format(t_hi))
+                    step = steps[self.n_accepted][1]
+                on_jump = bool(jumps) and t_hi < jumps[0] < t_hi + step
                 if on_jump:
                     step = jumps[0] - t_hi
-                y1, ks, ratio = self._attempt(t_hi, step, y0, f0)
+                if steps is None:
+                    y1, ks, ratio = self._attempt(t_hi, step, y0, f0)
+                else:                            # a recorded step: accepted, no error estimate
+                    (y1, ks), ratio = self._stages(t_hi, step, y0, f0), 0.0
                 if ratio <= 1:
                     t_new = jumps[0] if on_jump else t_hi + step
                     if t_new >= target:          # the dense output is only ever evaluated inside the last step
@@ -270,8 +287,9 @@ class Dopri5:
         return total
 
 
-def odeint_dopri5(field, y0, times, rtol, atol, options=None, targets=None, norm=None):
-    """``times``: increasing Python floats.  Returns (len(times), *y0.shape).  ``norm``: the error norm (default RMS)."""
+def odeint_dopri5(field, y0, times, rtol, atol, options=None, targets=None, norm=None, steps=None):
+    """``times``: increasing Python floats.  Returns (len(times), *y0.shape).  ``norm``: the error norm (default RMS).
+    ``steps``: replay these accepted ``(t, dt)`` instead of running the controller (``Dopri5.integrate``)."""
     options = dict(options or {})
     jump_t = options.pop("jump_t", None)
     if isinstance(jump_t, torch.Tensor):
@@ -280,7 +298,7 @@ def odeint_dopri5(field, y0, times, rtol, atol, options=None, targets=None, norm
                     max_num_steps=options.pop("max_num_steps", 2 ** 31 - 1), norm=norm, jump_t=jump_t)
     if options:
         raise NotImplementedError("dopri5: unsupported options {}".format(sorted(options)))
-    out = solver.integrate(list(times), targets)
+    out = solver.integrate(list(times), targets, steps)
     return out, solver
 
 
@@ -342,6 +360,44 @@ def device_controller(launch, field, v0, times, rtol, atol, first_step, underflo
             if not math.isfinite(float(last[CTL_DT])) or float(last[CTL_DT]) == 0.0 or seq > 10_000_000:
                 raise RuntimeError(underflow.format(float(last[CTL_T])))
     return out, last, {"n_accepted": int(last[CTL_NACC]), "n_rejected": int(last[CTL_NREJ]), "launches": seq}
+
+
+def dense_output_weights(x, dt):
+    """The weights of ``Dopri5._evaluate(Dopri5._fit(y0, y1, y_mid, f0, f1, dt), 0, 1, x)`` on (y0, y1, y_mid, f0, f1):
+    the dense output is linear in them."""
+    x2, x3, x4 = x * x, x * x * x, x * x * x * x
+    return (1.0 - 11.0 * x2 + 18.0 * x3 - 8.0 * x4, -5.0 * x2 + 14.0 * x3 - 8.0 * x4, 16.0 * x2 - 32.0 * x3 + 16.0 * x4,
+            dt * (x - 4.0 * x2 + 5.0 * x3 - 2.0 * x4), dt * (x2 - 3.0 * x3 + 2.0 * x4))
+
+
+def dopri5_backward_tables(steps, times):
+    """The host tables of ``tcde_dopri5_linear_backward`` for the accepted ``steps`` [(t, dt), ...] of a solve over the
+    increasing output times ``times``, in double, cast to float32 at the end:
+      coef [n, 36]: (float)(beta[s][j] * dt), the forward's own stage coefficients;
+      inj_range [n + 1], inj_out [m], inj_w [m, 8]: the outputs each step emits (the kernel's rule: the first accepted step
+      whose end is at or past the output time; output 0 is y(t0) itself) and their weights on (y_n, y_{n+1}, k1, k3, k4,
+      k5, k6, k7) -- ``dense_output_weights`` with y_mid = y_n + dt sum_j c_mid[j] k_j folded in."""
+    import numpy as np
+    n = len(steps)
+    dts = np.array([dt for _t, dt in steps], dtype=np.float64)
+    beta = np.zeros((6, 6))
+    for s, row in enumerate(_BETA):
+        beta[s, :len(row)] = row
+    coef = (beta.reshape(1, 36) * dts.reshape(n, 1)).astype(np.float32)
+    inj_range, inj_out, inj_w = [0], [], []
+    nxt = 1
+    for t, dt in steps:
+        t_hi = t + dt
+        while nxt < len(times) and times[nxt] <= t_hi:
+            w_y0, w_y1, w_ym, w_f0, w_f1 = dense_output_weights((times[nxt] - t) / (t_hi - t), dt)
+            cm = [c * dt * w_ym for c in _C_MID]
+            inj_out.append(nxt)
+            inj_w.append([w_y0 + w_ym, w_y1, w_f0 + cm[0], cm[2], cm[3], cm[4], cm[5], w_f1 + cm[6]])
+            nxt += 1
+        inj_range.append(len(inj_out))
+    return {"coef": torch.from_numpy(coef), "inj_range": torch.tensor(inj_range, dtype=torch.int32),
+            "inj_out": torch.tensor(inj_out or [0], dtype=torch.int32),
+            "inj_w": torch.tensor(inj_w or [[0.0] * 8], dtype=torch.float64).to(torch.float32)}
 
 
 # ------------------------------------------------------------------------- fixed grids (generic)

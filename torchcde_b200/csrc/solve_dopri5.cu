@@ -87,6 +87,12 @@ struct Args {
     float* q_frac;
     float* q_weight;
     int max_slots;
+    // recording mode (the forward pass of cdeint(adjoint=False) with gradients; null otherwise): every attempt leaves its
+    // step, its stage locations and the inputs of its six evaluations in slot [accepted steps so far - C_BASE]
+    float* rec_z;             // [max_slots][6][n_paths][32]: inputs of stages 2..7 (stage 7's is the step's result y1); may be null
+    double* rec_step;         // [max_slots][2]: (t, dt)
+    int32_t* rec_index;       // [max_slots][6]: spline interval and fraction of stages 2..7
+    float* rec_frac;
 };
 
 struct Smem {
@@ -137,7 +143,10 @@ __device__ __forceinline__ double next_step(double dt, double ratio) {          
     return dt * fmin(10.0, fmax(f, dfactor));
 }
 
-__global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args a) {
+// One launch of the solve.  RECORD: the recording mode (Args::rec_*); the kernels with RECORD = false are the plain and
+// paired modes.
+template <bool RECORD>
+__device__ __forceinline__ void attempt(const Args& a) {
     extern __shared__ unsigned char smem_unaligned[];
     unsigned char* smem = smem_unaligned + ((128u - (smem_u32(smem_unaligned) & 127u)) & 127u);
     Plan* plan = reinterpret_cast<Plan*>(smem + Smem::misc);
@@ -200,7 +209,7 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
         }
         int overflow = (int)in[C_OVERFLOW];
         const int base = (int)in[C_BASE];
-        if (a.weight2 != nullptr && !done && nacc - base >= a.max_slots) {   // no trajectory slot left for another attempt
+        if ((a.weight2 != nullptr || RECORD) && !done && nacc - base >= a.max_slots) {   // no trajectory slot left for another attempt
             overflow = 1;
             done = 1;
         }
@@ -220,6 +229,14 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
                 for (int j = 0; j < 6; ++j) p.cs[s][j] = (float)(c_beta[s][j] * dt);
                 const double ti = (c_alpha[s] == 1.0) ? t + dt : t + c_alpha[s] * dt;
                 locate_stage(a, ti, p.stage_index[s], p.stage_frac[s]);
+                if (RECORD && blockIdx.x == 0) {
+                    a.rec_index[p.slot * 6 + s] = p.stage_index[s];
+                    a.rec_frac[p.slot * 6 + s] = p.stage_frac[s];
+                }
+            }
+            if (RECORD && blockIdx.x == 0) {
+                a.rec_step[2 * p.slot] = t;
+                a.rec_step[2 * p.slot + 1] = dt;
             }
             for (int j = 0; j < 7; ++j) {
                 p.ce[j] = (float)(c_err[j] * dt);
@@ -329,6 +346,13 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
             for (int c4 = 0; c4 < 8; ++c4) dst[c4] = make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
         };
 
+        auto record_stage = [&](int k, const float* v) {         // input of stage k + 2 (0..5) of this attempt
+            if (!RECORD || !live || a.rec_z == nullptr) return;
+            float4* dst = reinterpret_cast<float4*>(a.rec_z + ((size_t)(plan->slot * 6 + k) * a.n_paths + path) * kHid);
+#pragma unroll
+            for (int c4 = 0; c4 < 8; ++c4) dst[c4] = make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
+        };
+
         auto fetch_row = [&](int idx) {
             const float* src = crow + (int64_t)idx * row_stride;
             const int parts = cubic ? 6 : 2;
@@ -383,11 +407,13 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
         // s = 0: k1
 #pragma unroll
         for (int h = 0; h < kHid; ++h) kv[h] = fmaf(plan->cs[0][0], k1[h], y[h]);
+        record_stage(0, kv);
         evaluate(kv, 0, kA, nothing);                                        // kA = k2
         // s = 1: k1, k2
 #pragma unroll
         for (int h = 0; h < kHid; ++h) kv[h] = fmaf(plan->cs[1][1], kA[h], fmaf(plan->cs[1][0], k1[h], y[h]));
         dump_stage(1, kv);
+        record_stage(1, kv);
         evaluate(kv, 1, kv, nothing);                                        // kv = k3
 #pragma unroll
         for (int h = 0; h < kHid; ++h) park[(size_t)(0 * kHid + h) * kRows] = kv[h];
@@ -396,6 +422,7 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
         for (int h = 0; h < kHid; ++h)
             kv[h] = fmaf(plan->cs[2][2], kv[h], fmaf(plan->cs[2][1], kA[h], fmaf(plan->cs[2][0], k1[h], y[h])));
         dump_stage(2, kv);
+        record_stage(2, kv);
         evaluate(kv, 2, kv, nothing);                                        // kv = k4
 #pragma unroll
         for (int h = 0; h < kHid; ++h) park[(size_t)(1 * kHid + h) * kRows] = kv[h];
@@ -407,6 +434,7 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
             kv[h] = fmaf(plan->cs[3][3], kv[h], v);
         }
         dump_stage(3, kv);
+        record_stage(3, kv);
         evaluate(kv, 3, kv, nothing);                                        // kv = k5
 #pragma unroll
         for (int h = 0; h < kHid; ++h) park[(size_t)(2 * kHid + h) * kRows] = kv[h];
@@ -419,6 +447,7 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
             kv[h] = fmaf(plan->cs[4][4], kv[h], v);
         }
         dump_stage(4, kv);
+        record_stage(4, kv);
         evaluate(kv, 4, kA, nothing);                                        // kA = k6 (k2 is not used again)
         // s = 5: the 5th-order solution y1 = y + dt (b1 k1 + b3 k3 + b4 k4 + b5 k5 + b6 k6); k7 = f(t + dt, y1)
         float y1[kHid];
@@ -430,6 +459,7 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
             v = fmaf(plan->cs[5][4], park[(size_t)(2 * kHid + h) * kRows], v);
             y1[h] = fmaf(plan->cs[5][5], kA[h], v);
         }
+        record_stage(5, y1);
         float e6[kHid];                                   // error estimate without its k7 term, formed in the MMAs' shadow
         evaluate(y1, 5, kv, [&] {
             if (live) {
@@ -489,6 +519,182 @@ __global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args 
     }
 }
 
+__global__ void __launch_bounds__(kThreads, 1) dopri5_attempt_kernel(const Args a) { attempt<false>(a); }
+__global__ void __launch_bounds__(kThreads, 1) dopri5_record_kernel(const Args a) { attempt<true>(a); }
+
+// ---- the backward pass of the recording mode: the transposed Dormand-Prince recurrence over the accepted steps --------
+//
+// For this linear field J = df/dz does not depend on z, so the cotangents need no forward state.  Per step n (last to
+// first), with A the cotangent of y_{n+1} and K the cotangent still pending on the evaluation k7 of step n (= k1 of step
+// n + 1, one evaluation under FSAL):
+//   kappa7 = K + injections;  Zbar7 = A + J7^T kappa7 + injections;  then stages 6 .. 2: kappa_i = the accumulated cotangent
+//   of k_i, Zbar_i = J_i^T kappa_i, and Zbar_i flows to y_n (weight 1) and to k_j, j < i (weight (float)(beta[i-2][j-1] dt));
+//   the new A is the cotangent of y_n, the new K that of k1.
+// The output cotangents enter through the transposed dense output (y_mid folded into y_n and the k_j on the host): weights
+// [y_n, y_{n+1}, k1, k3, k4, k5, k6, k7] per (step, output).  kappa_i goes to item 6n + i - 2 of the record, the slot of its
+// evaluation's input, for tcde_linear_field_param_grads.
+struct BwdArgs {
+    const float* control;
+    const float* weight_t;    // [256][32] W with rows regrouped as (k, c): the field product with it is J^T
+    const float* zeros;       // [256] zero bias
+    const float* grad_out;    // [n_paths][n_out][32]
+    float* carry;             // [2][n_paths][32]: (A, K) at step n_steps, replaced by (A, K) at step 0
+    float* kappa;             // [n_steps][6][n_paths][32], or null
+    const float* coef;        // [n_steps][36]: (float)(beta[s][j] dt_n), as the forward's Plan.cs
+    const int32_t* stage_index;   // [n_steps][6]: the forward's stage locations
+    const float* stage_frac;
+    const int32_t* inj_range;     // [n_steps + 1]: injections of step n are [inj_range[n], inj_range[n + 1])
+    const int32_t* inj_out;       // [n_inj]: output index
+    const float* inj_w;           // [n_inj][8]
+    int64_t n_paths, n_rows;
+    int control_kind, n_out, n_steps;
+    float sign;
+};
+enum { W_Y0 = 0, W_Y1, W_K1, W_K3, W_K4, W_K5, W_K6, W_K7 };
+
+struct BwdSmem {
+    static constexpr int b = 0;
+    static constexpr int a = (BSmem<1>::bytes + 127) & ~127;
+    static constexpr int park = a + (kThreads / 32) * WarpSmem<1>::bytes;   // [4][32][kThreads] floats: cotangents of k2..k5
+    static constexpr int total = park + 4 * kHid * kThreads * 4;
+};
+
+__global__ void __launch_bounds__(kThreads, 1) dopri5_backward_kernel(const BwdArgs a) {
+    extern __shared__ unsigned char smem_unaligned[];
+    unsigned char* smem = smem_unaligned + ((128u - (smem_u32(smem_unaligned) & 127u)) & 127u);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    float inv_w_scale, beta;
+    prepare_b<1>(smem + BwdSmem::b, a.weight_t, a.zeros, tid, kThreads, inv_w_scale, beta);
+    __syncthreads();
+    unsigned char* ws = smem + BwdSmem::a + warp * WarpSmem<1>::bytes;
+    float* park = reinterpret_cast<float*>(smem + BwdSmem::park) + tid;          // cotangent of k_j: park[((j - 2) * 32 + h) * kThreads]
+    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
+    const int row_stride = cubic ? 4 * kCh : kCh;
+    const size_t item = (size_t)a.n_paths * kHid;
+
+    for (int64_t w = (int64_t)blockIdx.x * (kThreads / 32) + warp; w * 32 < a.n_paths; w += (int64_t)gridDim.x * (kThreads / 32)) {
+        const int64_t path = w * 32 + lane;
+        const bool live = path < a.n_paths;
+        const int64_t lpath = live ? path : a.n_paths - 1;
+        const float* crow = a.control + lpath * a.n_rows * row_stride + (cubic ? kCh : 0);
+        const float* grow = a.grad_out + lpath * a.n_out * kHid;
+
+        // v = J^T v at stage location s of step n (every lane of the warp together)
+        auto transposed = [&](int n, int s, float* v) {
+            const int idx = a.stage_index[n * 6 + s];
+            const float frac = a.stage_frac[n * 6 + s];
+            const float4* src = reinterpret_cast<const float4*>(crow + (int64_t)idx * row_stride);
+            float dx[kCh];
+            if (cubic) {
+                float r[24];
+#pragma unroll
+                for (int j = 0; j < 6; ++j) {
+                    const float4 q = src[j];
+                    r[4 * j] = q.x; r[4 * j + 1] = q.y; r[4 * j + 2] = q.z; r[4 * j + 3] = q.w;
+                }
+#pragma unroll
+                for (int c = 0; c < kCh; ++c)
+                    dx[c] = __fmul_rn(__fadd_rn(r[c], __fmul_rn(__fadd_rn(r[8 + c], __fmul_rn(r[16 + c], frac)), frac)), a.sign);
+            } else {
+                const float4 q0 = src[0], q1 = src[1];
+                dx[0] = q0.x * a.sign; dx[1] = q0.y * a.sign; dx[2] = q0.z * a.sign; dx[3] = q0.w * a.sign;
+                dx[4] = q1.x * a.sign; dx[5] = q1.y * a.sign; dx[6] = q1.z * a.sign; dx[7] = q1.w * a.sign;
+            }
+            warp_field<1>(v, dx, v, ws, smem + BwdSmem::b, beta, inv_w_scale);
+        };
+        auto store = [&](float* dst, const float* v) {
+            if (!live || dst == nullptr) return;
+            float4* d = reinterpret_cast<float4*>(dst + path * kHid);
+#pragma unroll
+            for (int c4 = 0; c4 < 8; ++c4) d[c4] = make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
+        };
+        auto load = [&](const float* src, float* v) {
+            const float4* s4 = reinterpret_cast<const float4*>(src);
+#pragma unroll
+            for (int c4 = 0; c4 < 8; ++c4) {
+                const float4 q = s4[c4];
+                v[4 * c4] = q.x; v[4 * c4 + 1] = q.y; v[4 * c4 + 2] = q.z; v[4 * c4 + 3] = q.w;
+            }
+        };
+
+        float A[kHid], K[kHid], v[kHid];
+        load(a.carry + lpath * kHid, A);
+        load(a.carry + item + lpath * kHid, K);
+        for (int n = a.n_steps - 1; n >= 0; --n) {
+            const float* cs = a.coef + n * 36;
+            float* kap = a.kappa;                                      // null: no parameter gradient wanted
+            const int e0 = a.inj_range[n], e1 = a.inj_range[n + 1];
+            // stage 7: kappa7 = K + injections, then Zbar7 = A + J7^T kappa7 + injections (in A)
+#pragma unroll
+            for (int h = 0; h < kHid; ++h) v[h] = K[h];
+            for (int e = e0; e < e1; ++e) {
+                float gv[kHid];
+                load(grow + a.inj_out[e] * kHid, gv);
+                const float wk = a.inj_w[8 * e + W_K7];
+#pragma unroll
+                for (int h = 0; h < kHid; ++h) v[h] = fmaf(wk, gv[h], v[h]);
+            }
+            store(kap ? kap + ((size_t)n * 6 + 5) * item : nullptr, v);
+            transposed(n, 5, v);
+#pragma unroll
+            for (int h = 0; h < kHid; ++h) A[h] += v[h];
+            for (int e = e0; e < e1; ++e) {
+                float gv[kHid];
+                load(grow + a.inj_out[e] * kHid, gv);
+                const float wy = a.inj_w[8 * e + W_Y1];
+#pragma unroll
+                for (int h = 0; h < kHid; ++h) A[h] = fmaf(wy, gv[h], A[h]);
+            }
+            // Zbar7 -> y_n (K now holds ybar_n), k1 (v), k2..k5 (park), k6 (A)
+#pragma unroll
+            for (int h = 0; h < kHid; ++h) {
+                K[h] = A[h];
+                v[h] = cs[5 * 6 + 0] * A[h];
+#pragma unroll
+                for (int j = 2; j <= 5; ++j) park[((j - 2) * kHid + h) * kThreads] = cs[5 * 6 + j - 1] * A[h];
+                A[h] = cs[5 * 6 + 5] * A[h];
+            }
+            for (int e = e0; e < e1; ++e) {
+                float gv[kHid];
+                load(grow + a.inj_out[e] * kHid, gv);
+                const float* we = a.inj_w + 8 * e;
+#pragma unroll
+                for (int h = 0; h < kHid; ++h) {
+                    K[h] = fmaf(we[W_Y0], gv[h], K[h]);
+                    v[h] = fmaf(we[W_K1], gv[h], v[h]);
+#pragma unroll
+                    for (int j = 3; j <= 5; ++j)
+                        park[((j - 2) * kHid + h) * kThreads] = fmaf(we[W_K3 + j - 3], gv[h], park[((j - 2) * kHid + h) * kThreads]);
+                    A[h] = fmaf(we[W_K6], gv[h], A[h]);
+                }
+            }
+            // stages 6 .. 2: A = kappa_i on entry
+#pragma unroll
+            for (int i = 6; i >= 2; --i) {
+                store(kap ? kap + ((size_t)n * 6 + i - 2) * item : nullptr, A);
+                transposed(n, i - 2, A);                                   // A = Zbar_i
+                const float* c = cs + (i - 2) * 6;
+#pragma unroll
+                for (int h = 0; h < kHid; ++h) {
+                    K[h] += A[h];
+                    v[h] = fmaf(c[0], A[h], v[h]);
+#pragma unroll
+                    for (int j = 2; j <= i - 2; ++j)
+                        park[((j - 2) * kHid + h) * kThreads] = fmaf(c[j - 1], A[h], park[((j - 2) * kHid + h) * kThreads]);
+                    if (i > 2) A[h] = fmaf(c[i - 2], A[h], park[((i - 3) * kHid + h) * kThreads]);   // kappa_{i-1}
+                }
+            }
+#pragma unroll
+            for (int h = 0; h < kHid; ++h) {
+                A[h] = K[h];
+                K[h] = v[h];
+            }
+        }
+        store(a.carry, A);
+        store(a.carry + item, K);
+    }
+}
+
 }  // namespace dp5
 
 }  // namespace tcde
@@ -501,13 +707,14 @@ extern "C" int tcde_dopri5_linear_grid(int64_t n_paths) {
     return (int)(pairs < sm_count() ? pairs : sm_count());
 }
 
-static int launch_attempts(dp5::Args a, int64_t first_seq, int64_t n_launches, cudaStream_t s) {
+static int launch_attempts(dp5::Args a, int64_t first_seq, int64_t n_launches, cudaStream_t s,
+                           void (*kernel)(const dp5::Args) = dp5::dopri5_attempt_kernel) {
     constexpr int smem = dp5::Smem::total + 1024;
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(dp5::dopri5_attempt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     const int grid = tcde_dopri5_linear_grid(a.n_paths);
     for (int64_t i = 0; i < n_launches; ++i) {
         a.seq = (int)((first_seq + i) & 0x3fffffff);
-        dp5::dopri5_attempt_kernel<<<grid, dp5::kThreads, smem, s>>>(a);
+        kernel<<<grid, dp5::kThreads, smem, s>>>(a);
     }
     TCDE_CHECK_CUDA(cudaGetLastError());
     return TCDE_OK;
@@ -556,4 +763,56 @@ extern "C" int tcde_dopri5_linear_paired_attempts(const void* control, int contr
                 (int)n_out, 0, (float)sign, (const float*)weight2, (const float*)bias2, n_ctrl, (float*)dump_z, (float*)dump_a,
                 q_index, (float*)q_frac, (float*)q_weight, (int)max_slots};
     return launch_attempts(a, first_seq, n_launches, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int tcde_dopri5_linear_record_attempts(const void* control, int control_kind, int64_t n_rows, const void* knots,
+                                                  const void* weight, const void* bias, void* state, void* partials, void* ctl,
+                                                  void* out, const void* out_times, int64_t n_out, int64_t n_paths,
+                                                  int64_t channels, int64_t hidden, double sign, void* rec_z, void* rec_step,
+                                                  int32_t* rec_index, void* rec_frac, int64_t max_slots, int64_t first_seq,
+                                                  int64_t n_launches, int dtype, void* stream) {
+    TCDE_CHECK_ARG(control && knots && weight && bias && state && partials && ctl && out && out_times, "null pointer");
+    TCDE_CHECK_ARG(rec_step && rec_index && rec_frac && max_slots >= 1 && max_slots < (1ll << 24), "null record / bad slot count");
+    TCDE_CHECK_ARG(n_paths >= 1 && n_rows >= 1 && n_out >= 2 && n_launches >= 0 && first_seq >= 0, "bad sizes");
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d", control_kind);
+    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && hidden == dp5::kHid && channels == dp5::kCh,
+                         "device-controlled dopri5: built for float32, hidden=32, channels=8");
+    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(state) | reinterpret_cast<uintptr_t>(out) |
+                           reinterpret_cast<uintptr_t>(rec_z)) & 15) == 0,
+                         "device-controlled dopri5: control, state, out and the record must be 16-byte aligned");
+    TCDE_CHECK_SUPPORTED(n_paths * 32 * 6 * max_slots < (1ll << 40), "record too large");
+    dp5::Args a{(const float*)control, (const float*)knots, (const float*)weight, (const float*)bias, (float*)state,
+                (double*)partials, (double*)ctl, (float*)out, (const double*)out_times, n_paths, n_rows, control_kind,
+                (int)n_out, 0, (float)sign, nullptr, nullptr, n_paths, nullptr, nullptr, nullptr, nullptr, nullptr,
+                (int)max_slots, (float*)rec_z, (double*)rec_step, rec_index, (float*)rec_frac};
+    return launch_attempts(a, first_seq, n_launches, static_cast<cudaStream_t>(stream), dp5::dopri5_record_kernel);
+}
+
+extern "C" int tcde_dopri5_linear_backward(const void* control, int control_kind, int64_t n_rows, const void* weight_t,
+                                           const void* zeros, const void* grad_out, void* carry, void* kappa, const void* coef,
+                                           const int32_t* stage_index, const void* stage_frac, const int32_t* inj_range,
+                                           const int32_t* inj_out, const void* inj_w, int64_t n_out, int64_t n_steps,
+                                           int64_t n_paths, int64_t channels, int64_t hidden, double sign, int dtype,
+                                           void* stream) {
+    TCDE_CHECK_ARG(control && weight_t && zeros && grad_out && carry && coef && stage_index && stage_frac && inj_range &&
+                   (inj_out || n_steps == 0) && inj_w, "null pointer");
+    TCDE_CHECK_ARG(n_paths >= 1 && n_rows >= 1 && n_out >= 2 && n_steps >= 0 && n_steps < (1ll << 24), "bad sizes");
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d", control_kind);
+    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && hidden == dp5::kHid && channels == dp5::kCh,
+                         "dopri5 backward: built for float32, hidden=32, channels=8");
+    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(grad_out) | reinterpret_cast<uintptr_t>(carry) |
+                           reinterpret_cast<uintptr_t>(kappa)) & 15) == 0,
+                         "dopri5 backward: control, grad_out, carry and kappa must be 16-byte aligned");
+    if (n_steps == 0) return TCDE_OK;
+    dp5::BwdArgs a{(const float*)control, (const float*)weight_t, (const float*)zeros, (const float*)grad_out, (float*)carry,
+                   (float*)kappa, (const float*)coef, stage_index, (const float*)stage_frac, inj_range, inj_out,
+                   (const float*)inj_w, n_paths, n_rows, control_kind, (int)n_out, (int)n_steps, (float)sign};
+    constexpr int smem = dp5::BwdSmem::total + 1024;
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(dp5::dopri5_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const int64_t warps = (n_paths + 31) / 32;
+    const int64_t blocks = (warps + dp5::kThreads / 32 - 1) / (dp5::kThreads / 32);
+    const int grid = (int)(blocks < sm_count() ? blocks : sm_count());
+    dp5::dopri5_backward_kernel<<<grid, dp5::kThreads, smem, static_cast<cudaStream_t>(stream)>>>(a);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    return TCDE_OK;
 }

@@ -437,6 +437,185 @@ def fixed_backprop(kernels, z0, t, method, step_size, loop):
         return None
 
 
+class _NoRoom(Exception):
+    """The record of a recording dopri5 solve would not fit in the device memory."""
+
+
+class Dopri5Backprop:
+    """``cdeint(..., adjoint=False)`` of the device-controlled dopri5 solve of this linear field with gradients for z0, the
+    weight and / or the bias: the exact gradient of the discrete solve, without autograd.
+
+    The forward is the recording mode of the device controller (``tcde_dopri5_linear_record_attempts``: the outputs and
+    the accepted / rejected steps of the same call without gradients, bit for bit); every accepted step leaves its (t, dt),
+    its stage locations and, with a parameter gradient, the inputs of its six evaluations in a slot.  The slots come in
+    chunks of ``slots`` steps; a full chunk pauses the device, which resumes on a fresh chunk.  The backward is, per chunk
+    and last chunk first, ONE launch of ``tcde_dopri5_linear_backward`` (the transposed Dormand-Prince recurrence) and,
+    with a parameter gradient, ONE launch of ``tcde_linear_field_param_grads`` over (stage input, kappa); then one launch of
+    ``tcde_vector_field_linear_vjp`` closes the start slope f(t0, z0).  ``replay(steps)``: the differentiable
+    torch-operator solve of the same problem taking the recorded steps, which a backward with ``create_graph``
+    differentiates instead (the kernels give no higher-order derivatives; the forward cannot know which backward will
+    come, so it records either way).  Memory: the first chunk is checked before the solve starts, each further chunk when
+    the device pauses for it; a chunk that does not fit discards the partial solve and the caller runs the
+    torch-operator solve from the start."""
+
+    slots = 64                # accepted steps per record chunk
+
+    def __init__(self, kernels, times, rtol, atol, sign, first_step, replay, want_params):
+        self.kernels, self.times, self.rtol, self.atol = kernels, list(times), rtol, atol
+        self.sign, self.first_step, self.replay, self.want_params = float(sign), first_step, replay, want_params
+
+    def _chunk_bytes(self, n_paths):
+        return self.slots * 6 * n_paths * self.kernels.hidden * 4 if self.want_params else 0
+
+    def fits(self, n_paths):
+        """Whether one more record chunk, the kappa chunk of the backward and the parameter-gradient scratch fit in 0.7 of
+        the free device memory (the bound of ``FixedBackprop.fits``)."""
+        k = self.kernels
+        need = 2 * self._chunk_bytes(n_paths)
+        if self.want_params:
+            scratch_bytes = k.param_grad_scratch_bytes(n_paths, 6 * self.slots)
+            if scratch_bytes < 0:
+                return False
+            need += scratch_bytes
+        with torch.cuda.device(k.device):
+            free, _total = torch.cuda.mem_get_info()
+        return need <= 0.7 * free
+
+    def _new_chunk(self, n_paths):
+        k, dev = self.kernels, self.kernels.device
+        return {"z": torch.empty(self.slots * 6, n_paths, k.hidden, dtype=torch.float32, device=dev)
+                if self.want_params else None,
+                "step": torch.zeros(self.slots, 2, dtype=torch.float64, device=dev),
+                "index": torch.zeros(self.slots, 6, dtype=torch.int32, device=dev),
+                "frac": torch.zeros(self.slots, 6, dtype=torch.float32, device=dev)}
+
+    def forward(self, z0):
+        """(the outputs ``(..., len(times), H)``, the record: per chunk its stage inputs (None without a parameter
+        gradient), stage intervals and fractions).  The route keeps only the accepted steps on the host, so the record
+        lives exactly as long as its holder (the autograd Function saves it for the backward).  Raises ``_NoRoom``
+        (nothing kept) when the record does not fit."""
+        k = self.kernels
+        with torch.cuda.device(k.device):
+            yf = z0.detach().reshape(-1, k.hidden).contiguous()
+            n_paths = yf.size(0)
+            if not self.fits(n_paths):
+                raise _NoRoom()
+            field = k.field() if self.sign > 0 else _reverse(k.field())
+            knots = k.time_knots.detach().to(device=k.device, dtype=torch.float32).contiguous()
+            stream = _lib.stream_of(yf)
+            chunks = [self._new_chunk(n_paths)]
+
+            def launch(state, partials, ctl, out, out_times, first_seq):
+                c = chunks[-1]
+                _lib.call("tcde_dopri5_linear_record_attempts", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(knots),
+                          _lib.ptr(k.w), _lib.ptr(k.b), _lib.ptr(state), _lib.ptr(partials), _lib.ptr(ctl), _lib.ptr(out),
+                          _lib.ptr(out_times), len(self.times), n_paths, k.channels, k.hidden, self.sign, _lib.ptr(c["z"]),
+                          _lib.ptr(c["step"]), _lib.ptr(c["index"]), _lib.ptr(c["frac"]), self.slots, first_seq,
+                          adaptive._DEVICE_CHUNK, _lib.F32, stream)
+
+            def grow(last):                          # the chunk is full: the device resumes on a fresh one
+                if not self.fits(n_paths):
+                    raise _NoRoom()
+                chunks.append(self._new_chunk(n_paths))
+
+            out, _last, stats = adaptive.device_controller(
+                launch, field, yf, self.times, self.rtol, self.atol, self.first_step,
+                "dopri5: step size underflow / non-finite error estimate at t = {}", on_overflow=grow)
+            n_acc = stats["n_accepted"]
+            self.counts = [min(self.slots, n_acc - i * self.slots) for i in range(len(chunks))]
+            steps = torch.cat([c["step"][:n] for c, n in zip(chunks, self.counts)]).cpu()
+            self.steps = [(float(t), float(dt)) for t, dt in steps.tolist()]
+        self.stats = dict(stats, device_controlled=True, steps=list(self.steps))
+        record = [(c["z"], c["index"], c["frac"]) for c in chunks]
+        return out.view(*z0.shape[:-1], len(self.times), k.hidden), record
+
+    def backward(self, g, z0, record, want_w, want_b):
+        """(dL/dz0, dL/dW or None, dL/db or None) for output gradients ``g`` ``(..., len(times), H)`` from the solve of
+        ``z0`` and its ``record`` (``forward``'s)."""
+        k = self.kernels
+        hidden, dev, n_out = k.hidden, k.device, len(self.times)
+        with torch.cuda.device(dev):
+            gf = g.reshape(-1, n_out, hidden)
+            if not gf.is_contiguous() or gf.data_ptr() % 16:
+                gf = gf.clone(memory_format=torch.contiguous_format)
+            n_paths = gf.size(0)
+            stream = _lib.stream_of(gf)
+            gw = torch.zeros_like(k.w) if want_w else None
+            gb = torch.zeros_like(k.b) if want_b else None
+            params = gw is not None or gb is not None
+            tables = adaptive.dopri5_backward_tables(self.steps, self.times)
+            coef, inj_range = tables["coef"].to(dev), tables["inj_range"].to(dev)
+            inj_out, inj_w = tables["inj_out"].to(dev), tables["inj_w"].to(dev)
+            w_t, zeros = k.transposed_weights
+            carry = torch.zeros(2, n_paths, hidden, dtype=torch.float32, device=dev)
+            kappa = torch.empty(self.slots * 6, n_paths, hidden, dtype=torch.float32, device=dev) if params else None
+            weights = torch.full((self.slots * 6,), self.sign, dtype=torch.float32, device=dev) if params else None
+            for i in range(len(record) - 1, -1, -1):
+                (stage_z, stage_index, stage_frac), n = record[i], self.counts[i]
+                lo = i * self.slots
+                if n <= 0:
+                    continue
+                _lib.call("tcde_dopri5_linear_backward", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(w_t),
+                          _lib.ptr(zeros), _lib.ptr(gf), _lib.ptr(carry), _lib.ptr(kappa), _lib.ptr(coef[lo:lo + n]),
+                          _lib.ptr(stage_index), _lib.ptr(stage_frac), _lib.ptr(inj_range[lo:lo + n + 1]), _lib.ptr(inj_out),
+                          _lib.ptr(inj_w), n_out, n, n_paths, k.channels, hidden, self.sign, _lib.F32, stream)
+                if params and not k.param_grads(stage_z, kappa, stage_index.view(-1), stage_frac.view(-1), weights, 6 * n,
+                                                gw, gb):
+                    raise RuntimeError("cdeint backward: the parameter-gradient kernel is not built for this problem")
+            # the start slope f(t0, z0): its cotangent is carry[1]
+            index, frac = k.where(self.sign * self.times[0])
+            z0 = z0.detach().reshape(-1, hidden).contiguous()
+            f_tmp, vjp = torch.empty_like(z0), torch.empty_like(z0)
+            scratch_bytes = _lib.load().tcde_vector_field_linear_vjp_scratch_bytes(n_paths, k.channels, hidden)
+            scratch = torch.empty(max(scratch_bytes // 4, 4), dtype=torch.float32, device=dev)
+            _lib.call("tcde_vector_field_linear_vjp", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w), _lib.ptr(k.b),
+                      _lib.ptr(z0), _lib.ptr(carry[1]), _lib.ptr(f_tmp), _lib.ptr(vjp), _lib.ptr(gw), _lib.ptr(gb),
+                      _lib.ptr(scratch), n_paths, k.channels, hidden, index, float(frac), 1.0, self.sign, self.sign,
+                      _lib.F32, stream)
+            gz = carry[0] + vjp + gf[:, 0]
+        return gz.view(g.shape[:-2] + (hidden,)), gw, gb
+
+
+class _Dopri5BackpropFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, route, z0, weight, bias):
+        out, record = route.forward(z0)
+        ctx.route = route                      # host-side metadata only: the record goes through save_for_backward, so a
+        ctx.save_for_backward(z0, weight, bias, *(x for chunk in record for x in chunk))   # backward frees it
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        z0, weight, bias, *flat = ctx.saved_tensors
+        record = [tuple(flat[i:i + 3]) for i in range(0, len(flat), 3)]
+        _route_needs, want_z, want_w, want_b = ctx.needs_input_grad
+        if torch.is_grad_enabled():
+            # create_graph: differentiate the torch-operator replay of the recorded steps, whose gradients are themselves
+            # differentiable and belong to the same discrete solve
+            inputs = [x for x, want in ((z0, want_z), (weight, want_w), (bias, want_b)) if want]
+            got = iter(torch.autograd.grad(ctx.route.replay(ctx.route.steps)(z0), inputs, g, create_graph=True,
+                                           allow_unused=True))
+            return (None,) + tuple(next(got) if want else None for want in (want_z, want_w, want_b))
+        gz, gw, gb = ctx.route.backward(g, z0, record, want_w, want_b)
+        return None, gz if want_z else None, gw, gb
+
+
+def dopri5_backprop(kernels, z0, times, rtol, atol, sign, first_step, replay):
+    """``cdeint(..., adjoint=False)``'s outputs ``(..., len(times), H)`` and statistics on the route of ``Dopri5Backprop``,
+    or None when the route does not serve the problem (the caller runs the torch-operator solve).  ``times``: increasing
+    floats (negated when ``sign`` < 0); ``replay(steps)`` returns the torch-operator solve ``z0 -> outputs`` on ``steps``."""
+    k = kernels
+    if k.dtype != torch.float32 or k.hidden != 32 or k.channels != 8 or k.n_paths == 0 or len(times) < 2:
+        return None
+    want_params = any(p is not None and p.requires_grad for p in (k.weight, k.bias))
+    route = Dopri5Backprop(k, times, rtol, atol, sign, first_step, replay, want_params)
+    try:
+        return _Dopri5BackpropFn.apply(route, z0, k.weight, k.bias), route.stats
+    except (_NoRoom, NotImplementedError):
+        # the record does not fit, or the recording solve refuses the problem (control rows off a 16-byte boundary)
+        return None
+
+
 class AdjointStage:
     """The adjoint stage of the linear field: ``stage(t, y, a, scale) -> (f, scale * a^T df/dy, [scale * a^T df/dp for
     p in params])`` as ONE launch of ``tcde_vector_field_linear_vjp``, plus the whole-segment backward routes that

@@ -15,7 +15,8 @@ import torch
 
 from . import _lib, adaptive
 from .controls import CubicSpline, _control_signature, _schedule_knots
-from .linear_field import LinearFieldKernels, LinearVectorField, _reverse, fixed_backprop, linear_field_of  # noqa: F401
+from .linear_field import (LinearFieldKernels, LinearVectorField, _reverse, dopri5_backprop, fixed_backprop,  # noqa: F401
+                           linear_field_of)
 from .mlp_field import MlpFieldKernels, mlp_backprop, mlp_field_of
 from .schedule import FIXED_METHODS, build_schedule, host_locator
 
@@ -377,7 +378,10 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     linear field at fp32, hidden 32, channels 8 with gradients for z0 / weight / bias in three
     launches (``linear_field.FixedBackprop``), likewise for the examples' MLP field at fp32, hidden
     32, channels 8, width 128 with gradients for z0 and its two layers (``mlp_field.MlpBackprop``),
-    otherwise through the differentiable generic stage loop.
+    for the linear field under dopri5 from a recording device-controlled forward and one transposed
+    Dormand-Prince launch per record chunk (``linear_field.Dopri5Backprop``; ``cdeint.last_stats["steps"]``
+    then lists the accepted ``(t, dt)``, in ``-t`` for a decreasing ``t``), otherwise through the
+    differentiable generic stage loop.
 
     ``backend="torchsde"`` is built for ``method="reversible_heun"`` (torchsde's reversible Heun
     method with zero diffusion, fixed step ``dt``, default 1e-3; ``z0`` of shape (batch, hidden),
@@ -533,17 +537,22 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                              "device_controlled": False}
         return out
 
-    # adjoint=False with gradients of a fixed-step linear-field solve: the three-launch route of linear_field.FixedBackprop
-    # serves gradients for z0, the weight and the bias of an fp32 problem at hidden 32 / channels 8; a gradient for
-    # anything else (t, the control's knots or coefficients) keeps the torch-operator solve
-    backprop = (field_params is not None and not adjoint and wants_grad and method in FIXED_METHODS
-                and not t.requires_grad and not any(b.requires_grad for b in X.buffers())
-                and z0.dtype == torch.float32 and z0.size(-1) == 32 and sig[2] == 8
-                and all(b.dtype == torch.float32 and b.device == z0.device for b in X.buffers() if b.is_floating_point())
-                and all(p.dtype == torch.float32 and p.device == z0.device for p in field_params if p is not None))
+    # adjoint=False with gradients of a linear-field solve: the kernel routes of linear_field.FixedBackprop (fixed step)
+    # and linear_field.Dopri5Backprop (dopri5, controller on the device) serve gradients for z0, the weight and the bias of
+    # an fp32 problem at hidden 32 / channels 8; a gradient for anything else (t, the control's knots or coefficients)
+    # keeps the torch-operator solve
+    served = (field_params is not None and not adjoint and wants_grad
+              and not t.requires_grad and not any(b.requires_grad for b in X.buffers())
+              and z0.dtype == torch.float32 and z0.size(-1) == 32 and sig[2] == 8
+              and all(b.dtype == torch.float32 and b.device == z0.device for b in X.buffers() if b.is_floating_point())
+              and all(p.dtype == torch.float32 and p.device == z0.device for p in field_params if p is not None))
+    backprop = served and method in FIXED_METHODS
+    # dopri5: the options the device controller takes (no jump_t)
+    dp5_backprop = (served and method == "dopri5" and not options.get("jump_t")
+                    and set(options) <= {"first_step", "jump_t"})
     # the routes that call a kernel own the linear-field problem; building it checks dtypes and devices
     kernels = None
-    if field_params is not None and (adjoint or not wants_grad or backprop):
+    if field_params is not None and (adjoint or not wants_grad or backprop or dp5_backprop):
         kernels = LinearFieldKernels(X, field_params[0], field_params[1], z0)
     # the examples' MLP field (no gradient, or adjoint=True): the fixed-step forward is one launch, a dopri5 field
     # evaluation and an adjoint stage one call each where its CUDA-core kernels serve the shape
@@ -606,6 +615,15 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                 if ys is not None:
                     return ys
         return _generic_solve(X, func, z0, t, method, step_size, is_prod, sig is not None)
+    if dp5_backprop:
+        def replay(steps):
+            return lambda y0: _time_first_to_reference_layout(
+                adaptive.odeint_dopri5(autograd_field(), y0, times, rtol, atol, options, steps=steps)[0])
+
+        done = dopri5_backprop(kernels, z0, times, rtol, atol, -1.0 if flipped else 1.0, options.get("first_step"), replay)
+        if done is not None:
+            ys, cdeint.last_stats = done
+            return ys
     targets = None
     if t.requires_grad:
         targets = (-t if flipped else t).to(z0.device)
