@@ -392,6 +392,35 @@ TCDE_API int tcde_reversible_heun_mlp_backward_segment(
     const void* stage_frac, int64_t lo, int64_t hi, int64_t n_paths, int64_t channels, int64_t hidden, int64_t width,
     void* dump_z, void* dump_a, int dtype, void* stream);
 
+/* The backward pass of cdeint(adjoint=False) with dopri5 for the MLP field of tcde_cdeint_fixed_mlp, over one record chunk
+ * of a host-driven solve, its n_steps accepted steps last to first, in ONE launch (one thread per path, fp32 or fp64): the
+ * transposed Dormand-Prince recurrence of tcde_dopri5_linear_backward, with J^T of every evaluation formed at its recorded
+ * input (the forward's ReLU masks and tanh values).
+ *   rec_z     [n_items][n_paths][hidden]: the inputs of the chunk's evaluations, n_items = step_item[n_steps]; the items
+ *             of step n are [step_item[n], step_item[n + 1]): stages 2..7 (stage 7's input is the step's result), preceded
+ *             by the step's own start slope f(t_n, y_n) when k1 of step n is not the previous step's k7 (step 0 of the
+ *             solve, and the step after a jump of jump_t): 7 items then, 6 otherwise
+ *   item_index int32 / item_frac [n_items]: the spline interval and fraction of every evaluation
+ *   grad_out  [n_paths][n_out][hidden]: dL/d(outputs)
+ *   carry     [2][n_paths][hidden]: in, the cotangent of the state after the chunk's last step and the cotangent still
+ *             pending on that step's last evaluation (zero for the last chunk); out, the same before the chunk's first step
+ *             (the second is zero when that step's start slope was its own evaluation)
+ *   kappa     [n_items][n_paths][hidden] or NULL: the cotangent of every evaluation, in its item, for
+ *             tcde_mlp_field_param_grads (item_index / item_frac, n_items, sign = the solve's, scale 1)
+ *   coef      [n_steps][36]: beta[s][j] dt of the Dormand-Prince tableau in the state dtype, rows s = 0..5, zero padded
+ *   inj_range int32 [n_steps + 1], inj_out int32 [n_inj], inj_w [n_inj][8]: as tcde_dopri5_linear_backward's, in the state
+ *             dtype
+ *   sign      +1, or -1 for a decreasing t solved in -t (dX/dt is negated)
+ * Served where tcde_cdeint_fixed_mlp_stages runs the CUDA cores (by default hidden <= 8, fp32 and fp64; under solve variant 1
+ * also hidden * channels <= 32) at widths whose columns fit shared memory; TCDE_ERR_UNSUPPORTED elsewhere, the tensor-core
+ * shape 32 / 8 / 128 included.  n_paths == 0 validates the problem and launches nothing. */
+TCDE_API int tcde_dopri5_mlp_backward(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
+                             const void* w2, const void* b2, const void* rec_z, const void* grad_out, void* carry,
+                             void* kappa, const void* coef, const int32_t* step_item, const int32_t* item_index,
+                             const void* item_frac, const int32_t* inj_range, const int32_t* inj_out, const void* inj_w,
+                             int64_t n_out, int64_t n_steps, int64_t n_paths, int64_t channels, int64_t hidden,
+                             int64_t width, double sign, int dtype, void* stream);
+
 /* The parameter gradients of a whole backward solve (the stage trajectories of tcde_cdeint_fixed_linear_stages, or any
  * other list of (z, a, stage) triples) in one launch:
  *   grad_weight[h*C+c][k] += scale * sum_e sum_p stage_weight[e] * a_stages[e][p][h] * dXdt_e[p][c] * z_stages[e][p][k]

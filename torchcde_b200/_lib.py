@@ -67,6 +67,8 @@ SIGNATURES = {
                                          _p, _p, _p, _i64, _p, _p, _int, _p], _int),
     "tcde_reversible_heun_mlp_backward_segment": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _i64,
                                                    _p, _p, _p, _i64, _i64, _i64, _i64, _i64, _i64, _p, _p, _int, _p], _int),
+    "tcde_dopri5_mlp_backward": ([_p, _int, _i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i64, _i64,
+                                  _i64, _i64, _i64, _i64, _dbl, _int, _p], _int),
     "tcde_linear_field_param_grads_scratch_bytes": ([_i64, _i64, _i64, _i64], _i64),
     "tcde_linear_field_param_grads": ([_p, _int, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _p, _i64, _i64, _i64, _dbl,
                                        _int, _p], _int),

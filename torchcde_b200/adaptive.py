@@ -202,13 +202,30 @@ class Dopri5:
         # no step may straddle one, and the slope is re-evaluated just after it
         self.jump_t = sorted(float(v) for v in jump_t) if jump_t is not None else []
 
+    # Hooks of a solve that records what its backward pass needs (mlp_field.Dopri5MlpBackprop); as defined here they
+    # leave the solve as it is.
+    def _stage_out(self, s):
+        """Where the input of stage s + 2 of the current attempt is written (None: a new tensor)."""
+        return None
+
+    def _stage_done(self, s):
+        """Called after the evaluation of stage s + 2 of the current attempt."""
+
+    def _start_slope(self, t, y, *nudge):
+        """f(t, y) where a step starts from a slope of its own: at t0, and just after a jump of ``jump_t``."""
+        return self.field(t, y, *nudge)
+
+    def _accepted(self, t, dt, t_new):
+        """Called when the attempt (t, dt) is accepted, before the next start slope; it ends at t_new."""
+
     def _stages(self, t0, dt, y0, f0):
         ks = [f0]
         y1 = y0
-        for alpha, beta in zip(_ALPHA, _BETA):
+        for s, (alpha, beta) in enumerate(zip(_ALPHA, _BETA)):
             ti = t0 + dt if alpha == 1.0 else t0 + alpha * dt
-            y1 = _combine(y0, ks, beta, dt)
+            y1 = _combine(y0, ks, beta, dt, out=self._stage_out(s))
             ks.append(self.field(ti, y1))
+            self._stage_done(s)
         # the last beta row equals the solution weights (FSAL): y1 is the 5th-order solution
         return y1, ks
 
@@ -224,7 +241,7 @@ class Dopri5:
         out = [self.y0]
         t0 = times[0]
         y0 = self.y0
-        f0 = self.field(t0, y0)
+        f0 = self._start_slope(t0, y0)
         if steps is not None:
             steps = list(steps)
             dt = steps[0][1] if steps else 0.0
@@ -244,7 +261,9 @@ class Dopri5:
                     if self.n_accepted == len(steps):
                         raise RuntimeError("dopri5 replay: the recorded steps end at t = {}".format(t_hi))
                     step = steps[self.n_accepted][1]
-                on_jump = bool(jumps) and t_hi < jumps[0] < t_hi + step
+                # a recorded step that ends on a jump is jumps[0] - t_hi, which t_hi + step may round onto or below the jump
+                on_jump = bool(jumps) and t_hi < jumps[0] and (jumps[0] < t_hi + step
+                                                                or (steps is not None and jumps[0] - t_hi == step))
                 if on_jump:
                     step = jumps[0] - t_hi
                 if steps is None:
@@ -253,6 +272,7 @@ class Dopri5:
                     (y1, ks), ratio = self._stages(t_hi, step, y0, f0), 0.0
                 if ratio <= 1:
                     t_new = jumps[0] if on_jump else t_hi + step
+                    self._accepted(t_hi, step, t_new)
                     if t_new >= target:          # the dense output is only ever evaluated inside the last step
                         y_mid = _combine(y0, ks, _C_MID, step)
                         coeff = self._fit(y0, y1, y_mid, ks[0], ks[-1], step)
@@ -260,7 +280,7 @@ class Dopri5:
                     y0, f0 = y1, ks[-1]
                     if on_jump:
                         jumps.pop(0)
-                        f0 = self.field(t_hi, y0, 1)      # the slope just AFTER the discontinuity
+                        f0 = self._start_slope(t_hi, y0, 1)      # the slope just AFTER the discontinuity
                     self.n_accepted += 1
                 else:
                     self.n_rejected += 1
@@ -370,24 +390,28 @@ def dense_output_weights(x, dt):
             dt * (x - 4.0 * x2 + 5.0 * x3 - 2.0 * x4), dt * (x2 - 3.0 * x3 + 2.0 * x4))
 
 
-def dopri5_backward_tables(steps, times):
-    """The host tables of ``tcde_dopri5_linear_backward`` for the accepted ``steps`` [(t, dt), ...] of a solve over the
-    increasing output times ``times``, in double, cast to float32 at the end:
-      coef [n, 36]: (float)(beta[s][j] * dt), the forward's own stage coefficients;
+def dopri5_backward_tables(steps, times, dtype=torch.float32, ends=None):
+    """The host tables of ``tcde_dopri5_linear_backward`` / ``tcde_dopri5_mlp_backward`` for the accepted ``steps``
+    [(t, dt), ...] of a solve over the increasing output times ``times``, in double, cast to ``dtype`` (the state dtype:
+    the coefficients the forward's combinations used) at the end:
+      coef [n, 36]: beta[s][j] * dt, the forward's own stage coefficients;
       inj_range [n + 1], inj_out [m], inj_w [m, 8]: the outputs each step emits (the kernel's rule: the first accepted step
       whose end is at or past the output time; output 0 is y(t0) itself) and their weights on (y_n, y_{n+1}, k1, k3, k4,
-      k5, k6, k7) -- ``dense_output_weights`` with y_mid = y_n + dt sum_j c_mid[j] k_j folded in."""
+      k5, k6, k7) -- ``dense_output_weights`` with y_mid = y_n + dt sum_j c_mid[j] k_j folded in.
+    ``ends``: where each step ended as the solve took it (a step cut at a jump of ``jump_t`` ends exactly on the jump,
+    which t + dt may miss by a rounding); default t + dt."""
     import numpy as np
     n = len(steps)
+    np_dtype = np.float64 if dtype == torch.float64 else np.float32
     dts = np.array([dt for _t, dt in steps], dtype=np.float64)
     beta = np.zeros((6, 6))
     for s, row in enumerate(_BETA):
         beta[s, :len(row)] = row
-    coef = (beta.reshape(1, 36) * dts.reshape(n, 1)).astype(np.float32)
+    coef = (beta.reshape(1, 36) * dts.reshape(n, 1)).astype(np_dtype)
     inj_range, inj_out, inj_w = [0], [], []
     nxt = 1
-    for t, dt in steps:
-        t_hi = t + dt
+    for i, (t, dt) in enumerate(steps):
+        t_hi = t + dt if ends is None else ends[i]
         while nxt < len(times) and times[nxt] <= t_hi:
             w_y0, w_y1, w_ym, w_f0, w_f1 = dense_output_weights((times[nxt] - t) / (t_hi - t), dt)
             cm = [c * dt * w_ym for c in _C_MID]
@@ -397,7 +421,7 @@ def dopri5_backward_tables(steps, times):
         inj_range.append(len(inj_out))
     return {"coef": torch.from_numpy(coef), "inj_range": torch.tensor(inj_range, dtype=torch.int32),
             "inj_out": torch.tensor(inj_out or [0], dtype=torch.int32),
-            "inj_w": torch.tensor(inj_w or [[0.0] * 8], dtype=torch.float64).to(torch.float32)}
+            "inj_w": torch.tensor(inj_w or [[0.0] * 8], dtype=torch.float64).to(dtype)}
 
 
 # ------------------------------------------------------------------------- fixed grids (generic)

@@ -2396,6 +2396,257 @@ static int64_t mlp_param_grid(int64_t n_paths, int64_t n_total) {
     return g < 1 ? 1 : g;
 }
 
+// ---- the backward of cdeint(..., adjoint=False) under the host-driven dopri5 (tcde_dopri5_mlp_backward) ---------------
+//
+// The transposed Dormand-Prince recurrence of dopri5_backward_kernel (solve_dopri5.cu) for this field, one thread per path
+// over one record chunk, last step first.  J depends on the state here, so every J^T is one mlp_vjp pass at the
+// evaluation's recorded input and location (the forward's ReLU masks and tanh values, as in the Runge-Kutta backward).
+// Items [step_item[n], step_item[n + 1]) of the chunk are the evaluations of step n: 6 (stages 2..7; stage 7's input is
+// y_{n+1}), or 7 when k1 of step n is a fresh start slope f(t_n, y_n) (step 0 of the solve, and the step after a jump of
+// jump_t), whose item then comes first.  (A, K): the cotangents of y_{n+1} and of the evaluation k7 (= k1 of step n + 1
+// under FSAL: zero when that one was fresh).  Per step:
+//   kappa7 = K + inj;  Zbar7 = A + J7^T kappa7 + inj, to y_n (weight 1) and k_j (beta[5][j - 1] dt);  stages i = 6 .. 2:
+//   kappa_i = the accumulated cotangent of k_i, Zbar_i = J_i^T kappa_i to y_n and k_j, j < i;  (A, K) = (ybar_n, kbar_1);
+//   a fresh k1 gets its own J^T at y_n into A, and K = 0.
+// The output cotangents enter through the transposed dense output (adaptive.dopri5_backward_tables); kappa of every
+// evaluation goes to its item, for tcde_mlp_field_param_grads.  The cotangents of k2..k6 sit in the thread's shared-memory
+// columns, so that the stages run as one loop (one mlp_vjp site); A, K, J^T kappa and the input as the reversible
+// backward keeps its vectors (registers at HM = 8, 64-thread CTAs with shared columns at HM = 32).
+template <typename T> struct MlpDp5Bwd {
+    const T* rec_z;               // [n_items][n_paths][H]: the evaluations' inputs
+    T* kappa;                     // [n_items][n_paths][H], or null
+    const T* grad_out;            // [n_paths][n_out][H]
+    T* carry;                     // [2][n_paths][H]: (A, K) after the chunk's last step in, before its first step out
+    const T* coef;                // [n_steps][36]: beta[s][j] dt_n, rows s = 0..5 zero padded, as the forward combined
+    const int32_t* step_item;     // [n_steps + 1]
+    const int32_t* inj_range;     // [n_steps + 1]: the injections of step n are [inj_range[n], inj_range[n + 1])
+    const int32_t* inj_out;       // [n_inj]: output index
+    const T* inj_w;               // [n_inj][8]: weights on (y_n, y_{n+1}, k1, k3, k4, k5, k6, k7)
+    int n_steps;
+};
+enum { kDpY0 = 0, kDpY1 = 1, kDpK1 = 2, kDpK7 = 7 };               // inj_w columns; k_j (j = 3..6) is column j
+
+template <int HM> __host__ __device__ constexpr bool mlp_dp5_bwd_shared() { return HM == 32; }
+// per-thread values after the slopes: the cotangents of k2..k6 [5H], then at HM = 32 A, K, J^T kappa [H] and z [Hp]
+template <int HM> static int mlp_dp5_bwd_extra(int H) {
+    return 5 * H + (mlp_dp5_bwd_shared<HM>() ? 3 * H + (H + 3) / 4 * 4 : 0);
+}
+
+// a.stage_index / a.stage_frac: the items' locations; a.sign: the sign of the solve's time direction
+template <typename T, int HM>
+__global__ void __launch_bounds__(kMlpSimtThreads, 1) dopri5_mlp_backward_kernel(const MlpArgs<T> a,
+                                                                              const MlpSimtLayout<T> lay,
+                                                                              const MlpDp5Bwd<T> b) {
+    constexpr bool kShared = mlp_dp5_bwd_shared<HM>();
+    using E = exact<T>;
+    using P4 = Pack<T, 4>;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    T* smem = reinterpret_cast<T*>(smem_raw);
+    const int tid = threadIdx.x;
+    constexpr int nt = mlp_rev_bwd_threads<HM>();
+    const int H = a.H, C = a.C;
+    if (lay.staged) {
+        const int W = a.W, HC = a.H * a.C, Hp = lay.Hp, Nq = lay.Nq;
+        TCDE_MLP_STAGE_WEIGHTS()
+        __syncthreads();
+    }
+    T* dxs = smem + lay.cols + tid;
+    T* kvs = dxs + (size_t)C * nt;                                 // kvs[h * nt]: kappa of the evaluation transposed
+    T* park = kvs + (size_t)H * nt;                                // park[((j - 2) * H + h) * nt]: cotangent of k_j
+    const int64_t path = (int64_t)blockIdx.x * nt + tid;
+    const bool live = path < a.n_paths;
+    const int64_t lp = live ? path : a.n_paths - 1;
+    const bool cubic = (a.control_kind == TCDE_CONTROL_CUBIC);
+    const T* crow = a.control + lp * a.n_rows * (cubic ? 4 * C : C) + (cubic ? C : 0);
+    MlpRevVec<T, HM, kShared, nt> A, K, kv, zm;                    // kv: J^T kappa; zm: the evaluation's input
+    {
+        T* col = park + (size_t)5 * H * nt;
+        const size_t step = (size_t)H * nt;
+        A.bind(col);
+        K.bind(col + step);
+        kv.bind(col + 2 * step);
+        zm.bind(col + 3 * step);
+    }
+    struct Col {                                                   // the cotangent of k_j in the thread's column
+        T* p;
+        __device__ __forceinline__ T& operator[](int k) const { return p[(size_t)k * nt]; }
+    };
+    auto kbar = [&](int j) { return Col{park + (size_t)(j - 2) * H * nt}; };
+    const int64_t plane = a.n_paths * H;
+#pragma unroll
+    for (int h = 0; h < HM; ++h) {
+        if (!kShared || h < H) {
+            A[h] = h < H ? b.carry[lp * H + h] : T(0);
+            K[h] = h < H ? b.carry[plane + lp * H + h] : T(0);
+            kv[h] = T(0);
+        }
+        if (!kShared || h < lay.Hp) zm[h] = T(0);
+    }
+    // v += the step's output cotangents with weight column col
+    auto inject = [&](int e0, int e1, int col, auto&& v) {
+        for (int e = e0; e < e1; ++e) {
+            const T w = b.inj_w[8 * e + col];
+            const T* src = b.grad_out + (lp * a.n_out + b.inj_out[e]) * H;
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) v[h] = fma(w, src[h], v[h]);
+        }
+    };
+    // kv = J^T kappa (kappa in kvs) at item e's input and location; kappa also goes to item e of b.kappa
+    auto transposed = [&](int e) {
+        const T* zsrc = b.rec_z + (int64_t)e * plane + lp * H;
+        T* kdst = b.kappa ? b.kappa + (int64_t)e * plane + path * H : nullptr;
+#pragma unroll
+        for (int h = 0; h < HM; ++h) {
+            if (h < H) {
+                zm[h] = zsrc[h];
+                kv[h] = T(0);
+                if (kdst && live) kdst[h] = kvs[(size_t)h * nt];
+            }
+        }
+        {
+            TCDE_MLP_SLOPE(a.stage_index[e], a.stage_frac[e])
+        }
+        mlp_vjp<T, HM>(
+            a, lay, smem, zm.arg(), dxs, kvs, nt, [](int, const T*) {},
+            [&](int, int w, T pre, T sv) {
+                if (!(pre > T(0))) return;
+                if (lay.staged) {
+                    const T* wr = smem + lay.w1 + (size_t)w * lay.Hp;
+#pragma unroll
+                    for (int k4 = 0; k4 < HM / 4; ++k4) {
+                        if (4 * k4 < lay.Hp) {
+                            const P4 w4 = *reinterpret_cast<const P4*>(wr + 4 * k4);
+#pragma unroll
+                            for (int i = 0; i < 4; ++i)
+                                if (!kShared || 4 * k4 + i < H) kv[4 * k4 + i] = fma(w4.v[i], sv, kv[4 * k4 + i]);
+                        }
+                    }
+                } else {
+                    const T* wr = a.w1 + (size_t)w * H;
+#pragma unroll
+                    for (int k = 0; k < HM; ++k)
+                        if (k < H) kv[k] = fma(__ldg(wr + k), sv, kv[k]);
+                }
+            });
+    };
+
+    for (int n = b.n_steps - 1; n >= 0; --n) {
+        const T* cs = b.coef + (int64_t)n * 36;
+        const int e0 = b.inj_range[n], e1 = b.inj_range[n + 1];
+        const int first = b.step_item[n];
+        const bool fresh = b.step_item[n + 1] - first == 7;
+        const int s2 = first + (fresh ? 1 : 0);                    // the item of stage 2
+        // the evaluations of step n, last first: i = 7 .. 2 its stages, i = 1 its fresh start slope
+        for (int i = 7; i >= (fresh ? 1 : 2); --i) {
+            if (i == 7) inject(e0, e1, kDpK7, K);
+#pragma unroll
+            for (int h = 0; h < HM; ++h)
+                if (h < H) kvs[(size_t)h * nt] = (i == 7 || i == 1) ? K[h] : kbar(i)[h];
+            transposed(i == 1 ? first : s2 + i - 2);
+            if (i == 7) {
+#pragma unroll
+                for (int h = 0; h < HM; ++h)
+                    if (h < H) A[h] = E::add(A[h], kv[h]);
+                inject(e0, e1, kDpY1, A);
+                // Zbar7 (in A) -> y_n (A stays), k1 (K), k2 .. k6
+#pragma unroll
+                for (int h = 0; h < HM; ++h) {
+                    if (h < H) {
+                        const T z = A[h];
+                        K[h] = E::mul(cs[30], z);
+                        for (int j = 2; j <= 6; ++j) kbar(j)[h] = E::mul(cs[30 + j - 1], z);
+                    }
+                }
+                inject(e0, e1, kDpY0, A);
+                inject(e0, e1, kDpK1, K);
+                for (int j = 3; j <= 6; ++j) inject(e0, e1, j, kbar(j));
+            } else if (i == 1) {
+#pragma unroll
+                for (int h = 0; h < HM; ++h) {
+                    if (h < H) {
+                        A[h] = E::add(A[h], kv[h]);
+                        K[h] = T(0);
+                    }
+                }
+            } else {
+                const T* c = cs + (i - 2) * 6;
+#pragma unroll
+                for (int h = 0; h < HM; ++h) {
+                    if (h < H) {
+                        A[h] = E::add(A[h], kv[h]);
+                        K[h] = fma(c[0], kv[h], K[h]);
+                        for (int j = 2; j < i; ++j) kbar(j)[h] = fma(c[j - 1], kv[h], kbar(j)[h]);
+                    }
+                }
+            }
+        }
+    }
+    if (live) {
+#pragma unroll
+        for (int h = 0; h < HM; ++h) {
+            if (h < H) {
+                b.carry[path * H + h] = A[h];
+                b.carry[plane + path * H + h] = K[h];
+            }
+        }
+    }
+}
+
+// The layout of dopri5_mlp_backward_kernel at the HM the dispatch picks for H: the weights staged when everything fits,
+// else read from global memory; false if neither fits
+template <typename T, int HM> static bool mlp_dp5_bwd_layout(int H, int C, int W, MlpSimtLayout<T>& lay) {
+    for (int stage = 1; stage >= 0; --stage) {
+        lay = mlp_simt_layout<T>(H, C, W, stage != 0, mlp_rev_bwd_threads<HM>(), mlp_dp5_bwd_extra<HM>(H));
+        if (lay.total <= kMlpSimtMaxSmem) return true;
+    }
+    return false;
+}
+
+// Where tcde_dopri5_mlp_backward runs: the CUDA-core route of mlp_backprop_route (by default hidden <= 8, fp32 and fp64;
+// under solve variant 1 also hidden * channels <= 32), at widths whose columns fit shared memory; TCDE_ERR_UNSUPPORTED
+// elsewhere, the tensor-core shape 32 / 8 / 128 included, so that the caller keeps the torch-operator dopri5
+static int mlp_dopri5_route(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what) {
+    bool simt;
+    const int rc = mlp_backprop_route(hidden, channels, width, dtype, what, &simt);
+    if (rc != TCDE_OK) return rc;
+    TCDE_CHECK_SUPPORTED(simt, "%s is built for the CUDA-core shapes (hidden <= 8, or hidden * channels <= 32 under solve "
+                         "variant 1; got %lld, %lld, %lld)", what, (long long)hidden, (long long)channels,
+                         (long long)width);
+    MlpSimtLayout<double> lay;                       // the larger element size bounds both dtypes
+    const bool fits = hidden <= 8 ? mlp_dp5_bwd_layout<double, 8>((int)hidden, (int)channels, (int)width, lay)
+                                  : mlp_dp5_bwd_layout<double, 32>((int)hidden, (int)channels, (int)width, lay);
+    TCDE_CHECK_SUPPORTED(fits, "%s: hidden=%lld channels=%lld width=%lld do not fit the CUDA-core kernel's shared memory",
+                         what, (long long)hidden, (long long)channels, (long long)width);
+    return TCDE_OK;
+}
+
+template <typename T, int HM>
+static int launch_mlp_dp5_backward(const MlpArgs<T>& a, const MlpDp5Bwd<T>& b, cudaStream_t s) {
+    auto kern = dopri5_mlp_backward_kernel<T, HM>;
+    constexpr int nt = mlp_rev_bwd_threads<HM>();
+    MlpSimtLayout<T> lay;
+    const bool fits = mlp_dp5_bwd_layout<T, HM>(a.H, a.C, a.W, lay);
+    TCDE_CHECK_SUPPORTED(fits, "MLP dopri5 backward: the shape does not fit");
+    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
+    const int64_t ctas = (a.n_paths + nt - 1) / nt;
+    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
+    kern<<<(unsigned)ctas, nt, lay.total, s>>>(a, lay, b);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    return TCDE_OK;
+}
+
+template <typename T>
+static int mlp_dp5_backward(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
+                            const void* w2, const void* b2, const MlpDp5Bwd<T>& b, const int32_t* item_index,
+                            const void* item_frac, int64_t n_out, int64_t n_paths, int64_t channels, int64_t hidden,
+                            int64_t width, double sign, cudaStream_t s) {
+    const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths,
+                                          channels, hidden, width, TCDE_EULER, b.n_steps, nullptr, item_index, item_frac,
+                                          n_out, nullptr, nullptr, nullptr, sign);
+    return hidden <= 8 ? launch_mlp_dp5_backward<T, 8>(a, b, s) : launch_mlp_dp5_backward<T, 32>(a, b, s);
+}
+
 
 }  // namespace tcde
 
@@ -2749,4 +3000,37 @@ extern "C" int tcde_reversible_heun_mlp_backward_segment(
         MlpRevBwd<double>{(const double*)ckpt_lo, (const double*)ckpt_hi, (double*)carry, (const double*)g, inj_range,
                           (double*)dump_z, (double*)dump_a, (int)lo, (int)hi},
         s);
+}
+
+extern "C" int tcde_dopri5_mlp_backward(const void* control, int control_kind, int64_t n_rows, const void* w1,
+                                        const void* b1, const void* w2, const void* b2, const void* rec_z,
+                                        const void* grad_out, void* carry, void* kappa, const void* coef,
+                                        const int32_t* step_item, const int32_t* item_index, const void* item_frac,
+                                        const int32_t* inj_range, const int32_t* inj_out, const void* inj_w, int64_t n_out,
+                                        int64_t n_steps, int64_t n_paths, int64_t channels, int64_t hidden, int64_t width,
+                                        double sign, int dtype, void* stream) {
+    TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && rec_z && grad_out && carry, "null data pointer");
+    TCDE_CHECK_ARG(coef && step_item && item_index && item_frac && inj_range && inj_out && inj_w, "null table pointer");
+    TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_out >= 2 && n_out < (1ll << 31) && n_steps >= 0 &&
+                       n_steps < (1ll << 24) && channels >= 1 && hidden >= 1 && width >= 1, "bad sizes");
+    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    TCDE_CHECK_ARG(sign == 1.0 || sign == -1.0, "sign=%g", sign);
+    const int rc = mlp_dopri5_route(hidden, channels, width, dtype, "the MLP dopri5 backward");
+    if (rc != TCDE_OK) return rc;
+    TCDE_CHECK_SUPPORTED(n_paths * hidden * 7 * n_steps < (1ll << 62), "record too large");
+    if (n_paths == 0 || n_steps == 0) return TCDE_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    if (dtype == TCDE_F32)
+        return mlp_dp5_backward<float>(control, control_kind, n_rows, w1, b1, w2, b2,
+                                       MlpDp5Bwd<float>{(const float*)rec_z, (float*)kappa, (const float*)grad_out,
+                                                        (float*)carry, (const float*)coef, step_item, inj_range, inj_out,
+                                                        (const float*)inj_w, (int)n_steps},
+                                       item_index, item_frac, n_out, n_paths, channels, hidden, width, sign, s);
+    return mlp_dp5_backward<double>(control, control_kind, n_rows, w1, b1, w2, b2,
+                                    MlpDp5Bwd<double>{(const double*)rec_z, (double*)kappa, (const double*)grad_out,
+                                                      (double*)carry, (const double*)coef, step_item, inj_range, inj_out,
+                                                      (const double*)inj_w, (int)n_steps},
+                                    item_index, item_frac, n_out, n_paths, channels, hidden, width, sign, s);
 }

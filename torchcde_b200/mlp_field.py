@@ -5,7 +5,8 @@ example/time_series_classification.py:20-51 trains ``func(t, z) = tanh(Linear(W,
 its fixed-step forward as ONE launch of ``tcde_cdeint_fixed_mlp``; ``cdeint(..., adjoint=False)`` with gradients runs
 ``MlpBackprop`` (three launches) where it is built for the problem.  At the CUDA-core shapes ``MlpFieldKernels.field`` and
 ``MlpAdjointStage`` give the host-driven dopri5 one launch per field evaluation and the ``adjoint=True`` backward one
-launch per stage (``tcde_vector_field_mlp`` / ``tcde_vector_field_mlp_vjp``).  Under ``backend="torchsde"``
+launch per stage (``tcde_vector_field_mlp`` / ``tcde_vector_field_mlp_vjp``); ``cdeint(..., adjoint=False)`` with dopri5
+runs ``Dopri5MlpBackprop`` there (a recording host-driven forward, one backward launch per record chunk).  Under ``backend="torchsde"``
 (``reversible.py``) ``MlpFieldKernels`` supplies the reversible Heun forward and its segment backward on the CUDA cores."""
 import functools
 import math
@@ -13,9 +14,9 @@ import weakref
 
 import torch
 
-from . import _lib
+from . import _lib, adaptive
 from .controls import _control_signature, _schedule_knots
-from .linear_field import AdjointStage, _check_linear_problem, _probe, _schedules
+from .linear_field import AdjointStage, _NoRoom, _check_linear_problem, _probe, _reverse, _schedules
 from .schedule import backward_tables, host_locator
 
 # module -> {training flag: index of the accepted layer ordering, or -1}; kept apart from the linear probe's cache
@@ -403,4 +404,237 @@ def mlp_backprop(X, params, z0, t, method, step_size, loop):
         return _MlpBackpropFn.apply(route, z0, *leaves)
     except NotImplementedError:
         # the stage-dump solve refuses the problem (shape, solve variant, misaligned rows): nothing ran
+        return None
+
+
+class _Located:
+    """The field of a host-driven dopri5 that keeps the location ``where(t, nudge)`` of its last evaluation: the
+    locator the field itself calls, with the arguments it receives (under ``_reverse`` that is -s without the nudge)."""
+
+    def __init__(self, field, where):
+        self.field, self.where, self.loc = field, where, None
+
+    def __call__(self, t, y, nudge=0):
+        self.loc = self.where(t, nudge)
+        return self.field(t, y, nudge)
+
+
+class _RecordingDopri5(adaptive.Dopri5):
+    """``adaptive.Dopri5`` whose hooks fill the record of ``Dopri5MlpBackprop``: every attempt writes the inputs of its
+    evaluations 2..7 into the items of the step it would become (a rejected attempt's are overwritten by the next one), a
+    start slope of its own writes its input into the item before them, and the locations come from ``_Located``."""
+
+    def __init__(self, route, located, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.route, self.located = route, located
+        self.fresh = None                      # the location of the current step's own start slope, if it has one
+        self.locs = [None] * 6
+
+    def _start_slope(self, t, y, *nudge):
+        f = super()._start_slope(t, y, *nudge)
+        c = self.route.room()
+        c["z"][c["items"]].copy_(y)
+        self.fresh = self.located.loc
+        return f
+
+    def _stage_out(self, s):
+        c = self.route.room()
+        return c["z"][c["items"] + (self.fresh is not None) + s]
+
+    def _stage_done(self, s):
+        self.locs[s] = self.located.loc
+
+    def _accepted(self, t, dt, t_new):
+        c = self.route.chunks[-1]
+        locs = ([self.fresh] if self.fresh is not None else []) + self.locs
+        c["locs"] += locs
+        c["items"] += len(locs)
+        c["step_item"].append(c["items"])
+        self.route.steps.append((t, dt))
+        self.route.ends.append(t_new)
+        self.fresh = None
+
+
+class Dopri5MlpBackprop:
+    """``cdeint(..., adjoint=False)`` of the host-driven dopri5 solve of the MLP field with gradients for any of z0, W1,
+    b1, W2, b2: the exact gradient of the discrete solve, without autograd, where the CUDA-core kernels serve the shape
+    (the C dispatch's policy, ``tcde_dopri5_mlp_backward``).
+
+    The forward is ``adaptive.Dopri5`` under ``no_grad`` with the field the same call without gradients uses, so its
+    outputs and accepted / rejected steps are that call's, bit for bit; its hooks record, per accepted step, the inputs and
+    locations of its evaluations 2..7 and of its own start slope where it has one (step 0, and after a jump of
+    ``jump_t``), in chunks of ``slots`` steps.  The backward is, per chunk and last chunk first, ONE launch of
+    ``tcde_dopri5_mlp_backward`` (the transposed Dormand-Prince recurrence, J^T at the recorded inputs) and, with a
+    parameter gradient, ONE call of ``tcde_mlp_field_param_grads`` over (input, kappa) of the chunk's evaluations.
+    ``replay(steps)``: the differentiable torch-operator solve of the same problem taking the recorded steps, which a
+    backward with ``create_graph`` differentiates instead.  Memory: the first chunk is checked before the solve starts and
+    each further one before it is taken; a chunk that does not fit discards the partial solve (``_NoRoom``)."""
+
+    slots = 64                # accepted steps per record chunk
+
+    def __init__(self, kernels, field, times, rtol, atol, sign, options, replay, want_params):
+        self.kernels, self.field, self.times, self.rtol, self.atol = kernels, field, list(times), rtol, atol
+        self.sign, self.options, self.replay, self.want_params = float(sign), options, replay, want_params
+        # a step takes 6 items, 7 with a start slope of its own: only step 0 has one unless jump_t is given
+        self.cap = 7 * self.slots if options.get("jump_t") else 6 * self.slots + 1
+
+    def _elt(self):
+        return torch.empty(0, dtype=self.kernels.dtype).element_size()
+
+    def scratch_bytes(self, n_paths):
+        k = self.kernels
+        return _lib.load().tcde_mlp_field_param_grads_scratch_bytes(n_paths, self.cap, k.channels, k.hidden, k.width)
+
+    def fits(self, n_paths):
+        """Whether one more record chunk and, with a parameter gradient, the kappa chunk of the backward and the
+        parameter-gradient scratch fit in 0.7 of the free device memory (the bound of ``Dopri5Backprop.fits``)."""
+        k = self.kernels
+        chunk = self.cap * n_paths * k.hidden * self._elt()
+        need = 2 * chunk + self.scratch_bytes(n_paths) if self.want_params else chunk
+        with torch.cuda.device(k.device):
+            free, _total = torch.cuda.mem_get_info()
+        return need <= 0.7 * free
+
+    def room(self):
+        """The chunk the current step records into: a fresh one when the last is full (``_NoRoom`` if it does not fit)."""
+        if len(self.chunks[-1]["step_item"]) > self.slots:
+            if not self.fits(self.n_paths):
+                raise _NoRoom()
+            self._new_chunk()
+        return self.chunks[-1]
+
+    def _new_chunk(self):
+        k = self.kernels
+        self.chunks.append({"z": torch.empty((self.cap,) + self.shape, dtype=k.dtype, device=k.device),
+                            "items": 0, "step_item": [0], "locs": []})
+
+    def forward(self, z0):
+        """(the outputs ``(..., len(times), H)``, the record: per chunk its evaluations' inputs, interval indices and
+        fractions and its steps' first items).  Raises ``_NoRoom`` (nothing kept) when the record does not fit."""
+        k = self.kernels
+        with torch.cuda.device(k.device), torch.no_grad():
+            y0 = z0.detach()
+            self.shape, self.n_paths = tuple(y0.shape), k.n_paths
+            if not self.fits(self.n_paths):
+                raise _NoRoom()
+            self.chunks, self.steps, self.ends = [], [], []
+            self._new_chunk()
+            located = _Located(self.field, k.where)
+            opts = self.options
+            solver = _RecordingDopri5(self, located, _reverse(located) if self.sign < 0 else located, y0, self.rtol,
+                                      self.atol, first_step=opts.get("first_step"),
+                                      max_num_steps=opts.get("max_num_steps", 2 ** 31 - 1), jump_t=opts.get("jump_t"))
+            out = solver.integrate(self.times)
+            record = []
+            for c in self.chunks:
+                n_items = c["items"]
+                record.append((c["z"][:n_items],
+                               torch.tensor([i for i, _f in c["locs"]] or [0], dtype=torch.int32).to(k.device),
+                               torch.tensor([f for _i, f in c["locs"]] or [0.0], dtype=k.dtype).to(k.device),
+                               torch.tensor(c["step_item"], dtype=torch.int32).to(k.device)))
+            self.counts = [len(c["step_item"]) - 1 for c in self.chunks]
+            self.chunks = None                 # the record lives as long as its holder (the autograd Function saves it)
+        self.stats = {"n_accepted": solver.n_accepted, "n_rejected": solver.n_rejected, "device_controlled": False,
+                      "steps": list(self.steps)}
+        return out.movedim(0, -2), record
+
+    def backward(self, g, record, want):
+        """(dL/dz0, [dL/dW1, dL/db1, dL/dW2, dL/db2] with None where ``want`` is False) for output gradients ``g``
+        ``(..., len(times), H)`` from ``forward``'s record."""
+        k = self.kernels
+        hidden, dev, n_out, code = k.hidden, k.device, len(self.times), _lib.dtype_code(k.dtype)
+        with torch.cuda.device(dev):
+            gf = g.reshape(-1, n_out, hidden)
+            if not gf.is_contiguous():
+                gf = gf.contiguous()
+            n_paths = gf.size(0)
+            stream = _lib.stream_of(gf)
+            grads = [torch.zeros_like(p) if w else None for p, w in zip((k.w1, k.b1, k.w2, k.b2), want)]
+            params = any(want)
+            tables = adaptive.dopri5_backward_tables(self.steps, self.times, k.dtype, self.ends)
+            coef, inj_range = tables["coef"].to(dev), tables["inj_range"].to(dev)
+            inj_out, inj_w = tables["inj_out"].to(dev), tables["inj_w"].to(dev)
+            carry = torch.zeros(2, n_paths, hidden, dtype=k.dtype, device=dev)
+            kappa = torch.empty(self.cap, n_paths, hidden, dtype=k.dtype, device=dev) if params else None
+            scratch = (torch.empty(max(self.scratch_bytes(n_paths) // 4, 4), dtype=torch.float32, device=dev)
+                       if params else None)
+            starts = [sum(self.counts[:i]) for i in range(len(record))]
+            for i in range(len(record) - 1, -1, -1):
+                (z, index, frac, step_item), n, lo = record[i], self.counts[i], starts[i]
+                if n <= 0:
+                    continue
+                _lib.call("tcde_dopri5_mlp_backward", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1),
+                          _lib.ptr(k.b1), _lib.ptr(k.w2), _lib.ptr(k.b2), _lib.ptr(z), _lib.ptr(gf), _lib.ptr(carry),
+                          _lib.ptr(kappa), _lib.ptr(coef[lo:lo + n]), _lib.ptr(step_item), _lib.ptr(index),
+                          _lib.ptr(frac), _lib.ptr(inj_range[lo:lo + n + 1]), _lib.ptr(inj_out), _lib.ptr(inj_w), n_out,
+                          n, n_paths, k.channels, hidden, k.width, self.sign, code, stream)
+                if params:
+                    _lib.call("tcde_mlp_field_param_grads", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1),
+                              _lib.ptr(k.b1), _lib.ptr(k.w2), _lib.ptr(k.b2), _lib.ptr(z), _lib.ptr(kappa),
+                              _lib.ptr(index), _lib.ptr(frac), z.size(0), *(_lib.ptr(x) for x in grads),
+                              _lib.ptr(scratch), n_paths, k.channels, hidden, k.width, self.sign, 1.0, code, stream)
+            # step 0's start slope f(t0, z0) was closed by the first chunk's launch: carry[1] is zero
+            gz = carry[0] + gf[:, 0]
+        return gz.view(g.shape[:-2] + (hidden,)), grads
+
+
+class _Dopri5MlpBackpropFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, route, z0, *params):
+        out, record = route.forward(z0)
+        ctx.route = route                      # host-side metadata only: the record goes through save_for_backward, so a
+        ctx.save_for_backward(z0, *params, *(x for chunk in record for x in chunk))     # backward frees it
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        z0, w1, b1, w2, b2, *flat = ctx.saved_tensors
+        record = [tuple(flat[i:i + 4]) for i in range(0, len(flat), 4)]
+        want_z, *want = ctx.needs_input_grad[1:]
+        if torch.is_grad_enabled():
+            # create_graph: differentiate the torch-operator replay of the recorded steps, whose gradients are themselves
+            # differentiable and belong to the same discrete solve
+            inputs = [x for x, w in zip([z0, w1, b1, w2, b2], [want_z] + want) if w]
+            got = iter(torch.autograd.grad(ctx.route.replay(ctx.route.steps)(z0), inputs, g, create_graph=True,
+                                           allow_unused=True))
+            return (None,) + tuple(next(got) if w else None for w in [want_z] + want)
+        gz, grads = ctx.route.backward(g, record, want)
+        return (None, gz if want_z else None) + tuple(grads)
+
+
+def dopri5_mlp_backprop(X, params, z0, field_of, times, rtol, atol, sign, options, replay):
+    """``cdeint(..., adjoint=False)``'s outputs ``(..., len(times), H)`` and statistics on the route of
+    ``Dopri5MlpBackprop``, or None when the route does not serve the problem (the caller runs the torch-operator dopri5).
+    ``field_of(kernels)``: the dopri5 field of the same call without gradients (before ``_reverse``); ``times``: increasing floats
+    (negated when ``sign`` < 0); ``options``: the host driver's (``jump_t`` oriented like ``times``); ``replay(steps)``
+    returns the torch-operator solve ``z0 -> outputs`` on ``steps``.  Which shapes, dtypes and solve variants are served
+    is the C dispatch's call (``tcde_dopri5_mlp_backward``)."""
+    if (z0.dtype not in (torch.float32, torch.float64) or not z0.is_cuda or len(times) < 2
+            or any(p is not None and (p.dtype != z0.dtype or p.device != z0.device) for p in params)
+            or not set(options) <= {"first_step", "jump_t", "max_num_steps"}):
+        return None
+    k = MlpFieldKernels(X, params, z0)
+    if k.control.dtype != z0.dtype or k.control.device != z0.device or k.n_paths == 0:
+        return None
+    want_params = any(p is not None and p.requires_grad for p in params)
+    route = Dopri5MlpBackprop(k, None, times, rtol, atol, sign, options, replay, want_params)
+    if want_params and route.scratch_bytes(k.n_paths) < 0:
+        return None                            # the parameter-gradient staging does not fit this width
+    # the dispatch's verdict on the problem, from a call with no paths (it validates and launches nothing; one small
+    # buffer stands in for the per-path and table pointers)
+    s = torch.zeros(4, dtype=torch.float64, device=k.device)
+    p = _lib.ptr(s)
+    try:
+        with torch.cuda.device(k.device):
+            _lib.call("tcde_dopri5_mlp_backward", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1), _lib.ptr(k.b1),
+                      _lib.ptr(k.w2), _lib.ptr(k.b2), p, p, p, None, p, p, p, p, p, p, p, len(times), 0, 0, k.channels,
+                      k.hidden, k.width, float(sign), _lib.dtype_code(k.dtype), _lib.stream_of(s))
+    except NotImplementedError:
+        return None
+    with torch.no_grad():
+        route.field = field_of(k)
+    leaves = [q if q is not None else b for q, b in zip(params, (k.w1, k.b1, k.w2, k.b2))]
+    try:
+        return _Dopri5MlpBackpropFn.apply(route, z0, *leaves), route.stats
+    except _NoRoom:
         return None

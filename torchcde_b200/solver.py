@@ -17,7 +17,7 @@ from . import _lib, adaptive
 from .controls import CubicSpline, _control_signature, _schedule_knots
 from .linear_field import (LinearFieldKernels, LinearVectorField, _reverse, dopri5_backprop, fixed_backprop,  # noqa: F401
                            linear_field_of)
-from .mlp_field import MlpFieldKernels, mlp_backprop, mlp_field_of
+from .mlp_field import MlpFieldKernels, dopri5_mlp_backprop, mlp_backprop, mlp_field_of
 from .schedule import FIXED_METHODS, build_schedule, host_locator
 
 
@@ -380,8 +380,10 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     32, channels 8, width 128 with gradients for z0 and its two layers (``mlp_field.MlpBackprop``),
     for the linear field under dopri5 from a recording device-controlled forward and one transposed
     Dormand-Prince launch per record chunk (``linear_field.Dopri5Backprop``; ``cdeint.last_stats["steps"]``
-    then lists the accepted ``(t, dt)``, in ``-t`` for a decreasing ``t``), otherwise through the
-    differentiable generic stage loop.
+    then lists the accepted ``(t, dt)``, in ``-t`` for a decreasing ``t``), for the examples' MLP field
+    under dopri5 at its CUDA-core shapes from a recording host-driven forward and one transposed
+    Dormand-Prince launch per record chunk (``mlp_field.Dopri5MlpBackprop``, same ``last_stats``),
+    otherwise through the differentiable generic stage loop.
 
     ``backend="torchsde"`` is built for ``method="reversible_heun"`` (torchsde's reversible Heun
     method with zero diffusion, fixed step ``dt``, default 1e-3; ``z0`` of shape (batch, hidden),
@@ -488,6 +490,20 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
 
     rtol, atol = kwargs['rtol'], kwargs['atol']
 
+    def host_dopri5_field(owner, y0):
+        """The field of the host-driven dopri5 (before ``_reverse``): the kernel owner's where it answers one evaluation,
+        else the torch operators."""
+        if owner is not None:
+            field = owner.field()
+            try:
+                # one evaluation before the solve: the kernel field refuses a shape (e.g. hidden > 256, or the MLP's
+                # tensor-core shape) on every call, so a field that answers here answers every attempt
+                field(-times[0] if flipped else times[0], y0)
+                return field
+            except NotImplementedError:
+                pass                                          # the torch-operator field takes any shape
+        return _torch_field(X, func, is_prod, sig is not None, z0)
+
     def forward_values(y0):
         """Outputs only, time first, by the fastest route."""
         if method in FIXED_METHODS:
@@ -520,18 +536,7 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                 # host-driven loop below takes it, with the kernel field
                 pass
 
-        field = None
-        owner = kernels if kernels is not None else mlp
-        if owner is not None:
-            field = owner.field()
-            try:
-                # one evaluation before the solve: the kernel field refuses a shape (e.g. hidden > 256, or the MLP's
-                # tensor-core shape) on every call, so a field that answers here answers every attempt
-                field(-times[0] if flipped else times[0], y0)
-            except NotImplementedError:
-                field = None                                  # the torch-operator field takes any shape
-        if field is None:
-            field = _torch_field(X, func, is_prod, sig is not None, z0)
+        field = host_dopri5_field(kernels if kernels is not None else mlp, y0)
         out, solver_obj = adaptive.odeint_dopri5(_reverse(field) if flipped else field, y0, times, rtol, atol, options)
         cdeint.last_stats = {"n_accepted": solver_obj.n_accepted, "n_rejected": solver_obj.n_rejected,
                              "device_controlled": False}
@@ -615,15 +620,28 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                 if ys is not None:
                     return ys
         return _generic_solve(X, func, z0, t, method, step_size, is_prod, sig is not None)
-    if dp5_backprop:
-        def replay(steps):
-            return lambda y0: _time_first_to_reference_layout(
-                adaptive.odeint_dopri5(autograd_field(), y0, times, rtol, atol, options, steps=steps)[0])
+    def replay(steps):
+        return lambda y0: _time_first_to_reference_layout(
+            adaptive.odeint_dopri5(autograd_field(), y0, times, rtol, atol, options, steps=steps)[0])
 
+    if dp5_backprop:
         done = dopri5_backprop(kernels, z0, times, rtol, atol, -1.0 if flipped else 1.0, options.get("first_step"), replay)
         if done is not None:
             ys, cdeint.last_stats = done
             return ys
+    # the examples' MLP field under dopri5: the route of mlp_field.Dopri5MlpBackprop (a recording host-driven forward on
+    # the field the call without gradients uses, one backward launch per record chunk) serves gradients for z0 and the two
+    # layers' weights and biases where its CUDA-core kernels are built for the shape, under the conditions of the
+    # fixed-step route above
+    if (field_params is None and sig is not None and not is_prod and times and not t.requires_grad
+            and not any(b.requires_grad for b in X.buffers())):
+        mlp_params = mlp_field_of(func, z0, sig[2], times)
+        if mlp_params is not None:
+            done = dopri5_mlp_backprop(X, mlp_params, z0, lambda owner: host_dopri5_field(owner, z0), times, rtol, atol,
+                                       -1.0 if flipped else 1.0, options, replay)
+            if done is not None:
+                ys, cdeint.last_stats = done
+                return ys
     targets = None
     if t.requires_grad:
         targets = (-t if flipped else t).to(z0.device)
