@@ -27,7 +27,7 @@ import torchcde_b200 as cde  # noqa: E402
 from test_host_logic import FIXED_SCHEDULES, fixed_schedule_knots  # noqa: E402
 from torchcde_b200 import _lib  # noqa: E402
 from torchcde_b200.linear_field import FixedBackprop, LinearFieldKernels  # noqa: E402
-from torchcde_b200.schedule import backward_tables  # noqa: E402
+from torchcde_b200.schedule import backward_views  # noqa: E402
 
 PATHS, LENGTH, HIDDEN, CHANNELS = 1000, 40, 32, 8
 SAMPLE = [0, 63, 64, 999]
@@ -85,23 +85,18 @@ def compute(dev):
                 X, func, z0, t, step = _problem(dev, sname, "cubic")
                 k = LinearFieldKernels(X, func.linear.weight, func.linear.bias, z0)
                 route = FixedBackprop(k, t, method, step, None)
-                out, dump = route.forward(z0)
+                out, (dump,) = route.forward(z0)
                 sched = route.sched
                 g = _grads(out.shape, dev)
-                n_total = sched.n_steps * sched.n_stages
                 gz = torch.empty(PATHS, HIDDEN, device=dev)
                 kappa = torch.empty_like(dump)
-                tables = backward_tables(sched)
-                floats = torch.cat([tables["step_dt"], tables["stage_frac"], tables["inj_weight"]]).to(dev)
-                ints = torch.cat([tables["stage_index"], tables["inj_range"], tables["inj_out"]]).to(dev)
-                ns, nr = sched.n_steps, tables["inj_range"].numel()
+                v = backward_views(sched, dev)
                 w_t, zeros = k.transposed_weights
                 _lib.call("tcde_cdeint_fixed_linear_backward", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(w_t),
                           _lib.ptr(zeros), _lib.ptr(g), _lib.ptr(gz), _lib.ptr(kappa), PATHS, CHANNELS, HIDDEN,
-                          _lib.METHODS[method], ns, _lib.ptr(floats[:ns]), _lib.ptr(ints[:n_total]),
-                          _lib.ptr(floats[ns:ns + n_total]), sched.n_out, _lib.ptr(ints[n_total:n_total + nr]),
-                          _lib.ptr(ints[n_total + nr:]), _lib.ptr(floats[ns + n_total:]), float(sched.sign), _lib.F32,
-                          _lib.stream_of(g))
+                          _lib.METHODS[method], sched.n_steps, _lib.ptr(v["step_dt"]), _lib.ptr(v["stage_index"]),
+                          _lib.ptr(v["stage_frac"]), sched.n_out, _lib.ptr(v["inj_range"]), _lib.ptr(v["inj_out"]),
+                          _lib.ptr(v["inj_weight"]), float(sched.sign), _lib.F32, _lib.stream_of(g))
                 name = "dump/{}/{}/".format(sname, method)
                 got[name + "out"], got[name + "stages"] = out, dump.transpose(0, 1)
                 got[name + "dl_dz0"], got[name + "kappa"] = gz, kappa.transpose(0, 1)

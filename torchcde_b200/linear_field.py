@@ -7,9 +7,9 @@ import weakref
 
 import torch
 
-from . import _lib, adaptive
+from . import _lib, adaptive, backprop
 from .controls import _control_signature, _schedule_knots
-from .schedule import ScheduleCache, backward_tables, host_locator, locate
+from .schedule import ScheduleCache, backward_views, host_locator, locate
 
 _schedules = ScheduleCache()
 
@@ -323,6 +323,17 @@ class LinearFieldKernels:
         return AdjointStage(self, roles, torch.empty(max(scratch_bytes // 4, 4), dtype=torch.float32, device=self.device))
 
 
+def _backprop_kernels(X, field_params, z0):
+    """The kernels of a problem the linear backprop routes are built for (fp32, hidden 32, channels 8, the control's
+    floating buffers and the parameters fp32 on z0's device), else None: nothing is built, so a mismatched call keeps
+    the torch operators' own dtype and device errors."""
+    if (z0.dtype != torch.float32 or z0.size(-1) != 32 or _control_signature(X)[2] != 8
+            or any(b.dtype != torch.float32 or b.device != z0.device for b in X.buffers() if b.is_floating_point())
+            or any(p is not None and (p.dtype != torch.float32 or p.device != z0.device) for p in field_params)):
+        return None
+    return LinearFieldKernels(X, field_params[0], field_params[1], z0)
+
+
 class FixedBackprop:
     """``cdeint(..., adjoint=False)`` of a fixed-step solve of this linear field with gradients for z0, the weight and /
     or the bias: the exact gradient of the discrete solve in three launches.  The forward is the stage-dump solve
@@ -330,64 +341,51 @@ class FixedBackprop:
     backward is ONE launch of ``tcde_cdeint_fixed_linear_backward`` (the transposed Runge-Kutta recurrence over every
     step, the cotangent kappa of every stage dumped in the forward's slot) and ONE launch of
     ``tcde_linear_field_param_grads`` over the two dumps (neither without a parameter gradient).
-    ``loop(z0)``: the differentiable torch-operator solve of the same problem, which a backward with ``create_graph``
-    differentiates instead (the kernels give no higher-order derivatives)."""
+    ``differentiable(z0)``: the torch-operator solve of the same problem, which a backward with ``create_graph``
+    differentiates instead."""
 
     def __init__(self, kernels, t, method, step_size, loop):
-        self.kernels, self.method, self.loop = kernels, method, loop
+        self.kernels, self.method, self.differentiable = kernels, method, loop
         self.sched, (_floats, _ints, self.views) = _schedules.get(t, kernels.knots, kernels.n_rows, method, step_size,
                                                                   kernels.dtype, kernels.device)
-
-    def fits(self, n_paths, want_params):
-        """Whether the stage dump, and with parameter gradients the kappa dump and the scratch of the parameter-gradient
-        kernel, fit in 0.7 of the free device memory (the bound of ``AdjointStage.segment``)."""
-        k = self.kernels
-        n_total = self.sched.n_steps * self.sched.n_stages
-        need = n_total * n_paths * k.hidden * 4
-        if want_params:
-            scratch_bytes = k.param_grad_scratch_bytes(n_paths, n_total)
-            if scratch_bytes < 0:
-                return False
-            need = 2 * need + scratch_bytes
-        with torch.cuda.device(k.device):
-            free, _total = torch.cuda.mem_get_info()
-        return need <= 0.7 * free
+        self.want_params = any(p is not None and p.requires_grad for p in kernels.field_params)
 
     def forward(self, z0):
-        """(the outputs ``(..., n_out, H)``, the input of every stage ``[n_steps * n_stages][paths][H]``)."""
+        """(the outputs ``(..., n_out, H)``, [the input of every stage ``[n_steps * n_stages][paths][H]``]).  Raises
+        ``NoRoom`` when the stage dump, and with a parameter gradient its kappa copy and the scratch, do not fit."""
         k, sched = self.kernels, self.sched
+        n_total = sched.n_steps * sched.n_stages
+        scratch_bytes = k.param_grad_scratch_bytes(k.n_paths, n_total) if self.want_params else None
+        if not backprop.fits(k.device, n_total * k.n_paths * k.hidden * 4, scratch_bytes):
+            raise backprop.NoRoom()
         with torch.cuda.device(k.device):
             zf = z0.detach().reshape(-1, k.hidden).contiguous()
             out = torch.empty(*z0.shape[:-1], sched.n_out, k.hidden, dtype=k.dtype, device=k.device)
-            dump = torch.empty(sched.n_steps * sched.n_stages, zf.size(0), k.hidden, dtype=k.dtype, device=k.device)
+            dump = torch.empty(n_total, zf.size(0), k.hidden, dtype=k.dtype, device=k.device)
             if zf.size(0) > 0:
                 k._fixed(sched, self.views, k.w, k.b, zf, out.view(-1, sched.n_out, k.hidden), dump)
-        return out, dump
+        return out, [dump]
 
-    def backward(self, g, dump, want_w, want_b):
-        """(dL/dz0, dL/dW or None, dL/db or None) for output gradients ``g`` ``(..., n_out, H)``."""
+    def backward(self, g, z0, saved, want):
+        """(dL/dz0, [dL/dW, dL/db], None where ``want`` is False) for output gradients ``g`` ``(..., n_out, H)``."""
         k, sched = self.kernels, self.sched
+        (dump,), (want_w, want_b) = saved, want
         hidden, dev = k.hidden, k.device
         n_total = sched.n_steps * sched.n_stages
         with torch.cuda.device(dev):
-            gf = g.reshape(-1, sched.n_out, hidden)
-            if not gf.is_contiguous() or gf.data_ptr() % 16:
-                gf = gf.clone(memory_format=torch.contiguous_format)
+            gf = backprop.cotangent(g, sched.n_out, hidden)
             n_paths = gf.size(0)
             gz = torch.empty(n_paths, hidden, dtype=k.dtype, device=dev)
             kappa = torch.empty_like(dump) if want_w or want_b else None
             if n_paths > 0:
-                tables = backward_tables(sched)
-                floats = torch.cat([tables["step_dt"], tables["stage_frac"], tables["inj_weight"]]).to(dev)
-                ints = torch.cat([tables["stage_index"], tables["inj_range"], tables["inj_out"]]).to(dev)
-                ns, nr = sched.n_steps, tables["inj_range"].numel()
+                tables = backward_views(sched, dev)
                 w_t, zeros = k.transposed_weights
                 _lib.call("tcde_cdeint_fixed_linear_backward", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(w_t),
                           _lib.ptr(zeros), _lib.ptr(gf), _lib.ptr(gz), _lib.ptr(kappa), n_paths, k.channels, hidden,
-                          _lib.METHODS[sched.method], ns, _lib.ptr(floats[:ns]), _lib.ptr(ints[:n_total]),
-                          _lib.ptr(floats[ns:ns + n_total]), sched.n_out, _lib.ptr(ints[n_total:n_total + nr]),
-                          _lib.ptr(ints[n_total + nr:]), _lib.ptr(floats[ns + n_total:]), float(sched.sign), _lib.F32,
-                          _lib.stream_of(gf))
+                          _lib.METHODS[sched.method], sched.n_steps, _lib.ptr(tables["step_dt"]),
+                          _lib.ptr(tables["stage_index"]), _lib.ptr(tables["stage_frac"]), sched.n_out,
+                          _lib.ptr(tables["inj_range"]), _lib.ptr(tables["inj_out"]), _lib.ptr(tables["inj_weight"]),
+                          float(sched.sign), _lib.F32, _lib.stream_of(gf))
             gw = torch.zeros_like(k.w) if want_w else None
             gb = torch.zeros_like(k.b) if want_b else None
             if (gw is not None or gb is not None) and n_paths > 0:
@@ -395,50 +393,15 @@ class FixedBackprop:
                 if not k.param_grads(dump, kappa, self.views["stage_index"], self.views["stage_frac"], weights, n_total,
                                      gw, gb):
                     raise RuntimeError("cdeint backward: the parameter-gradient kernel is not built for this problem")
-        return gz.view(g.shape[:-2] + (hidden,)), gw, gb
+        return gz.view(g.shape[:-2] + (hidden,)), [gw, gb]
 
 
-class _FixedBackpropFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, route, z0, weight, bias):
-        out, dump = route.forward(z0)
-        ctx.route = route
-        ctx.save_for_backward(z0, weight, bias, dump)
-        return out
-
-    @staticmethod
-    def backward(ctx, g):
-        z0, weight, bias, dump = ctx.saved_tensors
-        _route_needs, want_z, want_w, want_b = ctx.needs_input_grad
-        if torch.is_grad_enabled():
-            # create_graph: differentiate the torch-operator solve of the same problem, whose gradients are themselves
-            # differentiable
-            inputs = [x for x, want in ((z0, want_z), (weight, want_w), (bias, want_b)) if want]
-            got = iter(torch.autograd.grad(ctx.route.loop(z0), inputs, g, create_graph=True, allow_unused=True))
-            return (None,) + tuple(next(got) if want else None for want in (want_z, want_w, want_b))
-        gz, gw, gb = ctx.route.backward(g, dump, want_w, want_b)
-        return None, gz if want_z else None, gw, gb
-
-
-def fixed_backprop(kernels, z0, t, method, step_size, loop):
+def fixed_backprop(X, field_params, z0, t, method, step_size, loop):
     """``cdeint(..., adjoint=False)``'s outputs ``(..., n_out, H)`` on the three-launch route of ``FixedBackprop``, or
-    None when the route does not serve the problem (the caller runs the torch-operator solve)."""
-    k = kernels
-    if k.dtype != torch.float32 or k.hidden != 32 or k.channels != 8:
-        return None
-    route = FixedBackprop(k, t, method, step_size, loop)
-    want_params = any(p is not None and p.requires_grad for p in (k.weight, k.bias))
-    if not route.fits(k.n_paths, want_params):
-        return None
-    try:
-        return _FixedBackpropFn.apply(route, z0, k.weight, k.bias)
-    except NotImplementedError:
-        # the stage-dump solve refuses the problem (the CUDA-core kernel selected, misaligned rows): nothing ran
-        return None
-
-
-class _NoRoom(Exception):
-    """The record of a recording dopri5 solve would not fit in the device memory."""
+    None when the route does not serve the problem (the caller runs the torch-operator solve ``loop``).  The stage-dump
+    solve refuses the CUDA-core kernel's shapes and misaligned rows before it launches anything."""
+    k = _backprop_kernels(X, field_params, z0)
+    return None if k is None else backprop.run(FixedBackprop(k, t, method, step_size, loop), z0, k.field_params)
 
 
 class Dopri5Backprop:
@@ -453,33 +416,27 @@ class Dopri5Backprop:
     with a parameter gradient, ONE launch of ``tcde_linear_field_param_grads`` over (stage input, kappa); then one launch of
     ``tcde_vector_field_linear_vjp`` closes the start slope f(t0, z0).  ``replay(steps)``: the differentiable
     torch-operator solve of the same problem taking the recorded steps, which a backward with ``create_graph``
-    differentiates instead (the kernels give no higher-order derivatives; the forward cannot know which backward will
-    come, so it records either way).  Memory: the first chunk is checked before the solve starts, each further chunk when
-    the device pauses for it; a chunk that does not fit discards the partial solve and the caller runs the
-    torch-operator solve from the start."""
+    differentiates instead (the forward cannot know which backward will come, so it records either way).  Memory: the
+    first chunk is checked before the solve starts, each further chunk when the device pauses for it; a chunk that does
+    not fit discards the partial solve and the caller runs the torch-operator solve from the start."""
 
     slots = 64                # accepted steps per record chunk
 
-    def __init__(self, kernels, times, rtol, atol, sign, first_step, replay, want_params):
+    def __init__(self, kernels, times, rtol, atol, sign, first_step, replay):
         self.kernels, self.times, self.rtol, self.atol = kernels, list(times), rtol, atol
-        self.sign, self.first_step, self.replay, self.want_params = float(sign), first_step, replay, want_params
+        self.sign, self.first_step, self.replay = float(sign), first_step, replay
+        self.want_params = any(p is not None and p.requires_grad for p in kernels.field_params)
 
-    def _chunk_bytes(self, n_paths):
-        return self.slots * 6 * n_paths * self.kernels.hidden * 4 if self.want_params else 0
+    def differentiable(self, z0):
+        return self.replay(self.steps)(z0)
 
     def fits(self, n_paths):
-        """Whether one more record chunk, the kappa chunk of the backward and the parameter-gradient scratch fit in 0.7 of
-        the free device memory (the bound of ``FixedBackprop.fits``)."""
+        """Whether one more record chunk fits (``backprop.fits``; without a parameter gradient nothing is recorded)."""
         k = self.kernels
-        need = 2 * self._chunk_bytes(n_paths)
-        if self.want_params:
-            scratch_bytes = k.param_grad_scratch_bytes(n_paths, 6 * self.slots)
-            if scratch_bytes < 0:
-                return False
-            need += scratch_bytes
-        with torch.cuda.device(k.device):
-            free, _total = torch.cuda.mem_get_info()
-        return need <= 0.7 * free
+        if not self.want_params:
+            return backprop.fits(k.device, 0)
+        return backprop.fits(k.device, self.slots * 6 * n_paths * k.hidden * 4,
+                             k.param_grad_scratch_bytes(n_paths, 6 * self.slots))
 
     def _new_chunk(self, n_paths):
         k, dev = self.kernels, self.kernels.device
@@ -492,14 +449,13 @@ class Dopri5Backprop:
     def forward(self, z0):
         """(the outputs ``(..., len(times), H)``, the record: per chunk its stage inputs (None without a parameter
         gradient), stage intervals and fractions).  The route keeps only the accepted steps on the host, so the record
-        lives exactly as long as its holder (the autograd Function saves it for the backward).  Raises ``_NoRoom``
-        (nothing kept) when the record does not fit."""
+        lives exactly as long as its holder.  Raises ``NoRoom`` (nothing kept) when the record does not fit."""
         k = self.kernels
         with torch.cuda.device(k.device):
             yf = z0.detach().reshape(-1, k.hidden).contiguous()
             n_paths = yf.size(0)
             if not self.fits(n_paths):
-                raise _NoRoom()
+                raise backprop.NoRoom()
             field = k.field() if self.sign > 0 else _reverse(k.field())
             knots = k.time_knots.detach().to(device=k.device, dtype=torch.float32).contiguous()
             stream = _lib.stream_of(yf)
@@ -515,7 +471,7 @@ class Dopri5Backprop:
 
             def grow(last):                          # the chunk is full: the device resumes on a fresh one
                 if not self.fits(n_paths):
-                    raise _NoRoom()
+                    raise backprop.NoRoom()
                 chunks.append(self._new_chunk(n_paths))
 
             out, _last, stats = adaptive.device_controller(
@@ -526,18 +482,17 @@ class Dopri5Backprop:
             steps = torch.cat([c["step"][:n] for c, n in zip(chunks, self.counts)]).cpu()
             self.steps = [(float(t), float(dt)) for t, dt in steps.tolist()]
         self.stats = dict(stats, device_controlled=True, steps=list(self.steps))
-        record = [(c["z"], c["index"], c["frac"]) for c in chunks]
+        record = [x for c in chunks for x in (c["z"], c["index"], c["frac"])]
         return out.view(*z0.shape[:-1], len(self.times), k.hidden), record
 
-    def backward(self, g, z0, record, want_w, want_b):
-        """(dL/dz0, dL/dW or None, dL/db or None) for output gradients ``g`` ``(..., len(times), H)`` from the solve of
-        ``z0`` and its ``record`` (``forward``'s)."""
+    def backward(self, g, z0, saved, want):
+        """(dL/dz0, [dL/dW, dL/db], None where ``want`` is False) for output gradients ``g`` ``(..., len(times), H)`` from
+        the solve of ``z0`` and its record ``saved`` (``forward``'s)."""
         k = self.kernels
         hidden, dev, n_out = k.hidden, k.device, len(self.times)
+        want_w, want_b = want
         with torch.cuda.device(dev):
-            gf = g.reshape(-1, n_out, hidden)
-            if not gf.is_contiguous() or gf.data_ptr() % 16:
-                gf = gf.clone(memory_format=torch.contiguous_format)
+            gf = backprop.cotangent(g, n_out, hidden)
             n_paths = gf.size(0)
             stream = _lib.stream_of(gf)
             gw = torch.zeros_like(k.w) if want_w else None
@@ -550,8 +505,8 @@ class Dopri5Backprop:
             carry = torch.zeros(2, n_paths, hidden, dtype=torch.float32, device=dev)
             kappa = torch.empty(self.slots * 6, n_paths, hidden, dtype=torch.float32, device=dev) if params else None
             weights = torch.full((self.slots * 6,), self.sign, dtype=torch.float32, device=dev) if params else None
-            for i in range(len(record) - 1, -1, -1):
-                (stage_z, stage_index, stage_frac), n = record[i], self.counts[i]
+            for i in range(len(self.counts) - 1, -1, -1):
+                (stage_z, stage_index, stage_frac), n = saved[3 * i:3 * i + 3], self.counts[i]
                 lo = i * self.slots
                 if n <= 0:
                     continue
@@ -573,47 +528,23 @@ class Dopri5Backprop:
                       _lib.ptr(scratch), n_paths, k.channels, hidden, index, float(frac), 1.0, self.sign, self.sign,
                       _lib.F32, stream)
             gz = carry[0] + vjp + gf[:, 0]
-        return gz.view(g.shape[:-2] + (hidden,)), gw, gb
+        return gz.view(g.shape[:-2] + (hidden,)), [gw, gb]
 
 
-class _Dopri5BackpropFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, route, z0, weight, bias):
-        out, record = route.forward(z0)
-        ctx.route = route                      # host-side metadata only: the record goes through save_for_backward, so a
-        ctx.save_for_backward(z0, weight, bias, *(x for chunk in record for x in chunk))   # backward frees it
-        return out
-
-    @staticmethod
-    def backward(ctx, g):
-        z0, weight, bias, *flat = ctx.saved_tensors
-        record = [tuple(flat[i:i + 3]) for i in range(0, len(flat), 3)]
-        _route_needs, want_z, want_w, want_b = ctx.needs_input_grad
-        if torch.is_grad_enabled():
-            # create_graph: differentiate the torch-operator replay of the recorded steps, whose gradients are themselves
-            # differentiable and belong to the same discrete solve
-            inputs = [x for x, want in ((z0, want_z), (weight, want_w), (bias, want_b)) if want]
-            got = iter(torch.autograd.grad(ctx.route.replay(ctx.route.steps)(z0), inputs, g, create_graph=True,
-                                           allow_unused=True))
-            return (None,) + tuple(next(got) if want else None for want in (want_z, want_w, want_b))
-        gz, gw, gb = ctx.route.backward(g, z0, record, want_w, want_b)
-        return None, gz if want_z else None, gw, gb
-
-
-def dopri5_backprop(kernels, z0, times, rtol, atol, sign, first_step, replay):
+def dopri5_backprop(X, field_params, z0, times, rtol, atol, sign, options, replay):
     """``cdeint(..., adjoint=False)``'s outputs ``(..., len(times), H)`` and statistics on the route of ``Dopri5Backprop``,
     or None when the route does not serve the problem (the caller runs the torch-operator solve).  ``times``: increasing
-    floats (negated when ``sign`` < 0); ``replay(steps)`` returns the torch-operator solve ``z0 -> outputs`` on ``steps``."""
-    k = kernels
-    if k.dtype != torch.float32 or k.hidden != 32 or k.channels != 8 or k.n_paths == 0 or len(times) < 2:
+    floats (negated when ``sign`` < 0); ``options``: the host driver's (the device controller takes ``first_step`` and no
+    ``jump_t``); ``replay(steps)`` returns the torch-operator solve ``z0 -> outputs`` on ``steps``.  The recording solve
+    refuses control rows off a 16-byte boundary before it launches anything."""
+    if options.get("jump_t") or not set(options) <= {"first_step", "jump_t"} or len(times) < 2:
         return None
-    want_params = any(p is not None and p.requires_grad for p in (k.weight, k.bias))
-    route = Dopri5Backprop(k, times, rtol, atol, sign, first_step, replay, want_params)
-    try:
-        return _Dopri5BackpropFn.apply(route, z0, k.weight, k.bias), route.stats
-    except (_NoRoom, NotImplementedError):
-        # the record does not fit, or the recording solve refuses the problem (control rows off a 16-byte boundary)
+    k = _backprop_kernels(X, field_params, z0)
+    if k is None or k.n_paths == 0:
         return None
+    route = Dopri5Backprop(k, times, rtol, atol, sign, options.get("first_step"), replay)
+    ys = backprop.run(route, z0, k.field_params)
+    return None if ys is None else (ys, route.stats)
 
 
 class AdjointStage:
@@ -682,14 +613,9 @@ class AdjointStage:
         tt = torch.tensor([t_hi, t_lo], dtype=torch.float64)
         sched, (_floats, _ints, v) = _schedules.get(tt, k.knots, k.n_rows, method, step_size, dtype, dev)
         n_total = sched.n_steps * sched.n_stages
-        scratch_bytes = k.param_grad_scratch_bytes(n_paths, n_total)
-        if scratch_bytes < 0:
+        if not backprop.fits(dev, n_total * n_paths * hidden * 4, k.param_grad_scratch_bytes(n_paths, n_total)):
             return None
-        need = 2 * n_total * n_paths * hidden * 4
         with torch.cuda.device(dev):
-            free, _total = torch.cuda.mem_get_info()
-            if need + scratch_bytes > 0.7 * free:
-                return None
             w2, b2 = k.adjoint_weights
             z_stages = torch.empty(n_total, n_paths, hidden, dtype=dtype, device=dev)
             a_stages = torch.empty_like(z_stages)

@@ -14,10 +14,10 @@ import weakref
 
 import torch
 
-from . import _lib, adaptive
+from . import _lib, adaptive, backprop
 from .controls import _control_signature, _schedule_knots
-from .linear_field import AdjointStage, _NoRoom, _check_linear_problem, _probe, _reverse, _schedules
-from .schedule import backward_tables, host_locator
+from .linear_field import AdjointStage, _check_linear_problem, _probe, _reverse, _schedules
+from .schedule import backward_views, host_locator
 
 # module -> {training flag: index of the accepted layer ordering, or -1}; kept apart from the linear probe's cache
 _recognised = weakref.WeakKeyDictionary()
@@ -178,19 +178,30 @@ class MlpFieldKernels:
         return hi - lo + (1 if hi == n_steps else 0)
 
     def reversible_param_grads(self, bw, lo, n):
-        """dW1, db1, dW2, db2 += the segment's dump of ``n`` steps from ``lo``: ONE call of ``tcde_mlp_field_param_grads``
-        (its kernel and its fixed-order reduction)."""
-        n_paths = bw.g.size(0)
+        """dW1, db1, dW2, db2 += the segment's dump of ``n`` steps from ``lo`` (``param_grads``, its scratch kept on ``bw``)."""
         if getattr(bw, "scratch", None) is None:
-            nbytes = _lib.load().tcde_mlp_field_param_grads_scratch_bytes(n_paths, bw.dump_z.size(0), self.channels,
-                                                                           self.hidden, self.width)
-            bw.scratch = torch.empty(max(nbytes // 4, 4), dtype=torch.float32, device=self.device)
+            bw.scratch = self.param_grad_scratch(bw.g.size(0), bw.dump_z.size(0))
         v = bw.views
+        self.param_grads(bw.dump_z, bw.dump_a, v["stage_index"][lo:], v["stage_frac"][lo:], n, bw.grads, bw.scratch)
+
+    def param_grad_scratch_bytes(self, n_paths, n_total):
+        return _lib.load().tcde_mlp_field_param_grads_scratch_bytes(n_paths, n_total, self.channels, self.hidden,
+                                                                    self.width)
+
+    def param_grad_scratch(self, n_paths, n_total):
+        """The scratch of ``param_grads`` for ``n_paths`` paths and up to ``n_total`` stages."""
+        return torch.empty(max(self.param_grad_scratch_bytes(n_paths, n_total) // 4, 4), dtype=torch.float32,
+                           device=self.device)
+
+    def param_grads(self, z_stages, a_stages, index, frac, n_total, grads, scratch, weight=1.0):
+        """``grads`` (dW1, db1, dW2, db2, None where not wanted) += ``weight`` times the sum over ``n_total`` stages of
+        a^T df/dtheta at the stage inputs ``z_stages`` and cotangents ``a_stages`` ``[stage][paths][H]`` (``z_stages`` may
+        keep the batch shape): ONE call of ``tcde_mlp_field_param_grads`` (its kernel and its fixed-order reduction)."""
         _lib.call("tcde_mlp_field_param_grads", _lib.ptr(self.control), self.kind, self.n_rows, _lib.ptr(self.w1),
-                  _lib.ptr(self.b1), _lib.ptr(self.w2), _lib.ptr(self.b2), _lib.ptr(bw.dump_z), _lib.ptr(bw.dump_a),
-                  _lib.ptr(v["stage_index"][lo:]), _lib.ptr(v["stage_frac"][lo:]), n, *(_lib.ptr(g) for g in bw.grads),
-                  _lib.ptr(bw.scratch), n_paths, self.channels, self.hidden, self.width, 1.0, 1.0,
-                  _lib.dtype_code(self.dtype), bw.stream)
+                  _lib.ptr(self.b1), _lib.ptr(self.w2), _lib.ptr(self.b2), _lib.ptr(z_stages), _lib.ptr(a_stages),
+                  _lib.ptr(index), _lib.ptr(frac), n_total, *(_lib.ptr(g) for g in grads), _lib.ptr(scratch),
+                  a_stages.size(1), self.channels, self.hidden, self.width, float(weight), 1.0,
+                  _lib.dtype_code(self.dtype), _lib.stream_of(z_stages))
 
     def adjoint_stage(self, params):
         """The adjoint stage of this problem for ``params``, or None when the kernel is not built for it (then autograd
@@ -284,36 +295,25 @@ class MlpBackprop:
     stage-dump solve
     (``tcde_cdeint_fixed_mlp_stages``: the outputs of the same call without gradients, bit for bit); the backward is ONE
     launch of ``tcde_cdeint_fixed_mlp_backward`` (the transposed Runge-Kutta recurrence over every step at the dumped stage
-    inputs) and, with parameter gradients, ONE launch of ``tcde_mlp_field_param_grads`` over the two dumps.  ``loop(z0)``:
-    the differentiable torch-operator solve of the same problem, which a backward with ``create_graph`` differentiates."""
+    inputs) and, with parameter gradients, ONE launch of ``tcde_mlp_field_param_grads`` over the two dumps.
+    ``differentiable(z0)``: the torch-operator solve of the same problem, which a backward with ``create_graph``
+    differentiates instead."""
 
     def __init__(self, kernels, t, method, step_size, loop):
-        self.kernels, self.method, self.loop = kernels, method, loop
+        self.kernels, self.method, self.differentiable = kernels, method, loop
         self.sched, (_floats, _ints, self.views) = _schedules.get(t, kernels.knots, kernels.n_rows, method, step_size,
                                                                   kernels.dtype, kernels.device)
         self.n_total = self.sched.n_steps * self.sched.n_stages
-
-    def scratch_bytes(self, n_paths):
-        k = self.kernels
-        return _lib.load().tcde_mlp_field_param_grads_scratch_bytes(n_paths, self.n_total, k.channels, k.hidden, k.width)
-
-    def fits(self, n_paths, want_params):
-        """Whether the stage dump, and with parameter gradients the kappa dump and the parameter-gradient scratch, fit in
-        0.7 of the free device memory."""
-        k = self.kernels
-        need = self.n_total * n_paths * k.hidden * torch.empty(0, dtype=k.dtype).element_size()
-        if want_params:
-            scratch = self.scratch_bytes(n_paths)
-            if scratch < 0:
-                return False
-            need = 2 * need + scratch
-        with torch.cuda.device(k.device):
-            free, _total = torch.cuda.mem_get_info()
-        return need <= 0.7 * free
+        self.want_params = any(p is not None and p.requires_grad for p in kernels.field_params)
 
     def forward(self, z0):
-        """(the outputs ``(..., n_out, H)``, the input of every stage ``[n_steps * n_stages][paths][H]``)."""
+        """(the outputs ``(..., n_out, H)``, [the input of every stage ``[n_steps * n_stages][paths][H]``]).  Raises
+        ``NoRoom`` when the stage dump, and with a parameter gradient its kappa copy and the scratch, do not fit."""
         k, sched, v = self.kernels, self.sched, self.views
+        scratch_bytes = k.param_grad_scratch_bytes(k.n_paths, self.n_total) if self.want_params else None
+        elt = torch.empty(0, dtype=k.dtype).element_size()
+        if not backprop.fits(k.device, self.n_total * k.n_paths * k.hidden * elt, scratch_bytes):
+            raise backprop.NoRoom()
         with torch.cuda.device(k.device):
             zf = z0.detach().reshape(-1, k.hidden).contiguous()
             out = torch.empty(zf.size(0), sched.n_out, k.hidden, dtype=k.dtype, device=k.device)
@@ -325,86 +325,52 @@ class MlpBackprop:
                           _lib.ptr(v["step_dt"]), _lib.ptr(v["stage_index"]), _lib.ptr(v["stage_frac"]), sched.n_out,
                           _lib.ptr(v["out_step"]), _lib.ptr(v["out_mode"]), _lib.ptr(v["out_slope"]), float(sched.sign),
                           _lib.dtype_code(k.dtype), _lib.stream_of(zf))
-        return out.view(*z0.shape[:-1], sched.n_out, k.hidden), dump
+        return out.view(*z0.shape[:-1], sched.n_out, k.hidden), [dump]
 
-    def backward(self, g, dump, want):
+    def backward(self, g, z0, saved, want):
         """(dL/dz0, [dL/dW1, dL/db1, dL/dW2, dL/db2] with None where ``want`` is False) for output gradients ``g``."""
         k, sched = self.kernels, self.sched
-        hidden, dev, n_total = k.hidden, k.device, self.n_total
+        (dump,), hidden, dev = saved, k.hidden, k.device
         with torch.cuda.device(dev):
-            gf = g.reshape(-1, sched.n_out, hidden)
-            if not gf.is_contiguous() or gf.data_ptr() % 16:
-                gf = gf.clone(memory_format=torch.contiguous_format)
+            gf = backprop.cotangent(g, sched.n_out, hidden)
             n_paths = gf.size(0)
             gz = torch.empty(n_paths, hidden, dtype=k.dtype, device=dev)
             kappa = torch.empty_like(dump) if any(want) else None
             grads = [torch.zeros_like(p) if w else None for p, w in zip((k.w1, k.b1, k.w2, k.b2), want)]
             if n_paths > 0:
-                tables = backward_tables(sched)
-                floats = torch.cat([tables["step_dt"], tables["stage_frac"], tables["inj_weight"]]).to(dev)
-                ints = torch.cat([tables["stage_index"], tables["inj_range"], tables["inj_out"]]).to(dev)
-                ns, nr = sched.n_steps, tables["inj_range"].numel()
+                tables = backward_views(sched, dev)
                 _lib.call("tcde_cdeint_fixed_mlp_backward", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1),
                           _lib.ptr(k.b1), _lib.ptr(k.w2), _lib.ptr(k.b2), _lib.ptr(dump), _lib.ptr(gf), _lib.ptr(gz),
-                          _lib.ptr(kappa), n_paths, k.channels, hidden, k.width, _lib.METHODS[sched.method], ns,
-                          _lib.ptr(floats[:ns]), _lib.ptr(ints[:n_total]), _lib.ptr(floats[ns:ns + n_total]), sched.n_out,
-                          _lib.ptr(ints[n_total:n_total + nr]), _lib.ptr(ints[n_total + nr:]),
-                          _lib.ptr(floats[ns + n_total:]), float(sched.sign), _lib.dtype_code(k.dtype),
-                          _lib.stream_of(gf))
+                          _lib.ptr(kappa), n_paths, k.channels, hidden, k.width, _lib.METHODS[sched.method], sched.n_steps,
+                          _lib.ptr(tables["step_dt"]), _lib.ptr(tables["stage_index"]), _lib.ptr(tables["stage_frac"]),
+                          sched.n_out, _lib.ptr(tables["inj_range"]), _lib.ptr(tables["inj_out"]),
+                          _lib.ptr(tables["inj_weight"]), float(sched.sign), _lib.dtype_code(k.dtype), _lib.stream_of(gf))
                 if kappa is not None:
-                    scratch = torch.empty(max(self.scratch_bytes(n_paths) // 4, 4), dtype=torch.float32, device=dev)
-                    _lib.call("tcde_mlp_field_param_grads", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1),
-                              _lib.ptr(k.b1), _lib.ptr(k.w2), _lib.ptr(k.b2), _lib.ptr(dump), _lib.ptr(kappa),
-                              _lib.ptr(self.views["stage_index"]), _lib.ptr(self.views["stage_frac"]), n_total,
-                              *(_lib.ptr(x) for x in grads), _lib.ptr(scratch), n_paths, k.channels, hidden, k.width,
-                              float(sched.sign), 1.0, _lib.dtype_code(k.dtype), _lib.stream_of(gf))
+                    k.param_grads(dump, kappa, self.views["stage_index"], self.views["stage_frac"], self.n_total, grads,
+                                  k.param_grad_scratch(n_paths, self.n_total), sched.sign)
         return gz.view(g.shape[:-2] + (hidden,)), grads
 
 
-class _MlpBackpropFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, route, z0, *params):
-        out, dump = route.forward(z0)
-        ctx.route = route
-        ctx.save_for_backward(z0, dump, *params)
-        return out
-
-    @staticmethod
-    def backward(ctx, g):
-        z0, dump, *params = ctx.saved_tensors
-        want_z, *want = ctx.needs_input_grad[1:]
-        if torch.is_grad_enabled():
-            # create_graph: differentiate the torch-operator solve of the same problem, whose gradients are themselves
-            # differentiable
-            inputs = [x for x, w in zip([z0] + params, [want_z] + want) if w]
-            got = iter(torch.autograd.grad(ctx.route.loop(z0), inputs, g, create_graph=True, allow_unused=True))
-            return (None,) + tuple(next(got) if w else None for w in [want_z] + want)
-        gz, grads = ctx.route.backward(g, dump, want)
-        return (None, gz if want_z else None) + tuple(grads)
-
-
-def mlp_backprop(X, params, z0, t, method, step_size, loop):
-    """``cdeint(..., adjoint=False)``'s outputs ``(..., n_out, H)`` on the three-launch route of ``MlpBackprop``, or None
-    when the route does not serve the problem (the caller runs the torch-operator solve).  ``params``: (W1, b1, W2, b2)
-    of the recognised field, a bias may be None.  Which shapes, dtypes and solve variants are served is the C dispatch's
-    call: a refusal (``TCDE_ERR_UNSUPPORTED``, as a -1 scratch size or NotImplementedError) keeps the loop."""
+def _backprop_kernels(X, params, z0):
+    """The kernels of a problem the MLP backprop routes may serve (z0 fp32 or fp64 on a CUDA device, the parameters and
+    the control of its dtype and device), else None.  Which shapes, dtypes and solve variants are served is the C
+    dispatch's call: a refusal (``TCDE_ERR_UNSUPPORTED``, as a -1 scratch size or NotImplementedError) keeps the
+    torch-operator solve."""
     if (z0.dtype not in (torch.float32, torch.float64) or not z0.is_cuda
             or any(p is not None and (p.dtype != z0.dtype or p.device != z0.device) for p in params)):
         return None
     k = MlpFieldKernels(X, params, z0)
     if k.control.dtype != z0.dtype or k.control.device != z0.device:
         return None
-    route = MlpBackprop(k, t, method, step_size, loop)
-    present = [p for p in params if p is not None]
-    if not route.fits(k.n_paths, any(p.requires_grad for p in present)):
-        return None
-    # a missing bias is the kernels' zero vector, which wants no gradient
-    leaves = [p if p is not None else b for p, b in zip(params, (k.w1, k.b1, k.w2, k.b2))]
-    try:
-        return _MlpBackpropFn.apply(route, z0, *leaves)
-    except NotImplementedError:
-        # the stage-dump solve refuses the problem (shape, solve variant, misaligned rows): nothing ran
-        return None
+    return k
+
+
+def mlp_backprop(X, params, z0, t, method, step_size, loop):
+    """``cdeint(..., adjoint=False)``'s outputs ``(..., n_out, H)`` on the three-launch route of ``MlpBackprop``, or None
+    when the route does not serve the problem (the caller runs the torch-operator solve ``loop``).  ``params``: (W1, b1,
+    W2, b2) of the recognised field, a bias may be None (the kernels' zero vector, which wants no gradient)."""
+    k = _backprop_kernels(X, params, z0)
+    return None if k is None else backprop.run(MlpBackprop(k, t, method, step_size, loop), z0, params)
 
 
 class _Located:
@@ -468,38 +434,32 @@ class Dopri5MlpBackprop:
     parameter gradient, ONE call of ``tcde_mlp_field_param_grads`` over (input, kappa) of the chunk's evaluations.
     ``replay(steps)``: the differentiable torch-operator solve of the same problem taking the recorded steps, which a
     backward with ``create_graph`` differentiates instead.  Memory: the first chunk is checked before the solve starts and
-    each further one before it is taken; a chunk that does not fit discards the partial solve (``_NoRoom``)."""
+    each further one before it is taken; a chunk that does not fit discards the partial solve (``NoRoom``)."""
 
     slots = 64                # accepted steps per record chunk
 
-    def __init__(self, kernels, field, times, rtol, atol, sign, options, replay, want_params):
+    def __init__(self, kernels, field, times, rtol, atol, sign, options, replay):
         self.kernels, self.field, self.times, self.rtol, self.atol = kernels, field, list(times), rtol, atol
-        self.sign, self.options, self.replay, self.want_params = float(sign), options, replay, want_params
+        self.sign, self.options, self.replay = float(sign), options, replay
+        self.want_params = any(p is not None and p.requires_grad for p in kernels.field_params)
         # a step takes 6 items, 7 with a start slope of its own: only step 0 has one unless jump_t is given
         self.cap = 7 * self.slots if options.get("jump_t") else 6 * self.slots + 1
 
-    def _elt(self):
-        return torch.empty(0, dtype=self.kernels.dtype).element_size()
-
-    def scratch_bytes(self, n_paths):
-        k = self.kernels
-        return _lib.load().tcde_mlp_field_param_grads_scratch_bytes(n_paths, self.cap, k.channels, k.hidden, k.width)
+    def differentiable(self, z0):
+        return self.replay(self.steps)(z0)
 
     def fits(self, n_paths):
-        """Whether one more record chunk and, with a parameter gradient, the kappa chunk of the backward and the
-        parameter-gradient scratch fit in 0.7 of the free device memory (the bound of ``Dopri5Backprop.fits``)."""
+        """Whether one more record chunk fits (``backprop.fits``)."""
         k = self.kernels
-        chunk = self.cap * n_paths * k.hidden * self._elt()
-        need = 2 * chunk + self.scratch_bytes(n_paths) if self.want_params else chunk
-        with torch.cuda.device(k.device):
-            free, _total = torch.cuda.mem_get_info()
-        return need <= 0.7 * free
+        chunk = self.cap * n_paths * k.hidden * torch.empty(0, dtype=k.dtype).element_size()
+        return backprop.fits(k.device, chunk,
+                             k.param_grad_scratch_bytes(n_paths, self.cap) if self.want_params else None)
 
     def room(self):
-        """The chunk the current step records into: a fresh one when the last is full (``_NoRoom`` if it does not fit)."""
+        """The chunk the current step records into: a fresh one when the last is full (``NoRoom`` if it does not fit)."""
         if len(self.chunks[-1]["step_item"]) > self.slots:
             if not self.fits(self.n_paths):
-                raise _NoRoom()
+                raise backprop.NoRoom()
             self._new_chunk()
         return self.chunks[-1]
 
@@ -510,13 +470,13 @@ class Dopri5MlpBackprop:
 
     def forward(self, z0):
         """(the outputs ``(..., len(times), H)``, the record: per chunk its evaluations' inputs, interval indices and
-        fractions and its steps' first items).  Raises ``_NoRoom`` (nothing kept) when the record does not fit."""
+        fractions and its steps' first items).  Raises ``NoRoom`` (nothing kept) when the record does not fit."""
         k = self.kernels
         with torch.cuda.device(k.device), torch.no_grad():
             y0 = z0.detach()
             self.shape, self.n_paths = tuple(y0.shape), k.n_paths
             if not self.fits(self.n_paths):
-                raise _NoRoom()
+                raise backprop.NoRoom()
             self.chunks, self.steps, self.ends = [], [], []
             self._new_chunk()
             located = _Located(self.field, k.where)
@@ -528,25 +488,23 @@ class Dopri5MlpBackprop:
             record = []
             for c in self.chunks:
                 n_items = c["items"]
-                record.append((c["z"][:n_items],
-                               torch.tensor([i for i, _f in c["locs"]] or [0], dtype=torch.int32).to(k.device),
-                               torch.tensor([f for _i, f in c["locs"]] or [0.0], dtype=k.dtype).to(k.device),
-                               torch.tensor(c["step_item"], dtype=torch.int32).to(k.device)))
+                record += [c["z"][:n_items],
+                           torch.tensor([i for i, _f in c["locs"]] or [0], dtype=torch.int32).to(k.device),
+                           torch.tensor([f for _i, f in c["locs"]] or [0.0], dtype=k.dtype).to(k.device),
+                           torch.tensor(c["step_item"], dtype=torch.int32).to(k.device)]
             self.counts = [len(c["step_item"]) - 1 for c in self.chunks]
-            self.chunks = None                 # the record lives as long as its holder (the autograd Function saves it)
+            self.chunks = None                 # the record lives as long as its holder (the autograd shell saves it)
         self.stats = {"n_accepted": solver.n_accepted, "n_rejected": solver.n_rejected, "device_controlled": False,
                       "steps": list(self.steps)}
         return out.movedim(0, -2), record
 
-    def backward(self, g, record, want):
+    def backward(self, g, z0, saved, want):
         """(dL/dz0, [dL/dW1, dL/db1, dL/dW2, dL/db2] with None where ``want`` is False) for output gradients ``g``
-        ``(..., len(times), H)`` from ``forward``'s record."""
+        ``(..., len(times), H)`` from ``forward``'s record ``saved``."""
         k = self.kernels
         hidden, dev, n_out, code = k.hidden, k.device, len(self.times), _lib.dtype_code(k.dtype)
         with torch.cuda.device(dev):
-            gf = g.reshape(-1, n_out, hidden)
-            if not gf.is_contiguous():
-                gf = gf.contiguous()
+            gf = backprop.cotangent(g, n_out, hidden)
             n_paths = gf.size(0)
             stream = _lib.stream_of(gf)
             grads = [torch.zeros_like(p) if w else None for p, w in zip((k.w1, k.b1, k.w2, k.b2), want)]
@@ -556,11 +514,10 @@ class Dopri5MlpBackprop:
             inj_out, inj_w = tables["inj_out"].to(dev), tables["inj_w"].to(dev)
             carry = torch.zeros(2, n_paths, hidden, dtype=k.dtype, device=dev)
             kappa = torch.empty(self.cap, n_paths, hidden, dtype=k.dtype, device=dev) if params else None
-            scratch = (torch.empty(max(self.scratch_bytes(n_paths) // 4, 4), dtype=torch.float32, device=dev)
-                       if params else None)
-            starts = [sum(self.counts[:i]) for i in range(len(record))]
-            for i in range(len(record) - 1, -1, -1):
-                (z, index, frac, step_item), n, lo = record[i], self.counts[i], starts[i]
+            scratch = k.param_grad_scratch(n_paths, self.cap) if params else None
+            starts = [sum(self.counts[:i]) for i in range(len(self.counts))]
+            for i in range(len(self.counts) - 1, -1, -1):
+                (z, index, frac, step_item), n, lo = saved[4 * i:4 * i + 4], self.counts[i], starts[i]
                 if n <= 0:
                     continue
                 _lib.call("tcde_dopri5_mlp_backward", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1),
@@ -569,56 +526,25 @@ class Dopri5MlpBackprop:
                           _lib.ptr(frac), _lib.ptr(inj_range[lo:lo + n + 1]), _lib.ptr(inj_out), _lib.ptr(inj_w), n_out,
                           n, n_paths, k.channels, hidden, k.width, self.sign, code, stream)
                 if params:
-                    _lib.call("tcde_mlp_field_param_grads", _lib.ptr(k.control), k.kind, k.n_rows, _lib.ptr(k.w1),
-                              _lib.ptr(k.b1), _lib.ptr(k.w2), _lib.ptr(k.b2), _lib.ptr(z), _lib.ptr(kappa),
-                              _lib.ptr(index), _lib.ptr(frac), z.size(0), *(_lib.ptr(x) for x in grads),
-                              _lib.ptr(scratch), n_paths, k.channels, hidden, k.width, self.sign, 1.0, code, stream)
+                    k.param_grads(z, kappa, index, frac, z.size(0), grads, scratch, self.sign)
             # step 0's start slope f(t0, z0) was closed by the first chunk's launch: carry[1] is zero
             gz = carry[0] + gf[:, 0]
         return gz.view(g.shape[:-2] + (hidden,)), grads
 
 
-class _Dopri5MlpBackpropFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, route, z0, *params):
-        out, record = route.forward(z0)
-        ctx.route = route                      # host-side metadata only: the record goes through save_for_backward, so a
-        ctx.save_for_backward(z0, *params, *(x for chunk in record for x in chunk))     # backward frees it
-        return out
-
-    @staticmethod
-    def backward(ctx, g):
-        z0, w1, b1, w2, b2, *flat = ctx.saved_tensors
-        record = [tuple(flat[i:i + 4]) for i in range(0, len(flat), 4)]
-        want_z, *want = ctx.needs_input_grad[1:]
-        if torch.is_grad_enabled():
-            # create_graph: differentiate the torch-operator replay of the recorded steps, whose gradients are themselves
-            # differentiable and belong to the same discrete solve
-            inputs = [x for x, w in zip([z0, w1, b1, w2, b2], [want_z] + want) if w]
-            got = iter(torch.autograd.grad(ctx.route.replay(ctx.route.steps)(z0), inputs, g, create_graph=True,
-                                           allow_unused=True))
-            return (None,) + tuple(next(got) if w else None for w in [want_z] + want)
-        gz, grads = ctx.route.backward(g, record, want)
-        return (None, gz if want_z else None) + tuple(grads)
-
-
 def dopri5_mlp_backprop(X, params, z0, field_of, times, rtol, atol, sign, options, replay):
     """``cdeint(..., adjoint=False)``'s outputs ``(..., len(times), H)`` and statistics on the route of
     ``Dopri5MlpBackprop``, or None when the route does not serve the problem (the caller runs the torch-operator dopri5).
-    ``field_of(kernels)``: the dopri5 field of the same call without gradients (before ``_reverse``); ``times``: increasing floats
-    (negated when ``sign`` < 0); ``options``: the host driver's (``jump_t`` oriented like ``times``); ``replay(steps)``
-    returns the torch-operator solve ``z0 -> outputs`` on ``steps``.  Which shapes, dtypes and solve variants are served
-    is the C dispatch's call (``tcde_dopri5_mlp_backward``)."""
-    if (z0.dtype not in (torch.float32, torch.float64) or not z0.is_cuda or len(times) < 2
-            or any(p is not None and (p.dtype != z0.dtype or p.device != z0.device) for p in params)
-            or not set(options) <= {"first_step", "jump_t", "max_num_steps"}):
+    ``field_of(kernels)``: the dopri5 field of the same call without gradients (before ``_reverse``); ``times``: increasing
+    floats (negated when ``sign`` < 0); ``options``: the host driver's (``jump_t`` oriented like ``times``); ``replay(steps)``
+    returns the torch-operator solve ``z0 -> outputs`` on ``steps``."""
+    if len(times) < 2 or not set(options) <= {"first_step", "jump_t", "max_num_steps"}:
         return None
-    k = MlpFieldKernels(X, params, z0)
-    if k.control.dtype != z0.dtype or k.control.device != z0.device or k.n_paths == 0:
+    k = _backprop_kernels(X, params, z0)
+    if k is None or k.n_paths == 0:
         return None
-    want_params = any(p is not None and p.requires_grad for p in params)
-    route = Dopri5MlpBackprop(k, None, times, rtol, atol, sign, options, replay, want_params)
-    if want_params and route.scratch_bytes(k.n_paths) < 0:
+    route = Dopri5MlpBackprop(k, None, times, rtol, atol, sign, options, replay)
+    if route.want_params and k.param_grad_scratch_bytes(k.n_paths, route.cap) < 0:
         return None                            # the parameter-gradient staging does not fit this width
     # the dispatch's verdict on the problem, from a call with no paths (it validates and launches nothing; one small
     # buffer stands in for the per-path and table pointers)
@@ -633,8 +559,5 @@ def dopri5_mlp_backprop(X, params, z0, field_of, times, rtol, atol, sign, option
         return None
     with torch.no_grad():
         route.field = field_of(k)
-    leaves = [q if q is not None else b for q, b in zip(params, (k.w1, k.b1, k.w2, k.b2))]
-    try:
-        return _Dopri5MlpBackpropFn.apply(route, z0, *leaves), route.stats
-    except _NoRoom:
-        return None
+    ys = backprop.run(route, z0, params)
+    return None if ys is None else (ys, route.stats)

@@ -186,6 +186,17 @@ def backward_tables(sched):
     }
 
 
+def backward_views(sched, device):
+    """``backward_tables(sched)`` on ``device`` in two copies: the float tables packed into one buffer, the int tables
+    into another, returned as views named like the tables."""
+    tables = backward_tables(sched)
+    views = {}
+    for names in (("step_dt", "stage_frac", "inj_weight"), ("stage_index", "inj_range", "inj_out")):
+        packed = torch.cat([tables[n] for n in names]).to(device)
+        views.update(zip(names, packed.split([tables[n].numel() for n in names])))
+    return views
+
+
 def build_sde_schedule(t, knots, n_intervals, dt, state_dtype):
     """The schedule of torchsde's fixed-step ``integrate`` loop with the reversible Heun method, in the table format of
     ``build_schedule`` (``tcde_cdeint_reversible_heun_linear`` reads it):

@@ -542,30 +542,22 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                              "device_controlled": False}
         return out
 
-    # adjoint=False with gradients of a linear-field solve: the kernel routes of linear_field.FixedBackprop (fixed step)
-    # and linear_field.Dopri5Backprop (dopri5, controller on the device) serve gradients for z0, the weight and the bias of
-    # an fp32 problem at hidden 32 / channels 8; a gradient for anything else (t, the control's knots or coefficients)
-    # keeps the torch-operator solve
-    served = (field_params is not None and not adjoint and wants_grad
-              and not t.requires_grad and not any(b.requires_grad for b in X.buffers())
-              and z0.dtype == torch.float32 and z0.size(-1) == 32 and sig[2] == 8
-              and all(b.dtype == torch.float32 and b.device == z0.device for b in X.buffers() if b.is_floating_point())
-              and all(p.dtype == torch.float32 and p.device == z0.device for p in field_params if p is not None))
-    backprop = served and method in FIXED_METHODS
-    # dopri5: the options the device controller takes (no jump_t)
-    dp5_backprop = (served and method == "dopri5" and not options.get("jump_t")
-                    and set(options) <= {"first_step", "jump_t"})
-    # the routes that call a kernel own the linear-field problem; building it checks dtypes and devices
+    # adjoint=False with gradients: the kernel routes serve gradients for z0 and the field's parameters; a gradient for
+    # anything else (t, the control's knots or coefficients) keeps the torch-operator solve
+    route_may_serve = (not adjoint and wants_grad and sig is not None and not t.requires_grad
+                       and not any(b.requires_grad for b in X.buffers()))
+    # the routes that call a kernel own the problem; building it checks dtypes and devices (the adjoint=False routes
+    # build their own where they serve the problem)
+    kernel_forward = adjoint or not wants_grad
     kernels = None
-    if field_params is not None and (adjoint or not wants_grad or backprop or dp5_backprop):
+    if field_params is not None and kernel_forward:
         kernels = LinearFieldKernels(X, field_params[0], field_params[1], z0)
-    # the examples' MLP field (no gradient, or adjoint=True): the fixed-step forward is one launch, a dopri5 field
-    # evaluation and an adjoint stage one call each where its CUDA-core kernels serve the shape
-    mlp = None
-    if (field_params is None and sig is not None and not is_prod and times
-            and (adjoint or not wants_grad)):
+    # the examples' MLP field: the fixed-step forward is one launch, a dopri5 field evaluation and an adjoint stage one
+    # call each where its CUDA-core kernels serve the shape
+    mlp_params = mlp = None
+    if field_params is None and sig is not None and not is_prod and times and (kernel_forward or route_may_serve):
         mlp_params = mlp_field_of(func, z0, sig[2], times)
-        if mlp_params is not None:
+        if mlp_params is not None and kernel_forward:
             mlp = MlpFieldKernels(X, mlp_params, z0)
 
     if not wants_grad:
@@ -603,45 +595,32 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                                          fused_vjp, fixed_spec, t_grad, flipped)
         return _time_first_to_reference_layout(ys)
 
-    # adjoint=False: backpropagate through the solver's own operations, like torchdiffeq.odeint
+    # adjoint=False: backpropagate through the solver's own operations, like torchdiffeq.odeint, or through a kernel
+    # route's solve where one serves the problem (linear_field.FixedBackprop / Dopri5Backprop, mlp_field.MlpBackprop /
+    # Dopri5MlpBackprop)
     if method in FIXED_METHODS:
         loop = lambda y0: _generic_solve(X, func, y0, t, method, step_size, is_prod, True)  # noqa: E731
-        if backprop:
-            ys = fixed_backprop(kernels, z0, t, method, step_size, loop)
-            if ys is not None:
-                return ys
-        # the examples' MLP field: the three-launch route of mlp_field.MlpBackprop serves gradients for z0 and the two
-        # layers' weights and biases where its kernels are built for the shape; a gradient for t or the control keeps the loop
-        if (field_params is None and sig is not None and not is_prod and times and not t.requires_grad
-                and not any(b.requires_grad for b in X.buffers())):
-            mlp_params = mlp_field_of(func, z0, sig[2], times)
-            if mlp_params is not None:
-                ys = mlp_backprop(X, mlp_params, z0, t, method, step_size, loop)
-                if ys is not None:
-                    return ys
-        return _generic_solve(X, func, z0, t, method, step_size, is_prod, sig is not None)
+        ys = None
+        if route_may_serve and field_params is not None:
+            ys = fixed_backprop(X, field_params, z0, t, method, step_size, loop)
+        elif route_may_serve and mlp_params is not None:
+            ys = mlp_backprop(X, mlp_params, z0, t, method, step_size, loop)
+        return ys if ys is not None else _generic_solve(X, func, z0, t, method, step_size, is_prod, sig is not None)
+
     def replay(steps):
         return lambda y0: _time_first_to_reference_layout(
             adaptive.odeint_dopri5(autograd_field(), y0, times, rtol, atol, options, steps=steps)[0])
 
-    if dp5_backprop:
-        done = dopri5_backprop(kernels, z0, times, rtol, atol, -1.0 if flipped else 1.0, options.get("first_step"), replay)
-        if done is not None:
-            ys, cdeint.last_stats = done
-            return ys
-    # the examples' MLP field under dopri5: the route of mlp_field.Dopri5MlpBackprop (a recording host-driven forward on
-    # the field the call without gradients uses, one backward launch per record chunk) serves gradients for z0 and the two
-    # layers' weights and biases where its CUDA-core kernels are built for the shape, under the conditions of the
-    # fixed-step route above
-    if (field_params is None and sig is not None and not is_prod and times and not t.requires_grad
-            and not any(b.requires_grad for b in X.buffers())):
-        mlp_params = mlp_field_of(func, z0, sig[2], times)
-        if mlp_params is not None:
-            done = dopri5_mlp_backprop(X, mlp_params, z0, lambda owner: host_dopri5_field(owner, z0), times, rtol, atol,
-                                       -1.0 if flipped else 1.0, options, replay)
-            if done is not None:
-                ys, cdeint.last_stats = done
-                return ys
+    sign, done = -1.0 if flipped else 1.0, None
+    if route_may_serve and field_params is not None:
+        done = dopri5_backprop(X, field_params, z0, times, rtol, atol, sign, options, replay)
+    elif route_may_serve and mlp_params is not None:
+        # the dopri5 field of the same call without gradients
+        done = dopri5_mlp_backprop(X, mlp_params, z0, lambda owner: host_dopri5_field(owner, z0), times, rtol, atol, sign,
+                                   options, replay)
+    if done is not None:
+        ys, cdeint.last_stats = done
+        return ys
     targets = None
     if t.requires_grad:
         targets = (-t if flipped else t).to(z0.device)
