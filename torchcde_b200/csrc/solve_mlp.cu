@@ -7,6 +7,7 @@
 //   * cdeint_mlp_simt_kernel<T, HM, DUMP> (fp32 / fp64, H <= HM, any C and W): one thread per path on the CUDA cores; the
 //     fp64 instantiation is the reference solve of the parity tests.
 // Each has a stage-dump variant, a Runge-Kutta backward and a parameter-gradient kernel for cdeint(..., adjoint=False).
+#include <optional>
 #include <type_traits>
 
 #include "wg_common.cuh"
@@ -267,36 +268,45 @@ __global__ void __launch_bounds__(kMlpSimtThreads) cdeint_mlp_simt_kernel(const 
     }
 }
 
-// The layout of a CUDA-core kernel: the weights staged when everything fits in kMax bytes, else read from global memory
+// The layout of a CUDA-core kernel of nt threads per CTA with `extra` values per thread after the slopes: the weights
+// staged when everything fits in kMlpSimtMaxSmem bytes, else read from global memory; none if neither fits
 constexpr size_t kMlpSimtMaxSmem = 200 * 1024;
-template <typename T> static int mlp_simt_pick_layout(int H, int C, int W, MlpSimtLayout<T>& lay, int extra = 0) {
-    lay = mlp_simt_layout<T>(H, C, W, true, kMlpSimtThreads, extra);
-    if (lay.total > kMlpSimtMaxSmem) lay = mlp_simt_layout<T>(H, C, W, false, kMlpSimtThreads, extra);
-    TCDE_CHECK_SUPPORTED(lay.total <= kMlpSimtMaxSmem, "MLP solve: hidden=%d channels=%d do not fit the CUDA-core "
-                         "kernel's shared memory", H, C);
-    return TCDE_OK;
+template <typename T>
+static std::optional<MlpSimtLayout<T>> mlp_simt_fit(int H, int C, int W, int nt, int extra) {
+    for (const bool stage : {true, false}) {
+        const MlpSimtLayout<T> lay = mlp_simt_layout<T>(H, C, W, stage, nt, extra);
+        if (lay.total <= kMlpSimtMaxSmem) return lay;
+    }
+    return std::nullopt;
 }
 
-template <typename T, int HM>
-static int launch_mlp_simt(const MlpArgs<T>& a, T* stage_dump, cudaStream_t stream) {
-    auto kern = stage_dump ? cdeint_mlp_simt_kernel<T, HM, true> : cdeint_mlp_simt_kernel<T, HM, false>;
-    MlpSimtLayout<T> lay;
-    const int rc = mlp_simt_pick_layout<T>(a.H, a.C, a.W, lay);
-    if (rc != TCDE_OK) return rc;
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
-    const int64_t ctas = (a.n_paths + kMlpSimtThreads - 1) / kMlpSimtThreads;
-    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
-    kern<<<(unsigned)ctas, kMlpSimtThreads, lay.total, stream>>>(a, lay, stage_dump);
+// kern<<<grid, threads, smem, s>>>(args...), with smem bytes of dynamic shared memory allowed
+template <typename... P, typename... A>
+static int mlp_launch(void (*kern)(P...), int64_t grid, int threads, size_t smem, cudaStream_t s, const A&... args) {
+    if (smem > 0) TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
+    kern<<<(unsigned)grid, threads, smem, s>>>(args...);
     TCDE_CHECK_CUDA(cudaGetLastError());
     return TCDE_OK;
 }
 
-template <typename T>
-static int solve_mlp_simt(const MlpArgs<T>& a, cudaStream_t stream, T* stage_dump = nullptr) {
-    TCDE_CHECK_SUPPORTED(a.H <= 32, "MLP solve: hidden=%d > 32 is not built for the CUDA-core kernel", a.H);
-    if (a.H <= 8) return launch_mlp_simt<T, 8>(a, stage_dump, stream);
-    return launch_mlp_simt<T, 32>(a, stage_dump, stream);
+// kern(a, layout, args...) on the CUDA cores: one thread per path in CTAs of nt threads, the layout fitted for them
+template <typename T, typename... P, typename... A>
+static int mlp_launch_simt(void (*kern)(P...), const MlpArgs<T>& a, int nt, int extra, cudaStream_t s,
+                           const A&... args) {
+    const auto lay = mlp_simt_fit<T>(a.H, a.C, a.W, nt, extra);
+    TCDE_CHECK_SUPPORTED(lay.has_value(), "MLP kernel on the CUDA cores: hidden=%d channels=%d width=%d do not fit its "
+                         "shared memory", a.H, a.C, a.W);
+    return mlp_launch(kern, (a.n_paths + nt - 1) / nt, nt, lay->total, s, a, *lay, args...);
 }
+
+// f(std::integral_constant<int, HM>()) at the CUDA-core instantiation hm (8 or 32)
+template <typename F> static int mlp_hm(int hm, F&& f) {
+    return hm == 8 ? f(std::integral_constant<int, 8>()) : f(std::integral_constant<int, 32>());
+}
+
+// f(T()) at the element type of dtype: float for TCDE_F32, else double (the checks have refused every other code)
+template <typename F> static int mlp_dtype(int dtype, F&& f) { return dtype == TCDE_F32 ? f(float()) : f(double()); }
 
 // ---- the backward of the CUDA-core solve (cdeint(..., adjoint=False)): one thread per path ---------------------------
 //
@@ -468,20 +478,6 @@ __global__ void __launch_bounds__(kMlpSimtThreads) cdeint_mlp_simt_backward_kern
     }
 }
 
-template <typename T, int HM>
-static int launch_mlp_simt_backward(const MlpArgs<T>& a, const MlpSimtBwd<T>& b, cudaStream_t stream) {
-    auto kern = cdeint_mlp_simt_backward_kernel<T, HM>;
-    MlpSimtLayout<T> lay;
-    const int rc = mlp_simt_pick_layout<T>(a.H, a.C, a.W, lay);
-    if (rc != TCDE_OK) return rc;
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
-    const int64_t ctas = (a.n_paths + kMlpSimtThreads - 1) / kMlpSimtThreads;
-    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
-    kern<<<(unsigned)ctas, kMlpSimtThreads, lay.total, stream>>>(a, lay, b);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
-}
-
 // ---- the parameter gradients of the CUDA-core backward ---------------------------------------------------------------
 //
 //   dW2 = sum_e g_e h_e^T,  db2 = sum_e g_e,  dW1 = sum_e ub_e z_e^T,  db1 = sum_e ub_e
@@ -515,10 +511,11 @@ template <typename T> static MlpSimtPg mlp_simt_pg_layout(const MlpSimtLayout<T>
     return p;
 }
 
-// The widest block (128, 64 or 32 items) whose staging fits, with the weights staged if they fit too; false if none does
+// The widest block (ni_max, ni_max / 2, ... 32 items) whose staging fits, with the weights staged if they fit too; false
+// if none does.  Not mlp_simt_fit: the staging after the columns decides, and its rows are ni + 1 elements apart.
 template <typename T>
-static bool mlp_simt_pg_pick(int H, int C, int W, MlpSimtLayout<T>& lay, MlpSimtPg& pg) {
-    for (int ni = kMlpSimtThreads; ni >= 32; ni /= 2) {
+static bool mlp_simt_pg_pick(int H, int C, int W, int ni_max, MlpSimtLayout<T>& lay, MlpSimtPg& pg) {
+    for (int ni = ni_max; ni >= 32; ni /= 2) {
         for (int stage = 1; stage >= 0; --stage) {
             lay = mlp_simt_layout<T>(H, C, W, stage != 0, ni);
             pg = mlp_simt_pg_layout<T>(lay, H, C, W, ni);
@@ -656,9 +653,8 @@ template <typename T> struct MlpFieldEval {
 template <typename T, int HM, bool VJP> __host__ __device__ constexpr bool mlp_field_kv_shared() {
     return VJP && sizeof(T) == 8 && HM == 32;
 }
-static int mlp_field_extra_shared(int H) { return 2 * H + (H + 3) / 4 * 4; }
 template <typename T, int HM, bool VJP> static int mlp_field_extra(int H) {
-    return !VJP ? 0 : mlp_field_kv_shared<T, HM, VJP>() ? mlp_field_extra_shared(H) : H;
+    return !VJP ? 0 : mlp_field_kv_shared<T, HM, VJP>() ? 2 * H + (H + 3) / 4 * 4 : H;
 }
 
 // a.z0: z [n_paths][H]; a.out: f_scale f [n_paths][H]; a.sign = 1
@@ -2096,57 +2092,6 @@ __global__ void mlp_param_reduce_kernel(const float* scratch, int n_parts, float
 }  // namespace mlp
 }  // namespace tc
 
-static bool mlp_tc_shape(int64_t H, int64_t C, int64_t W) { return H == tc::kHid && C == tc::kCh && W == tc::mlp::kWidth; }
-
-// cdeint_mlp_wgmma_kernel, with a stage dump when u.stage_dump is set
-static int launch_mlp_tc(const UmmaArgs& u, const float* w2, const float* b2, cudaStream_t s) {
-    const int64_t grid = (u.n_paths + tc::mlp::kPaths - 1) / tc::mlp::kPaths;
-    TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
-    auto kern = u.stage_dump ? tc::mlp::cdeint_mlp_wgmma_kernel<true> : tc::mlp::cdeint_mlp_wgmma_kernel<false>;
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::mlp::kSmem));
-    kern<<<(unsigned)grid, tc::mlp::kThreads, tc::mlp::kSmem, s>>>(u, w2, b2);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
-}
-
-// Where automatic selection runs the CUDA-core kernel: the shapes at which it measured faster than cdeint's stage loop on
-// an H100 (DESIGN 4.2): at most 8 hidden units (the HM = 8 instantiation) or one chunk of outputs (H C <= 32).  Elsewhere
-// it recomputes the first product per chunk of 32 outputs and runs at low occupancy, and was 1.3-4.5x (fp32) and up to
-// 13.6x (fp64) slower than the loop, so automatic selection refuses the shape and the caller keeps its stage loop.
-static bool mlp_simt_preferred(int64_t H, int64_t C) { return H <= 8 || H * C <= kMlpChunk; }
-
-// What the stage-dump solve, its backward and the parameter gradients are built for: fp32 at 32 / 8 / 128 under a solve
-// variant that runs the tensor-core kernel (0, 4, 5)
-static int check_mlp_backprop(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what) {
-    const int variant = current_solve_variant();
-    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && mlp_tc_shape(hidden, channels, width) && (variant == 0 || variant >= 4) &&
-                             variant != 6,
-                         "%s is built for fp32, hidden=32, channels=8, width=128 on the tensor-core kernel (got dtype=%d, "
-                         "%lld, %lld, %lld, solve variant %d)", what, dtype, (long long)hidden, (long long)channels,
-                         (long long)width, variant);
-    return TCDE_OK;
-}
-
-// Which kernels the stage-dump solve, its backward and the parameter gradients run: the CUDA-core ones (*simt = true) at
-// shapes where the CUDA-core forward runs by default (mlp_simt_preferred; fp32 or fp64, solve variant 0 or 1), the
-// tensor-core ones at fp32 32 / 8 / 128 under variant 0, 4 or 5 (check_mlp_backprop); TCDE_ERR_UNSUPPORTED otherwise.
-// Variant 1 serves only the shapes mlp_simt_preferred admits, so that elsewhere the caller keeps its own loop.  By default
-// the CUDA-core route also needs hidden <= 8 (the HM = 8 instantiations): at hidden 32, channels 1 a training step on it
-// measured slower per sequence than the torch-operator loop on an H100 (DESIGN 4.2), so variant 1 alone runs HM = 32.
-static int mlp_backprop_route(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what, bool* simt) {
-    TCDE_CHECK_ARG(channels >= 1 && hidden >= 1 && width >= 1, "bad sizes");
-    TCDE_CHECK_SUPPORTED(width < (1 << 20) && channels < (1 << 20) && hidden * channels < (1 << 20), "MLP too wide");
-    *simt = mlp_simt_preferred(hidden, channels);
-    if (!*simt) return check_mlp_backprop(hidden, channels, width, dtype, what);
-    const int variant = current_solve_variant();
-    TCDE_CHECK_SUPPORTED(hidden <= 8 || variant == 1, "%s: at hidden=%lld the CUDA-core route is slower than the stage "
-                         "loop; automatic selection does not run it (variant 1 forces it)", what, (long long)hidden);
-    TCDE_CHECK_SUPPORTED((dtype == TCDE_F32 || dtype == TCDE_F64) && variant <= 1 && width >= 1 && width < (1 << 20),
-                         "%s on the CUDA cores is built for fp32 / fp64 under solve variant 0 or 1 (got dtype=%d, "
-                         "width %lld, solve variant %d)", what, dtype, (long long)width, variant);
-    return TCDE_OK;
-}
-
 template <typename T>
 static MlpArgs<T> mlp_simt_args(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
                                 const void* w2, const void* b2, const void* z0, void* out, int64_t n_paths,
@@ -2158,12 +2103,6 @@ static MlpArgs<T> mlp_simt_args(const void* control, int control_kind, int64_t n
                       (const T*)step_dt, stage_index, (const T*)stage_frac, out_step, out_mode, (const T*)out_slope,
                       n_paths, n_rows, (int)channels, (int)hidden, (int)width, control_kind, method, n_stages,
                       (int)n_steps, (int)n_out, (T)sign};
-}
-
-template <typename T>
-static int mlp_simt_backward(const MlpArgs<T>& a, const MlpSimtBwd<T>& b, cudaStream_t s) {
-    if (a.H <= 8) return launch_mlp_simt_backward<T, 8>(a, b, s);
-    return launch_mlp_simt_backward<T, 32>(a, b, s);
 }
 
 // the persistent grid of mlp_simt_param_grad_kernel (independent of the dtype: the scratch size has no dtype)
@@ -2179,106 +2118,44 @@ static int64_t mlp_simt_param_grid(int64_t n_paths, int64_t n_total, int ni) {
 static int mlp_simt_param_items(int64_t H, int64_t C, int64_t W) {
     MlpSimtLayout<double> lay;
     MlpSimtPg pg;
-    return mlp_simt_pg_pick<double>((int)H, (int)C, (int)W, lay, pg) ? pg.ni : 0;
-}
-
-template <typename T, int HM>
-static int launch_mlp_simt_param_grads(const MlpArgs<T>& a, const MlpSimtPgArgs<T>& p, int64_t grid, int ni,
-                                       cudaStream_t s) {
-    auto kern = mlp_simt_param_grad_kernel<T, HM>;
-    MlpSimtLayout<T> lay;
-    MlpSimtPg pg;
-    // the same block width as the scratch was sized for; fp32 may then also stage the weights
-    lay = mlp_simt_layout<T>(a.H, a.C, a.W, true, ni);
-    pg = mlp_simt_pg_layout<T>(lay, a.H, a.C, a.W, ni);
-    if (pg.total > kMlpSimtMaxSmem) {
-        lay = mlp_simt_layout<T>(a.H, a.C, a.W, false, ni);
-        pg = mlp_simt_pg_layout<T>(lay, a.H, a.C, a.W, ni);
-    }
-    TCDE_CHECK_SUPPORTED(pg.total <= kMlpSimtMaxSmem, "MLP parameter gradients: the shape does not fit");
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pg.total));
-    kern<<<(unsigned)grid, ni, pg.total, s>>>(a, lay, pg, p);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
+    return mlp_simt_pg_pick<double>((int)H, (int)C, (int)W, kMlpSimtThreads, lay, pg) ? pg.ni : 0;
 }
 
 template <typename T>
-static int mlp_simt_param_grads(const MlpArgs<T>& a, const T* z_stages, const T* kappa, int64_t n_total, void* grad_w1,
-                                void* grad_b1, void* grad_w2, void* grad_b2, void* scratch, double scale,
+static int mlp_simt_param_grads(const MlpArgs<T>& a, int hm, const T* z_stages, const T* kappa, int64_t n_total,
+                                void* grad_w1, void* grad_b1, void* grad_w2, void* grad_b2, void* scratch, double scale,
                                 cudaStream_t s) {
     const int ni = mlp_simt_param_items(a.H, a.C, a.W);
     TCDE_CHECK_SUPPORTED(ni > 0, "MLP parameter gradients: hidden=%d channels=%d width=%d do not fit the CUDA-core "
                          "kernel's shared memory", a.H, a.C, a.W);
+    // the same block width as the scratch was sized for; fp32 may then also stage the weights
+    MlpSimtLayout<T> lay;
+    MlpSimtPg pg;
+    TCDE_CHECK_SUPPORTED(mlp_simt_pg_pick<T>(a.H, a.C, a.W, ni, lay, pg) && pg.ni == ni,
+                         "MLP parameter gradients: the shape does not fit");
     const int64_t grid = mlp_simt_param_grid(a.n_paths, n_total, ni);
     const int64_t n_params = mlp_simt_n_params(a.H, a.C, a.W);
     const MlpSimtPgArgs<T> p{z_stages, kappa, (T*)scratch, n_params, (int)n_total};
-    const int rc = a.H <= 8 ? launch_mlp_simt_param_grads<T, 8>(a, p, grid, ni, s)
-                            : launch_mlp_simt_param_grads<T, 32>(a, p, grid, ni, s);
-    if (rc != TCDE_OK) return rc;
-    if (grad_w1 || grad_b1 || grad_w2 || grad_b2) {
-        const int64_t o_b1 = (int64_t)a.W * a.H, o_w2 = o_b1 + a.W, o_b2 = o_w2 + (int64_t)a.H * a.C * a.W;
-        mlp_simt_param_reduce_kernel<T><<<(unsigned)((n_params + 255) / 256), 256, 0, s>>>(
-            (const T*)scratch, (int)grid, n_params, o_b1, o_w2, o_b2, (T)scale, (T*)grad_w1, (T*)grad_b1, (T*)grad_w2,
-            (T*)grad_b2);
-        TCDE_CHECK_CUDA(cudaGetLastError());
-    }
-    return TCDE_OK;
-}
-
-// The shapes tcde_vector_field_mlp[_vjp] are built for: those where mlp_backprop_route runs the CUDA cores, the
-// parameter-gradient staging included, so that a stage the scratch query admits runs every call.  By default they serve
-// only fp32 with hidden * channels <= 32 (one chunk of outputs: the first product is formed once per pass) and width <=
-// 128, where an adjoint=True training step on them measured faster than autograd per stage on an H100 (DESIGN 8);
-// fp64, channels 14 and width 366 at hidden 8 measured 0.13-0.83x of autograd's speed, so automatic selection refuses
-// them and solve variant 1 forces them (as it does for the HM = 32 kernels)
-static int mlp_field_route(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what) {
-    bool simt;
-    const int rc = mlp_backprop_route(hidden, channels, width, dtype, what, &simt);
-    if (rc != TCDE_OK) return rc;
-    TCDE_CHECK_SUPPORTED(simt, "%s is built for the CUDA-core shapes (hidden <= 8, or hidden * channels <= 32 under solve "
-                         "variant 1; got %lld, %lld, %lld)", what, (long long)hidden, (long long)channels,
-                         (long long)width);
-    TCDE_CHECK_SUPPORTED(current_solve_variant() == 1 || (dtype == TCDE_F32 && hidden * channels <= kMlpChunk &&
-                                                          width <= 128),
-                         "%s: at dtype=%d hidden=%lld channels=%lld width=%lld it is slower than autograd per stage; "
-                         "automatic selection does not run it (variant 1 forces it)", what, dtype, (long long)hidden,
-                         (long long)channels, (long long)width);
-    // the largest field layout: fp64, unstaged, with the HM = 32 vjp's shared columns past hidden 8
-    const int extra = hidden > 8 ? mlp_field_extra_shared((int)hidden) : (int)hidden;
-    TCDE_CHECK_SUPPORTED(mlp_simt_param_items(hidden, channels, width) > 0 &&
-                             mlp_simt_layout<double>((int)hidden, (int)channels, (int)width, false, kMlpSimtThreads,
-                                                     extra).total <= kMlpSimtMaxSmem,
-                         "%s: hidden=%lld channels=%lld width=%lld do not fit the CUDA-core kernels' shared memory", what,
-                         (long long)hidden, (long long)channels, (long long)width);
-    return TCDE_OK;
+    const int rc = mlp_hm(hm, [&](auto HM) {
+        return mlp_launch(mlp_simt_param_grad_kernel<T, HM.value>, grid, ni, pg.total, s, a, lay, pg, p);
+    });
+    if (rc != TCDE_OK || !(grad_w1 || grad_b1 || grad_w2 || grad_b2)) return rc;
+    const int64_t o_b1 = (int64_t)a.W * a.H, o_w2 = o_b1 + a.W, o_b2 = o_w2 + (int64_t)a.H * a.C * a.W;
+    return mlp_launch(mlp_simt_param_reduce_kernel<T>, (n_params + 255) / 256, 256, 0, s, (const T*)scratch, (int)grid,
+                      n_params, o_b1, o_w2, o_b2, (T)scale, (T*)grad_w1, (T*)grad_b1, (T*)grad_w2, (T*)grad_b2);
 }
 
 // the parameter-gradient scratch of tcde_vector_field_mlp_vjp starts after the stage's (index, frac)
 constexpr int64_t kMlpFieldScratchHead = 16;
 
-template <typename T, int HM, bool VJP>
-static int launch_mlp_field(const MlpArgs<T>& a, const MlpFieldEval<T>& e, cudaStream_t s) {
-    auto kern = mlp_field_kernel<T, HM, VJP>;
-    MlpSimtLayout<T> lay;
-    const int rc = mlp_simt_pick_layout<T>(a.H, a.C, a.W, lay, mlp_field_extra<T, HM, VJP>(a.H));
-    if (rc != TCDE_OK) return rc;
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
-    const int64_t ctas = (a.n_paths + kMlpSimtThreads - 1) / kMlpSimtThreads;
-    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
-    kern<<<(unsigned)ctas, kMlpSimtThreads, lay.total, s>>>(a, lay, e);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
-}
-
 // One field evaluation (no cotangent) or one adjoint stage: at most three launches (the field kernel, then with a
 // parameter gradient mlp_simt_param_grad_kernel over this one stage and mlp_simt_param_reduce_kernel)
 template <typename T>
-static int mlp_field_eval(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
+static int mlp_field_eval(int hm, const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
                           const void* w2, const void* b2, const void* z, void* f_out, int64_t n_paths, int64_t channels,
                           int64_t hidden, int64_t width, int32_t index, double frac, const void* adj, void* vjp_out,
                           void* grad_w1, void* grad_b1, void* grad_w2, void* grad_b2, void* scratch, double f_scale,
                           double vjp_scale, double grad_scale, cudaStream_t s) {
-    const bool vjp = adj != nullptr;
     const bool grads = grad_w1 || grad_b1 || grad_w2 || grad_b2;
     int32_t* q_index = grads ? static_cast<int32_t*>(scratch) : nullptr;
     T* q_frac = grads ? reinterpret_cast<T*>(static_cast<char*>(scratch) + 8) : nullptr;
@@ -2286,107 +2163,17 @@ static int mlp_field_eval(const void* control, int control_kind, int64_t n_rows,
                                           hidden, width, TCDE_EULER, 1, nullptr, q_index, q_frac, 1, nullptr, nullptr,
                                           nullptr, 1.0);
     const MlpFieldEval<T> e{(const T*)adj, (T*)vjp_out, q_index, q_frac, index, (T)frac, (T)f_scale, (T)vjp_scale};
-    int rc;
-    if (!vjp) rc = hidden <= 8 ? launch_mlp_field<T, 8, false>(a, e, s) : launch_mlp_field<T, 32, false>(a, e, s);
-    else rc = hidden <= 8 ? launch_mlp_field<T, 8, true>(a, e, s) : launch_mlp_field<T, 32, true>(a, e, s);
+    const auto field = [&](auto vjp) {
+        constexpr bool VJP = decltype(vjp)::value;
+        return mlp_hm(hm, [&](auto HM) {
+            return mlp_launch_simt(mlp_field_kernel<T, HM.value, VJP>, a, kMlpSimtThreads,
+                                   mlp_field_extra<T, HM.value, VJP>(a.H), s, e);
+        });
+    };
+    const int rc = adj == nullptr ? field(std::false_type()) : field(std::true_type());
     if (rc != TCDE_OK || !grads) return rc;
-    return mlp_simt_param_grads(a, (const T*)z, (const T*)adj, 1, grad_w1, grad_b1, grad_w2, grad_b2,
+    return mlp_simt_param_grads(a, hm, (const T*)z, (const T*)adj, 1, grad_w1, grad_b1, grad_w2, grad_b2,
                                 static_cast<char*>(scratch) + kMlpFieldScratchHead, grad_scale, s);
-}
-
-// The layouts of the reversible Heun forward and segment backward at the HM the dispatch picks for H: the weights staged
-// when everything fits, else read from global memory; false if neither fits
-template <typename T, int HM> static bool mlp_rev_fwd_layout(int H, int C, int W, MlpSimtLayout<T>& lay) {
-    for (int stage = 1; stage >= 0; --stage) {
-        lay = mlp_simt_layout<T>(H, C, W, stage != 0, kMlpSimtThreads, mlp_rev_fwd_extra<T, HM>(H));
-        if (lay.total <= kMlpSimtMaxSmem) return true;
-    }
-    return false;
-}
-template <typename T, int HM> static bool mlp_rev_bwd_layout(int H, int C, int W, MlpSimtLayout<T>& lay) {
-    for (int stage = 1; stage >= 0; --stage) {
-        lay = mlp_simt_layout<T>(H, C, W, stage != 0, mlp_rev_bwd_threads<HM>(), mlp_rev_bwd_extra<HM>(H));
-        if (lay.total <= kMlpSimtMaxSmem) return true;
-    }
-    return false;
-}
-
-// Where tcde_cdeint_reversible_heun_mlp and tcde_reversible_heun_mlp_backward_segment run: the CUDA-core route of
-// mlp_backprop_route (hidden <= 8 by default; variant 4 and the tensor-core shape refused), by default only at hidden *
-// channels <= 32 (one chunk of outputs), fp32 and fp64, at widths where the parameter-gradient staging and both kernels'
-// columns fit shared memory.  A training step on it measured faster than the torch-operator forward and per-step autograd
-// it replaces at (8, 3, 128) fp32 and fp64 and at (5, 3, 37) on an H100, but 7.7x slower at (8, 14, 128) (four chunks:
-// the backward recomputes the first product per chunk, and its parameter gradients stage 112 outputs per item), so
-// automatic selection refuses more than one chunk of outputs and solve variant 1 forces every shape the kernels are built
-// for (DESIGN, "torchsde backend").  TCDE_ERR_UNSUPPORTED elsewhere, so that the caller keeps the torch-operator route.
-static int mlp_reversible_route(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what) {
-    bool simt;
-    const int rc = mlp_backprop_route(hidden, channels, width, dtype, what, &simt);
-    if (rc != TCDE_OK) return rc;
-    TCDE_CHECK_SUPPORTED(simt, "%s is built for the CUDA-core shapes (hidden <= 8, or hidden * channels <= 32 under solve "
-                         "variant 1; got %lld, %lld, %lld)", what, (long long)hidden, (long long)channels,
-                         (long long)width);
-    TCDE_CHECK_SUPPORTED(current_solve_variant() == 1 || hidden * channels <= kMlpChunk,
-                         "%s: at hidden=%lld channels=%lld the backward is slower than per-step autograd; automatic "
-                         "selection does not run it (variant 1 forces it)", what, (long long)hidden, (long long)channels);
-    const int H = (int)hidden, C = (int)channels, W = (int)width;
-    MlpSimtLayout<double> fwd, bwd;                 // the larger element size bounds both dtypes
-    const bool fits = H <= 8 ? mlp_rev_fwd_layout<double, 8>(H, C, W, fwd) && mlp_rev_bwd_layout<double, 8>(H, C, W, bwd)
-                             : mlp_rev_fwd_layout<double, 32>(H, C, W, fwd) && mlp_rev_bwd_layout<double, 32>(H, C, W, bwd);
-    TCDE_CHECK_SUPPORTED(fits && mlp_simt_param_items(hidden, channels, width) > 0,
-                         "%s: hidden=%lld channels=%lld width=%lld do not fit the CUDA-core kernels' shared memory", what,
-                         (long long)hidden, (long long)channels, (long long)width);
-    return TCDE_OK;
-}
-
-template <typename T, int HM>
-static int launch_mlp_rev(const MlpArgs<T>& a, T* ckpt, int ckpt_stride, cudaStream_t s) {
-    auto kern = cdeint_mlp_rev_kernel<T, HM>;
-    MlpSimtLayout<T> lay;
-    const bool fits = mlp_rev_fwd_layout<T, HM>(a.H, a.C, a.W, lay);
-    TCDE_CHECK_SUPPORTED(fits, "MLP reversible Heun: the shape does not fit");
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
-    const int64_t ctas = (a.n_paths + kMlpSimtThreads - 1) / kMlpSimtThreads;
-    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
-    kern<<<(unsigned)ctas, kMlpSimtThreads, lay.total, s>>>(a, lay, ckpt, ckpt_stride);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
-}
-
-template <typename T, int HM>
-static int launch_mlp_rev_backward(const MlpArgs<T>& a, const MlpRevBwd<T>& b, cudaStream_t s) {
-    auto kern = mlp_rev_backward_kernel<T, HM>;
-    constexpr int nt = mlp_rev_bwd_threads<HM>();
-    MlpSimtLayout<T> lay;
-    const bool fits = mlp_rev_bwd_layout<T, HM>(a.H, a.C, a.W, lay);
-    TCDE_CHECK_SUPPORTED(fits, "MLP reversible backward: the shape does not fit");
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
-    const int64_t ctas = (a.n_paths + nt - 1) / nt;
-    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
-    kern<<<(unsigned)ctas, nt, lay.total, s>>>(a, lay, b);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
-}
-
-template <typename T>
-static MlpArgs<T> mlp_rev_args(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
-                               const void* w2, const void* b2, const void* z0, void* out, int64_t n_paths,
-                               int64_t channels, int64_t hidden, int64_t width, int64_t n_steps, const void* step_dt,
-                               const int32_t* stage_index, const void* stage_frac, int64_t n_out, const int32_t* out_step,
-                               const void* out_weights) {
-    return mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths, channels, hidden, width,
-                            TCDE_REVERSIBLE_HEUN, n_steps, step_dt, stage_index, stage_frac, n_out, out_step, nullptr,
-                            out_weights, 1.0);
-}
-
-template <typename T>
-static int mlp_rev_forward(const MlpArgs<T>& a, void* ckpt, int ckpt_stride, cudaStream_t s) {
-    return a.H <= 8 ? launch_mlp_rev<T, 8>(a, (T*)ckpt, ckpt_stride, s) : launch_mlp_rev<T, 32>(a, (T*)ckpt, ckpt_stride, s);
-}
-
-template <typename T>
-static int mlp_rev_backward(const MlpArgs<T>& a, const MlpRevBwd<T>& b, cudaStream_t s) {
-    return a.H <= 8 ? launch_mlp_rev_backward<T, 8>(a, b, s) : launch_mlp_rev_backward<T, 32>(a, b, s);
 }
 
 static int64_t mlp_param_grid(int64_t n_paths, int64_t n_total) {
@@ -2593,60 +2380,163 @@ __global__ void __launch_bounds__(kMlpSimtThreads, 1) dopri5_mlp_backward_kernel
     }
 }
 
-// The layout of dopri5_mlp_backward_kernel at the HM the dispatch picks for H: the weights staged when everything fits,
-// else read from global memory; false if neither fits
-template <typename T, int HM> static bool mlp_dp5_bwd_layout(int H, int C, int W, MlpSimtLayout<T>& lay) {
-    for (int stage = 1; stage >= 0; --stage) {
-        lay = mlp_simt_layout<T>(H, C, W, stage != 0, mlp_rev_bwd_threads<HM>(), mlp_dp5_bwd_extra<HM>(H));
-        if (lay.total <= kMlpSimtMaxSmem) return true;
-    }
-    return false;
+// ---- which kernels serve an entry point: the one route policy of the MLP field ----------------------------------------
+//
+// What is asked, then what serves it (every ask first needs 1 <= width, channels < 2^20 and hidden * channels < 2^20).
+// "simt shapes": hidden <= 8 (the HM = 8 instantiations) or hidden * channels <= 32 (one chunk of outputs); "tc": fp32
+// at hidden 32, channels 8, width 128 with 16-byte aligned buffers; "CUDA-core route": fp32 or fp64 at the simt shapes
+// under solve variant 0 (hidden <= 8) or variant 1.
+//   solve                fp32: tc under variant 0 (if not tc, as fp64) and only tc under 4 / 5; 2 / 3 / 6 (3xTF32) not
+//                        built.  fp64 under any variant: the CUDA cores at the simt shapes, or at hidden <= 32 under 1.
+//   stages, backward,    tc under variant 0, 4 or 5 past the simt shapes, the CUDA-core route at them.
+//   param_grads
+//   param_scratch        as param_grads, whatever the dtype and the variant.
+//   field                the CUDA-core route; by default also only fp32 at hidden * channels <= 32 and width <= 128.
+//   reversible           the CUDA-core route; by default also only hidden * channels <= 32.
+//   dopri5_backward      the CUDA-core route.
+// For field, reversible and dopri5_backward the width must also let the kernels' layouts (mlp_simt_fit, with 8-byte
+// elements: one answer for both dtypes) and, but for the dopri5 backward, the parameter-gradient staging fit shared memory.
+// Elsewhere TCDE_ERR_UNSUPPORTED, and the caller keeps its own route (the stage loop, autograd, torch operators).
+//
+// Why, from measurements on an H100 (DESIGN 4.2, 8 and "torchsde backend"):
+//   * past the simt shapes the CUDA-core forward recomputes the first product per chunk of 32 outputs and runs at low
+//     occupancy: 1.3-4.5x (fp32) and up to 13.6x (fp64) slower than cdeint's stage loop;
+//   * at hidden 32, channels 1 a training step on the CUDA-core backprop was slower per sequence than the torch-operator
+//     loop, so variant 0 runs it only at hidden <= 8 (variant 1 forces the HM = 32 kernels);
+//   * an adjoint=True training step on the field kernels beat autograd per stage only at fp32, hidden * channels <= 32 and
+//     width <= 128; fp64, channels 14 and width 366 at hidden 8 measured 0.13-0.83x of autograd's speed;
+//   * reversible Heun beat the torch-operator forward and per-step autograd at (8, 3, 128) fp32 and fp64 and at
+//     (5, 3, 37), but was 7.7x slower at (8, 14, 128): four chunks, the backward recomputes the first product per chunk
+//     and its parameter gradients stage 112 outputs per item.
+enum MlpAsk { kMlpSolve, kMlpStages, kMlpBackward, kMlpParamGrads, kMlpParamScratch, kMlpField, kMlpReversible,
+              kMlpDopri5Backward };
+
+struct MlpRoute {
+    bool tc;                      // the tensor-core kernels
+    int hm;                       // else the CUDA-core instantiation: HM = 8 up to 8 hidden units, else 32
+};
+
+// The checks of the entry points' enum arguments.  The solve and the reversible Heun and dopri5 entries reject an unknown
+// dtype as an argument; to the others it is a dtype the route policy does not serve.
+static int mlp_check_args(MlpAsk ask, int control_kind, int dtype, int method = TCDE_EULER) {
+    const bool dtype_arg = ask == kMlpSolve || ask == kMlpReversible || ask == kMlpDopri5Backward;
+    TCDE_CHECK_ARG(!dtype_arg || dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
+    return TCDE_OK;
 }
 
-// Where tcde_dopri5_mlp_backward runs: the CUDA-core route of mlp_backprop_route (by default hidden <= 8, fp32 and fp64;
-// under solve variant 1 also hidden * channels <= 32), at widths whose columns fit shared memory; TCDE_ERR_UNSUPPORTED
-// elsewhere, the tensor-core shape 32 / 8 / 128 included, so that the caller keeps the torch-operator dopri5
-static int mlp_dopri5_route(int64_t hidden, int64_t channels, int64_t width, int dtype, const char* what) {
-    bool simt;
-    const int rc = mlp_backprop_route(hidden, channels, width, dtype, what, &simt);
-    if (rc != TCDE_OK) return rc;
-    TCDE_CHECK_SUPPORTED(simt, "%s is built for the CUDA-core shapes (hidden <= 8, or hidden * channels <= 32 under solve "
-                         "variant 1; got %lld, %lld, %lld)", what, (long long)hidden, (long long)channels,
-                         (long long)width);
-    MlpSimtLayout<double> lay;                       // the larger element size bounds both dtypes
-    const bool fits = hidden <= 8 ? mlp_dp5_bwd_layout<double, 8>((int)hidden, (int)channels, (int)width, lay)
-                                  : mlp_dp5_bwd_layout<double, 32>((int)hidden, (int)channels, (int)width, lay);
-    TCDE_CHECK_SUPPORTED(fits, "%s: hidden=%lld channels=%lld width=%lld do not fit the CUDA-core kernel's shared memory",
+static int mlp_check_shape(int64_t hidden, int64_t channels, int64_t width) {
+    TCDE_CHECK_ARG(channels >= 1 && hidden >= 1 && width >= 1, "bad sizes");
+    TCDE_CHECK_SUPPORTED(width < (1 << 20) && channels < (1 << 20) && hidden * channels < (1 << 20), "MLP too wide");
+    return TCDE_OK;
+}
+
+static int mlp_route(MlpAsk ask, int64_t hidden, int64_t channels, int64_t width, int dtype, bool aligned,
+                     const char* what, MlpRoute* r) {
+    if (const int rc = mlp_check_shape(hidden, channels, width); rc != TCDE_OK) return rc;
+    const int variant = current_solve_variant();
+    const bool simt = hidden <= 8 || hidden * channels <= kMlpChunk;
+    const bool tc_shape = hidden == tc::kHid && channels == tc::kCh && width == tc::mlp::kWidth;
+    *r = MlpRoute{false, hidden <= 8 ? 8 : 32};
+    if (ask == kMlpParamScratch) {
+        r->tc = !simt;
+        TCDE_CHECK_SUPPORTED(simt ? mlp_simt_param_items(hidden, channels, width) > 0 : tc_shape,
+                             "%s: hidden=%lld channels=%lld width=%lld are not served", what, (long long)hidden,
+                             (long long)channels, (long long)width);
+        return TCDE_OK;
+    }
+    if (ask == kMlpSolve) {
+        if (dtype == TCDE_F32) {
+            TCDE_CHECK_SUPPORTED(variant <= 1 || variant == 4 || variant == 5,
+                                 "%s: solve variant %d (3xTF32) is not built for the MLP field", what, variant);
+            TCDE_CHECK_SUPPORTED(variant <= 1 || (tc_shape && aligned), "%s: the tensor-core kernel is built for "
+                                 "hidden=32, channels=8, width=128 with 16-byte aligned control, z0 and out (got %lld, "
+                                 "%lld, %lld)", what, (long long)hidden, (long long)channels, (long long)width);
+            r->tc = variant >= 4 || (variant == 0 && tc_shape && aligned);
+            if (r->tc) return TCDE_OK;
+        }
+        TCDE_CHECK_SUPPORTED(simt || variant == 1, "%s: at hidden=%lld channels=%lld the CUDA-core kernel is slower than "
+                             "the stage loop; automatic selection does not run it (variant 1 forces it)", what,
+                             (long long)hidden, (long long)channels);
+        TCDE_CHECK_SUPPORTED(hidden <= 32, "%s: hidden=%lld > 32 is not built for the CUDA-core kernel", what,
+                             (long long)hidden);
+        return TCDE_OK;
+    }
+    if (!simt) {
+        r->tc = true;
+        TCDE_CHECK_SUPPORTED((ask == kMlpStages || ask == kMlpBackward || ask == kMlpParamGrads) && dtype == TCDE_F32 &&
+                                 tc_shape && (variant == 0 || variant == 4 || variant == 5),
+                             "%s is built for fp32, hidden=32, channels=8, width=128 on the tensor-core kernel where it "
+                             "has one, else for the CUDA-core shapes (hidden <= 8, or hidden * channels <= 32 under solve "
+                             "variant 1; got dtype=%d, %lld, %lld, %lld, solve variant %d)", what, dtype,
+                             (long long)hidden, (long long)channels, (long long)width, variant);
+        TCDE_CHECK_SUPPORTED(aligned, "%s: the tensor-core kernel needs 16-byte aligned buffers", what);
+        return TCDE_OK;
+    }
+    TCDE_CHECK_SUPPORTED(hidden <= 8 || variant == 1, "%s: at hidden=%lld the CUDA-core route is slower than the stage "
+                         "loop; automatic selection does not run it (variant 1 forces it)", what, (long long)hidden);
+    TCDE_CHECK_SUPPORTED((dtype == TCDE_F32 || dtype == TCDE_F64) && variant <= 1, "%s on the CUDA cores is built for "
+                         "fp32 / fp64 under solve variant 0 or 1 (got dtype=%d, solve variant %d)", what, dtype,
+                         variant);
+    TCDE_CHECK_SUPPORTED(ask != kMlpField || variant == 1 ||
+                             (dtype == TCDE_F32 && hidden * channels <= kMlpChunk && width <= 128),
+                         "%s: at dtype=%d hidden=%lld channels=%lld width=%lld it is slower than autograd per stage; "
+                         "automatic selection does not run it (variant 1 forces it)", what, dtype, (long long)hidden,
+                         (long long)channels, (long long)width);
+    TCDE_CHECK_SUPPORTED(ask != kMlpReversible || variant == 1 || hidden * channels <= kMlpChunk,
+                         "%s: at hidden=%lld channels=%lld the backward is slower than per-step autograd; automatic "
+                         "selection does not run it (variant 1 forces it)", what, (long long)hidden, (long long)channels);
+    const int H = (int)hidden, C = (int)channels, W = (int)width;
+    const bool fits = mlp_hm(r->hm, [&](auto HM) {
+        const bool staging = mlp_simt_param_items(H, C, W) > 0;
+        switch (ask) {
+        case kMlpField:
+            return staging && mlp_simt_fit<double>(H, C, W, kMlpSimtThreads, mlp_field_extra<double, HM.value, true>(H));
+        case kMlpReversible:
+            return staging && mlp_simt_fit<double>(H, C, W, kMlpSimtThreads, mlp_rev_fwd_extra<double, HM.value>(H)) &&
+                   mlp_simt_fit<double>(H, C, W, mlp_rev_bwd_threads<HM.value>(), mlp_rev_bwd_extra<HM.value>(H));
+        case kMlpDopri5Backward:
+            return mlp_simt_fit<double>(H, C, W, mlp_rev_bwd_threads<HM.value>(), mlp_dp5_bwd_extra<HM.value>(H))
+                .has_value();
+        default:
+            return true;          // the solve's layouts are fitted at launch
+        }
+    });
+    TCDE_CHECK_SUPPORTED(fits, "%s: hidden=%lld channels=%lld width=%lld do not fit the CUDA-core kernels' shared memory",
                          what, (long long)hidden, (long long)channels, (long long)width);
     return TCDE_OK;
 }
 
-template <typename T, int HM>
-static int launch_mlp_dp5_backward(const MlpArgs<T>& a, const MlpDp5Bwd<T>& b, cudaStream_t s) {
-    auto kern = dopri5_mlp_backward_kernel<T, HM>;
-    constexpr int nt = mlp_rev_bwd_threads<HM>();
-    MlpSimtLayout<T> lay;
-    const bool fits = mlp_dp5_bwd_layout<T, HM>(a.H, a.C, a.W, lay);
-    TCDE_CHECK_SUPPORTED(fits, "MLP dopri5 backward: the shape does not fit");
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lay.total));
-    const int64_t ctas = (a.n_paths + nt - 1) / nt;
-    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
-    kern<<<(unsigned)ctas, nt, lay.total, s>>>(a, lay, b);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
+// The fixed-step solve, with a stage dump when stage_dump is set
+static int mlp_fixed_solve(const MlpRoute& r, const void* control, int control_kind, int64_t n_rows, const void* w1,
+                           const void* b1, const void* w2, const void* b2, const void* z0, void* out, void* stage_dump,
+                           int64_t n_paths, int64_t channels, int64_t hidden, int64_t width, int method,
+                           int64_t n_steps, const void* step_dt, const int32_t* stage_index, const void* stage_frac,
+                           int64_t n_out, const int32_t* out_step, const int32_t* out_mode, const void* out_slope,
+                           double sign, int dtype, cudaStream_t s) {
+    return mlp_dtype(dtype, [&](auto t) {
+        using T = decltype(t);
+        const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths, channels,
+                                              hidden, width, method, n_steps, step_dt, stage_index, stage_frac, n_out,
+                                              out_step, out_mode, out_slope, sign);
+        if (r.tc) {
+            const UmmaArgs u{(const float*)a.control, (const float*)a.w1, (const float*)a.b1, (const float*)a.z0,
+                             (float*)a.out, (const float*)a.step_dt, a.stage_index, (const float*)a.stage_frac,
+                             a.out_step, a.out_mode, (const float*)a.out_slope, a.n_paths, a.n_rows, a.control_kind,
+                             a.method, a.n_stages, a.n_steps, a.n_out, (float)a.sign, (float*)stage_dump, 0};
+            return mlp_launch(stage_dump ? tc::mlp::cdeint_mlp_wgmma_kernel<true> : tc::mlp::cdeint_mlp_wgmma_kernel<false>,
+                              (n_paths + tc::mlp::kPaths - 1) / tc::mlp::kPaths, tc::mlp::kThreads, tc::mlp::kSmem, s,
+                              u, (const float*)w2, (const float*)b2);
+        }
+        return mlp_hm(r.hm, [&](auto HM) {
+            return mlp_launch_simt(stage_dump ? cdeint_mlp_simt_kernel<T, HM.value, true>
+                                              : cdeint_mlp_simt_kernel<T, HM.value, false>,
+                                   a, kMlpSimtThreads, 0, s, (T*)stage_dump);
+        });
+    });
 }
-
-template <typename T>
-static int mlp_dp5_backward(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
-                            const void* w2, const void* b2, const MlpDp5Bwd<T>& b, const int32_t* item_index,
-                            const void* item_frac, int64_t n_out, int64_t n_paths, int64_t channels, int64_t hidden,
-                            int64_t width, double sign, cudaStream_t s) {
-    const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths,
-                                          channels, hidden, width, TCDE_EULER, b.n_steps, nullptr, item_index, item_frac,
-                                          n_out, nullptr, nullptr, nullptr, sign);
-    return hidden <= 8 ? launch_mlp_dp5_backward<T, 8>(a, b, s) : launch_mlp_dp5_backward<T, 32>(a, b, s);
-}
-
 
 }  // namespace tcde
 
@@ -2662,55 +2552,18 @@ extern "C" int tcde_cdeint_fixed_mlp(const void* control, int control_kind, int6
     TCDE_CHECK_ARG(step_dt && stage_index && stage_frac && out_step && out_mode && out_slope, "null schedule pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1, "bad sizes");
     TCDE_CHECK_ARG(n_steps >= 1 && n_out >= 1, "n_steps=%lld n_out=%lld", (long long)n_steps, (long long)n_out);
-    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
+    if (const int rc = mlp_check_args(kMlpSolve, control_kind, dtype, method); rc != TCDE_OK) return rc;
     TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
-    TCDE_CHECK_SUPPORTED(width < (1 << 20) && channels < (1 << 20) && hidden * channels < (1 << 20), "MLP too wide");
+    if (const int rc = mlp_check_shape(hidden, channels, width); rc != TCDE_OK) return rc;
     if (n_paths == 0) return TCDE_OK;
-    const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const int variant = current_solve_variant();
-    const bool simt_ok = variant == 1 || mlp_simt_preferred(hidden, channels);
-    if (dtype == TCDE_F32) {
-        // 0: the tensor-core kernel where it is built for the shape and the buffers are 16-byte aligned, else the CUDA
-        // cores where they beat the stage loop; 1: the CUDA cores; 4 / 5: the tensor-core kernel or TCDE_ERR_UNSUPPORTED;
-        // 2 / 3 / 6 (3xTF32): not built
-        const bool aligned = ((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z0) |
-                               reinterpret_cast<uintptr_t>(out)) & 15) == 0;
-        const bool tc_ok = mlp_tc_shape(hidden, channels, width) && aligned;
-        TCDE_CHECK_SUPPORTED(variant <= 1 || variant == 4 || variant == 5,
-                             "MLP solve: solve variant %d (3xTF32) is not built for the MLP field", variant);
-        if (variant >= 4) {
-            TCDE_CHECK_SUPPORTED(tc_ok, "MLP solve: the tensor-core kernel is built for hidden=32, channels=8, width=128 "
-                                 "with 16-byte aligned control, z0 and out (got %lld, %lld, %lld)", (long long)hidden,
-                                 (long long)channels, (long long)width);
-        }
-        if (variant >= 4 || (variant == 0 && tc_ok)) {
-            UmmaArgs u{(const float*)control, (const float*)w1, (const float*)b1, (const float*)z0, (float*)out,
-                       (const float*)step_dt, stage_index, (const float*)stage_frac, out_step, out_mode,
-                       (const float*)out_slope, n_paths, n_rows, control_kind, method, n_stages, (int)n_steps, (int)n_out,
-                       (float)sign, nullptr, 0};
-            return launch_mlp_tc(u, (const float*)w2, (const float*)b2, s);
-        }
-        MlpArgs<float> a{(const float*)control, (const float*)w1, (const float*)b1, (const float*)w2, (const float*)b2,
-                         (const float*)z0, (float*)out, (const float*)step_dt, stage_index, (const float*)stage_frac,
-                         out_step, out_mode, (const float*)out_slope, n_paths, n_rows, (int)channels, (int)hidden,
-                         (int)width, control_kind, method, n_stages, (int)n_steps, (int)n_out, (float)sign};
-        TCDE_CHECK_SUPPORTED(simt_ok, "MLP solve: at hidden=%lld channels=%lld the CUDA-core kernel is slower than the "
-                             "stage loop; automatic selection does not run it (variant 1 forces it)", (long long)hidden,
-                             (long long)channels);
-        return solve_mlp_simt(a, s);
-    }
-    TCDE_CHECK_SUPPORTED(simt_ok, "MLP solve: at hidden=%lld channels=%lld the CUDA-core kernel is slower than the stage "
-                         "loop; automatic selection does not run it (variant 1 forces it)", (long long)hidden,
-                         (long long)channels);
-    MlpArgs<double> a{(const double*)control, (const double*)w1, (const double*)b1, (const double*)w2, (const double*)b2,
-                      (const double*)z0, (double*)out, (const double*)step_dt, stage_index, (const double*)stage_frac,
-                      out_step, out_mode, (const double*)out_slope, n_paths, n_rows, (int)channels, (int)hidden,
-                      (int)width, control_kind, method, n_stages, (int)n_steps, (int)n_out, sign};
-    return solve_mlp_simt(a, s);
+    MlpRoute r;
+    if (const int rc = mlp_route(kMlpSolve, hidden, channels, width, dtype,
+                                 aligned16(control) && aligned16(z0) && aligned16(out), "the MLP solve", &r);
+        rc != TCDE_OK)
+        return rc;
+    return mlp_fixed_solve(r, control, control_kind, n_rows, w1, b1, w2, b2, z0, out, nullptr, n_paths, channels, hidden,
+                           width, method, n_steps, step_dt, stage_index, stage_frac, n_out, out_step, out_mode,
+                           out_slope, sign, dtype, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int tcde_cdeint_fixed_mlp_stages(const void* control, int control_kind, int64_t n_rows, const void* w1,
@@ -2723,37 +2576,19 @@ extern "C" int tcde_cdeint_fixed_mlp_stages(const void* control, int control_kin
     TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z0 && out && stage_dump, "null data pointer");
     TCDE_CHECK_ARG(step_dt && stage_index && stage_frac && out_step && out_mode && out_slope, "null schedule pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_steps >= 1 && n_out >= 1, "bad sizes");
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
+    if (const int rc = mlp_check_args(kMlpStages, control_kind, dtype, method); rc != TCDE_OK) return rc;
     TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
-    bool simt;
-    const int rc = mlp_backprop_route(hidden, channels, width, dtype, "the MLP stage-dump solve", &simt);
-    if (rc != TCDE_OK) return rc;
-    if (simt) {
-        TCDE_CHECK_SUPPORTED(n_paths * hidden * n_steps * 4 < (1ll << 62), "stage dump too large");
-        if (n_paths == 0) return TCDE_OK;
-        cudaStream_t s = static_cast<cudaStream_t>(stream);
-        if (dtype == TCDE_F32)
-            return solve_mlp_simt(mlp_simt_args<float>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths,
-                                                       channels, hidden, width, method, n_steps, step_dt, stage_index,
-                                                       stage_frac, n_out, out_step, out_mode, out_slope, sign),
-                                  s, (float*)stage_dump);
-        return solve_mlp_simt(mlp_simt_args<double>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths,
-                                                    channels, hidden, width, method, n_steps, step_dt, stage_index,
-                                                    stage_frac, n_out, out_step, out_mode, out_slope, sign),
-                              s, (double*)stage_dump);
-    }
-    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z0) |
-                           reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(stage_dump)) & 15) == 0,
-                         "MLP stage-dump solve: control, z0, out and the dump must be 16-byte aligned");
+    MlpRoute r;
+    if (const int rc = mlp_route(kMlpStages, hidden, channels, width, dtype,
+                                 aligned16(control) && aligned16(z0) && aligned16(out) && aligned16(stage_dump),
+                                 "the MLP stage-dump solve", &r);
+        rc != TCDE_OK)
+        return rc;
+    TCDE_CHECK_SUPPORTED(r.tc || n_paths * hidden * n_steps * 4 < (1ll << 62), "stage dump too large");
     if (n_paths == 0) return TCDE_OK;
-    const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
-    UmmaArgs u{(const float*)control, (const float*)w1, (const float*)b1, (const float*)z0, (float*)out,
-               (const float*)step_dt, stage_index, (const float*)stage_frac, out_step, out_mode, (const float*)out_slope,
-               n_paths, n_rows, control_kind, method, n_stages, (int)n_steps, (int)n_out, (float)sign, (float*)stage_dump,
-               0};
-    return launch_mlp_tc(u, (const float*)w2, (const float*)b2, static_cast<cudaStream_t>(stream));
+    return mlp_fixed_solve(r, control, control_kind, n_rows, w1, b1, w2, b2, z0, out, stage_dump, n_paths, channels,
+                           hidden, width, method, n_steps, step_dt, stage_index, stage_frac, n_out, out_step, out_mode,
+                           out_slope, sign, dtype, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int tcde_cdeint_fixed_mlp_backward(
@@ -2766,65 +2601,51 @@ extern "C" int tcde_cdeint_fixed_mlp_backward(
     TCDE_CHECK_ARG(step_dt_rev && stage_index_rev && stage_frac_rev && inj_range && inj_out && inj_weight,
                    "null schedule pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_steps >= 1 && n_out >= 1, "bad sizes");
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
+    if (const int rc = mlp_check_args(kMlpBackward, control_kind, dtype, method); rc != TCDE_OK) return rc;
     TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
-    bool simt;
-    const int rc = mlp_backprop_route(hidden, channels, width, dtype, "the MLP Runge-Kutta backward", &simt);
-    if (rc != TCDE_OK) return rc;
-    if (simt) {
-        if (n_paths == 0) return TCDE_OK;
-        cudaStream_t s = static_cast<cudaStream_t>(stream);
-        if (dtype == TCDE_F32)
-            return mlp_simt_backward(
-                mlp_simt_args<float>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, grad_z0, n_paths, channels,
-                                     hidden, width, method, n_steps, step_dt_rev, stage_index_rev, stage_frac_rev, n_out,
-                                     nullptr, nullptr, nullptr, sign),
-                MlpSimtBwd<float>{(const float*)stage_dump, (float*)kappa_dump, (const float*)grad_out, inj_range,
-                                  inj_out, (const float*)inj_weight},
-                s);
-        return mlp_simt_backward(
-            mlp_simt_args<double>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, grad_z0, n_paths, channels,
-                                  hidden, width, method, n_steps, step_dt_rev, stage_index_rev, stage_frac_rev, n_out,
-                                  nullptr, nullptr, nullptr, sign),
-            MlpSimtBwd<double>{(const double*)stage_dump, (double*)kappa_dump, (const double*)grad_out, inj_range,
-                               inj_out, (const double*)inj_weight},
-            s);
-    }
-    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(stage_dump) |
-                           reinterpret_cast<uintptr_t>(grad_out) | reinterpret_cast<uintptr_t>(grad_z0) |
-                           reinterpret_cast<uintptr_t>(kappa_dump)) & 15) == 0,
-                         "MLP Runge-Kutta backward: control, the dumps, grad_out and grad_z0 must be 16-byte aligned");
+    MlpRoute r;
+    if (const int rc = mlp_route(kMlpBackward, hidden, channels, width, dtype,
+                                 aligned16(control) && aligned16(stage_dump) && aligned16(grad_out) &&
+                                     aligned16(grad_z0) && aligned16(kappa_dump),
+                                 "the MLP Runge-Kutta backward", &r);
+        rc != TCDE_OK)
+        return rc;
     if (n_paths == 0) return TCDE_OK;
-    const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
-    UmmaArgs u{(const float*)control, (const float*)w1, (const float*)b1, nullptr, (float*)grad_z0,
-               (const float*)step_dt_rev, stage_index_rev, (const float*)stage_frac_rev, nullptr, nullptr, nullptr,
-               n_paths, n_rows, control_kind, method, n_stages, (int)n_steps, (int)n_out, (float)sign,
-               (float*)kappa_dump, 0, (const float*)grad_out, inj_range, inj_out, (const float*)inj_weight};
-    const int64_t grid = (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths;
-    TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(tc::mlp::cdeint_mlp_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         tc::mlp::kBwdSmem));
-    tc::mlp::cdeint_mlp_backward_kernel<<<(unsigned)grid, tc::mlp::kBwdThreads, tc::mlp::kBwdSmem,
-                                          static_cast<cudaStream_t>(stream)>>>(u, (const float*)w2, (const float*)b2,
-                                                                               (const float*)stage_dump);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
+    cudaStream_t s = static_cast<cudaStream_t>(stream);
+    return mlp_dtype(dtype, [&](auto t) {
+        using T = decltype(t);
+        const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, grad_z0, n_paths,
+                                              channels, hidden, width, method, n_steps, step_dt_rev, stage_index_rev,
+                                              stage_frac_rev, n_out, nullptr, nullptr, nullptr, sign);
+        if (r.tc) {
+            const UmmaArgs u{(const float*)control, (const float*)w1, (const float*)b1, nullptr, (float*)grad_z0,
+                             (const float*)step_dt_rev, stage_index_rev, (const float*)stage_frac_rev, nullptr, nullptr,
+                             nullptr, n_paths, n_rows, control_kind, method, a.n_stages, (int)n_steps, (int)n_out,
+                             (float)sign, (float*)kappa_dump, 0, (const float*)grad_out, inj_range, inj_out,
+                             (const float*)inj_weight};
+            return mlp_launch(tc::mlp::cdeint_mlp_backward_kernel, (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths,
+                              tc::mlp::kBwdThreads, tc::mlp::kBwdSmem, s, u, (const float*)w2, (const float*)b2,
+                              (const float*)stage_dump);
+        }
+        const MlpSimtBwd<T> b{(const T*)stage_dump, (T*)kappa_dump, (const T*)grad_out, inj_range, inj_out,
+                              (const T*)inj_weight};
+        return mlp_hm(r.hm, [&](auto HM) {
+            return mlp_launch_simt(cdeint_mlp_simt_backward_kernel<T, HM.value>, a, kMlpSimtThreads, 0, s, b);
+        });
+    });
 }
 
 extern "C" int64_t tcde_mlp_field_param_grads_scratch_bytes(int64_t n_paths, int64_t n_stages_total, int64_t channels,
                                                            int64_t hidden, int64_t width) {
-    if (n_paths < 0 || n_stages_total < 1 || hidden < 1 || channels < 1 || width < 1) return -1;
-    if (width >= (1 << 20) || channels >= (1 << 20) || hidden * channels >= (1 << 20)) return -1;
-    if (mlp_simt_preferred(hidden, channels)) {               // the CUDA-core kernel, sized for 8-byte elements
-        const int ni = mlp_simt_param_items(hidden, channels, width);
-        if (ni == 0) return -1;
-        return mlp_simt_param_grid(n_paths, n_stages_total, ni) * mlp_simt_n_params(hidden, channels, width) *
-               (int64_t)sizeof(double);
-    }
-    if (!mlp_tc_shape(hidden, channels, width)) return -1;
-    return mlp_param_grid(n_paths, n_stages_total) * tc::mlp::kPgParams * (int64_t)sizeof(float);
+    MlpRoute r;
+    if (n_paths < 0 || n_stages_total < 1 ||
+        mlp_route(kMlpParamScratch, hidden, channels, width, TCDE_F32, true, "the MLP parameter-gradient scratch",
+                  &r) != TCDE_OK)
+        return -1;
+    if (r.tc) return mlp_param_grid(n_paths, n_stages_total) * tc::mlp::kPgParams * (int64_t)sizeof(float);
+    // the CUDA-core kernel, sized for 8-byte elements
+    return mlp_simt_param_grid(n_paths, n_stages_total, mlp_simt_param_items(hidden, channels, width)) *
+           mlp_simt_n_params(hidden, channels, width) * (int64_t)sizeof(double);
 }
 
 extern "C" int tcde_mlp_field_param_grads(const void* control, int control_kind, int64_t n_rows, const void* w1,
@@ -2836,49 +2657,40 @@ extern "C" int tcde_mlp_field_param_grads(const void* control, int control_kind,
     TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z_stages && kappa_stages && stage_index && stage_frac && scratch,
                    "null data pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_stages_total >= 1 && n_stages_total < (1ll << 31), "bad sizes");
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    bool simt;
-    const int rc = mlp_backprop_route(hidden, channels, width, dtype, "the MLP parameter gradients", &simt);
-    if (rc != TCDE_OK) return rc;
-    if (simt) {
-        if (n_paths == 0) return TCDE_OK;
-        cudaStream_t s = static_cast<cudaStream_t>(stream);
-        // the forward's stage tables; the solve's method and steps do not matter here
-        if (dtype == TCDE_F32)
-            return mlp_simt_param_grads(
-                mlp_simt_args<float>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths, channels,
-                                     hidden, width, TCDE_EULER, 1, nullptr, stage_index, stage_frac, 1, nullptr, nullptr,
-                                     nullptr, sign),
-                (const float*)z_stages, (const float*)kappa_stages, n_stages_total, grad_w1, grad_b1, grad_w2, grad_b2,
-                scratch, scale, s);
-        return mlp_simt_param_grads(
-            mlp_simt_args<double>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths, channels,
-                                  hidden, width, TCDE_EULER, 1, nullptr, stage_index, stage_frac, 1, nullptr, nullptr,
-                                  nullptr, sign),
-            (const double*)z_stages, (const double*)kappa_stages, n_stages_total, grad_w1, grad_b1, grad_w2, grad_b2,
-            scratch, scale, s);
-    }
-    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z_stages) |
-                           reinterpret_cast<uintptr_t>(kappa_stages) | reinterpret_cast<uintptr_t>(scratch)) & 15) == 0,
-                         "MLP parameter gradients: control, the dumps and scratch must be 16-byte aligned");
+    if (const int rc = mlp_check_args(kMlpParamGrads, control_kind, dtype); rc != TCDE_OK) return rc;
+    MlpRoute r;
+    if (const int rc = mlp_route(kMlpParamGrads, hidden, channels, width, dtype,
+                                 aligned16(control) && aligned16(z_stages) && aligned16(kappa_stages) &&
+                                     aligned16(scratch),
+                                 "the MLP parameter gradients", &r);
+        rc != TCDE_OK)
+        return rc;
     if (n_paths == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const int64_t grid = mlp_param_grid(n_paths, n_stages_total);
-    tc::mlp::PgArgs a{(const float*)control, (const float*)w1, (const float*)b1, (const float*)w2, (const float*)b2,
-                      (const float*)z_stages, (const float*)kappa_stages, stage_index, (const float*)stage_frac,
-                      (float*)scratch, n_paths, n_rows, control_kind, (int)n_stages_total, (float)sign};
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(tc::mlp::mlp_param_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         tc::mlp::kPgSmem));
-    tc::mlp::mlp_param_grad_kernel<<<dim3((unsigned)grid, tc::mlp::kPgY), tc::mlp::kBwdThreads, tc::mlp::kPgSmem, s>>>(a);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    if (grad_w1 || grad_b1 || grad_w2 || grad_b2) {
-        tc::mlp::mlp_param_reduce_kernel<<<(tc::mlp::kPgParams + 255) / 256, 256, 0, s>>>(
-            (const float*)scratch, (int)grid, (float)scale, (float*)grad_w1, (float*)grad_b1, (float*)grad_w2,
-            (float*)grad_b2);
+    if (r.tc) {
+        const int64_t grid = mlp_param_grid(n_paths, n_stages_total);
+        tc::mlp::PgArgs a{(const float*)control, (const float*)w1, (const float*)b1, (const float*)w2, (const float*)b2,
+                          (const float*)z_stages, (const float*)kappa_stages, stage_index, (const float*)stage_frac,
+                          (float*)scratch, n_paths, n_rows, control_kind, (int)n_stages_total, (float)sign};
+        TCDE_CHECK_CUDA(cudaFuncSetAttribute(tc::mlp::mlp_param_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             tc::mlp::kPgSmem));
+        tc::mlp::mlp_param_grad_kernel<<<dim3((unsigned)grid, tc::mlp::kPgY), tc::mlp::kBwdThreads, tc::mlp::kPgSmem,
+                                         s>>>(a);
         TCDE_CHECK_CUDA(cudaGetLastError());
+        if (!(grad_w1 || grad_b1 || grad_w2 || grad_b2)) return TCDE_OK;
+        return mlp_launch(tc::mlp::mlp_param_reduce_kernel, (tc::mlp::kPgParams + 255) / 256, 256, 0, s,
+                          (const float*)scratch, (int)grid, (float)scale, (float*)grad_w1, (float*)grad_b1,
+                          (float*)grad_w2, (float*)grad_b2);
     }
-    return TCDE_OK;
+    // the forward's stage tables; the solve's method and steps do not matter here
+    return mlp_dtype(dtype, [&](auto t) {
+        using T = decltype(t);
+        return mlp_simt_param_grads(mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr,
+                                                     n_paths, channels, hidden, width, TCDE_EULER, 1, nullptr,
+                                                     stage_index, stage_frac, 1, nullptr, nullptr, nullptr, sign),
+                                    r.hm, (const T*)z_stages, (const T*)kappa_stages, n_stages_total, grad_w1, grad_b1,
+                                    grad_w2, grad_b2, scratch, scale, s);
+    });
 }
 
 extern "C" int tcde_vector_field_mlp(const void* control, int control_kind, int64_t n_rows, const void* w1, const void* b1,
@@ -2888,25 +2700,25 @@ extern "C" int tcde_vector_field_mlp(const void* control, int control_kind, int6
     TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z && out, "null data pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1, "bad sizes");
     TCDE_CHECK_ARG(index >= 0 && index < n_rows, "index=%d outside [0, %lld)", index, (long long)n_rows);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    const int rc = mlp_field_route(hidden, channels, width, dtype, "the MLP field evaluation");
-    if (rc != TCDE_OK) return rc;
+    if (const int rc = mlp_check_args(kMlpField, control_kind, dtype); rc != TCDE_OK) return rc;
+    MlpRoute r;
+    if (const int rc = mlp_route(kMlpField, hidden, channels, width, dtype, true, "the MLP field evaluation", &r);
+        rc != TCDE_OK)
+        return rc;
     if (n_paths == 0) return TCDE_OK;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (dtype == TCDE_F32)
-        return mlp_field_eval<float>(control, control_kind, n_rows, w1, b1, w2, b2, z, out, n_paths, channels, hidden,
-                                     width, index, frac, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                     1.0, 1.0, 1.0, s);
-    return mlp_field_eval<double>(control, control_kind, n_rows, w1, b1, w2, b2, z, out, n_paths, channels, hidden, width,
-                                  index, frac, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 1.0, 1.0,
-                                  1.0, s);
+    return mlp_dtype(dtype, [&](auto t) {
+        return mlp_field_eval<decltype(t)>(r.hm, control, control_kind, n_rows, w1, b1, w2, b2, z, out, n_paths,
+                                           channels, hidden, width, index, frac, nullptr, nullptr, nullptr, nullptr,
+                                           nullptr, nullptr, nullptr, 1.0, 1.0, 1.0, static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int64_t tcde_vector_field_mlp_vjp_scratch_bytes(int64_t n_paths, int64_t channels, int64_t hidden,
                                                            int64_t width) {
-    if (n_paths < 0 || hidden < 1 || channels < 1 || width < 1) return -1;
-    if (mlp_field_route(hidden, channels, width, TCDE_F32, "the MLP adjoint stage") != TCDE_OK) return -1;
+    MlpRoute r;
+    if (n_paths < 0 ||
+        mlp_route(kMlpField, hidden, channels, width, TCDE_F32, true, "the MLP adjoint stage", &r) != TCDE_OK)
+        return -1;
     return kMlpFieldScratchHead + mlp_simt_param_grid(n_paths, 1, mlp_simt_param_items(hidden, channels, width)) *
                                       mlp_simt_n_params(hidden, channels, width) * (int64_t)sizeof(double);
 }
@@ -2920,20 +2732,19 @@ extern "C" int tcde_vector_field_mlp_vjp(const void* control, int control_kind, 
     TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z && a && f_out && vjp_z_out && scratch, "null data pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1, "bad sizes");
     TCDE_CHECK_ARG(index >= 0 && index < n_rows, "index=%d outside [0, %lld)", index, (long long)n_rows);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    TCDE_CHECK_ARG((reinterpret_cast<uintptr_t>(scratch) & 15) == 0, "scratch must be 16-byte aligned");
-    const int rc = mlp_field_route(hidden, channels, width, dtype, "the MLP adjoint stage");
-    if (rc != TCDE_OK) return rc;
+    if (const int rc = mlp_check_args(kMlpField, control_kind, dtype); rc != TCDE_OK) return rc;
+    TCDE_CHECK_ARG(aligned16(scratch), "scratch must be 16-byte aligned");
+    MlpRoute r;
+    if (const int rc = mlp_route(kMlpField, hidden, channels, width, dtype, true, "the MLP adjoint stage", &r);
+        rc != TCDE_OK)
+        return rc;
     if (n_paths == 0) return TCDE_OK;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (dtype == TCDE_F32)
-        return mlp_field_eval<float>(control, control_kind, n_rows, w1, b1, w2, b2, z, f_out, n_paths, channels, hidden,
-                                     width, index, frac, a, vjp_z_out, grad_w1, grad_b1, grad_w2, grad_b2, scratch,
-                                     f_scale, vjp_scale, grad_scale, s);
-    return mlp_field_eval<double>(control, control_kind, n_rows, w1, b1, w2, b2, z, f_out, n_paths, channels, hidden,
-                                  width, index, frac, a, vjp_z_out, grad_w1, grad_b1, grad_w2, grad_b2, scratch, f_scale,
-                                  vjp_scale, grad_scale, s);
+    return mlp_dtype(dtype, [&](auto t) {
+        return mlp_field_eval<decltype(t)>(r.hm, control, control_kind, n_rows, w1, b1, w2, b2, z, f_out, n_paths,
+                                           channels, hidden, width, index, frac, a, vjp_z_out, grad_w1, grad_b1, grad_w2,
+                                           grad_b2, scratch, f_scale, vjp_scale, grad_scale,
+                                           static_cast<cudaStream_t>(stream));
+    });
 }
 
 extern "C" int tcde_cdeint_reversible_heun_mlp(const void* control, int control_kind, int64_t n_rows, const void* w1,
@@ -2949,23 +2760,25 @@ extern "C" int tcde_cdeint_reversible_heun_mlp(const void* control, int control_
     TCDE_CHECK_ARG(n_steps >= 1 && n_out >= 1, "n_steps=%lld n_out=%lld", (long long)n_steps, (long long)n_out);
     TCDE_CHECK_ARG(checkpoint_stride >= 1 && checkpoint_stride < (1ll << 30), "checkpoint_stride=%lld",
                    (long long)checkpoint_stride);
-    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
+    if (const int rc = mlp_check_args(kMlpReversible, control_kind, dtype); rc != TCDE_OK) return rc;
     TCDE_CHECK_SUPPORTED(n_steps + 1 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
-    const int rc = mlp_reversible_route(hidden, channels, width, dtype, "the MLP reversible Heun solve");
-    if (rc != TCDE_OK) return rc;
+    MlpRoute r;
+    if (const int rc = mlp_route(kMlpReversible, hidden, channels, width, dtype, true, "the MLP reversible Heun solve",
+                                 &r);
+        rc != TCDE_OK)
+        return rc;
     if (n_paths == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (dtype == TCDE_F32)
-        return mlp_rev_forward(mlp_rev_args<float>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths,
-                                                   channels, hidden, width, n_steps, step_dt, stage_index, stage_frac,
-                                                   n_out, out_step, out_weights),
-                               checkpoints, (int)checkpoint_stride, s);
-    return mlp_rev_forward(mlp_rev_args<double>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths, channels,
-                                                hidden, width, n_steps, step_dt, stage_index, stage_frac, n_out, out_step,
-                                                out_weights),
-                           checkpoints, (int)checkpoint_stride, s);
+    return mlp_dtype(dtype, [&](auto t) {
+        using T = decltype(t);
+        const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths, channels,
+                                              hidden, width, TCDE_REVERSIBLE_HEUN, n_steps, step_dt, stage_index,
+                                              stage_frac, n_out, out_step, nullptr, out_weights, 1.0);
+        return mlp_hm(r.hm, [&](auto HM) {
+            return mlp_launch_simt(cdeint_mlp_rev_kernel<T, HM.value>, a, kMlpSimtThreads,
+                                   mlp_rev_fwd_extra<T, HM.value>(a.H), s, (T*)checkpoints, (int)checkpoint_stride);
+        });
+    });
 }
 
 extern "C" int tcde_reversible_heun_mlp_backward_segment(
@@ -2980,26 +2793,25 @@ extern "C" int tcde_reversible_heun_mlp_backward_segment(
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1 && n_out >= 1, "bad sizes");
     TCDE_CHECK_ARG(lo >= 0 && hi > lo && hi <= n_steps && n_steps + 1 < (1ll << 31), "lo=%lld hi=%lld n_steps=%lld",
                    (long long)lo, (long long)hi, (long long)n_steps);
-    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    const int rc = mlp_reversible_route(hidden, channels, width, dtype, "the MLP reversible backward");
-    if (rc != TCDE_OK) return rc;
+    if (const int rc = mlp_check_args(kMlpReversible, control_kind, dtype); rc != TCDE_OK) return rc;
+    MlpRoute r;
+    if (const int rc = mlp_route(kMlpReversible, hidden, channels, width, dtype, true, "the MLP reversible backward", &r);
+        rc != TCDE_OK)
+        return rc;
     if (n_paths == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (dtype == TCDE_F32)
-        return mlp_rev_backward(
-            mlp_rev_args<float>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths, channels,
-                                hidden, width, n_steps, step_dt, stage_index, stage_frac, n_out, out_step, out_weights),
-            MlpRevBwd<float>{(const float*)ckpt_lo, (const float*)ckpt_hi, (float*)carry, (const float*)g, inj_range,
-                             (float*)dump_z, (float*)dump_a, (int)lo, (int)hi},
-            s);
-    return mlp_rev_backward(
-        mlp_rev_args<double>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths, channels, hidden,
-                             width, n_steps, step_dt, stage_index, stage_frac, n_out, out_step, out_weights),
-        MlpRevBwd<double>{(const double*)ckpt_lo, (const double*)ckpt_hi, (double*)carry, (const double*)g, inj_range,
-                          (double*)dump_z, (double*)dump_a, (int)lo, (int)hi},
-        s);
+    return mlp_dtype(dtype, [&](auto t) {
+        using T = decltype(t);
+        const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths,
+                                              channels, hidden, width, TCDE_REVERSIBLE_HEUN, n_steps, step_dt,
+                                              stage_index, stage_frac, n_out, out_step, nullptr, out_weights, 1.0);
+        const MlpRevBwd<T> b{(const T*)ckpt_lo, (const T*)ckpt_hi, (T*)carry, (const T*)g, inj_range, (T*)dump_z,
+                             (T*)dump_a, (int)lo, (int)hi};
+        return mlp_hm(r.hm, [&](auto HM) {
+            return mlp_launch_simt(mlp_rev_backward_kernel<T, HM.value>, a, mlp_rev_bwd_threads<HM.value>(),
+                                   mlp_rev_bwd_extra<HM.value>(a.H), s, b);
+        });
+    });
 }
 
 extern "C" int tcde_dopri5_mlp_backward(const void* control, int control_kind, int64_t n_rows, const void* w1,
@@ -3013,24 +2825,25 @@ extern "C" int tcde_dopri5_mlp_backward(const void* control, int control_kind, i
     TCDE_CHECK_ARG(coef && step_item && item_index && item_frac && inj_range && inj_out && inj_w, "null table pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_out >= 2 && n_out < (1ll << 31) && n_steps >= 0 &&
                        n_steps < (1ll << 24) && channels >= 1 && hidden >= 1 && width >= 1, "bad sizes");
-    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
+    if (const int rc = mlp_check_args(kMlpDopri5Backward, control_kind, dtype); rc != TCDE_OK) return rc;
     TCDE_CHECK_ARG(sign == 1.0 || sign == -1.0, "sign=%g", sign);
-    const int rc = mlp_dopri5_route(hidden, channels, width, dtype, "the MLP dopri5 backward");
-    if (rc != TCDE_OK) return rc;
+    MlpRoute r;
+    if (const int rc = mlp_route(kMlpDopri5Backward, hidden, channels, width, dtype, true, "the MLP dopri5 backward", &r);
+        rc != TCDE_OK)
+        return rc;
     TCDE_CHECK_SUPPORTED(n_paths * hidden * 7 * n_steps < (1ll << 62), "record too large");
     if (n_paths == 0 || n_steps == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (dtype == TCDE_F32)
-        return mlp_dp5_backward<float>(control, control_kind, n_rows, w1, b1, w2, b2,
-                                       MlpDp5Bwd<float>{(const float*)rec_z, (float*)kappa, (const float*)grad_out,
-                                                        (float*)carry, (const float*)coef, step_item, inj_range, inj_out,
-                                                        (const float*)inj_w, (int)n_steps},
-                                       item_index, item_frac, n_out, n_paths, channels, hidden, width, sign, s);
-    return mlp_dp5_backward<double>(control, control_kind, n_rows, w1, b1, w2, b2,
-                                    MlpDp5Bwd<double>{(const double*)rec_z, (double*)kappa, (const double*)grad_out,
-                                                      (double*)carry, (const double*)coef, step_item, inj_range, inj_out,
-                                                      (const double*)inj_w, (int)n_steps},
-                                    item_index, item_frac, n_out, n_paths, channels, hidden, width, sign, s);
+    return mlp_dtype(dtype, [&](auto t) {
+        using T = decltype(t);
+        const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths,
+                                              channels, hidden, width, TCDE_EULER, n_steps, nullptr, item_index,
+                                              item_frac, n_out, nullptr, nullptr, nullptr, sign);
+        const MlpDp5Bwd<T> b{(const T*)rec_z, (T*)kappa, (const T*)grad_out, (T*)carry, (const T*)coef, step_item,
+                             inj_range, inj_out, (const T*)inj_w, (int)n_steps};
+        return mlp_hm(r.hm, [&](auto HM) {
+            return mlp_launch_simt(dopri5_mlp_backward_kernel<T, HM.value>, a, mlp_rev_bwd_threads<HM.value>(),
+                                   mlp_dp5_bwd_extra<HM.value>(a.H), s, b);
+        });
+    });
 }
