@@ -1,4 +1,4 @@
-// Error plumbing and device queries behind the C ABI (include/torchcde_b200.h).
+// Error plumbing, device queries and the solve-variant switch behind the C ABI (include/torchcde_b200.h).
 #include <stdarg.h>
 
 #include "common.cuh"
@@ -35,6 +35,9 @@ int sm_count() {
     return cached;
 }
 
+static int g_solve_variant = kVariantAuto;
+int current_solve_variant() { return g_solve_variant; }
+
 }  // namespace tcde
 
 extern "C" int tcde_abi_version(void) { return TCDE_ABI_VERSION; }
@@ -51,5 +54,18 @@ extern "C" int tcde_device_info(int* sm_count, int* cc_major, int* cc_minor) {
     if (sm_count) *sm_count = n;
     if (cc_major) *cc_major = major;
     if (cc_minor) *cc_minor = minor;
+    return TCDE_OK;
+}
+
+extern "C" int tcde_set_solve_variant(int variant) {
+    using namespace tcde;
+    TCDE_CHECK_ARG(variant >= 0 && (variant & 15) <= 6,
+                   "variant=%d (0 auto, 1 CUDA-core kernel, 3 / 4 tensor-core kernel with the 3xTF32 / 2xFP16 operand split; "
+                   "2, 6 / 5 are aliases of 3 / 4)", variant);
+    // bits above 15 (profiling switches of earlier kernels) are accepted and ignored; 2, 6 and 5 are aliases from the
+    // development history
+    static const SolveVariant canonical[7] = {kVariantAuto, kVariantSimt, kVariantTf32, kVariantTf32,
+                                              kVariantFp16, kVariantFp16, kVariantTf32};
+    g_solve_variant = canonical[variant & 15];
     return TCDE_OK;
 }

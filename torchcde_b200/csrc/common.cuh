@@ -92,7 +92,65 @@ template <int N> __device__ __forceinline__ void cp_async_wait() {
     asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+// ---- host plumbing shared by the entry points of the linear and MLP fields ------------------------------------------
+
+// return the status of call if it is not TCDE_OK
+#define TCDE_TRY(call)                                \
+    do {                                              \
+        const int rc_ = (call);                       \
+        if (rc_ != TCDE_OK) return rc_;               \
+    } while (0)
+
+// every pointer 16-byte aligned (a null pointer counts as aligned)
+template <typename... P> inline bool aligned16(const P*... p) {
+    return (((reinterpret_cast<uintptr_t>(p) & 15u) == 0) && ...);
+}
+
+inline int check_dtype(int dtype) {
+    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
+    return TCDE_OK;
+}
+inline int check_control_kind(int control_kind) {
+    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
+                   control_kind);
+    return TCDE_OK;
+}
+inline int check_method(int method) {
+    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
+    return TCDE_OK;
+}
+
+// f(T()) at the element type of dtype: float for TCDE_F32, else double (the checks have refused every other code)
+template <typename F> inline int by_dtype(int dtype, F&& f) { return dtype == TCDE_F32 ? f(float()) : f(double()); }
+
+// a persistent grid: one CTA per item, at most ctas_per_sm per SM, at least one
+inline int capped_grid(int64_t items, int ctas_per_sm) {
+    const int64_t cap = (int64_t)sm_count() * ctas_per_sm;
+    return (int)(items < 1 ? 1 : items < cap ? items : cap);
+}
+
+// kern<<<grid, threads, smem, s>>>(args...), with smem bytes of dynamic shared memory allowed
+template <typename... P, typename... A>
+inline int launch(void (*kern)(P...), int64_t grid, int threads, size_t smem, cudaStream_t s, const A&... args) {
+    TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
+    if (smem > 0) TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<(unsigned)grid, threads, smem, s>>>(args...);
+    TCDE_CHECK_CUDA(cudaGetLastError());
+    return TCDE_OK;
+}
+
+// ---- the solve variant (tcde_set_solve_variant, api.cu), with its aliases folded in when it is set ------------------
+enum SolveVariant { kVariantAuto = 0, kVariantSimt = 1, kVariantTf32 = 3, kVariantFp16 = 4 };
+int current_solve_variant();
+
+// ---- which kernels serve an entry point of the linear field (linear_route, solve_simt.cu) ---------------------------
+enum LinearAsk { kLinSolve, kLinStages, kLinField, kLinBackward, kLinVjp, kLinParamGrads, kLinScratch, kLinDopri5 };
+struct LinearRoute {
+    bool tc;                      // the tensor-core kernels, else the CUDA-core ones
+    int split;                    // tensor cores: 0 = 3xTF32, 1 = the 16-bit split (2xFP16 solve, 2xBF16 gradients)
+};
+int linear_route(LinearAsk ask, int64_t hidden, int64_t channels, int dtype, bool aligned, const char* what,
+                 LinearRoute* r);
 
 // ---- arguments of the tensor-core solve (solve_tc.cu), filled in by the C entry points of solve_simt.cu ----
 struct UmmaArgs {
@@ -122,11 +180,9 @@ struct UmmaArgs {
     const int32_t* inj_out;      // output index of each entry
     const float* inj_weight;     // its weight
 };
-bool solve_tc_supported(int H, int C);
 // tensor-core kernel (solve_tc.cu): Runge-Kutta state in registers; mode 0 = 3xTF32 operand split, mode 1 = 2xFP16 with
 // per-path power-of-two scaling
 int solve_tc_f32(const UmmaArgs& a, int H, int C, int mode, cudaStream_t stream);
-int current_solve_variant();          // tcde_set_solve_variant: 0 auto, 1 CUDA-core, 2 / 3 tensor cores 3xTF32, 4 tensor cores 2xFP16
 
 // parameter gradients of a whole backward solve on the tensor cores (param_grad_mma.cu): mode 0 = 3xTF32, 1 = 2xBF16 split
 int param_grad_mma_grid(int64_t n_paths, int64_t n_stage_total);

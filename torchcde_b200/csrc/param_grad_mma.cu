@@ -192,21 +192,15 @@ param_grad_mma_kernel(const float* __restrict__ control, int control_kind, int64
 }  // namespace pg
 
 int param_grad_mma_grid(int64_t n_paths, int64_t n_stage_total) {
-    const int64_t items = ((n_paths + pg::TB - 1) / pg::TB) * n_stage_total;
-    int64_t g = (int64_t)sm_count() * 2;
-    if (g > items) g = items;
-    if (g < 1) g = 1;
-    return (int)g;
+    return capped_grid(((n_paths + pg::TB - 1) / pg::TB) * n_stage_total, 2);
 }
 
 int param_grad_mma_f32(const float* control, int control_kind, int64_t n_rows, const float* z_stages, const float* a_stages,
                        const int32_t* stage_index, const float* stage_frac, const float* stage_weight, int n_stage_total,
                        float* scratch, int64_t n_paths, int mode, int grid, cudaStream_t stream) {
-    auto kern = (mode & 1) ? pg::param_grad_mma_kernel<1> : pg::param_grad_mma_kernel<0>;
-    kern<<<grid, pg::kThreads, 0, stream>>>(control, control_kind, n_rows, z_stages, a_stages, stage_index, stage_frac,
-                                             stage_weight, n_stage_total, scratch, n_paths);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
+    return launch((mode & 1) ? pg::param_grad_mma_kernel<1> : pg::param_grad_mma_kernel<0>, grid, pg::kThreads, 0,
+                  stream, control, control_kind, n_rows, z_stages, a_stages, stage_index, stage_frac, stage_weight,
+                  n_stage_total, scratch, n_paths);
 }
 
 }  // namespace tcde

@@ -703,10 +703,10 @@ using namespace tcde;
 
 extern "C" int tcde_dopri5_linear_grid(int64_t n_paths) {
     if (n_paths < 1) return -1;
-    const int64_t pairs = (n_paths + dp5::kRows * dp5::kTiles - 1) / (dp5::kRows * dp5::kTiles);
-    return (int)(pairs < sm_count() ? pairs : sm_count());
+    return capped_grid((n_paths + dp5::kRows * dp5::kTiles - 1) / (dp5::kRows * dp5::kTiles), 1);
 }
 
+// n_launches launches of one attempt kernel, each the next in the sequence, behind one shared-memory attribute call
 static int launch_attempts(dp5::Args a, int64_t first_seq, int64_t n_launches, cudaStream_t s,
                            void (*kernel)(const dp5::Args) = dp5::dopri5_attempt_kernel) {
     constexpr int smem = dp5::Smem::total + 1024;
@@ -727,10 +727,10 @@ extern "C" int tcde_dopri5_linear_attempts(const void* control, int control_kind
                                            void* stream) {
     TCDE_CHECK_ARG(control && knots && weight && bias && state && partials && ctl && out && out_times, "null pointer");
     TCDE_CHECK_ARG(n_paths >= 1 && n_rows >= 1 && n_out >= 2 && n_launches >= 0 && first_seq >= 0, "bad sizes");
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d", control_kind);
-    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && hidden == dp5::kHid && channels == dp5::kCh,
-                         "device-controlled dopri5: built for float32, hidden=32, channels=8");
-    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(state) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
+    TCDE_TRY(check_control_kind(control_kind));
+    LinearRoute r;
+    TCDE_TRY(linear_route(kLinDopri5, hidden, channels, dtype, true, "device-controlled dopri5: ", &r));
+    TCDE_CHECK_SUPPORTED(aligned16(control, state, out),
                          "device-controlled dopri5: control, state and out must be 16-byte aligned");
     TCDE_CHECK_SUPPORTED(n_paths * 32 * 5 < (1ll << 40), "batch too large");
     dp5::Args a{(const float*)control, (const float*)knots, (const float*)weight, (const float*)bias, (float*)state,
@@ -748,14 +748,13 @@ extern "C" int tcde_dopri5_linear_paired_attempts(const void* control, int contr
     TCDE_CHECK_ARG(control && knots && weight && bias && weight2 && bias2 && state && partials && ctl && out && out_times, "null pointer");
     TCDE_CHECK_ARG(dump_z && dump_a && q_index && q_frac && q_weight && max_slots >= 1 && max_slots < (1ll << 24), "null trajectory / bad slot count");
     TCDE_CHECK_ARG(n_ctrl >= 1 && n_rows >= 1 && n_out >= 2 && n_launches >= 0 && first_seq >= 0, "bad sizes");
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d", control_kind);
-    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && hidden == dp5::kHid && channels == dp5::kCh,
-                         "device-controlled dopri5: built for float32, hidden=32, channels=8");
+    TCDE_TRY(check_control_kind(control_kind));
+    LinearRoute r;
+    TCDE_TRY(linear_route(kLinDopri5, hidden, channels, dtype, true, "device-controlled dopri5: ", &r));
     TCDE_CHECK_SUPPORTED(n_ctrl % (dp5::kRows * dp5::kTiles) == 0,
                          "device-controlled dopri5 adjoint: the batch (%lld paths) must be a multiple of %d", (long long)n_ctrl,
                          dp5::kRows * dp5::kTiles);
-    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(state) | reinterpret_cast<uintptr_t>(out) |
-                           reinterpret_cast<uintptr_t>(dump_z) | reinterpret_cast<uintptr_t>(dump_a)) & 15) == 0,
+    TCDE_CHECK_SUPPORTED(aligned16(control, state, out, dump_z, dump_a),
                          "device-controlled dopri5: control, state, out and the trajectories must be 16-byte aligned");
     TCDE_CHECK_SUPPORTED(n_ctrl * 2 * 32 * 5 < (1ll << 40), "batch too large");
     dp5::Args a{(const float*)control, (const float*)knots, (const float*)weight, (const float*)bias, (float*)state,
@@ -774,11 +773,10 @@ extern "C" int tcde_dopri5_linear_record_attempts(const void* control, int contr
     TCDE_CHECK_ARG(control && knots && weight && bias && state && partials && ctl && out && out_times, "null pointer");
     TCDE_CHECK_ARG(rec_step && rec_index && rec_frac && max_slots >= 1 && max_slots < (1ll << 24), "null record / bad slot count");
     TCDE_CHECK_ARG(n_paths >= 1 && n_rows >= 1 && n_out >= 2 && n_launches >= 0 && first_seq >= 0, "bad sizes");
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d", control_kind);
-    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && hidden == dp5::kHid && channels == dp5::kCh,
-                         "device-controlled dopri5: built for float32, hidden=32, channels=8");
-    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(state) | reinterpret_cast<uintptr_t>(out) |
-                           reinterpret_cast<uintptr_t>(rec_z)) & 15) == 0,
+    TCDE_TRY(check_control_kind(control_kind));
+    LinearRoute r;
+    TCDE_TRY(linear_route(kLinDopri5, hidden, channels, dtype, true, "device-controlled dopri5: ", &r));
+    TCDE_CHECK_SUPPORTED(aligned16(control, state, out, rec_z),
                          "device-controlled dopri5: control, state, out and the record must be 16-byte aligned");
     TCDE_CHECK_SUPPORTED(n_paths * 32 * 6 * max_slots < (1ll << 40), "record too large");
     dp5::Args a{(const float*)control, (const float*)knots, (const float*)weight, (const float*)bias, (float*)state,
@@ -797,22 +795,17 @@ extern "C" int tcde_dopri5_linear_backward(const void* control, int control_kind
     TCDE_CHECK_ARG(control && weight_t && zeros && grad_out && carry && coef && stage_index && stage_frac && inj_range &&
                    (inj_out || n_steps == 0) && inj_w, "null pointer");
     TCDE_CHECK_ARG(n_paths >= 1 && n_rows >= 1 && n_out >= 2 && n_steps >= 0 && n_steps < (1ll << 24), "bad sizes");
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d", control_kind);
-    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && hidden == dp5::kHid && channels == dp5::kCh,
-                         "dopri5 backward: built for float32, hidden=32, channels=8");
-    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(grad_out) | reinterpret_cast<uintptr_t>(carry) |
-                           reinterpret_cast<uintptr_t>(kappa)) & 15) == 0,
+    TCDE_TRY(check_control_kind(control_kind));
+    LinearRoute r;
+    TCDE_TRY(linear_route(kLinDopri5, hidden, channels, dtype, true, "dopri5 backward: ", &r));
+    TCDE_CHECK_SUPPORTED(aligned16(control, grad_out, carry, kappa),
                          "dopri5 backward: control, grad_out, carry and kappa must be 16-byte aligned");
     if (n_steps == 0) return TCDE_OK;
-    dp5::BwdArgs a{(const float*)control, (const float*)weight_t, (const float*)zeros, (const float*)grad_out, (float*)carry,
-                   (float*)kappa, (const float*)coef, stage_index, (const float*)stage_frac, inj_range, inj_out,
-                   (const float*)inj_w, n_paths, n_rows, control_kind, (int)n_out, (int)n_steps, (float)sign};
-    constexpr int smem = dp5::BwdSmem::total + 1024;
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(dp5::dopri5_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    const dp5::BwdArgs a{(const float*)control, (const float*)weight_t, (const float*)zeros, (const float*)grad_out,
+                         (float*)carry, (float*)kappa, (const float*)coef, stage_index, (const float*)stage_frac,
+                         inj_range, inj_out, (const float*)inj_w, n_paths, n_rows, control_kind, (int)n_out,
+                         (int)n_steps, (float)sign};
     const int64_t warps = (n_paths + 31) / 32;
-    const int64_t blocks = (warps + dp5::kThreads / 32 - 1) / (dp5::kThreads / 32);
-    const int grid = (int)(blocks < sm_count() ? blocks : sm_count());
-    dp5::dopri5_backward_kernel<<<grid, dp5::kThreads, smem, static_cast<cudaStream_t>(stream)>>>(a);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
+    return launch(dp5::dopri5_backward_kernel, capped_grid((warps + dp5::kThreads / 32 - 1) / (dp5::kThreads / 32), 1),
+                  dp5::kThreads, dp5::BwdSmem::total + 1024, static_cast<cudaStream_t>(stream), a);
 }

@@ -280,16 +280,6 @@ static std::optional<MlpSimtLayout<T>> mlp_simt_fit(int H, int C, int W, int nt,
     return std::nullopt;
 }
 
-// kern<<<grid, threads, smem, s>>>(args...), with smem bytes of dynamic shared memory allowed
-template <typename... P, typename... A>
-static int mlp_launch(void (*kern)(P...), int64_t grid, int threads, size_t smem, cudaStream_t s, const A&... args) {
-    if (smem > 0) TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
-    kern<<<(unsigned)grid, threads, smem, s>>>(args...);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
-}
-
 // kern(a, layout, args...) on the CUDA cores: one thread per path in CTAs of nt threads, the layout fitted for them
 template <typename T, typename... P, typename... A>
 static int mlp_launch_simt(void (*kern)(P...), const MlpArgs<T>& a, int nt, int extra, cudaStream_t s,
@@ -297,16 +287,13 @@ static int mlp_launch_simt(void (*kern)(P...), const MlpArgs<T>& a, int nt, int 
     const auto lay = mlp_simt_fit<T>(a.H, a.C, a.W, nt, extra);
     TCDE_CHECK_SUPPORTED(lay.has_value(), "MLP kernel on the CUDA cores: hidden=%d channels=%d width=%d do not fit its "
                          "shared memory", a.H, a.C, a.W);
-    return mlp_launch(kern, (a.n_paths + nt - 1) / nt, nt, lay->total, s, a, *lay, args...);
+    return launch(kern, (a.n_paths + nt - 1) / nt, nt, lay->total, s, a, *lay, args...);
 }
 
 // f(std::integral_constant<int, HM>()) at the CUDA-core instantiation hm (8 or 32)
 template <typename F> static int mlp_hm(int hm, F&& f) {
     return hm == 8 ? f(std::integral_constant<int, 8>()) : f(std::integral_constant<int, 32>());
 }
-
-// f(T()) at the element type of dtype: float for TCDE_F32, else double (the checks have refused every other code)
-template <typename F> static int mlp_dtype(int dtype, F&& f) { return dtype == TCDE_F32 ? f(float()) : f(double()); }
 
 // ---- the backward of the CUDA-core solve (cdeint(..., adjoint=False)): one thread per path ---------------------------
 //
@@ -2107,10 +2094,7 @@ static MlpArgs<T> mlp_simt_args(const void* control, int control_kind, int64_t n
 
 // the persistent grid of mlp_simt_param_grad_kernel (independent of the dtype: the scratch size has no dtype)
 static int64_t mlp_simt_param_grid(int64_t n_paths, int64_t n_total, int ni) {
-    const int64_t blocks = ((n_paths + ni - 1) / ni) * n_total;
-    int64_t g = (int64_t)sm_count() * kMlpPgCtasPerSm;
-    if (g > blocks) g = blocks;
-    return g < 1 ? 1 : g;
+    return capped_grid(((n_paths + ni - 1) / ni) * n_total, kMlpPgCtasPerSm);
 }
 
 // the items per block of the parameter gradients at this shape (sized for 8-byte elements, so that both dtypes use the
@@ -2137,11 +2121,11 @@ static int mlp_simt_param_grads(const MlpArgs<T>& a, int hm, const T* z_stages, 
     const int64_t n_params = mlp_simt_n_params(a.H, a.C, a.W);
     const MlpSimtPgArgs<T> p{z_stages, kappa, (T*)scratch, n_params, (int)n_total};
     const int rc = mlp_hm(hm, [&](auto HM) {
-        return mlp_launch(mlp_simt_param_grad_kernel<T, HM.value>, grid, ni, pg.total, s, a, lay, pg, p);
+        return launch(mlp_simt_param_grad_kernel<T, HM.value>, grid, ni, pg.total, s, a, lay, pg, p);
     });
     if (rc != TCDE_OK || !(grad_w1 || grad_b1 || grad_w2 || grad_b2)) return rc;
     const int64_t o_b1 = (int64_t)a.W * a.H, o_w2 = o_b1 + a.W, o_b2 = o_w2 + (int64_t)a.H * a.C * a.W;
-    return mlp_launch(mlp_simt_param_reduce_kernel<T>, (n_params + 255) / 256, 256, 0, s, (const T*)scratch, (int)grid,
+    return launch(mlp_simt_param_reduce_kernel<T>, (n_params + 255) / 256, 256, 0, s, (const T*)scratch, (int)grid,
                       n_params, o_b1, o_w2, o_b2, (T)scale, (T*)grad_w1, (T*)grad_b1, (T*)grad_w2, (T*)grad_b2);
 }
 
@@ -2177,10 +2161,7 @@ static int mlp_field_eval(int hm, const void* control, int control_kind, int64_t
 }
 
 static int64_t mlp_param_grid(int64_t n_paths, int64_t n_total) {
-    const int64_t items = ((n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths) * n_total;
-    int64_t g = sm_count();
-    if (g > items) g = items;
-    return g < 1 ? 1 : g;
+    return capped_grid(((n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths) * n_total, 1);
 }
 
 // ---- the backward of cdeint(..., adjoint=False) under the host-driven dopri5 (tcde_dopri5_mlp_backward) ---------------
@@ -2419,12 +2400,9 @@ struct MlpRoute {
 // The checks of the entry points' enum arguments.  The solve and the reversible Heun and dopri5 entries reject an unknown
 // dtype as an argument; to the others it is a dtype the route policy does not serve.
 static int mlp_check_args(MlpAsk ask, int control_kind, int dtype, int method = TCDE_EULER) {
-    const bool dtype_arg = ask == kMlpSolve || ask == kMlpReversible || ask == kMlpDopri5Backward;
-    TCDE_CHECK_ARG(!dtype_arg || dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
-    return TCDE_OK;
+    if (ask == kMlpSolve || ask == kMlpReversible || ask == kMlpDopri5Backward) TCDE_TRY(check_dtype(dtype));
+    TCDE_TRY(check_control_kind(control_kind));
+    return check_method(method);
 }
 
 static int mlp_check_shape(int64_t hidden, int64_t channels, int64_t width) {
@@ -2435,7 +2413,7 @@ static int mlp_check_shape(int64_t hidden, int64_t channels, int64_t width) {
 
 static int mlp_route(MlpAsk ask, int64_t hidden, int64_t channels, int64_t width, int dtype, bool aligned,
                      const char* what, MlpRoute* r) {
-    if (const int rc = mlp_check_shape(hidden, channels, width); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_shape(hidden, channels, width));
     const int variant = current_solve_variant();
     const bool simt = hidden <= 8 || hidden * channels <= kMlpChunk;
     const bool tc_shape = hidden == tc::kHid && channels == tc::kCh && width == tc::mlp::kWidth;
@@ -2449,15 +2427,17 @@ static int mlp_route(MlpAsk ask, int64_t hidden, int64_t channels, int64_t width
     }
     if (ask == kMlpSolve) {
         if (dtype == TCDE_F32) {
-            TCDE_CHECK_SUPPORTED(variant <= 1 || variant == 4 || variant == 5,
+            TCDE_CHECK_SUPPORTED(variant != kVariantTf32,
                                  "%s: solve variant %d (3xTF32) is not built for the MLP field", what, variant);
-            TCDE_CHECK_SUPPORTED(variant <= 1 || (tc_shape && aligned), "%s: the tensor-core kernel is built for "
+            TCDE_CHECK_SUPPORTED(variant <= kVariantSimt || (tc_shape && aligned),
+                                 "%s: the tensor-core kernel is built for "
                                  "hidden=32, channels=8, width=128 with 16-byte aligned control, z0 and out (got %lld, "
                                  "%lld, %lld)", what, (long long)hidden, (long long)channels, (long long)width);
-            r->tc = variant >= 4 || (variant == 0 && tc_shape && aligned);
+            r->tc = variant == kVariantFp16 || (variant == kVariantAuto && tc_shape && aligned);
             if (r->tc) return TCDE_OK;
         }
-        TCDE_CHECK_SUPPORTED(simt || variant == 1, "%s: at hidden=%lld channels=%lld the CUDA-core kernel is slower than "
+        TCDE_CHECK_SUPPORTED(simt || variant == kVariantSimt,
+                             "%s: at hidden=%lld channels=%lld the CUDA-core kernel is slower than "
                              "the stage loop; automatic selection does not run it (variant 1 forces it)", what,
                              (long long)hidden, (long long)channels);
         TCDE_CHECK_SUPPORTED(hidden <= 32, "%s: hidden=%lld > 32 is not built for the CUDA-core kernel", what,
@@ -2467,7 +2447,7 @@ static int mlp_route(MlpAsk ask, int64_t hidden, int64_t channels, int64_t width
     if (!simt) {
         r->tc = true;
         TCDE_CHECK_SUPPORTED((ask == kMlpStages || ask == kMlpBackward || ask == kMlpParamGrads) && dtype == TCDE_F32 &&
-                                 tc_shape && (variant == 0 || variant == 4 || variant == 5),
+                                 tc_shape && (variant == kVariantAuto || variant == kVariantFp16),
                              "%s is built for fp32, hidden=32, channels=8, width=128 on the tensor-core kernel where it "
                              "has one, else for the CUDA-core shapes (hidden <= 8, or hidden * channels <= 32 under solve "
                              "variant 1; got dtype=%d, %lld, %lld, %lld, solve variant %d)", what, dtype,
@@ -2475,17 +2455,19 @@ static int mlp_route(MlpAsk ask, int64_t hidden, int64_t channels, int64_t width
         TCDE_CHECK_SUPPORTED(aligned, "%s: the tensor-core kernel needs 16-byte aligned buffers", what);
         return TCDE_OK;
     }
-    TCDE_CHECK_SUPPORTED(hidden <= 8 || variant == 1, "%s: at hidden=%lld the CUDA-core route is slower than the stage "
+    TCDE_CHECK_SUPPORTED(hidden <= 8 || variant == kVariantSimt,
+                         "%s: at hidden=%lld the CUDA-core route is slower than the stage "
                          "loop; automatic selection does not run it (variant 1 forces it)", what, (long long)hidden);
-    TCDE_CHECK_SUPPORTED((dtype == TCDE_F32 || dtype == TCDE_F64) && variant <= 1, "%s on the CUDA cores is built for "
+    TCDE_CHECK_SUPPORTED((dtype == TCDE_F32 || dtype == TCDE_F64) && variant <= kVariantSimt,
+                         "%s on the CUDA cores is built for "
                          "fp32 / fp64 under solve variant 0 or 1 (got dtype=%d, solve variant %d)", what, dtype,
                          variant);
-    TCDE_CHECK_SUPPORTED(ask != kMlpField || variant == 1 ||
+    TCDE_CHECK_SUPPORTED(ask != kMlpField || variant == kVariantSimt ||
                              (dtype == TCDE_F32 && hidden * channels <= kMlpChunk && width <= 128),
                          "%s: at dtype=%d hidden=%lld channels=%lld width=%lld it is slower than autograd per stage; "
                          "automatic selection does not run it (variant 1 forces it)", what, dtype, (long long)hidden,
                          (long long)channels, (long long)width);
-    TCDE_CHECK_SUPPORTED(ask != kMlpReversible || variant == 1 || hidden * channels <= kMlpChunk,
+    TCDE_CHECK_SUPPORTED(ask != kMlpReversible || variant == kVariantSimt || hidden * channels <= kMlpChunk,
                          "%s: at hidden=%lld channels=%lld the backward is slower than per-step autograd; automatic "
                          "selection does not run it (variant 1 forces it)", what, (long long)hidden, (long long)channels);
     const int H = (int)hidden, C = (int)channels, W = (int)width;
@@ -2516,7 +2498,7 @@ static int mlp_fixed_solve(const MlpRoute& r, const void* control, int control_k
                            int64_t n_steps, const void* step_dt, const int32_t* stage_index, const void* stage_frac,
                            int64_t n_out, const int32_t* out_step, const int32_t* out_mode, const void* out_slope,
                            double sign, int dtype, cudaStream_t s) {
-    return mlp_dtype(dtype, [&](auto t) {
+    return by_dtype(dtype, [&](auto t) {
         using T = decltype(t);
         const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths, channels,
                                               hidden, width, method, n_steps, step_dt, stage_index, stage_frac, n_out,
@@ -2526,7 +2508,7 @@ static int mlp_fixed_solve(const MlpRoute& r, const void* control, int control_k
                              (float*)a.out, (const float*)a.step_dt, a.stage_index, (const float*)a.stage_frac,
                              a.out_step, a.out_mode, (const float*)a.out_slope, a.n_paths, a.n_rows, a.control_kind,
                              a.method, a.n_stages, a.n_steps, a.n_out, (float)a.sign, (float*)stage_dump, 0};
-            return mlp_launch(stage_dump ? tc::mlp::cdeint_mlp_wgmma_kernel<true> : tc::mlp::cdeint_mlp_wgmma_kernel<false>,
+            return launch(stage_dump ? tc::mlp::cdeint_mlp_wgmma_kernel<true> : tc::mlp::cdeint_mlp_wgmma_kernel<false>,
                               (n_paths + tc::mlp::kPaths - 1) / tc::mlp::kPaths, tc::mlp::kThreads, tc::mlp::kSmem, s,
                               u, (const float*)w2, (const float*)b2);
         }
@@ -2552,15 +2534,12 @@ extern "C" int tcde_cdeint_fixed_mlp(const void* control, int control_kind, int6
     TCDE_CHECK_ARG(step_dt && stage_index && stage_frac && out_step && out_mode && out_slope, "null schedule pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1, "bad sizes");
     TCDE_CHECK_ARG(n_steps >= 1 && n_out >= 1, "n_steps=%lld n_out=%lld", (long long)n_steps, (long long)n_out);
-    if (const int rc = mlp_check_args(kMlpSolve, control_kind, dtype, method); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_args(kMlpSolve, control_kind, dtype, method));
     TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
-    if (const int rc = mlp_check_shape(hidden, channels, width); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_shape(hidden, channels, width));
     if (n_paths == 0) return TCDE_OK;
     MlpRoute r;
-    if (const int rc = mlp_route(kMlpSolve, hidden, channels, width, dtype,
-                                 aligned16(control) && aligned16(z0) && aligned16(out), "the MLP solve", &r);
-        rc != TCDE_OK)
-        return rc;
+    TCDE_TRY(mlp_route(kMlpSolve, hidden, channels, width, dtype, aligned16(control, z0, out), "the MLP solve", &r));
     return mlp_fixed_solve(r, control, control_kind, n_rows, w1, b1, w2, b2, z0, out, nullptr, n_paths, channels, hidden,
                            width, method, n_steps, step_dt, stage_index, stage_frac, n_out, out_step, out_mode,
                            out_slope, sign, dtype, static_cast<cudaStream_t>(stream));
@@ -2576,14 +2555,11 @@ extern "C" int tcde_cdeint_fixed_mlp_stages(const void* control, int control_kin
     TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z0 && out && stage_dump, "null data pointer");
     TCDE_CHECK_ARG(step_dt && stage_index && stage_frac && out_step && out_mode && out_slope, "null schedule pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_steps >= 1 && n_out >= 1, "bad sizes");
-    if (const int rc = mlp_check_args(kMlpStages, control_kind, dtype, method); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_args(kMlpStages, control_kind, dtype, method));
     TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
     MlpRoute r;
-    if (const int rc = mlp_route(kMlpStages, hidden, channels, width, dtype,
-                                 aligned16(control) && aligned16(z0) && aligned16(out) && aligned16(stage_dump),
-                                 "the MLP stage-dump solve", &r);
-        rc != TCDE_OK)
-        return rc;
+    TCDE_TRY(mlp_route(kMlpStages, hidden, channels, width, dtype, aligned16(control, z0, out, stage_dump),
+                       "the MLP stage-dump solve", &r));
     TCDE_CHECK_SUPPORTED(r.tc || n_paths * hidden * n_steps * 4 < (1ll << 62), "stage dump too large");
     if (n_paths == 0) return TCDE_OK;
     return mlp_fixed_solve(r, control, control_kind, n_rows, w1, b1, w2, b2, z0, out, stage_dump, n_paths, channels,
@@ -2601,18 +2577,15 @@ extern "C" int tcde_cdeint_fixed_mlp_backward(
     TCDE_CHECK_ARG(step_dt_rev && stage_index_rev && stage_frac_rev && inj_range && inj_out && inj_weight,
                    "null schedule pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_steps >= 1 && n_out >= 1, "bad sizes");
-    if (const int rc = mlp_check_args(kMlpBackward, control_kind, dtype, method); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_args(kMlpBackward, control_kind, dtype, method));
     TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
     MlpRoute r;
-    if (const int rc = mlp_route(kMlpBackward, hidden, channels, width, dtype,
-                                 aligned16(control) && aligned16(stage_dump) && aligned16(grad_out) &&
-                                     aligned16(grad_z0) && aligned16(kappa_dump),
-                                 "the MLP Runge-Kutta backward", &r);
-        rc != TCDE_OK)
-        return rc;
+    TCDE_TRY(mlp_route(kMlpBackward, hidden, channels, width, dtype,
+                       aligned16(control, stage_dump, grad_out, grad_z0, kappa_dump),
+                       "the MLP Runge-Kutta backward", &r));
     if (n_paths == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    return mlp_dtype(dtype, [&](auto t) {
+    return by_dtype(dtype, [&](auto t) {
         using T = decltype(t);
         const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, grad_z0, n_paths,
                                               channels, hidden, width, method, n_steps, step_dt_rev, stage_index_rev,
@@ -2623,7 +2596,7 @@ extern "C" int tcde_cdeint_fixed_mlp_backward(
                              nullptr, n_paths, n_rows, control_kind, method, a.n_stages, (int)n_steps, (int)n_out,
                              (float)sign, (float*)kappa_dump, 0, (const float*)grad_out, inj_range, inj_out,
                              (const float*)inj_weight};
-            return mlp_launch(tc::mlp::cdeint_mlp_backward_kernel, (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths,
+            return launch(tc::mlp::cdeint_mlp_backward_kernel, (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths,
                               tc::mlp::kBwdThreads, tc::mlp::kBwdSmem, s, u, (const float*)w2, (const float*)b2,
                               (const float*)stage_dump);
         }
@@ -2657,14 +2630,11 @@ extern "C" int tcde_mlp_field_param_grads(const void* control, int control_kind,
     TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z_stages && kappa_stages && stage_index && stage_frac && scratch,
                    "null data pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_stages_total >= 1 && n_stages_total < (1ll << 31), "bad sizes");
-    if (const int rc = mlp_check_args(kMlpParamGrads, control_kind, dtype); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_args(kMlpParamGrads, control_kind, dtype));
     MlpRoute r;
-    if (const int rc = mlp_route(kMlpParamGrads, hidden, channels, width, dtype,
-                                 aligned16(control) && aligned16(z_stages) && aligned16(kappa_stages) &&
-                                     aligned16(scratch),
-                                 "the MLP parameter gradients", &r);
-        rc != TCDE_OK)
-        return rc;
+    TCDE_TRY(mlp_route(kMlpParamGrads, hidden, channels, width, dtype,
+                       aligned16(control, z_stages, kappa_stages, scratch),
+                       "the MLP parameter gradients", &r));
     if (n_paths == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     if (r.tc) {
@@ -2678,12 +2648,12 @@ extern "C" int tcde_mlp_field_param_grads(const void* control, int control_kind,
                                          s>>>(a);
         TCDE_CHECK_CUDA(cudaGetLastError());
         if (!(grad_w1 || grad_b1 || grad_w2 || grad_b2)) return TCDE_OK;
-        return mlp_launch(tc::mlp::mlp_param_reduce_kernel, (tc::mlp::kPgParams + 255) / 256, 256, 0, s,
+        return launch(tc::mlp::mlp_param_reduce_kernel, (tc::mlp::kPgParams + 255) / 256, 256, 0, s,
                           (const float*)scratch, (int)grid, (float)scale, (float*)grad_w1, (float*)grad_b1,
                           (float*)grad_w2, (float*)grad_b2);
     }
     // the forward's stage tables; the solve's method and steps do not matter here
-    return mlp_dtype(dtype, [&](auto t) {
+    return by_dtype(dtype, [&](auto t) {
         using T = decltype(t);
         return mlp_simt_param_grads(mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr,
                                                      n_paths, channels, hidden, width, TCDE_EULER, 1, nullptr,
@@ -2700,13 +2670,11 @@ extern "C" int tcde_vector_field_mlp(const void* control, int control_kind, int6
     TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z && out, "null data pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1, "bad sizes");
     TCDE_CHECK_ARG(index >= 0 && index < n_rows, "index=%d outside [0, %lld)", index, (long long)n_rows);
-    if (const int rc = mlp_check_args(kMlpField, control_kind, dtype); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_args(kMlpField, control_kind, dtype));
     MlpRoute r;
-    if (const int rc = mlp_route(kMlpField, hidden, channels, width, dtype, true, "the MLP field evaluation", &r);
-        rc != TCDE_OK)
-        return rc;
+    TCDE_TRY(mlp_route(kMlpField, hidden, channels, width, dtype, true, "the MLP field evaluation", &r));
     if (n_paths == 0) return TCDE_OK;
-    return mlp_dtype(dtype, [&](auto t) {
+    return by_dtype(dtype, [&](auto t) {
         return mlp_field_eval<decltype(t)>(r.hm, control, control_kind, n_rows, w1, b1, w2, b2, z, out, n_paths,
                                            channels, hidden, width, index, frac, nullptr, nullptr, nullptr, nullptr,
                                            nullptr, nullptr, nullptr, 1.0, 1.0, 1.0, static_cast<cudaStream_t>(stream));
@@ -2732,14 +2700,12 @@ extern "C" int tcde_vector_field_mlp_vjp(const void* control, int control_kind, 
     TCDE_CHECK_ARG(control && w1 && b1 && w2 && b2 && z && a && f_out && vjp_z_out && scratch, "null data pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1, "bad sizes");
     TCDE_CHECK_ARG(index >= 0 && index < n_rows, "index=%d outside [0, %lld)", index, (long long)n_rows);
-    if (const int rc = mlp_check_args(kMlpField, control_kind, dtype); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_args(kMlpField, control_kind, dtype));
     TCDE_CHECK_ARG(aligned16(scratch), "scratch must be 16-byte aligned");
     MlpRoute r;
-    if (const int rc = mlp_route(kMlpField, hidden, channels, width, dtype, true, "the MLP adjoint stage", &r);
-        rc != TCDE_OK)
-        return rc;
+    TCDE_TRY(mlp_route(kMlpField, hidden, channels, width, dtype, true, "the MLP adjoint stage", &r));
     if (n_paths == 0) return TCDE_OK;
-    return mlp_dtype(dtype, [&](auto t) {
+    return by_dtype(dtype, [&](auto t) {
         return mlp_field_eval<decltype(t)>(r.hm, control, control_kind, n_rows, w1, b1, w2, b2, z, f_out, n_paths,
                                            channels, hidden, width, index, frac, a, vjp_z_out, grad_w1, grad_b1, grad_w2,
                                            grad_b2, scratch, f_scale, vjp_scale, grad_scale,
@@ -2760,16 +2726,14 @@ extern "C" int tcde_cdeint_reversible_heun_mlp(const void* control, int control_
     TCDE_CHECK_ARG(n_steps >= 1 && n_out >= 1, "n_steps=%lld n_out=%lld", (long long)n_steps, (long long)n_out);
     TCDE_CHECK_ARG(checkpoint_stride >= 1 && checkpoint_stride < (1ll << 30), "checkpoint_stride=%lld",
                    (long long)checkpoint_stride);
-    if (const int rc = mlp_check_args(kMlpReversible, control_kind, dtype); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_args(kMlpReversible, control_kind, dtype));
     TCDE_CHECK_SUPPORTED(n_steps + 1 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
     MlpRoute r;
-    if (const int rc = mlp_route(kMlpReversible, hidden, channels, width, dtype, true, "the MLP reversible Heun solve",
-                                 &r);
-        rc != TCDE_OK)
-        return rc;
+    TCDE_TRY(mlp_route(kMlpReversible, hidden, channels, width, dtype, true, "the MLP reversible Heun solve",
+                       &r));
     if (n_paths == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    return mlp_dtype(dtype, [&](auto t) {
+    return by_dtype(dtype, [&](auto t) {
         using T = decltype(t);
         const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, z0, out, n_paths, channels,
                                               hidden, width, TCDE_REVERSIBLE_HEUN, n_steps, step_dt, stage_index,
@@ -2793,14 +2757,12 @@ extern "C" int tcde_reversible_heun_mlp_backward_segment(
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && width >= 1 && n_rows >= 1 && n_out >= 1, "bad sizes");
     TCDE_CHECK_ARG(lo >= 0 && hi > lo && hi <= n_steps && n_steps + 1 < (1ll << 31), "lo=%lld hi=%lld n_steps=%lld",
                    (long long)lo, (long long)hi, (long long)n_steps);
-    if (const int rc = mlp_check_args(kMlpReversible, control_kind, dtype); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_args(kMlpReversible, control_kind, dtype));
     MlpRoute r;
-    if (const int rc = mlp_route(kMlpReversible, hidden, channels, width, dtype, true, "the MLP reversible backward", &r);
-        rc != TCDE_OK)
-        return rc;
+    TCDE_TRY(mlp_route(kMlpReversible, hidden, channels, width, dtype, true, "the MLP reversible backward", &r));
     if (n_paths == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    return mlp_dtype(dtype, [&](auto t) {
+    return by_dtype(dtype, [&](auto t) {
         using T = decltype(t);
         const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths,
                                               channels, hidden, width, TCDE_REVERSIBLE_HEUN, n_steps, step_dt,
@@ -2825,16 +2787,14 @@ extern "C" int tcde_dopri5_mlp_backward(const void* control, int control_kind, i
     TCDE_CHECK_ARG(coef && step_item && item_index && item_frac && inj_range && inj_out && inj_w, "null table pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_out >= 2 && n_out < (1ll << 31) && n_steps >= 0 &&
                        n_steps < (1ll << 24) && channels >= 1 && hidden >= 1 && width >= 1, "bad sizes");
-    if (const int rc = mlp_check_args(kMlpDopri5Backward, control_kind, dtype); rc != TCDE_OK) return rc;
+    TCDE_TRY(mlp_check_args(kMlpDopri5Backward, control_kind, dtype));
     TCDE_CHECK_ARG(sign == 1.0 || sign == -1.0, "sign=%g", sign);
     MlpRoute r;
-    if (const int rc = mlp_route(kMlpDopri5Backward, hidden, channels, width, dtype, true, "the MLP dopri5 backward", &r);
-        rc != TCDE_OK)
-        return rc;
+    TCDE_TRY(mlp_route(kMlpDopri5Backward, hidden, channels, width, dtype, true, "the MLP dopri5 backward", &r));
     TCDE_CHECK_SUPPORTED(n_paths * hidden * 7 * n_steps < (1ll << 62), "record too large");
     if (n_paths == 0 || n_steps == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    return mlp_dtype(dtype, [&](auto t) {
+    return by_dtype(dtype, [&](auto t) {
         using T = decltype(t);
         const MlpArgs<T> a = mlp_simt_args<T>(control, control_kind, n_rows, w1, b1, w2, b2, nullptr, nullptr, n_paths,
                                               channels, hidden, width, TCDE_EULER, n_steps, nullptr, item_index,

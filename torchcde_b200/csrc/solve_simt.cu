@@ -471,6 +471,7 @@ vector_field_kernel(const T* __restrict__ control, int control_kind, int64_t n_r
 template <typename T, int ST, int CT>
 static int launch_solve_ct(SolveArgs<T> a, cudaStream_t stream) {
     auto kern = (a.method == TCDE_REVERSIBLE_HEUN) ? cdeint_simt_kernel<T, ST, CT, true> : cdeint_simt_kernel<T, ST, CT, false>;
+    // the occupancy queries below see the kernel with the largest shared memory any CTA size would need
     TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
     int g_max = 256 / a.H;
     if (g_max < 1) g_max = 1;
@@ -507,30 +508,22 @@ static int launch_solve_ct(SolveArgs<T> a, cudaStream_t stream) {
                          a.C);
     a.groups = best_g;
     a.threads = ((best_g * a.H + 31) / 32) * 32;
-    const int64_t ctas = (a.n_paths + best_lay.TB - 1) / best_lay.TB;
-    TCDE_CHECK_SUPPORTED(ctas < (1ll << 31), "too many paths");
-    kern<<<(unsigned)ctas, a.threads, best_lay.total, stream>>>(a, best_lay);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
+    return launch(kern, (a.n_paths + best_lay.TB - 1) / best_lay.TB, a.threads, best_lay.total, stream, a, best_lay);
 }
 
-template <typename T, int ST>
-static int launch_solve(const SolveArgs<T>& a_in, cudaStream_t stream) {
-    SolveArgs<T> a = a_in;
-    TCDE_CHECK_SUPPORTED(a.H <= 256, "fused solve: hidden=%d > 256 is not supported by the CUDA-core kernel", a.H);
+// the CUDA-core solve at hidden <= 256 (linear_route): 8 channels per pass where the padded channels allow it, else 4
+template <typename T>
+static int launch_solve(SolveArgs<T> a, cudaStream_t stream) {
+    constexpr int ST = sizeof(T) == 4 ? 8 : 4;
     a.Cp = ((a.C + 3) / 4) * 4;
     if (a.Cp % 8 == 0) return launch_solve_ct<T, ST, 8>(a, stream);
     return launch_solve_ct<T, ST, 4>(a, stream);
 }
 
-int solve_simt_f32(const SolveArgs<float>& a, cudaStream_t s) { return launch_solve<float, 8>(a, s); }
-int solve_simt_f64(const SolveArgs<double>& a, cudaStream_t s) { return launch_solve<double, 4>(a, s); }
-
 template <typename T>
 static int launch_field(const void* control, int control_kind, int64_t n_rows, const void* weight, const void* bias,
                         const void* z, void* out, int64_t n_paths, int C, int H, int index, double frac,
                         cudaStream_t stream) {
-    TCDE_CHECK_SUPPORTED(H <= 256, "vector field: hidden=%d > 256", H);
     {
         // the register-tiled stage of the fused solve, run for exactly one evaluation
         SolveArgs<T> a{};
@@ -540,39 +533,92 @@ static int launch_field(const void* control, int control_kind, int64_t n_rows, c
         a.control_kind = control_kind; a.method = TCDE_EULER; a.n_stages = 1; a.n_steps = 1; a.n_out = 1;
         a.sign = T(1);
         a.eval_only = 1; a.eval_index = index; a.eval_frac = (T)frac;
-        const int rc = launch_solve<T, (sizeof(T) == 4 ? 8 : 4)>(a, stream);
+        const int rc = launch_solve<T>(a, stream);
         if (rc != TCDE_ERR_UNSUPPORTED) return rc;
     }
     const int ppc = 256 / H;
     const int threads = ppc * H;
     const size_t smem = (size_t)ppc * (H + C) * sizeof(T);
     TCDE_CHECK_SUPPORTED(smem <= 48 * 1024, "vector field: channels=%d too large", C);
-    const int64_t ctas = (n_paths + ppc - 1) / ppc;
-    vector_field_kernel<T><<<(unsigned)ctas, threads, smem, stream>>>(
-        (const T*)control, control_kind, n_rows, (const T*)weight, (const T*)bias, (const T*)z, (T*)out, n_paths, C, H,
-        index, (T)frac);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
+    return launch(vector_field_kernel<T>, (n_paths + ppc - 1) / ppc, threads, smem, stream, (const T*)control,
+                  control_kind, n_rows, (const T*)weight, (const T*)bias, (const T*)z, (T*)out, n_paths, C, H, index,
+                  (T)frac);
 }
 
-// ---- tensor-core variant (solve_tc.cu) ---------------------------------------------------------
+// ---- which kernels serve an entry point: the one route policy of the linear field -------------------------------------
+//
+// What is asked, then what serves it ("tc": fp32 at hidden 32, channels 8; the solve variant is the canonical one of
+// tcde_set_solve_variant: auto, CUDA cores, 3xTF32, 2xFP16).
+//   solve (fixed-step       fp32: tc under 3xTF32 and 2xFP16 at every shape (solve_tc_f32 then refuses any shape but 32 / 8
+//   and reversible Heun     and misaligned control, z0, out or dump); under auto tc at 32 / 8 with `aligned` buffers, with
+//   forward), stages        the TCDE_DEFAULT_TC_MODE split; else, and for fp64 under every variant, the CUDA cores at
+//                           hidden <= 256.  stages: the dump is written by tc only, so the CUDA-core answer is refused.
+//   field                   the CUDA cores at hidden <= 256, every dtype and variant.
+//   backward (Runge-Kutta,  tc, 2xFP16 wgmma under every variant, at fp32 32 / 8 only.
+//   reversible segment)
+//   vjp                     the CUDA cores, at fp32 32 / 8 only.
+//   param_grads             tc with the 3xTF32 split under 3xTF32, the 2xBF16 split under auto and 2xFP16; the CUDA
+//                           cores under the CUDA-core variant; fp32 32 / 8 only.
+//   scratch (of vjp and     32 / 8, whatever the dtype and the variant.
+//   param_grads)
+//   dopri5 (attempts,       tc, at fp32 32 / 8 only.
+//   paired, record,
+//   backward)
+// Elsewhere TCDE_ERR_UNSUPPORTED, and the caller keeps its own route.  `what` begins the refusal messages of the
+// fixed-shape asks.  What the entry points keep outside the policy, each as it always was:
+//   * the fixed-step solve, its stage dump, the reversible Heun forward and the field return TCDE_OK for an empty batch
+//     before they ask;
+//   * every other entry point checks the alignment of its own buffers after the answer, with its own message: an
+//     argument error (TCDE_ERR_ARGUMENT) in the vjp and the parameter gradients, TCDE_ERR_UNSUPPORTED elsewhere;
+//   * the dopri5 entry points demand at least one path, and the paired attempts a batch that is a multiple of 256;
+//   * the field falls back from the register-tiled stage of the fused solve to vector_field_kernel when that stage does
+//     not fit shared memory.
 #ifndef TCDE_DEFAULT_TC_MODE
 #define TCDE_DEFAULT_TC_MODE 1      // bit 0: 2xFP16 operand split (warpgroup wgmma) instead of 3xTF32 (warp-level mma.sync)
 #endif
-static int g_solve_variant = 0;     // 0 auto, 1 CUDA-core kernel, 2 / 3 tensor cores 3xTF32, 4 tensor cores 2xFP16
-int current_solve_variant() { return g_solve_variant; }
+
+int linear_route(LinearAsk ask, int64_t hidden, int64_t channels, int dtype, bool aligned, const char* what,
+                 LinearRoute* r) {
+    const int variant = current_solve_variant();
+    const bool tc_shape = hidden == 32 && channels == 8;
+    *r = LinearRoute{false, 1};
+    switch (ask) {
+    case kLinSolve:
+    case kLinStages:
+        if (dtype == TCDE_F32) {
+            r->tc = variant == kVariantTf32 || variant == kVariantFp16 || (variant == kVariantAuto && tc_shape && aligned);
+            r->split = variant == kVariantTf32 ? 0 : variant == kVariantFp16 ? 1 : TCDE_DEFAULT_TC_MODE;
+            if (r->tc) return TCDE_OK;
+            TCDE_CHECK_SUPPORTED(ask != kLinStages, "the stage dump is written by the tensor-core solve only "
+                                 "(fp32, hidden=32, channels=8, 16-byte aligned buffers)");
+        }
+        TCDE_CHECK_SUPPORTED(ask != kLinStages, "the stage dump is written by the fp32 tensor-core solve only");
+        TCDE_CHECK_SUPPORTED(hidden <= 256, "%shidden=%d > 256 is not supported by the CUDA-core kernel", what,
+                             (int)hidden);
+        return TCDE_OK;
+    case kLinField:
+        TCDE_CHECK_SUPPORTED(hidden <= 256, "%shidden=%d > 256", what, (int)hidden);
+        return TCDE_OK;
+    case kLinScratch:
+        TCDE_CHECK_SUPPORTED(tc_shape, "%shidden=%lld channels=%lld are not served", what, (long long)hidden,
+                             (long long)channels);
+        return TCDE_OK;
+    case kLinDopri5:
+        TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && tc_shape, "%sbuilt for float32, hidden=32, channels=8", what);
+        r->tc = true;
+        return TCDE_OK;
+    default:
+        TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && tc_shape, "%sbuilt for fp32, hidden=32, channels=8 (got dtype=%d, "
+                             "hidden=%lld, channels=%lld)", what, dtype, (long long)hidden, (long long)channels);
+        r->tc = ask == kLinBackward || (ask == kLinParamGrads && variant != kVariantSimt);
+        r->split = ask == kLinParamGrads && variant == kVariantTf32 ? 0 : 1;
+        return TCDE_OK;
+    }
+}
 
 }  // namespace tcde
 
 using namespace tcde;
-
-extern "C" int tcde_set_solve_variant(int variant) {
-    TCDE_CHECK_ARG(variant >= 0 && (variant & 15) <= 6,
-                   "variant=%d (0 auto, 1 CUDA-core kernel, 3 / 4 tensor-core kernel with the 3xTF32 / 2xFP16 operand split; "
-                   "2, 6 / 5 are aliases of 3 / 4)", variant);
-    g_solve_variant = variant & 15;      // bits above 15 (profiling switches of earlier kernels) are accepted and ignored
-    return TCDE_OK;
-}
 
 extern "C" int tcde_vector_field_linear(const void* control, int control_kind, int64_t n_rows, const void* weight,
                                         const void* bias, const void* z, void* out, int64_t n_paths, int64_t channels,
@@ -580,16 +626,44 @@ extern "C" int tcde_vector_field_linear(const void* control, int control_kind, i
     TCDE_CHECK_ARG(control && weight && bias && z && out, "null data pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && n_rows >= 1, "bad sizes");
     TCDE_CHECK_ARG(index >= 0 && index < n_rows, "index=%d outside [0, %lld)", index, (long long)n_rows);
-    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
+    TCDE_TRY(check_dtype(dtype));
+    TCDE_TRY(check_control_kind(control_kind));
     if (n_paths == 0) return TCDE_OK;
+    LinearRoute r;
+    TCDE_TRY(linear_route(kLinField, hidden, channels, dtype, true, "vector field: ", &r));
+    return by_dtype(dtype, [&](auto t) {
+        return launch_field<decltype(t)>(control, control_kind, n_rows, weight, bias, z, out, n_paths, (int)channels,
+                                         (int)hidden, index, frac, static_cast<cudaStream_t>(stream));
+    });
+}
+
+// The fixed-step solve, its stage dump and the reversible Heun forward, on the kernel linear_route answers.  dump: the
+// stage dump, or the reversible Heun checkpoints of every ckpt_stride-th step; out_mode is null for reversible Heun.
+static int solve_linear(LinearAsk ask, bool aligned, const void* control, int control_kind, int64_t n_rows,
+                        const void* weight, const void* bias, const void* z0, void* out, int64_t n_paths,
+                        int64_t channels, int64_t hidden, int method, int64_t n_steps, const void* step_dt,
+                        const int32_t* stage_index, const void* stage_frac, int64_t n_out, const int32_t* out_step,
+                        const int32_t* out_mode, const void* out_slope, double sign, int dtype, void* dump,
+                        int64_t ckpt_stride, void* stream) {
+    LinearRoute r;
+    TCDE_TRY(linear_route(ask, hidden, channels, dtype, aligned, "fused solve: ", &r));
+    const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (dtype == TCDE_F32)
-        return launch_field<float>(control, control_kind, n_rows, weight, bias, z, out, n_paths, (int)channels,
-                                   (int)hidden, index, frac, s);
-    return launch_field<double>(control, control_kind, n_rows, weight, bias, z, out, n_paths, (int)channels,
-                                (int)hidden, index, frac, s);
+    if (r.tc) {
+        const UmmaArgs u{(const float*)control, (const float*)weight, (const float*)bias, (const float*)z0, (float*)out,
+                         (const float*)step_dt, stage_index, (const float*)stage_frac, out_step, out_mode,
+                         (const float*)out_slope, n_paths, n_rows, control_kind, method, n_stages, (int)n_steps,
+                         (int)n_out, (float)sign, (float*)dump, (int)ckpt_stride};
+        return solve_tc_f32(u, (int)hidden, (int)channels, r.split, s);
+    }
+    return by_dtype(dtype, [&](auto t) {
+        using T = decltype(t);
+        const SolveArgs<T> a{(const T*)control, (const T*)weight, (const T*)bias, (const T*)z0, (T*)out,
+                             (const T*)step_dt, stage_index, (const T*)stage_frac, out_step, out_mode,
+                             (const T*)out_slope, n_paths, n_rows, (int)channels, 0, (int)hidden, control_kind, method,
+                             n_stages, (int)n_steps, (int)n_out, 0, 0, (T)sign, 0, 0, T(0), (int)ckpt_stride, (T*)dump};
+        return launch_solve<T>(a, s);
+    });
 }
 
 static int solve_fixed_linear(const void* control, int control_kind, int64_t n_rows, const void* weight,
@@ -602,45 +676,15 @@ static int solve_fixed_linear(const void* control, int control_kind, int64_t n_r
     TCDE_CHECK_ARG(step_dt && stage_index && stage_frac && out_step && out_mode && out_slope, "null schedule pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && n_rows >= 1, "bad sizes");
     TCDE_CHECK_ARG(n_steps >= 1 && n_out >= 1, "n_steps=%lld n_out=%lld", (long long)n_steps, (long long)n_out);
-    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
+    TCDE_TRY(check_dtype(dtype));
+    TCDE_TRY(check_control_kind(control_kind));
+    TCDE_TRY(check_method(method));
     TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
     if (n_paths == 0) return TCDE_OK;
-    const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (dtype == TCDE_F32) {
-        // auto: the tensor-core kernel wherever it is built for the shape (parity-tested against the
-        // CUDA-core kernel and the fp64 oracle), the CUDA-core kernel for every other shape
-        const bool tc_ok = solve_tc_supported((int)hidden, (int)channels) &&
-                           ((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z0) |
-                             reinterpret_cast<uintptr_t>(out)) & 15) == 0;
-        const bool want_tc = (g_solve_variant >= 2) || (g_solve_variant == 0 && tc_ok);
-        if (want_tc) {
-            UmmaArgs u{(const float*)control, (const float*)weight, (const float*)bias, (const float*)z0, (float*)out,
-                       (const float*)step_dt, stage_index, (const float*)stage_frac, out_step, out_mode,
-                       (const float*)out_slope, n_paths, n_rows, control_kind, method, n_stages, (int)n_steps,
-                       (int)n_out, (float)sign, (float*)stage_dump};
-            // 2 / 3 / 6 = 3xTF32 split, 4 / 5 = 2xFP16 split (2, 5, 6: aliases from the development history)
-            const int mode = (g_solve_variant == 2 || g_solve_variant == 3 || g_solve_variant == 6) ? 0
-                             : (g_solve_variant == 4 || g_solve_variant == 5) ? 1 : TCDE_DEFAULT_TC_MODE;
-            return solve_tc_f32(u, (int)hidden, (int)channels, mode, s);
-        }
-        TCDE_CHECK_SUPPORTED(stage_dump == nullptr, "the stage dump is written by the tensor-core solve only "
-                             "(fp32, hidden=32, channels=8, 16-byte aligned buffers)");
-        SolveArgs<float> a{(const float*)control, (const float*)weight, (const float*)bias, (const float*)z0,
-                           (float*)out, (const float*)step_dt, stage_index, (const float*)stage_frac, out_step,
-                           out_mode, (const float*)out_slope, n_paths, n_rows, (int)channels, 0, (int)hidden,
-                           control_kind, method, n_stages, (int)n_steps, (int)n_out, 0, 0, (float)sign, 0, 0, 0.f};
-        return solve_simt_f32(a, s);
-    }
-    TCDE_CHECK_SUPPORTED(stage_dump == nullptr, "the stage dump is written by the fp32 tensor-core solve only");
-    SolveArgs<double> a{(const double*)control, (const double*)weight, (const double*)bias, (const double*)z0,
-                        (double*)out, (const double*)step_dt, stage_index, (const double*)stage_frac, out_step,
-                        out_mode, (const double*)out_slope, n_paths, n_rows, (int)channels, 0, (int)hidden,
-                        control_kind, method, n_stages, (int)n_steps, (int)n_out, 0, 0, (double)sign, 0, 0, 0.0};
-    return solve_simt_f64(a, s);
+    // the alignment that automatic selection asks of the tensor-core solve leaves the dump to the kernel's own check
+    return solve_linear(stage_dump ? kLinStages : kLinSolve, aligned16(control, z0, out), control, control_kind, n_rows,
+                        weight, bias, z0, out, n_paths, channels, hidden, method, n_steps, step_dt, stage_index,
+                        stage_frac, n_out, out_step, out_mode, out_slope, sign, dtype, stage_dump, 0, stream);
 }
 
 extern "C" int tcde_cdeint_fixed_linear(const void* control, int control_kind, int64_t n_rows, const void* weight,
@@ -667,39 +711,14 @@ extern "C" int tcde_cdeint_reversible_heun_linear(const void* control, int contr
     TCDE_CHECK_ARG(n_steps >= 1 && n_out >= 1, "n_steps=%lld n_out=%lld", (long long)n_steps, (long long)n_out);
     TCDE_CHECK_ARG(checkpoint_stride >= 1 && checkpoint_stride < (1ll << 30), "checkpoint_stride=%lld",
                    (long long)checkpoint_stride);
-    TCDE_CHECK_ARG(dtype == TCDE_F32 || dtype == TCDE_F64, "dtype=%d", dtype);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
+    TCDE_TRY(check_dtype(dtype));
+    TCDE_TRY(check_control_kind(control_kind));
     TCDE_CHECK_SUPPORTED(n_steps + 1 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
     if (n_paths == 0) return TCDE_OK;
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    if (dtype == TCDE_F32) {
-        // the tensor-core kernel wherever the fixed-step solve uses it (same variant switch), the CUDA-core kernel otherwise
-        const bool tc_ok = solve_tc_supported((int)hidden, (int)channels) &&
-                           ((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(z0) |
-                             reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(checkpoints)) & 15) == 0;
-        if ((g_solve_variant >= 2) || (g_solve_variant == 0 && tc_ok)) {
-            UmmaArgs u{(const float*)control, (const float*)weight, (const float*)bias, (const float*)z0, (float*)out,
-                       (const float*)step_dt, stage_index, (const float*)stage_frac, out_step, nullptr,
-                       (const float*)out_weights, n_paths, n_rows, control_kind, TCDE_REVERSIBLE_HEUN, 1, (int)n_steps,
-                       (int)n_out, 1.f, (float*)checkpoints, (int)checkpoint_stride};
-            const int mode = (g_solve_variant == 2 || g_solve_variant == 3 || g_solve_variant == 6) ? 0
-                             : (g_solve_variant == 4 || g_solve_variant == 5) ? 1 : TCDE_DEFAULT_TC_MODE;
-            return solve_tc_f32(u, (int)hidden, (int)channels, mode, s);
-        }
-        SolveArgs<float> a{(const float*)control, (const float*)weight, (const float*)bias, (const float*)z0,
-                           (float*)out, (const float*)step_dt, stage_index, (const float*)stage_frac, out_step,
-                           nullptr, (const float*)out_weights, n_paths, n_rows, (int)channels, 0, (int)hidden,
-                           control_kind, TCDE_REVERSIBLE_HEUN, 1, (int)n_steps, (int)n_out, 0, 0, 1.f, 0, 0, 0.f,
-                           (int)checkpoint_stride, (float*)checkpoints};
-        return solve_simt_f32(a, s);
-    }
-    SolveArgs<double> a{(const double*)control, (const double*)weight, (const double*)bias, (const double*)z0,
-                        (double*)out, (const double*)step_dt, stage_index, (const double*)stage_frac, out_step,
-                        nullptr, (const double*)out_weights, n_paths, n_rows, (int)channels, 0, (int)hidden,
-                        control_kind, TCDE_REVERSIBLE_HEUN, 1, (int)n_steps, (int)n_out, 0, 0, 1.0, 0, 0, 0.0,
-                        (int)checkpoint_stride, (double*)checkpoints};
-    return solve_simt_f64(a, s);
+    return solve_linear(kLinSolve, aligned16(control, z0, out, checkpoints), control, control_kind, n_rows, weight, bias,
+                        z0, out, n_paths, channels, hidden, TCDE_REVERSIBLE_HEUN, n_steps, step_dt, stage_index,
+                        stage_frac, n_out, out_step, nullptr, out_weights, 1.0, dtype, checkpoints, checkpoint_stride,
+                        stream);
 }
 
 extern "C" int tcde_cdeint_fixed_linear_stages(const void* control, int control_kind, int64_t n_rows, const void* weight,

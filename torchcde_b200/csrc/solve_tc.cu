@@ -672,37 +672,25 @@ __global__ void __launch_bounds__(wg::kThreads, 2) reversible_backward_kernel(co
 
 }  // namespace tc
 
-bool solve_tc_supported(int H, int C) { return H == tc::kHid && C == tc::kCh; }
-
-template <typename Kernel, typename Args>
-static int launch(Kernel kern, int64_t grid, int threads, int smem, const Args& a, cudaStream_t stream) {
-    TCDE_CHECK_SUPPORTED(grid < (1ll << 31), "too many paths");
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    kern<<<(unsigned)grid, threads, smem, stream>>>(a);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    return TCDE_OK;
-}
-
 int solve_tc_f32(const UmmaArgs& a, int H, int C, int mode, cudaStream_t stream) {
-    TCDE_CHECK_SUPPORTED(solve_tc_supported(H, C), "tensor-core solve: built for hidden=32, channels=8 (got %d, %d)", H, C);
-    TCDE_CHECK_SUPPORTED((reinterpret_cast<uintptr_t>(a.control) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.z0) & 15) == 0 &&
-                             (reinterpret_cast<uintptr_t>(a.out) & 15) == 0,
-                         "tensor-core solve: control, z0 and out must be 16-byte aligned");
-    TCDE_CHECK_SUPPORTED(a.stage_dump == nullptr || (reinterpret_cast<uintptr_t>(a.stage_dump) & 15) == 0,
-                         "tensor-core solve: the stage dump must be 16-byte aligned");
+    TCDE_CHECK_SUPPORTED(H == tc::kHid && C == tc::kCh, "tensor-core solve: built for hidden=32, channels=8 (got %d, %d)", H, C);
+    TCDE_CHECK_SUPPORTED(aligned16(a.control, a.z0, a.out), "tensor-core solve: control, z0 and out must be 16-byte aligned");
+    TCDE_CHECK_SUPPORTED(aligned16(a.stage_dump), "tensor-core solve: the stage dump must be 16-byte aligned");
     // mode: bit 0 = operand split (0 = 3xTF32, 1 = 2xFP16)
     const bool rev = (a.method == TCDE_REVERSIBLE_HEUN);
     if (mode & 1)
         return launch(rev ? (a.stage_dump ? tc::cdeint_wgmma_kernel<true, true> : tc::cdeint_wgmma_kernel<false, true>)
                           : (a.stage_dump ? tc::cdeint_wgmma_kernel<true, false> : tc::cdeint_wgmma_kernel<false, false>),
-                      (a.n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths, tc::wg::kThreads, tc::wg::kSmem, a, stream);
+                      (a.n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths, tc::wg::kThreads, tc::wg::kSmem, stream, a);
     return launch(rev ? (a.stage_dump ? tc::cdeint_tc_kernel<true, true> : tc::cdeint_tc_kernel<false, true>)
                       : (a.stage_dump ? tc::cdeint_tc_kernel<true, false> : tc::cdeint_tc_kernel<false, false>),
                   (a.n_paths + tc::kThreads - 1) / tc::kThreads, tc::kThreads,
-                  tc::Smem::total + 128, a, stream);               // slack for the 128-byte alignment of the tiles
+                  tc::Smem::total + 128, stream, a);               // slack for the 128-byte alignment of the tiles
 }
 
 }  // namespace tcde
+
+using namespace tcde;
 
 extern "C" int tcde_reversible_heun_linear_backward_segment(
     const void* control, int control_kind, int64_t n_rows, const void* weight, const void* bias, const void* weight_t,
@@ -710,29 +698,23 @@ extern "C" int tcde_reversible_heun_linear_backward_segment(
     const int32_t* out_step, const void* out_weights, const int32_t* inj_range, const void* step_dt,
     const int32_t* stage_index, const void* stage_frac, int64_t lo, int64_t hi, int64_t n_paths, int64_t channels,
     int64_t hidden, void* dump_z, void* dump_a, int dtype, void* stream) {
-    using namespace tcde;
     TCDE_CHECK_ARG(control && weight && bias && weight_t && zeros && ckpt_lo && ckpt_hi && carry && g && dump_z && dump_a,
                    "null data pointer");
     TCDE_CHECK_ARG(out_step && out_weights && inj_range && step_dt && stage_index && stage_frac, "null schedule pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_out >= 1 && lo >= 0 && hi > lo && hi < (1ll << 31), "bad sizes");
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && solve_tc_supported((int)hidden, (int)channels),
-                         "the reversible backward kernel is built for fp32, hidden=32, channels=8 (got dtype=%d, "
-                         "hidden=%lld, channels=%lld)", dtype, (long long)hidden, (long long)channels);
-    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(ckpt_lo) |
-                           reinterpret_cast<uintptr_t>(ckpt_hi) | reinterpret_cast<uintptr_t>(carry) |
-                           reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(dump_z) |
-                           reinterpret_cast<uintptr_t>(dump_a)) & 15) == 0,
+    TCDE_TRY(check_control_kind(control_kind));
+    LinearRoute r;
+    TCDE_TRY(linear_route(kLinBackward, hidden, channels, dtype, true, "the reversible backward kernel is ", &r));
+    TCDE_CHECK_SUPPORTED(aligned16(control, ckpt_lo, ckpt_hi, carry, g, dump_z, dump_a),
                          "reversible backward: buffers must be 16-byte aligned");
     if (n_paths == 0) return TCDE_OK;
-    tc::RevBwdArgs a{(const float*)control, (const float*)weight, (const float*)bias, (const float*)weight_t,
-                     (const float*)zeros, (const float*)ckpt_lo, (const float*)ckpt_hi, (float*)carry, (const float*)g,
-                     out_step, (const float*)out_weights, inj_range, (const float*)step_dt, stage_index,
-                     (const float*)stage_frac, (float*)dump_z, (float*)dump_a, n_paths, n_rows, control_kind, (int)n_out,
-                     (int)lo, (int)hi};
+    const tc::RevBwdArgs a{(const float*)control, (const float*)weight, (const float*)bias, (const float*)weight_t,
+                           (const float*)zeros, (const float*)ckpt_lo, (const float*)ckpt_hi, (float*)carry,
+                           (const float*)g, out_step, (const float*)out_weights, inj_range, (const float*)step_dt,
+                           stage_index, (const float*)stage_frac, (float*)dump_z, (float*)dump_a, n_paths, n_rows,
+                           control_kind, (int)n_out, (int)lo, (int)hi};
     return launch(tc::reversible_backward_kernel, (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths, tc::wg::kThreads,
-                  tc::kRevSmem, a, static_cast<cudaStream_t>(stream));
+                  tc::kRevSmem, static_cast<cudaStream_t>(stream), a);
 }
 
 extern "C" int tcde_cdeint_fixed_linear_backward(
@@ -740,28 +722,24 @@ extern "C" int tcde_cdeint_fixed_linear_backward(
     void* grad_z0, void* kappa_dump, int64_t n_paths, int64_t channels, int64_t hidden, int method, int64_t n_steps,
     const void* step_dt_rev, const int32_t* stage_index_rev, const void* stage_frac_rev, int64_t n_out,
     const int32_t* inj_range, const int32_t* inj_out, const void* inj_weight, double sign, int dtype, void* stream) {
-    using namespace tcde;
     TCDE_CHECK_ARG(control && weight_t && zeros && grad_out && grad_z0, "null data pointer");
     TCDE_CHECK_ARG(step_dt_rev && stage_index_rev && stage_frac_rev && inj_range && inj_out && inj_weight,
                    "null schedule pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_steps >= 1 && n_out >= 1, "bad sizes");
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    TCDE_CHECK_ARG(method == TCDE_EULER || method == TCDE_MIDPOINT || method == TCDE_RK4_38, "method=%d", method);
+    TCDE_TRY(check_control_kind(control_kind));
+    TCDE_TRY(check_method(method));
     TCDE_CHECK_SUPPORTED(n_steps * 4 < (1ll << 31) && n_out < (1ll << 31), "schedule too long");
-    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && solve_tc_supported((int)hidden, (int)channels),
-                         "the Runge-Kutta backward kernel is built for fp32, hidden=32, channels=8 (got dtype=%d, "
-                         "hidden=%lld, channels=%lld)", dtype, (long long)hidden, (long long)channels);
-    TCDE_CHECK_SUPPORTED(((reinterpret_cast<uintptr_t>(control) | reinterpret_cast<uintptr_t>(grad_out) |
-                           reinterpret_cast<uintptr_t>(grad_z0) | reinterpret_cast<uintptr_t>(kappa_dump)) & 15) == 0,
+    LinearRoute r;
+    TCDE_TRY(linear_route(kLinBackward, hidden, channels, dtype, true, "the Runge-Kutta backward kernel is ", &r));
+    TCDE_CHECK_SUPPORTED(aligned16(control, grad_out, grad_z0, kappa_dump),
                          "Runge-Kutta backward: control, grad_out, grad_z0 and the dump must be 16-byte aligned");
     if (n_paths == 0) return TCDE_OK;
     const int n_stages = (method == TCDE_RK4_38) ? 4 : (method == TCDE_MIDPOINT) ? 2 : 1;
-    UmmaArgs u{(const float*)control, (const float*)weight_t, (const float*)zeros, nullptr, (float*)grad_z0,
-               (const float*)step_dt_rev, stage_index_rev, (const float*)stage_frac_rev, nullptr, nullptr, nullptr,
-               n_paths, n_rows, control_kind, method, n_stages, (int)n_steps, (int)n_out, (float)sign,
-               (float*)kappa_dump, 0, (const float*)grad_out, inj_range, inj_out, (const float*)inj_weight};
+    const UmmaArgs u{(const float*)control, (const float*)weight_t, (const float*)zeros, nullptr, (float*)grad_z0,
+                     (const float*)step_dt_rev, stage_index_rev, (const float*)stage_frac_rev, nullptr, nullptr, nullptr,
+                     n_paths, n_rows, control_kind, method, n_stages, (int)n_steps, (int)n_out, (float)sign,
+                     (float*)kappa_dump, 0, (const float*)grad_out, inj_range, inj_out, (const float*)inj_weight};
     return launch(kappa_dump ? tc::cdeint_wgmma_kernel<true, false, true> : tc::cdeint_wgmma_kernel<false, false, true>,
-                  (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths, tc::wg::kThreads, tc::wg::kSmem, u,
-                  static_cast<cudaStream_t>(stream));
+                  (n_paths + tc::wg::kPaths - 1) / tc::wg::kPaths, tc::wg::kThreads, tc::wg::kSmem,
+                  static_cast<cudaStream_t>(stream), u);
 }

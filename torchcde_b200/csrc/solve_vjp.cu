@@ -312,19 +312,17 @@ param_grad_kernel(const float* __restrict__ control, int control_kind, int64_t n
 }
 
 static int param_grad_grid(int64_t n_paths, int64_t n_stage_total) {
-    const int64_t items = ((n_paths + TB - 1) / TB) * n_stage_total;
-    int64_t g = (int64_t)sm_count() * 3;
-    if (g > items) g = items;
-    if (g < 1) g = 1;
-    return (int)g;
+    return capped_grid(((n_paths + TB - 1) / TB) * n_stage_total, 3);
 }
 
-static int vjp_grid(int64_t n_paths) {
-    int64_t tiles = (n_paths + TB - 1) / TB;
-    int64_t g = (int64_t)sm_count() * 2;
-    if (g > tiles) g = tiles;
-    if (g < 1) g = 1;
-    return (int)g;
+static int vjp_grid(int64_t n_paths) { return capped_grid((n_paths + TB - 1) / TB, 2); }
+
+// grad_weight, grad_bias (either may be null) += scale * the sum of the grid's per-CTA partial sums in scratch
+static int reduce_param_grads(const void* scratch, int grid, double scale, void* grad_weight, void* grad_bias,
+                              cudaStream_t s) {
+    if (!(grad_weight || grad_bias)) return TCDE_OK;
+    return launch(field_vjp_reduce_kernel, (kParams + 31) / 32, 256, 0, s, (const float*)scratch, grid, (float)scale,
+                  (float*)grad_weight, (float*)grad_bias);
 }
 
 }  // namespace vjp
@@ -333,7 +331,10 @@ static int vjp_grid(int64_t n_paths) {
 using namespace tcde;
 
 extern "C" int64_t tcde_vector_field_linear_vjp_scratch_bytes(int64_t n_paths, int64_t channels, int64_t hidden) {
-    if (n_paths < 0 || channels != vjp::C || hidden != vjp::H) return -1;
+    LinearRoute r;
+    if (n_paths < 0 || linear_route(kLinScratch, hidden, channels, TCDE_F32, true,
+                                    "tcde_vector_field_linear_vjp_scratch_bytes: ", &r) != TCDE_OK)
+        return -1;
     return (int64_t)vjp::vjp_grid(n_paths) * vjp::kParams * (int64_t)sizeof(float);
 }
 
@@ -346,34 +347,27 @@ extern "C" int tcde_vector_field_linear_vjp(const void* control, int control_kin
     TCDE_CHECK_ARG(control && weight && bias && z && a && f_out && vjp_z_out && scratch, "null data pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && channels >= 1 && hidden >= 1 && n_rows >= 1, "bad sizes");
     TCDE_CHECK_ARG(index >= 0 && index < n_rows, "index=%d outside [0, %lld)", index, (long long)n_rows);
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && hidden == vjp::H && channels == vjp::C,
-                         "the fused adjoint stage is built for fp32, hidden=%d, channels=%d (got dtype=%d, hidden=%lld, "
-                         "channels=%lld)", vjp::H, vjp::C, dtype, (long long)hidden, (long long)channels);
-    TCDE_CHECK_ARG(((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(scratch)) & 15) == 0,
-                   "z, a and scratch must be 16-byte aligned");
+    TCDE_TRY(check_control_kind(control_kind));
+    LinearRoute r;
+    TCDE_TRY(linear_route(kLinVjp, hidden, channels, dtype, true, "the fused adjoint stage is ", &r));
+    TCDE_CHECK_ARG(aligned16(z, a, scratch), "z, a and scratch must be 16-byte aligned");
     if (n_paths == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     const int grid = vjp::vjp_grid(n_paths);
-    const size_t smem = (size_t)vjp::kSmemFloats * sizeof(float);
-    TCDE_CHECK_CUDA(cudaFuncSetAttribute(vjp::field_vjp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    vjp::field_vjp_kernel<<<grid, vjp::kThreads, smem, s>>>(
-        (const float*)control, control_kind, n_rows, (const float*)weight, (const float*)bias, (const float*)z,
-        (const float*)a, (float*)f_out, (float*)vjp_z_out, (float*)scratch, n_paths, (int)index, (float)frac,
-        (float)f_scale, (float)vjp_scale);
-    TCDE_CHECK_CUDA(cudaGetLastError());
-    if (grad_weight || grad_bias) {
-        vjp::field_vjp_reduce_kernel<<<(vjp::kParams + 31) / 32, 256, 0, s>>>((const float*)scratch, grid, (float)grad_scale,
-                                                                                (float*)grad_weight, (float*)grad_bias);
-        TCDE_CHECK_CUDA(cudaGetLastError());
-    }
-    return TCDE_OK;
+    TCDE_TRY(launch(vjp::field_vjp_kernel, grid, vjp::kThreads, (size_t)vjp::kSmemFloats * sizeof(float), s,
+                    (const float*)control, control_kind, n_rows, (const float*)weight, (const float*)bias,
+                    (const float*)z, (const float*)a, (float*)f_out, (float*)vjp_z_out, (float*)scratch, n_paths,
+                    (int)index, (float)frac, (float)f_scale, (float)vjp_scale));
+    return vjp::reduce_param_grads(scratch, grid, grad_scale, grad_weight, grad_bias, s);
 }
 
 extern "C" int64_t tcde_linear_field_param_grads_scratch_bytes(int64_t n_paths, int64_t n_stages_total, int64_t channels,
                                                               int64_t hidden) {
-    if (n_paths < 0 || n_stages_total < 1 || channels != vjp::C || hidden != vjp::H) return -1;
+    LinearRoute r;
+    if (n_paths < 0 || n_stages_total < 1 ||
+        linear_route(kLinScratch, hidden, channels, TCDE_F32, true, "tcde_linear_field_param_grads_scratch_bytes: ",
+                     &r) != TCDE_OK)
+        return -1;
     const int64_t g1 = vjp::param_grad_grid(n_paths, n_stages_total), g2 = param_grad_mma_grid(n_paths, n_stages_total);
     return (g1 > g2 ? g1 : g2) * vjp::kParams * (int64_t)sizeof(float);
 }
@@ -386,39 +380,21 @@ extern "C" int tcde_linear_field_param_grads(const void* control, int control_ki
     TCDE_CHECK_ARG(control && z_stages && a_stages && stage_index && stage_frac && stage_weight && scratch,
                    "null data pointer");
     TCDE_CHECK_ARG(n_paths >= 0 && n_rows >= 1 && n_stages_total >= 1 && n_stages_total < (1ll << 31), "bad sizes");
-    TCDE_CHECK_ARG(control_kind == TCDE_CONTROL_CUBIC || control_kind == TCDE_CONTROL_LINEAR, "control_kind=%d",
-                   control_kind);
-    TCDE_CHECK_SUPPORTED(dtype == TCDE_F32 && hidden == vjp::H && channels == vjp::C,
-                         "built for fp32, hidden=%d, channels=%d (got dtype=%d, hidden=%lld, channels=%lld)", vjp::H,
-                         vjp::C, dtype, (long long)hidden, (long long)channels);
-    TCDE_CHECK_ARG(((reinterpret_cast<uintptr_t>(z_stages) | reinterpret_cast<uintptr_t>(a_stages) |
-                     reinterpret_cast<uintptr_t>(scratch)) & 15) == 0, "stage buffers and scratch must be 16-byte aligned");
+    TCDE_TRY(check_control_kind(control_kind));
+    LinearRoute r;
+    TCDE_TRY(linear_route(kLinParamGrads, hidden, channels, dtype, true, "", &r));
+    TCDE_CHECK_ARG(aligned16(z_stages, a_stages, scratch), "stage buffers and scratch must be 16-byte aligned");
     if (n_paths == 0) return TCDE_OK;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    int grid;
-    const int variant = current_solve_variant();
-    if (variant != 1) {
-        // tensor cores: 2xBF16 split by default (and for 4 / 5), 3xTF32 for the variants that select it for the solve
-        const int mode = (variant == 2 || variant == 3 || variant == 6) ? 0 : 1;
-        grid = param_grad_mma_grid(n_paths, n_stages_total);
-        const int rc = param_grad_mma_f32((const float*)control, control_kind, n_rows, (const float*)z_stages,
-                                          (const float*)a_stages, stage_index, (const float*)stage_frac,
-                                          (const float*)stage_weight, (int)n_stages_total, (float*)scratch, n_paths, mode,
-                                          grid, s);
-        if (rc != TCDE_OK) return rc;
-    } else {
-        grid = vjp::param_grad_grid(n_paths, n_stages_total);
-        vjp::param_grad_kernel<<<grid, vjp::kThreads, 0, s>>>((const float*)control, control_kind, n_rows,
-                                                             (const float*)z_stages, (const float*)a_stages,
-                                                             stage_index, (const float*)stage_frac,
-                                                             (const float*)stage_weight, (int)n_stages_total,
-                                                             (float*)scratch, n_paths);
-        TCDE_CHECK_CUDA(cudaGetLastError());
-    }
-    if (grad_weight || grad_bias) {
-        vjp::field_vjp_reduce_kernel<<<(vjp::kParams + 31) / 32, 256, 0, s>>>((const float*)scratch, grid, (float)scale,
-                                                                              (float*)grad_weight, (float*)grad_bias);
-        TCDE_CHECK_CUDA(cudaGetLastError());
-    }
-    return TCDE_OK;
+    const int grid = r.tc ? param_grad_mma_grid(n_paths, n_stages_total) : vjp::param_grad_grid(n_paths, n_stages_total);
+    if (r.tc)
+        TCDE_TRY(param_grad_mma_f32((const float*)control, control_kind, n_rows, (const float*)z_stages,
+                                    (const float*)a_stages, stage_index, (const float*)stage_frac,
+                                    (const float*)stage_weight, (int)n_stages_total, (float*)scratch, n_paths, r.split,
+                                    grid, s));
+    else
+        TCDE_TRY(launch(vjp::param_grad_kernel, grid, vjp::kThreads, 0, s, (const float*)control, control_kind, n_rows,
+                        (const float*)z_stages, (const float*)a_stages, stage_index, (const float*)stage_frac,
+                        (const float*)stage_weight, (int)n_stages_total, (float*)scratch, n_paths));
+    return vjp::reduce_param_grads(scratch, grid, scale, grad_weight, grad_bias, s);
 }
