@@ -148,6 +148,22 @@ def test_torch_operator_backward_matches_autograd(dtype, bar, field):
         assert (a - b).abs().max() <= bar * b.abs().max().clamp(min=1e-30)
 
 
+@pytest.mark.parametrize("culprit", ["func", "func.prod", "X.derivative"])
+def test_a_non_tensor_answer_raises_the_reference_value_error(culprit):
+    """The reference's compatibility check: a ``func``, ``func.prod`` or ``X.derivative`` that answers with something
+    other than a tensor is a ValueError, before any solve."""
+    coeffs, z0, _func = _problem(4, 6, channels=4, hidden=16)
+    X = cde.CubicSpline(coeffs)
+    func = lambda t, z: [z]                                                         # noqa: E731
+    if culprit == "func.prod":
+        func = type("Prod", (), {"prod": staticmethod(lambda t, z, dx: [z])})()
+    elif culprit == "X.derivative":
+        X = type("Control", (), {"derivative": staticmethod(lambda t: [t])})()
+    with pytest.raises(ValueError, match="z0 is a tensor and so {} must return a tensor as well".format(culprit)):
+        cde.cdeint(X, func, z0, torch.tensor([0.0, 5.0], device=DEV), backend="torchsde", method="reversible_heun",
+                   dt=0.5)
+
+
 def _backward_peak(coeffs, z0, func, dt):
     X = cde.CubicSpline(coeffs)
     ts = torch.tensor([0.0, 255.0], device=DEV)

@@ -425,30 +425,47 @@ def dopri5_backward_tables(steps, times, dtype=torch.float32, ends=None):
 
 
 # ------------------------------------------------------------------------- fixed grids (generic)
+def _fixed_grid(times, step_size):
+    """The float grid of a fixed-step solve over ``times``: the times themselves without a step size, else
+    ``times[0] + i * step_size`` up to the end time, which replaces the last point."""
+    if step_size is None:
+        return list(times)
+    t0, t_end = times[0], times[-1]
+    n = int(math.ceil((t_end - t0) / step_size + 1))
+    grid = [t0 + i * step_size for i in range(n)]
+    grid[-1] = t_end
+    return grid
+
+
+def _stage_times(a, b, method):
+    """The times at which ``method`` evaluates the field in the step from ``a`` to ``b``."""
+    dt = b - a
+    if method == "rk4":
+        return a, a + dt / 3, a + dt * 2 / 3, b
+    if method == "midpoint":
+        return a, a + dt / 2
+    return (a,)
+
+
 def odeint_fixed(field, y0, times, method, step_size):
     """Fixed-grid euler / midpoint / rk4 (3/8 rule) on float times -- used by the adjoint pass."""
-    t0, t_end = times[0], times[-1]
-    if step_size is None:
-        grid = list(times)
-    else:
-        n = int(math.ceil((t_end - t0) / step_size + 1))
-        grid = [t0 + i * step_size for i in range(n)]
-        grid[-1] = t_end
+    grid = _fixed_grid(times, step_size)
     out = [y0]
     y = y0
     j = 1
     for a, b in zip(grid[:-1], grid[1:]):
         dt = b - a
+        ts = _stage_times(a, b, method)
         if method == "rk4":
-            k1 = field(a, y)
-            k2 = field(a + dt / 3, y + dt * k1 / 3)
-            k3 = field(a + dt * 2 / 3, y + dt * (k2 - k1 / 3))
-            k4 = field(b, y + dt * (k1 - k2 + k3))
+            k1 = field(ts[0], y)
+            k2 = field(ts[1], y + dt * k1 / 3)
+            k3 = field(ts[2], y + dt * (k2 - k1 / 3))
+            k4 = field(ts[3], y + dt * (k1 - k2 + k3))
             y1 = y + (k1 + 3 * (k2 + k3) + k4) * (dt * 0.125)
         elif method == "midpoint":
-            y1 = y + dt * field(a + dt / 2, y + field(a, y) * (dt / 2))
+            y1 = y + dt * field(ts[1], y + field(ts[0], y) * (dt / 2))
         else:
-            y1 = y + dt * field(a, y)
+            y1 = y + dt * field(ts[0], y)
         while j < len(times) and b >= times[j]:
             if times[j] == b:
                 out.append(y1)
@@ -633,22 +650,8 @@ def _fused_fixed_backward(stage, times, ys, grad_ys, method, step_size):
         if a_lo is not None:
             a_y = a_lo + grad_ys[i - 1]
             continue
-        s0, s_end = -times[i], -times[i - 1]
-        if step_size is None:
-            grid = [s0, s_end]
-        else:
-            n = int(math.ceil((s_end - s0) / step_size + 1))
-            grid = [s0 + j * step_size for j in range(n)]
-            grid[-1] = s_end
-        stage_times = []
-        for lo, hi in zip(grid[:-1], grid[1:]):
-            ds = hi - lo
-            if method == "rk4":
-                stage_times += [lo, lo + ds / 3, lo + ds * 2 / 3, hi]
-            elif method == "midpoint":
-                stage_times += [lo, lo + ds / 2]
-            else:
-                stage_times += [lo]
+        grid = _fixed_grid([-times[i], -times[i - 1]], step_size)
+        stage_times = [s for lo, hi in zip(grid[:-1], grid[1:]) for s in _stage_times(lo, hi, method)]
         index, frac = stage.locate_many([-s for s in stage_times])
         U[0].copy_(ys[i])
         U[1].copy_(a_y)

@@ -41,10 +41,10 @@ import torch
 
 from . import _lib
 from .controls import _control_signature, _schedule_knots
-from .linear_field import LinearFieldKernels, linear_field_of
+from .linear_field import LinearFieldKernels
 from .mlp_field import MlpFieldKernels, mlp_field_of
 from .schedule import build_sde_schedule, locate
-from .solver import _derivative_at, _shape_error_forward, _shape_error_prod
+from .solver import _adjoint_params, _derivative_at, _linear_field_or_check
 
 # the forward keeps (y, z, f) of every CHECKPOINT_STRIDE-th step; the backward restarts every segment from them
 CHECKPOINT_STRIDE = 16
@@ -333,22 +333,9 @@ def cdeint_reversible(X, func, z0, t, adjoint, kwargs):
     sig = _control_signature(X)
     is_prod = hasattr(func, "prod")
     times = [float(v) for v in t.detach().cpu().tolist()]
-    field_params = None
-    if sig is not None and not is_prod:
-        field_params = linear_field_of(func, z0, sig[2], times)
-    if field_params is not None:
-        _shape_error_forward(sig[1] + (sig[2],), tuple(z0.shape[:-1]) + (z0.size(-1), sig[2]), z0)
-    else:
-        dx = X.derivative(t[0].detach())
-        if is_prod:
-            _shape_error_prod(tuple(dx.shape), tuple(func.prod(t[0], z0, dx).shape), z0)
-        else:
-            _shape_error_forward(tuple(dx.shape), tuple(func(t[0], z0).shape), z0)
-
-    if "adjoint_params" in kwargs:
-        params = tuple(kwargs["adjoint_params"])
-    else:
-        params = tuple(func.parameters()) if isinstance(func, torch.nn.Module) else ()
+    field_params = _linear_field_or_check(X, func, z0, t, times, sig, is_prod)
+    params = _adjoint_params(func, kwargs)
+    # unlike cdeint's census: ``t`` takes no gradient here, and ``X.buffers()`` is read whatever the control's type
     differentiable = (z0,) + tuple(X.buffers()) + (tuple(func.parameters()) if isinstance(func, torch.nn.Module)
                                                     else ()) + params
     wants_grad = torch.is_grad_enabled() and any(isinstance(x, torch.Tensor) and x.requires_grad for x in differentiable)

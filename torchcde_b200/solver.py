@@ -14,7 +14,7 @@ import warnings
 import torch
 
 from . import _lib, adaptive
-from .controls import CubicSpline, _control_signature, _schedule_knots
+from .controls import CubicSpline, _control_signature, _eval_kernel, _schedule_knots
 from .linear_field import (LinearFieldKernels, LinearVectorField, _reverse, dopri5_backprop, fixed_backprop,  # noqa: F401
                            linear_field_of)
 from .mlp_field import MlpFieldKernels, dopri5_mlp_backprop, mlp_backprop, mlp_field_of
@@ -160,96 +160,61 @@ def _generic_solve(X, func, z0, t, method, step_size, is_prod, known_control):
 
 
 # ------------------------------------------------- generic func, no autograd: kernels + optional CUDA graph
+def _stage_loop(sched, y0, fields_of_step):
+    """The fixed-step time loop of ``sched`` from ``y0`` when nothing needs a gradient: ``fields_of_step(i)`` evaluates
+    dX/dt once for step i and returns ``field(s, z)``, the vector field at stage s of that step.  Every Runge-Kutta
+    combination and output interpolation is ONE launch of ``tcde_linear_combination``.  Returns the list of outputs."""
+    combine = adaptive._combine
+    outs = [None] * sched.n_out
+    j = 0
+    while j < sched.n_out and int(sched.out_step[j]) < 0:
+        outs[j] = y0
+        j += 1
+    y = y0
+    for i in range(sched.n_steps):
+        field = fields_of_step(i)
+        dt = float(sched.step_dt[i])
+        if sched.method == "rk4":
+            k1 = field(0, y)
+            k2 = field(1, combine(y, [k1], (1 / 3,), dt))
+            k3 = field(2, combine(y, [k1, k2], (-1 / 3, 1.0), dt))
+            k4 = field(3, combine(y, [k1, k2, k3], (1.0, -1.0, 1.0), dt))
+            y1 = combine(y, [k1, k2, k3, k4], (0.125, 0.375, 0.375, 0.125), dt)
+        elif sched.method == "midpoint":
+            k1 = field(0, y)
+            y1 = combine(y, [field(1, combine(y, [k1], (0.5,), dt))], (1.0,), dt)
+        else:
+            y1 = combine(y, [field(0, y)], (1.0,), dt)
+        while j < sched.n_out and int(sched.out_step[j]) == i:
+            mode = int(sched.out_mode[j])
+            outs[j] = y if mode == 0 else y1 if mode == 1 else combine(y, [y1, y], (1.0, -1.0), float(sched.out_slope[j]))
+            j += 1
+        y = y1
+    return outs
+
+
 _graphs = {}
 
 
-def _generic_solve_kernels(X, func, z0, t, method, step_size, is_prod, use_graph=False):
-    """The fixed-step stage loop for an arbitrary ``func`` when nothing needs a gradient: the control's derivative of
-    the four stages of a step is ONE launch of ``tcde_spline_eval`` (the reference: ~10 small kernels and 4 host syncs
-    per stage, interpolation_cubic.py:315-336), every Runge-Kutta combination is ONE launch of
-    ``tcde_linear_combination``; only ``func`` itself and the ``f @ dX`` contraction stay torch operators (they are the
-    user's code).  With ``use_graph`` the whole time loop is captured into a CUDA graph once per (func, X, shapes,
-    schedule) and replayed -- for small states the loop is launch-bound (12 launches per stage), which is what a graph
-    removes.  The graph reads ``func``'s parameters and X's coefficients from their own storage, so in-place updates of
-    either (``optimizer.step()``) are seen by a replay.  The cache key is everything a replay cannot see change: the
-    ``func`` and ``X`` objects, the state's shape, dtype and device, the method, step and output times, the ``training``
-    flag of every submodule of ``func`` (a branch on ``self.training`` is baked into the capture), and the storage address
-    of every parameter and buffer of ``func`` and of every buffer of ``X`` (``p.data = ...``, ``module.double().float()``
-    or ``load_state_dict(..., assign=True)`` give a parameter new storage, which the captured kernels would not read).
-    The cache entry keeps those tensors alive, so no address in a key can be reused while its graph is cached."""
-    kind, _, channels, n_rows = _control_signature(X)
-    dtype, device = z0.dtype, z0.device
-    sched = build_schedule(t, _schedule_knots(X), n_rows, method, step_size, dtype)
-    n_stages = sched.n_stages
-    control = (X._rows() if kind == _lib.CONTROL_CUBIC else X._coeffs).detach()
-    knots = X._t.detach().to(device=device, dtype=control.dtype).contiguous()
-    index_dev = sched.stage_index.to(device)
-    frac_dev = sched.stage_frac.to(device=device, dtype=control.dtype)
-    times_dev = sched.stage_times.to(device)
-    sign = sched.sign
-    from .controls import _eval_kernel
-    from .adaptive import _combine
-
-    def run(y0):
-        outs = [None] * sched.n_out
-        j = 0
-        while j < sched.n_out and int(sched.out_step[j]) < 0:
-            outs[j] = y0
-            j += 1
-        y = y0
-        for i in range(sched.n_steps):
-            # dX/dt of this step's stages: (..., n_stages, C) in one launch
-            dxs = _eval_kernel(control, knots, control.size(-2), channels, index_dev[i], frac_dev[i], kind, True)
-
-            def field(s, z):
-                ts = times_dev[i, s]
-                dx = dxs[..., s, :]
-                if is_prod:
-                    out = func.prod(ts, z, dx)
-                    out = out if sign > 0 else -1.0 * out
-                    return out if out.is_contiguous() else out.contiguous()
-                # solver.py:129-135: f(t, z) @ dX/dt as one streaming launch (the sign of a reversed solve folded in)
-                f = func(ts, z)
-                if (f.shape != z.shape + (channels,) or f.dtype != dtype or dxs.dtype != dtype or not f.is_cuda
-                        or dxs.shape[:-2] != z.shape[:-1]):
-                    out = (f @ dx.unsqueeze(-1)).squeeze(-1)          # an unusual func output: let torch broadcast / promote
-                    out = out if sign > 0 else -1.0 * out
-                    return out if out.is_contiguous() else out.contiguous()
-                f = f if f.is_contiguous() else f.contiguous()
-                out = torch.empty_like(z)
-                _lib.call("tcde_field_contract", _lib.ptr(f), _lib.ptr(dx), _lib.ptr(out), z.numel() // z.size(-1), z.size(-1),
-                          channels, n_stages * channels, float(sign),
-                          _lib.dtype_code(dtype), _lib.stream_of(z))
-                return out
-
-            dt = float(sched.step_dt[i])
-            if method == "rk4":
-                k1 = field(0, y)
-                k2 = field(1, _combine(y, [k1], (1 / 3,), dt))
-                k3 = field(2, _combine(y, [k1, k2], (-1 / 3, 1.0), dt))
-                k4 = field(3, _combine(y, [k1, k2, k3], (1.0, -1.0, 1.0), dt))
-                y1 = _combine(y, [k1, k2, k3, k4], (0.125, 0.375, 0.375, 0.125), dt)
-            elif method == "midpoint":
-                k1 = field(0, y)
-                y1 = _combine(y, [field(1, _combine(y, [k1], (0.5,), dt))], (1.0,), dt)
-            else:
-                y1 = _combine(y, [field(0, y)], (1.0,), dt)
-            while j < sched.n_out and int(sched.out_step[j]) == i:
-                mode = int(sched.out_mode[j])
-                outs[j] = y if mode == 0 else y1 if mode == 1 else _combine(y, [y1, y], (1.0, -1.0), float(sched.out_slope[j]))
-                j += 1
-            y = y1
-        return torch.stack(outs, dim=-2)
-
-    zc = z0.detach().contiguous()
-    if not use_graph:
-        return run(zc)
+def _graph_replay(run, zc, state_key, func, X, method, step_size, t):
+    """``run(zc)`` as a replay of a CUDA graph of ``run``, captured once per (func, X, state, schedule) -- for small
+    states the stage loop is launch-bound (12 launches per stage), which is what a graph removes.  The graph reads
+    ``func``'s parameters and X's coefficients from their own storage, so in-place updates of either
+    (``optimizer.step()``) are seen by a replay.  The cache key is everything a replay cannot see change: the ``func``
+    and ``X`` objects, the state (``state_key``: its shape, or its members' shapes), dtype and device, the method, step
+    and output times, the ``training`` flag of every submodule of ``func`` (a branch on ``self.training`` is baked into
+    the capture), and the storage address, shape and dtype of every parameter and buffer of ``func`` and of every buffer
+    of ``X`` (``p.data = ...``, ``module.double().float()`` or ``load_state_dict(..., assign=True)`` give a parameter
+    new storage, which the captured kernels would not read; a view of the same storage can start at the same address
+    with another extent).  The cache entry keeps those tensors alive, so no address in a key can be reused while its
+    graph is cached."""
+    dtype, device = zc.dtype, zc.device
     modules = list(func.modules()) if isinstance(func, torch.nn.Module) else []
     read = [x for m in modules for x in m.parameters(recurse=False)] + \
         [x for m in modules for x in m.buffers(recurse=False)] + list(X.buffers())
-    key = (id(func), id(X), tuple(zc.shape), dtype, str(device), method, step_size,
+    key = (id(func), id(X), state_key, dtype, str(device), method, step_size,
            tuple(float(v) for v in t.detach().cpu().tolist()), tuple(m.training for m in modules),
-           tuple(x.data_ptr() for x in read))
+           tuple((x.data_ptr(), tuple(x.shape), x.dtype) for x in read))
     hit = _graphs.get(key)
     if hit is None:
         static_in = zc.clone()
@@ -272,6 +237,60 @@ def _generic_solve_kernels(X, func, z0, t, method, step_size, is_prod, use_graph
     static_in.copy_(zc)
     graph.replay()
     return static_out.clone()
+
+
+def _generic_solve_kernels(X, func, z0, t, method, step_size, is_prod, use_graph=False):
+    """The fixed-step stage loop for an arbitrary ``func`` when nothing needs a gradient: the control's derivative of
+    the four stages of a step is ONE launch of ``tcde_spline_eval`` (the reference: ~10 small kernels and 4 host syncs
+    per stage, interpolation_cubic.py:315-336), every Runge-Kutta combination is ONE launch of
+    ``tcde_linear_combination``; only ``func`` itself and the ``f @ dX`` contraction stay torch operators (they are the
+    user's code).  With ``use_graph`` the whole time loop is captured into a CUDA graph and replayed
+    (``_graph_replay``)."""
+    kind, _, channels, n_rows = _control_signature(X)
+    dtype, device = z0.dtype, z0.device
+    sched = build_schedule(t, _schedule_knots(X), n_rows, method, step_size, dtype)
+    n_stages = sched.n_stages
+    control = (X._rows() if kind == _lib.CONTROL_CUBIC else X._coeffs).detach()
+    knots = X._t.detach().to(device=device, dtype=control.dtype).contiguous()
+    index_dev = sched.stage_index.to(device)
+    frac_dev = sched.stage_frac.to(device=device, dtype=control.dtype)
+    times_dev = sched.stage_times.to(device)
+    sign = sched.sign
+
+    def fields_of_step(i):
+        # dX/dt of this step's stages: (..., n_stages, C) in one launch
+        dxs = _eval_kernel(control, knots, control.size(-2), channels, index_dev[i], frac_dev[i], kind, True)
+
+        def field(s, z):
+            ts = times_dev[i, s]
+            dx = dxs[..., s, :]
+            if is_prod:
+                out = func.prod(ts, z, dx)
+                out = out if sign > 0 else -1.0 * out
+                return out if out.is_contiguous() else out.contiguous()
+            # solver.py:129-135: f(t, z) @ dX/dt as one streaming launch (the sign of a reversed solve folded in)
+            f = func(ts, z)
+            if (f.shape != z.shape + (channels,) or f.dtype != dtype or dxs.dtype != dtype or not f.is_cuda
+                    or dxs.shape[:-2] != z.shape[:-1]):
+                out = (f @ dx.unsqueeze(-1)).squeeze(-1)          # an unusual func output: let torch broadcast / promote
+                out = out if sign > 0 else -1.0 * out
+                return out if out.is_contiguous() else out.contiguous()
+            f = f if f.is_contiguous() else f.contiguous()
+            out = torch.empty_like(z)
+            _lib.call("tcde_field_contract", _lib.ptr(f), _lib.ptr(dx), _lib.ptr(out), z.numel() // z.size(-1), z.size(-1),
+                      channels, n_stages * channels, float(sign),
+                      _lib.dtype_code(dtype), _lib.stream_of(z))
+            return out
+
+        return field
+
+    def run(y0):
+        return torch.stack(_stage_loop(sched, y0, fields_of_step), dim=-2)
+
+    zc = z0.detach().contiguous()
+    if not use_graph:
+        return run(zc)
+    return _graph_replay(run, zc, tuple(zc.shape), func, X, method, step_size, t)
 
 
 def _host_locator(X, state_dtype):
@@ -355,6 +374,74 @@ def _oriented_times(times, method, options):
 def _time_first_to_reference_layout(out):
     dims = range(1, out.dim() - 1)
     return out.permute(*dims, 0, -1)
+
+
+def _linear_field_or_check(X, func, z0, t, times, sig, is_prod):
+    """``(weight, bias)`` when ``func`` is the README-form linear field on a built-in control, whose shapes are then
+    checked from metadata (nothing is evaluated on the batch); otherwise None, after the reference's own compatibility
+    check (solver.py:44-100): one evaluation at t[0]."""
+    if sig is not None and not is_prod and times:
+        field_params = linear_field_of(func, z0, sig[2], times)
+        if field_params is not None:
+            _shape_error_forward(sig[1] + (sig[2],), tuple(z0.shape[:-1]) + (z0.size(-1), sig[2]), z0)
+            return field_params
+    _lib.require_cuda(z0)
+    control_gradient = X.derivative(t[0].detach())
+    if not isinstance(control_gradient, torch.Tensor):
+        raise ValueError("z0 is a tensor and so X.derivative must return a tensor as well.")
+    if is_prod:
+        vector_field = func.prod(t[0], z0, control_gradient)
+        if not isinstance(vector_field, torch.Tensor):
+            raise ValueError("z0 is a tensor and so func.prod must return a tensor as well.")
+        _shape_error_prod(tuple(control_gradient.shape), tuple(vector_field.shape), z0)
+    else:
+        system = func(t[0], z0)
+        if not isinstance(system, torch.Tensor):
+            raise ValueError("z0 is a tensor and so func must return a tensor as well.")
+        _shape_error_forward(tuple(control_gradient.shape), tuple(system.shape), z0)
+    return None
+
+
+def _adjoint_params(func, kwargs):
+    """``kwargs['adjoint_params']``, by default the parameters of ``func``."""
+    if 'adjoint_params' in kwargs:
+        return tuple(kwargs['adjoint_params'])
+    return tuple(func.parameters()) if isinstance(func, torch.nn.Module) else ()
+
+
+def _wants_grad(states, t, X, func, adjoint_params):
+    """Whether grad mode is on and a gradient is wanted for a tensor of ``states``, the output times ``t``, the
+    control, ``func`` or ``adjoint_params``."""
+    # a user-defined control need not be a module: all it must have is ``derivative``
+    differentiable = tuple(states) + (t,) + (tuple(X.buffers()) if isinstance(X, torch.nn.Module) else ()) + \
+        (tuple(func.parameters()) if isinstance(func, torch.nn.Module) else ()) + adjoint_params
+    return torch.is_grad_enabled() and any(isinstance(x, torch.Tensor) and x.requires_grad for x in differentiable)
+
+
+def _adjoint_solve(kwargs, method, step_size, norm_of=None):
+    """The backward solve of ``adjoint=True``: ``solve_aug(f, v, ts)`` with ``adjoint_method`` (the forward's method by
+    default), and ``(method, step_size)`` of that solve when it is a fixed-step one, else None.  ``norm_of(v)``: the
+    error norm of a dopri5 backward on the augmented state ``v`` (default RMS)."""
+    a_method = kwargs.get("adjoint_method", None) or method
+    if a_method in FIXED_METHODS:
+        a_options = dict(kwargs.get("adjoint_options", None) or ({"step_size": step_size} if step_size else {}))
+        a_step = a_options.get("step_size", None)
+        return (lambda f, v, ts: adaptive.odeint_fixed(f, v, ts, a_method, a_step)), (a_method, a_step)
+    a_rtol, a_atol = kwargs["adjoint_rtol"], kwargs["adjoint_atol"]
+
+    def solve_aug(f, v, ts):
+        return adaptive.odeint_dopri5(f, v, ts, a_rtol, a_atol, norm=None if norm_of is None else norm_of(v))[0]
+
+    return solve_aug, None
+
+
+def _host_dopri5(field, y0, times, rtol, atol, options, norm=None):
+    """The host-driven dopri5 solve of the outputs (``adaptive.odeint_dopri5``); its step counts go to
+    ``cdeint.last_stats``."""
+    out, solver_obj = adaptive.odeint_dopri5(field, y0, times, rtol, atol, options, norm=norm)
+    cdeint.last_stats = {"n_accepted": solver_obj.n_accepted, "n_rejected": solver_obj.n_rejected,
+                         "device_controlled": False}
+    return out
 
 
 def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
@@ -447,40 +534,10 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
     _warn_control_gradients(X, adjoint, kwargs)
 
     # ---- what kind of problem is this? -----------------------------------------------------------
-    field_params = None
-    if sig is not None and not is_prod:
-        kind, batch, channels, _ = sig
-        field_params = linear_field_of(func, z0, channels, times) if times else None
-    if field_params is not None:
-        # shapes are checked from metadata: nothing is evaluated on the batch
-        _shape_error_forward(batch + (channels,), tuple(z0.shape[:-1]) + (z0.size(-1), channels), z0)
-    else:
-        # the reference's own compatibility check (solver.py:44-100): one evaluation at t[0]
-        _lib.require_cuda(z0)
-        control_gradient = X.derivative(t[0].detach())
-        if not isinstance(control_gradient, torch.Tensor):
-            raise ValueError("z0 is a tensor and so X.derivative must return a tensor as well.")
-        if is_prod:
-            vector_field = func.prod(t[0], z0, control_gradient)
-            if not isinstance(vector_field, torch.Tensor):
-                raise ValueError("z0 is a tensor and so func.prod must return a tensor as well.")
-            _shape_error_prod(tuple(control_gradient.shape), tuple(vector_field.shape), z0)
-        else:
-            system = func(t[0], z0)
-            if not isinstance(system, torch.Tensor):
-                raise ValueError("z0 is a tensor and so func must return a tensor as well.")
-            _shape_error_forward(tuple(control_gradient.shape), tuple(system.shape), z0)
+    field_params = _linear_field_or_check(X, func, z0, t, times, sig, is_prod)
     _lib.require_cuda(z0)
-
-    if 'adjoint_params' in kwargs:
-        adjoint_params = tuple(kwargs['adjoint_params'])
-    else:
-        adjoint_params = tuple(func.parameters()) if isinstance(func, torch.nn.Module) else ()
-    # a user-defined control need not be a module: all it must have is ``derivative``
-    differentiable = (z0, t) + (tuple(X.buffers()) if isinstance(X, torch.nn.Module) else ()) + \
-        (tuple(func.parameters()) if isinstance(func, torch.nn.Module) else ()) + adjoint_params
-    wants_grad = torch.is_grad_enabled() and any(isinstance(x, torch.Tensor) and x.requires_grad
-                                                 for x in differentiable)
+    adjoint_params = _adjoint_params(func, kwargs)
+    wants_grad = _wants_grad((z0,), t, X, func, adjoint_params)
 
     times, flipped = _oriented_times(times, method, options)
 
@@ -537,10 +594,7 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
                 pass
 
         field = host_dopri5_field(kernels if kernels is not None else mlp, y0)
-        out, solver_obj = adaptive.odeint_dopri5(_reverse(field) if flipped else field, y0, times, rtol, atol, options)
-        cdeint.last_stats = {"n_accepted": solver_obj.n_accepted, "n_rejected": solver_obj.n_rejected,
-                             "device_controlled": False}
-        return out
+        return _host_dopri5(_reverse(field) if flipped else field, y0, times, rtol, atol, options)
 
     # adjoint=False with gradients: the kernel routes serve gradients for z0 and the field's parameters; a gradient for
     # anything else (t, the control's knots or coefficients) keeps the torch-operator solve
@@ -565,15 +619,7 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
             return _time_first_to_reference_layout(forward_values(z0))
 
     if adjoint:
-        a_rtol, a_atol = kwargs["adjoint_rtol"], kwargs["adjoint_atol"]
-        a_method = kwargs.get("adjoint_method", None) or method
-        a_options = dict(kwargs.get("adjoint_options", None) or ({"step_size": step_size} if step_size else {}))
-
-        def solve_aug(f, v, ts):
-            if a_method in FIXED_METHODS:
-                return adaptive.odeint_fixed(f, v, ts, a_method, a_options.get("step_size", None))
-            return adaptive.odeint_dopri5(f, v, ts, a_rtol, a_atol)[0]
-
+        solve_aug, fixed_spec = _adjoint_solve(kwargs, method, step_size)
         t_grad = t if t.requires_grad else None
 
         def fused_vjp(params):
@@ -584,13 +630,12 @@ def cdeint(X, func, z0, t, adjoint=True, backend="torchdiffeq", **kwargs):
             if kernels is None:
                 return _mlp_vjp(mlp, params) if mlp is not None else None
             st = _kernel_vjp(kernels, params)
-            if (st is not None and a_method not in FIXED_METHODS and adaptive.device_dopri5_available(z0, sig[2])
+            if (st is not None and fixed_spec is None and adaptive.device_dopri5_available(z0, sig[2])
                     and not kwargs.get("adjoint_options", None)):
                 # dopri5 backward with the controller on the device; the forward pass's step count sizes the trajectory slots
-                st.adaptive_spec = (a_rtol, a_atol)
+                st.adaptive_spec = (kwargs["adjoint_rtol"], kwargs["adjoint_atol"])
             return st
 
-        fixed_spec = (a_method, a_options.get("step_size", None)) if a_method in FIXED_METHODS else None
         ys = adaptive.solve_with_adjoint(forward_values, autograd_field(), times, solve_aug, z0, adjoint_params,
                                          fused_vjp, fixed_spec, t_grad, flipped)
         return _time_first_to_reference_layout(ys)

@@ -20,10 +20,13 @@ from . import _lib, adaptive
 from .controls import TupleControl, _control_signature, _schedule_knots
 from .linear_field import _reverse
 from .schedule import FIXED_METHODS, build_schedule, host_locator
+from .solver import (_adjoint_params, _adjoint_solve, _generic_solve, _graph_replay, _host_dopri5, _shape_error_forward,
+                     _shape_error_prod, _stage_loop, _wants_grad)
+from .solver import _graphs  # noqa: F401 -- the one graph cache, which the grouped loop's captures share with solver's
 
 
 # ------------------------------------------------------------------------------- validation (solver.py:68-98)
-def check_compatability(X, func, z0, t, is_prod, shape_error_forward, shape_error_prod):
+def check_compatability(X, func, z0, t, is_prod):
     """The tuple branch of the reference's ``_check_compatability``, message for message."""
     control_gradient = X.derivative(t[0].detach())
     if is_prod:
@@ -44,7 +47,7 @@ def check_compatability(X, func, z0, t, is_prod, shape_error_forward, shape_erro
                 raise ValueError("X.derivative must return a tensor or tuple of tensors.")
             if not isinstance(vector_field_, torch.Tensor):
                 raise ValueError("func.prod must return a tensor or tuple/list of tensors.")
-            shape_error_prod(tuple(control_gradient_.shape), tuple(vector_field_.shape), z0_)
+            _shape_error_prod(tuple(control_gradient_.shape), tuple(vector_field_.shape), z0_)
     else:
         if not isinstance(system, (tuple, list)):
             raise ValueError("z0 is a tuple/list and so func must return a tuple/list as well.")
@@ -55,7 +58,7 @@ def check_compatability(X, func, z0, t, is_prod, shape_error_forward, shape_erro
                 raise ValueError("X.derivative must return a tensor or tuple of tensors.")
             if not isinstance(system_, torch.Tensor):
                 raise ValueError("func must return a tensor or tuple/list of tensors.")
-            shape_error_forward(tuple(control_gradient_.shape), tuple(system_.shape), z0_)
+            _shape_error_forward(tuple(control_gradient_.shape), tuple(system_.shape), z0_)
 
 
 # ------------------------------------------------------------------------------------------------ the packed state
@@ -164,12 +167,9 @@ def _apply_field(func, is_prod, ts, zs, dxs, stage, packing, out, sign):
 
 
 # ---------------------------------------------------------------------------- no gradient, fixed step: grouped loop
-_graphs = {}
-
-
 def grouped_solve(X, func, z0, t, method, step_size, is_prod, packing, use_graph=False):
-    """The fixed-step stage loop of a tuple state (the tuple form of ``solver._generic_solve_kernels``).  ``z0``: the
-    packed state.  Returns (len(t), numel)."""
+    """The fixed-step stage loop of a tuple state: ``solver._stage_loop`` with every member's dX/dt in one grouped
+    evaluation per step and one grouped contraction per stage.  ``z0``: the packed state.  Returns (len(t), numel)."""
     dtype, device = z0.dtype, z0.device
     gc = GroupedControls(list(X.controls), device)
     scheds = [build_schedule(t, _schedule_knots(m[0]), m[4], method, step_size, dtype) for m in gc.members]
@@ -178,70 +178,23 @@ def grouped_solve(X, func, z0, t, method, step_size, is_prod, packing, use_graph
     frac_dev = [s.stage_frac.to(device=device, dtype=gc.dtype) for s in scheds]
     times_dev = sched.stage_times.to(device)
     sign = sched.sign
-    from .adaptive import _combine
+
+    def fields_of_step(i):
+        dxs = gc.evaluate([ix[i] for ix in index_dev], [fr[i] for fr in frac_dev])       # every member, every stage
+
+        def field(s, z):
+            return _apply_field(func, is_prod, times_dev[i, s], packing.views(z), dxs, s, packing,
+                                torch.empty_like(z), sign)
+
+        return field
 
     def run(y0):
-        outs = [None] * sched.n_out
-        j = 0
-        while j < sched.n_out and int(sched.out_step[j]) < 0:
-            outs[j] = y0
-            j += 1
-        y = y0
-        for i in range(sched.n_steps):
-            dxs = gc.evaluate([ix[i] for ix in index_dev], [fr[i] for fr in frac_dev])       # every member, every stage
-
-            def field(s, z):
-                return _apply_field(func, is_prod, times_dev[i, s], packing.views(z), dxs, s, packing,
-                                    torch.empty_like(z), sign)
-
-            dt = float(sched.step_dt[i])
-            if method == "rk4":
-                k1 = field(0, y)
-                k2 = field(1, _combine(y, [k1], (1 / 3,), dt))
-                k3 = field(2, _combine(y, [k1, k2], (-1 / 3, 1.0), dt))
-                k4 = field(3, _combine(y, [k1, k2, k3], (1.0, -1.0, 1.0), dt))
-                y1 = _combine(y, [k1, k2, k3, k4], (0.125, 0.375, 0.375, 0.125), dt)
-            elif method == "midpoint":
-                k1 = field(0, y)
-                y1 = _combine(y, [field(1, _combine(y, [k1], (0.5,), dt))], (1.0,), dt)
-            else:
-                y1 = _combine(y, [field(0, y)], (1.0,), dt)
-            while j < sched.n_out and int(sched.out_step[j]) == i:
-                mode = int(sched.out_mode[j])
-                outs[j] = y if mode == 0 else y1 if mode == 1 else _combine(y, [y1, y], (1.0, -1.0), float(sched.out_slope[j]))
-                j += 1
-            y = y1
-        return torch.stack(outs, dim=0)
+        return torch.stack(_stage_loop(sched, y0, fields_of_step), dim=0)
 
     zc = z0.detach().contiguous()
     if not use_graph:
         return run(zc)
-    # the cache key of solver._generic_solve_kernels, over every member: what a replay cannot see change
-    modules = list(func.modules()) if isinstance(func, torch.nn.Module) else []
-    read = [x for m in modules for x in m.parameters(recurse=False)] + \
-        [x for m in modules for x in m.buffers(recurse=False)] + list(X.buffers())
-    key = (id(func), id(X), tuple(packing.shapes), dtype, str(device), method, step_size,
-           tuple(float(v) for v in t.detach().cpu().tolist()), tuple(m.training for m in modules),
-           tuple((x.data_ptr(), tuple(x.shape), x.dtype) for x in read))
-    hit = _graphs.get(key)
-    if hit is None:
-        static_in = zc.clone()
-        side = torch.cuda.Stream(device)
-        side.wait_stream(torch.cuda.current_stream(device))
-        with torch.cuda.stream(side):                      # warm-up outside the capture (lazy initialisations)
-            run(static_in)
-        torch.cuda.current_stream(device).wait_stream(side)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            static_out = run(static_in)
-        hit = (graph, static_in, static_out, func, X, run, read)
-        if len(_graphs) >= 8:
-            _graphs.clear()
-        _graphs[key] = hit
-    graph, static_in, static_out = hit[:3]
-    static_in.copy_(zc)
-    graph.replay()
-    return static_out.clone()
+    return _graph_replay(run, zc, tuple(packing.shapes), func, X, method, step_size, t)
 
 
 def grouped_field(X, func, is_prod, packing, dtype, device):
@@ -280,8 +233,7 @@ def torch_field(X, func, is_prod, packing, dtype):
 # ----------------------------------------------------------------------------------------------------- the driver
 def cdeint_tuple(X, func, z0, t, adjoint, kwargs, method, step_size, use_graph, options, times, flipped, is_prod):
     """``solver.cdeint`` for a tuple / list ``z0`` (after its argument parsing).  Returns the reference's output tuple."""
-    from .solver import _generic_solve, _shape_error_forward, _shape_error_prod
-    check_compatability(X, func, z0, t, is_prod, _shape_error_forward, _shape_error_prod)
+    check_compatability(X, func, z0, t, is_prod)
     _lib.require_cuda(*z0)
     packing = Packing(z0)
     y0 = packing.pack(z0)
@@ -291,14 +243,8 @@ def cdeint_tuple(X, func, z0, t, adjoint, kwargs, method, step_size, use_graph, 
                 and all(_control_signature(m) is not None for m in controls)
                 and all(b.device == device and b.dtype == dtype for m in controls for b in m.buffers()))
 
-    if 'adjoint_params' in kwargs:
-        adjoint_params = tuple(kwargs['adjoint_params'])
-    else:
-        adjoint_params = tuple(func.parameters()) if isinstance(func, torch.nn.Module) else ()
-    differentiable = tuple(z0) + (t,) + (tuple(X.buffers()) if isinstance(X, torch.nn.Module) else ()) + \
-        (tuple(func.parameters()) if isinstance(func, torch.nn.Module) else ()) + adjoint_params
-    wants_grad = torch.is_grad_enabled() and any(isinstance(x, torch.Tensor) and x.requires_grad
-                                                 for x in differentiable)
+    adjoint_params = _adjoint_params(func, kwargs)
+    wants_grad = _wants_grad(z0, t, X, func, adjoint_params)
     rtol, atol = kwargs['rtol'], kwargs['atol']
     prod = _PackedProd(func, is_prod, packing)
 
@@ -310,12 +256,8 @@ def cdeint_tuple(X, func, z0, t, adjoint, kwargs, method, step_size, use_graph, 
             return _generic_solve(X, prod, v0, t, method, step_size, True, False)
         field = grouped_field(X, func, is_prod, packing, dtype, device) if built_in and not torch.is_grad_enabled() \
             else torch_field(X, func, is_prod, packing, dtype)
-        out, solver_obj = adaptive.odeint_dopri5(_reverse(field) if flipped else field, v0, times, rtol, atol, options,
-                                                 norm=adaptive.tuple_norm(packing.sizes))
-        from .solver import cdeint
-        cdeint.last_stats = {"n_accepted": solver_obj.n_accepted, "n_rejected": solver_obj.n_rejected,
-                             "device_controlled": False}
-        return out
+        return _host_dopri5(_reverse(field) if flipped else field, v0, times, rtol, atol, options,
+                            norm=adaptive.tuple_norm(packing.sizes))
 
     if not wants_grad:
         with torch.no_grad():
@@ -326,20 +268,16 @@ def cdeint_tuple(X, func, z0, t, adjoint, kwargs, method, step_size, use_graph, 
         return _reverse(f) if flipped else f
 
     if adjoint:
-        a_rtol, a_atol = kwargs["adjoint_rtol"], kwargs["adjoint_atol"]
-        a_method = kwargs.get("adjoint_method", None) or method
-        a_options = dict(kwargs.get("adjoint_options", None) or ({"step_size": step_size} if step_size else {}))
         t_grad = t if t.requires_grad else None
         n_params = sum(p.numel() for p in adjoint_params if p.requires_grad and p is not t_grad)
 
-        def solve_aug(f, v, ts):
-            if a_method in FIXED_METHODS:
-                return adaptive.odeint_fixed(f, v, ts, a_method, a_options.get("step_size", None))
+        def aug_norm(v):
             # the augmented state (a_t?, y, a, params): the tuple norm on y and on a, the RMS of the rest
             lead = v.numel() - 2 * packing.numel - n_params
             sizes = ([lead] if lead else []) + packing.sizes + packing.sizes + ([n_params] if n_params else [])
-            return adaptive.odeint_dopri5(f, v, ts, a_rtol, a_atol, norm=adaptive.tuple_norm(sizes))[0]
+            return adaptive.tuple_norm(sizes)
 
+        solve_aug, _fixed_spec = _adjoint_solve(kwargs, method, step_size, aug_norm)
         ys = adaptive.solve_with_adjoint(forward_values, autograd_field(), times, solve_aug, y0, adjoint_params,
                                          None, None, t_grad, flipped)
         return packing.outputs(ys)
